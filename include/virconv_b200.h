@@ -286,6 +286,34 @@ int vc_group_points_grad(int B, int M, int C, int N, int nsample, const float* g
                          vc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Rotated-box IoU and NMS of the detector heads: the reference's `iou3d_nms_cuda` extension (pcdet/ops/iou3d_nms), whose
+ * rules csrc/iou3d_nms.cu states.  Boxes are (x, y, z, dx, dy, dz, heading) fp32; the pairwise calls take [n, 7] row-major.
+ *   vc_boxes_overlap_bev  <- boxesoverlapLauncher (iou3d_nms_kernel.cu:378-387): out [na, nb] = BEV intersection area.
+ *   vc_boxes_iou_bev      <- boxesioubevLauncher (:389-398): out [na, nb] = BEV IoU.
+ *   vc_boxes_iou3d        <- boxesoverlapLauncher + the torch glue of iou3d_nms_utils.boxes_iou3d_gpu (:67-100), fused:
+ *                            out [na, nb] = 3-D IoU.
+ *   vc_boxes_iou_bev_host <- boxes_iou_bev_cpu (iou3d_cpu.cpp:232-252): HOST pointers, no GPU needed; bit-identical to
+ *                            vc_boxes_iou_bev (shared geometry code).
+ *   vc_nms_boxes          <- nmsLauncher / nmsNormalLauncher plus the host side of nms_gpu / nms_normal_gpu
+ *                            (iou3d_nms.cpp:90-186), batched over segments and without a host read:
+ *                            boxes [batch, n_max, ld] (ld >= 7, columns 0..6 used; each segment sorted by descending
+ *                            score), counts [batch] device int32 = valid rows per segment (clamped to [0, n_max]),
+ *                            normal != 0: axis-aligned IoU (heading ignored).  Box j is dropped when an earlier kept box
+ *                            has IoU > thresh with it; at most post_max boxes are kept.  keep [batch, post_max] int32 =
+ *                            kept row indices in order, tail -1; num_keep [batch] int32.  Two launches (upper-triangle
+ *                            suppression mask into ws, then the greedy pass on the device), graph-capturable.
+ *                            ws >= vc_nms_ws_bytes(batch, n_max); n_max > VC_NMS_MAX_BOXES -> VC_ERR_UNSUPPORTED.
+ * ---------------------------------------------------------------------------------------------- */
+#define VC_NMS_MAX_BOXES 16384
+int vc_boxes_overlap_bev(const float* boxes_a, int na, const float* boxes_b, int nb, float* out, vc_stream_t stream);
+int vc_boxes_iou_bev(const float* boxes_a, int na, const float* boxes_b, int nb, float* out, vc_stream_t stream);
+int vc_boxes_iou3d(const float* boxes_a, int na, const float* boxes_b, int nb, float* out, vc_stream_t stream);
+int vc_boxes_iou_bev_host(const float* boxes_a /*host*/, int na, const float* boxes_b /*host*/, int nb, float* out /*host*/);
+size_t vc_nms_ws_bytes(int batch, int n_max);
+int vc_nms_boxes(const float* boxes, int batch, int n_max, int ld, const int32_t* counts, float thresh, int normal,
+                 int post_max, int32_t* keep, int32_t* num_keep, void* ws, size_t ws_bytes, vc_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Plan executor: a whole backbone forward / backward in ONE call.  Replaces the Python layer loop of
  * `VirConvL8x.forward` (spconv_backbone.py:609-699), `NRConvBlock.forward` (:207-229) and the two streams of
  * `VirConv8x.forward` (:339-535) together with autograd's reverse walk over them: the host side of ~100 operator

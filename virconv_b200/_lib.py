@@ -66,6 +66,12 @@ SIGNATURES = {
     'vc_voxel_query': (_I, [_I, _I, _I, _I, _I, _F, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     'vc_group_points': (_I, [_I, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
     'vc_group_points_grad': (_I, [_I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
+    'vc_boxes_overlap_bev': (_I, [_P, _I, _P, _I, _P, _P]),
+    'vc_boxes_iou_bev': (_I, [_P, _I, _P, _I, _P, _P]),
+    'vc_boxes_iou3d': (_I, [_P, _I, _P, _I, _P, _P]),
+    'vc_boxes_iou_bev_host': (_I, [_P, _I, _P, _I, _P]),
+    'vc_nms_ws_bytes': (_Z, [_I, _I]),
+    'vc_nms_boxes': (_I, [_P, _I, _I, _I, _P, _F, _I, _I, _P, _P, _P, _Z, _P]),
     'vc_exec_state_bytes': (_Z, []),
     'vc_exec_forward': (_I, [_P, _P, _I, _P, _P, _I, _P, _I, _P, _I, _HOST, _I, _P, _I, _I, _I, _P, _Z, _P, _P, _P, _Z, _P, _P, _I,
                              _P, _P, _P, _P]),

@@ -19,6 +19,13 @@ NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo',
          '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr',
          '-DVC_BUILDING']
+# per-source additions.  iou3d_nms.cu: no a*b+c contraction on either side, so that its __host__ __device__ box geometry
+# rounds identically on the host (vc_boxes_iou_bev_host) and on the GPU
+FILE_FLAGS = {'iou3d_nms.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off']}
+
+
+def flags_for(src):
+    return FLAGS + FILE_FLAGS.get(os.path.basename(src), [])
 
 
 def sources():
@@ -32,6 +39,7 @@ def _digest(paths):
             h.update(p.encode())
             h.update(f.read())
     h.update(' '.join(FLAGS).encode())
+    h.update(repr(sorted(FILE_FLAGS.items())).encode())
     return h.hexdigest()
 
 
@@ -52,7 +60,7 @@ def build(verbose: bool = False, force: bool = False, defines=(), suffix: str = 
 
     def compile_one(src):
         obj = os.path.join(LIBDIR, os.path.basename(src)[:-3] + '.o')
-        cmd = [NVCC] + FLAGS + (['-Xptxas', '-v'] if verbose else []) + ['-c', src, '-o', obj]
+        cmd = [NVCC] + flags_for(src) + (['-Xptxas', '-v'] if verbose else []) + ['-c', src, '-o', obj]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError('nvcc failed for %s:\n%s\n%s' % (src, r.stdout, r.stderr))
@@ -76,7 +84,7 @@ def _build_variant(defines, suffix, verbose):
     objs = []
     for src in sources():
         obj = os.path.join(LIBDIR, os.path.basename(src)[:-3] + f'_{suffix}.o')
-        r = subprocess.run([NVCC] + FLAGS + [f'-D{d}' for d in defines] + ['-c', src, '-o', obj], capture_output=True, text=True)
+        r = subprocess.run([NVCC] + flags_for(src) + [f'-D{d}' for d in defines] + ['-c', src, '-o', obj], capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError('nvcc failed for %s:\n%s' % (src, r.stderr))
         objs.append(obj)

@@ -14,9 +14,12 @@ What it registers (nothing is written into the reference tree, nothing from it i
       - `pointnet2_stack_cuda.voxel_query_wrapper / group_points_wrapper / group_points_grad_wrapper` run on this
         library's kernels (vc_voxel_query, vc_group_points, vc_group_points_grad: bit-exact against the reference's own
         CUDA, tests/test_gpu_roi_pool.py) — the voxel-RoI pooling of TEDMHead (ted_head.py:496-552);
+      - `iou3d_nms_cuda.boxes_overlap_bev_gpu / boxes_iou_bev_gpu / nms_gpu / nms_normal_gpu / boxes_iou_bev_cpu` run
+        on this library's rotated-box kernels (csrc/iou3d_nms.cu; the CPU one on its host entry point), with the
+        pybind signatures of iou3d_nms_api.cpp: the proposal / final NMS, RoI target assignment and GT sampling;
       - `roiaware_pool3d_cuda.points_in_boxes_cpu` (dataset-side augmentation) is restated in torch;
-      - everything else (rotated-box NMS / IoU, ball query, FPS, deformable conv, VOTR ops) is import-only: calling
-        it raises NotImplementedError naming the reference source that would have to be built.
+      - everything else (ball query, FPS, points_in_boxes_gpu, RoI-point pooling, deformable conv, VOTR ops) is
+        import-only: calling it raises NotImplementedError naming the reference source that would have to be built.
 With `use_fused_backbones` the detector registry (`pcdet.models.backbones_3d.__all__`) hands out this package's
 VirConvL8x / VirConv8x (plan executor, fused conv+BN+ReLU) instead of the reference classes over the compat layer.
 """
@@ -137,6 +140,61 @@ def _group_points_grad_wrapper(B, M, C, N, nsample, grad_out, idx, idx_batch_cnt
                'vc_group_points_grad')
 
 
+# ---- iou3d_nms: rotated-box IoU / NMS, on this library's kernels (iou3d_nms_api.cpp:8-14) -------------------------------
+def _pairwise_into(fn, boxes_a, boxes_b, out):
+    from . import _lib, ops
+    lib = _lib.load()
+    ops._require_cuda(boxes_a, boxes_b, out)
+    assert out.is_contiguous() and out.dtype == torch.float32
+    a, b = boxes_a.contiguous(), boxes_b.contiguous()
+    _lib.check(getattr(lib, fn)(a.data_ptr(), a.shape[0], b.data_ptr(), b.shape[0], out.data_ptr(), ops._stream()), fn)
+    return 1
+
+
+def _boxes_overlap_bev_gpu(boxes_a, boxes_b, ans_overlap):
+    """iou3d_nms_cuda.boxes_overlap_bev_gpu (iou3d_nms.cpp:49-68): fills ans_overlap [N, M] with the BEV intersection areas."""
+    return _pairwise_into('vc_boxes_overlap_bev', boxes_a, boxes_b, ans_overlap)
+
+
+def _boxes_iou_bev_gpu(boxes_a, boxes_b, ans_iou):
+    """iou3d_nms_cuda.boxes_iou_bev_gpu (iou3d_nms.cpp:70-88): fills ans_iou [N, M] with the BEV IoU."""
+    return _pairwise_into('vc_boxes_iou_bev', boxes_a, boxes_b, ans_iou)
+
+
+def _boxes_iou_bev_cpu(boxes_a, boxes_b, ans_iou):
+    """iou3d_nms_cuda.boxes_iou_bev_cpu (iou3d_cpu.cpp:232-252): CPU tensors, fills ans_iou [N, M]."""
+    from . import _lib
+    assert not (boxes_a.is_cuda or boxes_b.is_cuda or ans_iou.is_cuda), 'Only support CPU tensors'
+    assert ans_iou.is_contiguous() and ans_iou.dtype == torch.float32
+    a, b = boxes_a.float().contiguous(), boxes_b.float().contiguous()
+    _lib.check(_lib.load().vc_boxes_iou_bev_host(a.data_ptr(), a.shape[0], b.data_ptr(), b.shape[0], ans_iou.data_ptr()),
+               'vc_boxes_iou_bev_host')
+    return 1
+
+
+def _nms_into(boxes, keep, thresh, normal):
+    from . import iou3d_nms
+    n = boxes.shape[0]
+    if n == 0:
+        return 0
+    counts = torch.full((1,), n, dtype=torch.int32, device=boxes.device)
+    k, num = iou3d_nms._nms_sorted(boxes.float().contiguous().view(1, n, -1), counts, thresh, n, normal)
+    num_out = int(num.item())
+    keep[:num_out] = k[0, :num_out].cpu().to(keep.dtype)
+    return num_out
+
+
+def _nms_gpu(boxes, keep, nms_overlap_thresh):
+    """iou3d_nms_cuda.nms_gpu (iou3d_nms.cpp:90-136): boxes [N, 7] on the GPU, already in descending score order; writes the
+    kept row indices into the CPU LongTensor `keep` and returns their number."""
+    return _nms_into(boxes, keep, nms_overlap_thresh, False)
+
+
+def _nms_normal_gpu(boxes, keep, nms_overlap_thresh):
+    """iou3d_nms_cuda.nms_normal_gpu (iou3d_nms.cpp:139-186): the axis-aligned variant of _nms_gpu."""
+    return _nms_into(boxes, keep, nms_overlap_thresh, True)
+
+
 def _points_in_boxes_cpu(boxes, points, point_indices):
     """roiaware_pool3d_cuda.points_in_boxes_cpu (roiaware_pool3d_utils.py:9-26; src/roiaware_pool3d.cpp:106-140): CPU tensors,
     boxes [N, 7] (x, y, z, dx, dy, dz, heading) with z at the box centre, points [M, 3]; point_indices [N, M] int32 set to 1
@@ -195,8 +253,9 @@ def install(use_fused_backbones=False, reference_root=None):
         sk.io = _module('skimage.io', imread=_unbuilt('skimage.io', 'imread', 'scikit-image'))
 
     # the compiled extensions of pcdet/ops: module objects under the names the reference imports
-    _stub_ext('pcdet.ops.iou3d_nms.iou3d_nms_cuda', 'pcdet/ops/iou3d_nms/src',
-              ['boxes_overlap_bev_gpu', 'boxes_iou_bev_gpu', 'nms_gpu', 'nms_normal_gpu', 'boxes_iou_bev_cpu'])
+    _stub_ext('pcdet.ops.iou3d_nms.iou3d_nms_cuda', 'pcdet/ops/iou3d_nms/src', [],
+              boxes_overlap_bev_gpu=_boxes_overlap_bev_gpu, boxes_iou_bev_gpu=_boxes_iou_bev_gpu, nms_gpu=_nms_gpu,
+              nms_normal_gpu=_nms_normal_gpu, boxes_iou_bev_cpu=_boxes_iou_bev_cpu)
     _stub_ext('pcdet.ops.roiaware_pool3d.roiaware_pool3d_cuda', 'pcdet/ops/roiaware_pool3d/src',
               ['forward', 'backward', 'points_in_boxes_gpu'], points_in_boxes_cpu=_points_in_boxes_cpu)
     _stub_ext('pcdet.ops.roipoint_pool3d.roipoint_pool3d_cuda', 'pcdet/ops/roipoint_pool3d/src', ['forward'])
