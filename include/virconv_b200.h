@@ -353,6 +353,33 @@ int vc_nms_boxes(const float* boxes, int batch, int n_max, int ld, const int32_t
                  int post_max, int32_t* keep, int32_t* num_keep, void* ws, size_t ws_bytes, vc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Anchor-head targets of the RPN (AnchorHeadSingle), whose rules csrc/anchor_targets.cu states.  No call reads the
+ * device on the host; both are graph-capturable.
+ *   vc_anchor_mask    <- AnchorHeadSingle.get_anchor_mask (anchor_head_single.py:75-115): points [n_points, ld] fp32
+ *                        (column 1 = x, column 2 = y, all scenes together), min_x / min_y = point_cloud_range[0:2],
+ *                        inv_stride = 1.0f / float(round(voxel_size * 80)) -> mask [H, W] uint8 (0 / 1).  coarse
+ *                        [H/10 * W/10] uint8 is scratch, zeroed by the caller.  Two launches.
+ *   vc_anchor_targets <- AxisAlignedTargetAssigner.assign_targets (axis_aligned_target_assigner.py:46-243; POS_FRACTION
+ *                        < 0, MATCH_HEIGHT False, not multihead, NORM_BY_NUM_EXAMPLES False) for all scenes and anchor
+ *                        sets in one grid: anchors [N, 7] in the output order with anchor_set [N] int32 in [0, n_sets);
+ *                        matched / unmatched [n_sets] HOST fp32 thresholds; gt [B, M, ld] (ld >= 8, class in the last
+ *                        column); name_sets [n_names] HOST = bitmask of the anchor sets whose class name is class_names[k]
+ *                        -> labels [B, N] int32, targets [B, N, 7], reg_weights [B, N], gt_ious [B, N] fp32, every element
+ *                        written.  ws >= vc_anchor_targets_ws_bytes(B, n_sets, M); M > VC_ANCHOR_MAX_GT ->
+ *                        VC_ERR_UNSUPPORTED.  A memset and two launches.
+ * ---------------------------------------------------------------------------------------------- */
+#define VC_ANCHOR_MAX_GT 512
+#define VC_ANCHOR_MAX_SETS 8
+#define VC_ANCHOR_MAX_NAMES 32
+int vc_anchor_mask(const float* points, int n_points, int ld, float min_x, float min_y, float inv_stride, int H, int W,
+                   unsigned char* coarse, unsigned char* mask, vc_stream_t stream);
+size_t vc_anchor_targets_ws_bytes(int B, int n_sets, int M);
+int vc_anchor_targets(const float* anchors, const int32_t* anchor_set, int N, int n_sets, const float* matched /*host*/,
+                      const float* unmatched /*host*/, const float* gt, int B, int M, int ld, const int32_t* name_sets /*host*/,
+                      int n_names, int32_t* labels, float* targets, float* reg_weights, float* gt_ious, void* ws,
+                      size_t ws_bytes, vc_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Plan executor: a whole backbone forward / backward in ONE call.  Replaces the Python layer loop of
  * `VirConvL8x.forward` (spconv_backbone.py:609-699), `NRConvBlock.forward` (:207-229) and the two streams of
  * `VirConv8x.forward` (:339-535) together with autograd's reverse walk over them: the host side of ~100 operator

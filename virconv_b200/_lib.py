@@ -78,6 +78,9 @@ SIGNATURES = {
     'vc_boxes_iou_bev_host': (_I, [_P, _I, _P, _I, _P]),
     'vc_nms_ws_bytes': (_Z, [_I, _I]),
     'vc_nms_boxes': (_I, [_P, _I, _I, _I, _P, _F, _I, _I, _P, _P, _P, _Z, _P]),
+    'vc_anchor_mask': (_I, [_P, _I, _I, _F, _F, _F, _I, _I, _P, _P, _P]),
+    'vc_anchor_targets_ws_bytes': (_Z, [_I, _I, _I]),
+    'vc_anchor_targets': (_I, [_P, _P, _I, _I, _HOSTF, _HOSTF, _P, _I, _I, _I, _HOST, _I, _P, _P, _P, _P, _P, _Z, _P]),
     'vc_exec_state_bytes': (_Z, []),
     'vc_exec_forward': (_I, [_P, _P, _I, _P, _P, _I, _P, _I, _P, _I, _HOST, _I, _P, _I, _I, _I, _P, _Z, _P, _P, _P, _Z, _P, _P, _I,
                              _P, _P, _P, _P]),

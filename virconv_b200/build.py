@@ -21,7 +21,10 @@ FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-line
          '-DVC_BUILDING']
 # per-source additions.  iou3d_nms.cu: no a*b+c contraction on either side, so that its __host__ __device__ box geometry
 # rounds identically on the host (vc_boxes_iou_bev_host) and on the GPU
-FILE_FLAGS = {'iou3d_nms.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off']}
+# anchor_targets.cu: no contraction either, so that its IoU and box encoding round every operation as torch's elementwise
+# kernels do (the equality tests of the target assignment compare those values)
+FILE_FLAGS = {'iou3d_nms.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
+              'anchor_targets.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off']}
 
 
 def flags_for(src):

@@ -24,6 +24,9 @@ With `use_fused_backbones` the detector registry (`pcdet.models.backbones_3d.__a
 VirConvL8x / VirConv8x (plan executor, fused conv+BN+ReLU) instead of the reference classes over the compat layer.
 With `use_fused_roi_pool` `pcdet.ops.pointnet2.pointnet2_stack.voxel_pool_modules.NeighborVoxelSAModuleMSG` is this
 package's fused class (virconv_b200.voxel_pool), so TEDMHead's RoI grid pooling layers are built from it unchanged.
+With `use_fused_rpn_targets` `AnchorHeadSingle.get_anchor_mask` and the `AxisAlignedTargetAssigner` the anchor heads build
+(looked up in anchor_head_template, which imports the name at module level, and in its own module) are this package's
+device versions (virconv_b200.anchor_targets): the RPN's anchor mask and target assignment without a host read.
 """
 from __future__ import annotations
 
@@ -213,7 +216,7 @@ def _points_in_boxes_cpu(boxes, points, point_indices):
     return 1
 
 
-def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=False):
+def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=False, use_fused_rpn_targets=False):
     """Register everything listed in the module docstring.  `reference_root`: put that checkout first on sys.path."""
     if reference_root is not None and reference_root not in sys.path:
         sys.path.insert(0, reference_root)
@@ -282,4 +285,11 @@ def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=F
         vpm = importlib.import_module('pcdet.ops.pointnet2.pointnet2_stack.voxel_pool_modules')
         from .voxel_pool import NeighborVoxelSAModuleMSG
         vpm.NeighborVoxelSAModuleMSG = NeighborVoxelSAModuleMSG
+    if use_fused_rpn_targets:
+        from . import anchor_targets
+        for name in ('pcdet.models.dense_heads.target_assigner.axis_aligned_target_assigner',
+                     'pcdet.models.dense_heads.anchor_head_template'):
+            importlib.import_module(name).AxisAlignedTargetAssigner = anchor_targets.AxisAlignedTargetAssigner
+        ahs = importlib.import_module('pcdet.models.dense_heads.anchor_head_single')
+        ahs.AnchorHeadSingle.get_anchor_mask = anchor_targets.get_anchor_mask
     return True
