@@ -380,6 +380,37 @@ int vc_anchor_targets(const float* anchors, const int32_t* anchor_set, int N, in
                       size_t ws_bytes, vc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * RoI target sampling of the two-stage head (TEDMHead), whose rules csrc/roi_targets.cu states.  No host read;
+ * graph-capturable.
+ *   vc_roi_targets <- ProposalTargetLayer.forward (roi_heads/target_assigner/proposal_target_layer.py:32-353;
+ *                     SAMPLE_ROI_BY_EACH_CLASS True, CLS_SCORE_TYPE roi_iou_x) plus the canonical transform of
+ *                     RoIHeadTemplate.assign_targets (roi_head_template.py:133-158), all scenes in one call:
+ *                     rois [B, M, ldr] (ldr >= 7), roi_scores [B, M] fp32, roi_labels [B, M] int64, gt [B, G, ldg]
+ *                     (ldg >= 8, class in the last column); per-class HOST float64 thresholds [n_cls] as the config
+ *                     gives them (REG_FG_THRESH, CLS_FG_THRESH, CLS_BG_THRESH; HARD_SAMPLING_THRESH / _RATIO, read only
+ *                     with hard_sampling != 0), CLS_BG_THRESH_LO, R = ROI_PER_IMAGE, F = int(round(FG_RATIO * R)),
+ *                     HARD_BG_RATIO; uniforms in [0, 1): u_fg [B, ld_ufg >= max(M, R)], u_bg [B, R], u_hs [n_cls]
+ *                     -> rois [B, R, ldr], gt_of_rois_src / gt_of_rois [B, R, ldg], gt_iou_of_rois / roi_scores
+ *                     [B, R] fp32, roi_labels / reg_valid_mask [B, R] int64, rcnn_cls_labels [B, R] fp32, every element
+ *                     written; status [1] int32 = number of scenes with neither foreground nor background RoIs (the
+ *                     reference raises there; their rows are zero).  ws >= vc_roi_targets_ws_bytes(B, M, G) (G does
+ *                     not change the size).  M > VC_ROI_TARGETS_MAX_ROIS, G > VC_ROI_TARGETS_MAX_GT or
+ *                     ldg > VC_ROI_TARGETS_MAX_LDG -> VC_ERR_UNSUPPORTED.  A memset and two launches.
+ * ---------------------------------------------------------------------------------------------- */
+#define VC_ROI_TARGETS_MAX_ROIS 4096
+#define VC_ROI_TARGETS_MAX_GT 512
+#define VC_ROI_TARGETS_MAX_LDG 16
+#define VC_ROI_TARGETS_MAX_CLASSES 16
+size_t vc_roi_targets_ws_bytes(int B, int M, int G);
+int vc_roi_targets(const float* rois, const float* roi_scores, const int64_t* roi_labels, int B, int M, int ldr,
+                   const float* gt, int G, int ldg, int n_cls, const double* reg_fg /*host*/, const double* cls_fg /*host*/,
+                   const double* cls_bg /*host*/, double cls_bg_lo, const double* hs_thresh /*host*/,
+                   const double* hs_ratio /*host*/, int hard_sampling, int R, int F, double hard_bg_ratio,
+                   const float* u_fg, int ld_ufg, const float* u_bg, const float* u_hs, float* o_rois, float* o_gt_src,
+                   float* o_gt, float* o_iou, float* o_scores, int64_t* o_labels, int64_t* o_reg, float* o_cls,
+                   int32_t* status, void* ws, size_t ws_bytes, vc_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Plan executor: a whole backbone forward / backward in ONE call.  Replaces the Python layer loop of
  * `VirConvL8x.forward` (spconv_backbone.py:609-699), `NRConvBlock.forward` (:207-229) and the two streams of
  * `VirConv8x.forward` (:339-535) together with autograd's reverse walk over them: the host side of ~100 operator

@@ -7,7 +7,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import c_char_p, c_float, c_int, c_int32, c_size_t, c_void_p
+from ctypes import c_char_p, c_double, c_float, c_int, c_int32, c_size_t, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('VIRCONV_LIB') or os.path.join(_HERE, 'lib', 'libvirconv_sm90.so')
@@ -18,6 +18,8 @@ _F = c_float
 _Z = c_size_t
 _HOST = ctypes.POINTER(c_int32)
 _HOSTF = ctypes.POINTER(c_float)
+_HOSTD = ctypes.POINTER(c_double)
+_D = c_double
 
 # name -> (restype, argtypes).  Every symbol include/virconv_b200.h declares.
 SIGNATURES = {
@@ -81,6 +83,9 @@ SIGNATURES = {
     'vc_anchor_mask': (_I, [_P, _I, _I, _F, _F, _F, _I, _I, _P, _P, _P]),
     'vc_anchor_targets_ws_bytes': (_Z, [_I, _I, _I]),
     'vc_anchor_targets': (_I, [_P, _P, _I, _I, _HOSTF, _HOSTF, _P, _I, _I, _I, _HOST, _I, _P, _P, _P, _P, _P, _Z, _P]),
+    'vc_roi_targets_ws_bytes': (_Z, [_I, _I, _I]),
+    'vc_roi_targets': (_I, [_P, _P, _P, _I, _I, _I, _P, _I, _I, _I, _HOSTD, _HOSTD, _HOSTD, _D, _HOSTD, _HOSTD, _I, _I, _I,
+                            _D, _P, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _Z, _P]),
     'vc_exec_state_bytes': (_Z, []),
     'vc_exec_forward': (_I, [_P, _P, _I, _P, _P, _I, _P, _I, _P, _I, _HOST, _I, _P, _I, _I, _I, _P, _Z, _P, _P, _P, _Z, _P, _P, _I,
                              _P, _P, _P, _P]),
@@ -133,3 +138,7 @@ def host_i32(vals):
 
 def host_f32(vals):
     return (c_float * len(vals))(*[float(v) for v in vals])
+
+
+def host_f64(vals):
+    return (c_double * len(vals))(*[float(v) for v in vals])

@@ -23,8 +23,11 @@ FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-line
 # rounds identically on the host (vc_boxes_iou_bev_host) and on the GPU
 # anchor_targets.cu: no contraction either, so that its IoU and box encoding round every operation as torch's elementwise
 # kernels do (the equality tests of the target assignment compare those values)
+# roi_targets.cu: no contraction, so that the 3-D IoU it takes from box_geom.cuh is bit for bit vc_boxes_iou3d's and its
+# labels round as torch's elementwise kernels do
 FILE_FLAGS = {'iou3d_nms.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
-              'anchor_targets.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off']}
+              'anchor_targets.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
+              'roi_targets.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off']}
 
 
 def flags_for(src):

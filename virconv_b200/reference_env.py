@@ -27,6 +27,9 @@ package's fused class (virconv_b200.voxel_pool), so TEDMHead's RoI grid pooling 
 With `use_fused_rpn_targets` `AnchorHeadSingle.get_anchor_mask` and the `AxisAlignedTargetAssigner` the anchor heads build
 (looked up in anchor_head_template, which imports the name at module level, and in its own module) are this package's
 device versions (virconv_b200.anchor_targets): the RPN's anchor mask and target assignment without a host read.
+With `use_fused_roi_targets` the `ProposalTargetLayer` the RoI heads build (looked up in roi_head_template, which imports
+the name at module level, and in its own module) and `RoIHeadTemplate.assign_targets` are this package's device versions
+(virconv_b200.roi_targets): the RCNN's RoI sampling, labels and canonical transform in one call without a host read.
 """
 from __future__ import annotations
 
@@ -216,7 +219,8 @@ def _points_in_boxes_cpu(boxes, points, point_indices):
     return 1
 
 
-def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=False, use_fused_rpn_targets=False):
+def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=False, use_fused_rpn_targets=False,
+            use_fused_roi_targets=False):
     """Register everything listed in the module docstring.  `reference_root`: put that checkout first on sys.path."""
     if reference_root is not None and reference_root not in sys.path:
         sys.path.insert(0, reference_root)
@@ -292,4 +296,13 @@ def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=F
             importlib.import_module(name).AxisAlignedTargetAssigner = anchor_targets.AxisAlignedTargetAssigner
         ahs = importlib.import_module('pcdet.models.dense_heads.anchor_head_single')
         ahs.AnchorHeadSingle.get_anchor_mask = anchor_targets.get_anchor_mask
+    if use_fused_roi_targets:
+        from . import roi_targets
+        for name in ('pcdet.models.roi_heads.target_assigner.proposal_target_layer',
+                     'pcdet.models.roi_heads.roi_head_template'):
+            importlib.import_module(name).ProposalTargetLayer = roi_targets.ProposalTargetLayer
+        rht = importlib.import_module('pcdet.models.roi_heads.roi_head_template').RoIHeadTemplate
+        if rht.assign_targets is not roi_targets.assign_targets:
+            roi_targets._reference_assign_targets = rht.assign_targets
+        rht.assign_targets = roi_targets.assign_targets
     return True
