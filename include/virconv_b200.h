@@ -53,20 +53,14 @@ long long vc_launch_count(void);
 int vc_set_pdl(int enable);
 /* BatchNorm backward as ONE cooperative launch (reduction, grid-wide barrier, apply; default on) or as two launches (0). */
 int vc_set_bn_fused(int enable);
-/* Tensor-core conv forward / gather-dgrad kernel: 1 (default) = persistent kernel with a deep cp.async operand ring
- * (csrc/conv_tc2.cu; C in {8,16,32,64}); 0 = the round-1 one-tile-per-CTA kernel (csrc/conv_tc.cu; C in {16,32,64}).
- * A/B measurements only — weight images built under one variant are not valid under the other. */
+/* Tensor-core conv kernel selector: accepts 1 (the persistent kernel, csrc/conv_tc2.cu, the only one); else VC_ERR_INVALID. */
 int vc_set_tc_variant(int variant);
 /* A/B aid for the persistent tensor-core conv kernel (conv_tc2.cu): CTAs per SM, 0 = automatic (two when each still gets a
  * ring of >= 2 stages in half the shared memory), 1 or 2 = forced. */
 int vc_conv_tc2_config(int ctas_per_sm);
-/* The plan executor's weight-gradient kernel: variant 1 (default) = wgrad_tc3.cu (half-tile ring stages, <= 111 KB shared memory
- * and 416 threads per CTA: shares an SM with the dgrad kernels of the main stream), 0 = wgrad_tc2.cu (one CTA per SM,
- * 32 KB stages); max_ctas caps the CTAs of variant 1 (0 = half the SMs). */
+/* The plan executor's weight-gradient launches (csrc/wgrad_tc3.cu): variant must be 1 (the only kernel); max_ctas caps
+ * their CTAs (0, the default: half the SMs, so that each shares its SM with a dgrad CTA of the main stream). */
 int vc_conv_wgrad_tc3_config(int variant, int max_ctas);
-/* CTAs of the persistent tensor-core wgrad kernel (csrc/wgrad_tc2.cu): 0 (default) = one per SM.  Every CTA adds one
- * [K, C_in, C_out] partial with L2 vector reductions, so fewer CTAs trade main-loop parallelism for reduction traffic. */
-int vc_conv_wgrad_tc2_config(int max_ctas);
 
 /* ------------------------------------------------------------------------------------------------
  * Rulebooks.  Replaces spconv `ops.get_indice_pairs`, reached from every conv call site:
@@ -144,11 +138,13 @@ int vc_conv_wgrad_f32(const float* in, const float* dout, const int32_t* nbr, fl
                       int cout, int K, void* ws, size_t ws_bytes, vc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
- * bf16 tensor-core variants of forward / dgrad (wgmma, fp32 accumulators in registers).  Same tables,
- * same tiling, fp32 weights (converted per call) and fp32 outputs; the GATHERED operand (input features for
+ * bf16 tensor-core variants of forward / dgrad / wgrad (wgmma, fp32 accumulators in registers).  Same
+ * tables, fp32 weights (converted per call) and fp32 outputs; the GATHERED operand (input features for
  * forward, output gradients for dgrad) is bf16 [N, C] row major — vc_cast_f32_bf16 makes it.
- * cin, cout in {16,32,64}.  ws >= vc_conv_tc_ws_bytes(cin, cout, K).  err_flag (device int32, may be NULL)
- * is set to 1 if a pipeline wait ever times out (bounded spin instead of a hang); results are then invalid.
+ * cin, cout in {8,16,32,64} for forward, gather dgrad and wgrad; {16,32,64} for the scatter dgrad.
+ * ws >= vc_conv_tc_ws_bytes(cin, cout, K) for forward and both dgrads.  err_flag (device int32, may be
+ * NULL) is set non-zero if a pipeline wait ever times out (bounded wait instead of a hang); results are
+ * then invalid.
  * ---------------------------------------------------------------------------------------------- */
 int vc_cast_f32_bf16(const float* in, void* out_bf16, long long n_elements /* multiple of 4 */, vc_stream_t stream);
 size_t vc_conv_tc_ws_bytes(int cin, int cout, int K);
@@ -162,13 +158,9 @@ int vc_conv_dgrad_tc(const void* dout_bf16, const float* w, const int32_t* nbr_t
                      int cout, int K, int mirror, void* ws, size_t ws_bytes, int32_t* err_flag, vc_stream_t stream);
 /* dw[co,k,ci] = sum_o in[nbr[k,o],ci] * dout[o,co] on tensor cores: both operands bf16 (MN-major wgmma), 128/cin
  * kernel offsets stacked along the MMA M dimension, accumulators resident in registers across all tiles of a
- * persistent CTA, fixed-order reduction of the per-CTA partials.  ws >= vc_conv_wgrad_tc_ws_bytes(...). */
+ * persistent CTA, which adds them into one fp32 image with vector reductions: the summation order, and so the last
+ * bits of dw, vary from run to run.  ws >= vc_conv_wgrad_tc_ws_bytes(...). */
 size_t vc_conv_wgrad_tc_ws_bytes(int n_out, int cin, int cout, int K);
-/* Process-wide launch shape of vc_conv_wgrad_tc: at most max_ctas persistent CTAs (0, the default: one per SM), each asking
- * for at least smem_floor_bytes of dynamic shared memory (default 0).  The plan executor's backward uses (fewer CTAs,
- * a floor no gather-GEMM CTA fits beside) to run wgrad on its own stream next to the dgrad chain.  Affects
- * vc_conv_wgrad_tc_ws_bytes. */
-int vc_conv_wgrad_tc_config(int max_ctas, int smem_floor_bytes);
 int vc_conv_wgrad_tc(const void* in_bf16, const void* dout_bf16, const int32_t* nbr, float* dw, int n_out, int cin,
                      int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag, vc_stream_t stream);
 

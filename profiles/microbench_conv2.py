@@ -1,9 +1,8 @@
-"""A/B of the tensor-core conv kernels on the bench workload, per layer (round 2).
-    python profiles/microbench_conv2.py
-variant 0 = round-1 kernel (one 128-row tile per CTA, 2-deep ring), variant 1 = persistent kernel (conv_tc2.cu).
+"""The tensor-core conv kernel on the bench workload, per layer.
+    python profiles/microbench_conv2.py            # VIRCONV_LIB=<.so> times another build of the library
 For every conv layer of VirConv-L on the bench batch: forward and gather-dgrad through the C ABI (weight-image prep
 launch included in both), median of 7 CUDA-event timings with the L2 flushed in between, and the maximum relative
-difference between the two variants' results (C = 8 layers: variant 1 against the fp32 kernel fed bf16-rounded operands)."""
+difference to the fp32 kernel fed bf16-rounded operands."""
 import os
 import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -71,54 +70,27 @@ for li, (feats, weight, rb) in enumerate(calls):
     dout = torch.randn(rb.n_out, cout, device=dev)
     db = ops.cast_bf16(dout)
     ws = _ws(lib.vc_conv_tc_ws_bytes(cin, cout, rb.K), dev)
-    old_ok = ops.tc_supported(cin, cout)
     gather_dgrad = not (rb.subm and not rb.unique_coords)
-    res, outs = {}, {}
+    res = {}
 
-    def fwd(variant):
-        out = torch.empty((rb.n_out, cout), dtype=torch.float32, device=dev)
-
-        def run():
-            _lib.check(lib.vc_conv_fwd_tc(_p(fb), _p(weight), _p(rb.nbr), _p(out), rb.n_out, cin, cout, rb.K, None, _p(ws),
-                                          ws.numel(), _p(err), _stream()), 'vc_conv_fwd_tc')
-        _lib.check(lib.vc_set_tc_variant(variant), 'variant')
-        t = timed(run)
-        return t, out
-
-    def dgrad(variant):
-        din = torch.empty((rb.n_in, cin), dtype=torch.float32, device=dev)
-        table, mirror = (rb.nbr, 1) if rb.subm else (rb.nbr_bwd, 0)
-
-        def run():
-            _lib.check(lib.vc_conv_dgrad_tc(_p(db), _p(weight), _p(table), _p(din), rb.n_in, cin, cout, rb.K, mirror, _p(ws),
-                                            ws.numel(), _p(err), _stream()), 'vc_conv_dgrad_tc')
-        _lib.check(lib.vc_set_tc_variant(variant), 'variant')
-        t = timed(run)
-        return t, din
-
-    res['fwd1'], o1 = fwd(1)
-    if old_ok:
-        res['fwd0'], o0 = fwd(0)
-        d_f = rel(o1, o0)
-    else:
-        o0 = ops.conv_forward(bf16r(feats), bf16r(weight), rb, None, 'fp32')
-        d_f = rel(o1, o0)
+    out = torch.empty((rb.n_out, cout), dtype=torch.float32, device=dev)
+    res['fwd'] = timed(lambda: _lib.check(lib.vc_conv_fwd_tc(_p(fb), _p(weight), _p(rb.nbr), _p(out), rb.n_out, cin, cout, rb.K,
+                                                             None, _p(ws), ws.numel(), _p(err), _stream()), 'vc_conv_fwd_tc'))
+    d_f = rel(out, ops.conv_forward(bf16r(feats), bf16r(weight), rb, None, 'fp32'))
     d_d = None
     if gather_dgrad:
-        res['dgrad1'], g1 = dgrad(1)
-        if old_ok:
-            res['dgrad0'], g0 = dgrad(0)
-        else:
-            g0 = ops.conv_dgrad(bf16r(dout), bf16r(weight), rb, 'fp32')
-        d_d = rel(g1, g0)
-    lib.vc_set_tc_variant(1)
+        din = torch.empty((rb.n_in, cin), dtype=torch.float32, device=dev)
+        table, mirror = (rb.nbr, 1) if rb.subm else (rb.nbr_bwd, 0)
+        res['dgrad'] = timed(lambda: _lib.check(lib.vc_conv_dgrad_tc(_p(db), _p(weight), _p(table), _p(din), rb.n_in, cin, cout, rb.K,
+                                                                     mirror, _p(ws), ws.numel(), _p(err), _stream()), 'vc_conv_dgrad_tc'))
+        d_d = rel(din, ops.conv_dgrad(bf16r(dout), bf16r(weight), rb, 'fp32'))
     for k, v in res.items():
         tot[k] = tot.get(k, 0.0) + v
     P = rb.n_pairs()
     by = feats.shape[0] * cin * 2 + rb.n_out * cout * 4 + P * 8 + rb.K * cin * cout * 2
     print(f'L{li:02d} {"subm" if rb.subm else "conv"}{rb.ndim}d {cin:2d}->{cout:2d} K={rb.K:2d} N_in={feats.shape[0]:6d} N_out={rb.n_out:6d} '
           f'P={P:8d} ' + ' '.join(f'{k}={v:6.1f}us' for k, v in sorted(res.items())) +
-          f'  fwd1: {by / res["fwd1"] / 1e3:7.1f} GB/s {2 * P * cin * cout / res["fwd1"] / 1e6:6.1f} TF/s'
+          f'  fwd: {by / res["fwd"] / 1e3:7.1f} GB/s {2 * P * cin * cout / res["fwd"] / 1e6:6.1f} TF/s'
           f'  maxrel fwd {d_f:.1e}' + (f' dgrad {d_d:.1e}' if d_d is not None else ''), flush=True)
 print('TOTAL us', {k: round(v, 1) for k, v in sorted(tot.items())})
 print('error flag', int(err.item()))

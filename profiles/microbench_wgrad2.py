@@ -1,9 +1,8 @@
-"""A/B of the tensor-core weight-gradient kernels on the bench workload, per layer (round 2).
-    python profiles/microbench_wgrad2.py
-variant 0 = round-1 kernel (128 persistent CTAs, one [K,Cin,Cout] partial each + reduce kernel), variant 1 = persistent
-kernel of wgrad_tc2.cu (one scratch image, vector reductions, finalize).  Median of 7 CUDA-event timings per layer with the
-L2 flushed in between; maximum relative difference between the variants (C = 8 layers: variant 1 against the fp32 kernel fed
-bf16-rounded operands)."""
+"""The tensor-core weight-gradient kernel on the bench workload, per layer, through the per-operator C ABI.
+    python profiles/microbench_wgrad2.py            # VIRCONV_LIB=<.so> times another build of the library
+For every conv layer of VirConv-L on the bench batch: median of 7 CUDA-event timings of vc_conv_wgrad_tc (scratch zeroing and
+the transposing finalize included) with the L2 flushed in between, and the maximum relative difference to the fp32 kernel
+fed bf16-rounded operands."""
 import os
 import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -59,42 +58,22 @@ def bf16r(t):
     return t.to(torch.bfloat16).to(torch.float32)
 
 
-tot = {}
+tot = 0.0
 for li, (feats, weight, rb) in enumerate(calls):
     cout, cin = weight.shape[0], weight.shape[-1]
     feats = feats.contiguous()
     fb = ops.cast_bf16(feats)
     dout = torch.randn(rb.n_out, cout, device=dev)
     db = ops.cast_bf16(dout)
-    wsb = lib.vc_conv_wgrad_tc_ws_bytes(rb.n_out, cin, cout, rb.K)
-    ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-    old_ok = ops.tc_supported(cin, cout)
-    res = {}
-
-    def wgrad(variant):
-        dw = torch.empty(tuple(weight.shape), dtype=torch.float32, device=dev)
-
-        def run():
-            _lib.check(lib.vc_conv_wgrad_tc(_p(fb), _p(db), _p(rb.nbr), _p(dw), rb.n_out, cin, cout, rb.K, _p(ws), ws.numel(),
-                                            _p(err), _stream()), 'vc_conv_wgrad_tc')
-        _lib.check(lib.vc_set_tc_variant(variant), 'variant')
-        t = timed(run)
-        return t, dw
-
-    res['wgrad1'], w1 = wgrad(1)
-    if old_ok:
-        res['wgrad0'], w0 = wgrad(0)
-    else:
-        lib.vc_set_tc_variant(1)
-        w0 = ops.conv_wgrad(bf16r(feats), bf16r(dout), weight.shape, rb, 'fp32')
-    lib.vc_set_tc_variant(1)
-    d = rel(w1, w0)
-    for k, v in res.items():
-        tot[k] = tot.get(k, 0.0) + v
+    ws = _ws(lib.vc_conv_wgrad_tc_ws_bytes(rb.n_out, cin, cout, rb.K), dev)
+    dw = torch.empty(tuple(weight.shape), dtype=torch.float32, device=dev)
+    t = timed(lambda: _lib.check(lib.vc_conv_wgrad_tc(_p(fb), _p(db), _p(rb.nbr), _p(dw), rb.n_out, cin, cout, rb.K, _p(ws),
+                                                      ws.numel(), _p(err), _stream()), 'vc_conv_wgrad_tc'))
+    d = rel(dw, ops.conv_wgrad(bf16r(feats), bf16r(dout), weight.shape, rb, 'fp32'))
+    tot += t
     P = rb.n_pairs()
     by = (feats.shape[0] * cin + rb.n_out * cout) * 2 + P * 8 + rb.K * cin * cout * 4
     print(f'L{li:02d} {"subm" if rb.subm else "conv"}{rb.ndim}d {cin:2d}->{cout:2d} K={rb.K:2d} N_out={rb.n_out:6d} P={P:8d} '
-          + ' '.join(f'{k}={v:6.1f}us' for k, v in sorted(res.items()))
-          + f'  wgrad1: {by / res["wgrad1"] / 1e3:7.1f} GB/s {2 * P * cin * cout / res["wgrad1"] / 1e6:6.1f} TF/s  maxrel {d:.1e}', flush=True)
-print('TOTAL us', {k: round(v, 1) for k, v in sorted(tot.items())})
+          f'wgrad={t:6.1f}us  {by / t / 1e3:7.1f} GB/s {2 * P * cin * cout / t / 1e6:6.1f} TF/s  maxrel {d:.1e}', flush=True)
+print('TOTAL us', round(tot, 1))
 print('error flag', int(err.item()))

@@ -1,5 +1,5 @@
 """Run ONE conv layer of the bench workload a few times (for ncu captures of a single launch).
-    LAYER=6 VARIANT=1 REPS=4 python profiles/one_conv.py       # layer index as printed by microbench_conv2.py"""
+    LAYER=6 REPS=4 python profiles/one_conv.py       # layer index as printed by microbench_conv2.py"""
 import os
 import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -35,7 +35,6 @@ cout, cin = weight.shape[0], weight.shape[-1]
 fb = ops.cast_bf16(feats.contiguous())
 ws = ops._ws(lib.vc_conv_tc_ws_bytes(cin, cout, rb.K), dev)
 out = torch.empty((rb.n_out, cout), dtype=torch.float32, device=dev)
-_lib.check(lib.vc_set_tc_variant(int(os.environ.get('VARIANT', '1'))), 'variant')
 flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
 torch.cuda.synchronize()
 for _ in range(int(os.environ.get('REPS', '4'))):

@@ -1,5 +1,5 @@
 """Pipeline timeline of the persistent wgmma conv kernel (debug build -DVC_TC_TRACE: python -c "from virconv_b200 import
-build; build.build(defines=['VC_TC_TRACE'], suffix='trace')", run with VIRCONV_LIB=virconv_b200/lib/libvirconv_sm100_trace.so).
+build; build.build(defines=['VC_TC_TRACE'], suffix='trace')", run with VIRCONV_LIB=virconv_b200/lib/libvirconv_sm90_trace.so).
 CTA 0's events in ns since kernel start: tables published, stages issued / consumed, tiles committed, epilogue start / end."""
 import ctypes
 import os

@@ -411,44 +411,6 @@ def test_tc2_one_and_two_ctas_per_sm(lib_built, ctas):
         _lib.check(lib.vc_conv_tc2_config(0), 'vc_conv_tc2_config')
 
 
-def test_tc_round1_kernels(lib_built):
-    """The round-1 tensor-core kernels (vc_set_tc_variant(0): one tile per CTA, a 2-stage operand ring, per-CTA wgrad partials):
-    forward, dgrad and wgrad of a submanifold and a strided conv with every tile reaching many kernel offsets, against the
-    oracle fed the same bf16-rounded operands; the pipeline-timeout flag must stay 0."""
-    from virconv_b200 import _lib, ops
-    lib = _lib.load()
-    _lib.check(lib.vc_set_tc_variant(0), 'vc_set_tc_variant')
-    try:
-        rng = np.random.default_rng(91)
-        shape = [21, 40, 36]
-        c = _coords(rng, 6000, 2, shape)
-        n = c.shape[0]
-        torch.manual_seed(9)
-        for cin, cout, strided in ((16, 32, False), (64, 64, False), (32, 64, True)):
-            if strided:
-                rb = ops.build_conv_rulebook(torch.from_numpy(c).to(_dev()), 2, shape, 3, 2, 1)
-                oi, _, nf, _ = orb.conv_rulebook(c, shape, 3, 2, 1)
-                nbr, n_out = nf, oi.shape[0]
-            else:
-                rb = ops.build_subm_rulebook(torch.from_numpy(c).to(_dev()), 2, shape, 3)
-                nbr, n_out = orb.subm_rulebook(c, shape, 3), n
-            feats, weight, dout = torch.randn(n, cin), torch.randn(cout, 3, 3, 3, cin) * 0.1, torch.randn(n_out, cout)
-            f = feats.to(_dev()).requires_grad_(True)
-            w = weight.to(_dev()).requires_grad_(True)
-            out = ops.SparseConvFn.apply(f, w, rb, 'bf16')
-            out.backward(dout.to(_dev()))
-            torch.cuda.synchronize()
-            assert int(ops.tc_error_flag(_dev()).item()) == 0, (cin, cout, strided)
-            ro, _, _ = _oracle_conv(_bf(feats), _bf(weight), nbr, n_out, not strided, dout)
-            assert rel_err(out.detach().cpu(), ro) < TOL, (cin, cout, strided)
-            _, rdf, _ = _oracle_conv(feats, _bf(weight), nbr, n_out, not strided, _bf(dout))
-            assert rel_err(f.grad.cpu(), rdf) < TOL, (cin, cout, strided)
-            _, _, rdw = _oracle_conv(_bf(feats), weight, nbr, n_out, not strided, _bf(dout))
-            assert rel_err(w.grad.cpu(), rdw) < TOL, (cin, cout, strided)
-    finally:
-        _lib.check(lib.vc_set_tc_variant(1), 'vc_set_tc_variant')
-
-
 def test_tc_subm2d_duplicates_and_tails(lib_built):
     """image-branch table (forward and the scatter-form dgrad on tensor cores) + ragged tiles"""
     from virconv_b200 import ops

@@ -31,7 +31,6 @@ SIGNATURES = {
     'vc_set_tc_variant': (_I, [_I]),
     'vc_conv_tc2_config': (_I, [_I]),
     'vc_conv_wgrad_tc3_config': (_I, [_I, _I]),
-    'vc_conv_wgrad_tc2_config': (_I, [_I]),
     'vc_subm_rulebook_ws_bytes': (_Z, [_I]),
     'vc_subm_rulebook': (_I, [_P, _I, _I, _I, _HOST, _HOST, _HOST, _P, _P, _P, _Z, _P]),
     'vc_conv_rulebook_ws_bytes': (_Z, [_I, _I, _HOST]),
@@ -90,7 +89,6 @@ SIGNATURES = {
     'vc_exec_forward': (_I, [_P, _P, _I, _P, _P, _I, _P, _I, _P, _I, _HOST, _I, _P, _I, _I, _I, _P, _Z, _P, _P, _P, _Z, _P, _P, _I,
                              _P, _P, _P, _P]),
     'vc_exec_backward': (_I, [_P, _P, _I, _P, _P, _I, _P, _P, _I, _P, _Z, _P, _P, _P, _P]),
-    'vc_conv_wgrad_tc_config': (_I, [_I, _I]),
     'vc_exec_query': (_I, [_P, _I, _I, _P]),
     'vc_exec_timing': (_I, [_I]),
     'vc_exec_timing_read': (_I, [_P, _P, _I]),

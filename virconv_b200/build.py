@@ -50,8 +50,8 @@ def _digest(paths):
 
 
 def build(verbose: bool = False, force: bool = False, defines=(), suffix: str = '') -> str:
-    """`defines` / `suffix`: experiment variants (e.g. -DVC_TC_STAGES=6 -> libvirconv_sm90_s6.so, picked up through
-    the VIRCONV_LIB environment variable); the default build has neither."""
+    """`defines` / `suffix`: debug variants (e.g. -DVC_TC_TRACE -> libvirconv_sm90_trace.so, picked up through the
+    VIRCONV_LIB environment variable); the default build has neither."""
     os.makedirs(LIBDIR, exist_ok=True)
     if suffix:
         return _build_variant(list(defines), suffix, verbose)

@@ -155,14 +155,14 @@ int cat2_dev(const float* a, const float* b, float* out, void* out_bf16, int n, 
 int index2uv_dev(const int32_t* indices, int n, const int* n_dev, int batch_size, const float* params, const float* grid,
                  int stride, int u_max, int v_max, int32_t* uv_out, cudaStream_t stream);
 
-// ---- shared between conv_tc.cu and executor.cu ----
+// ---- shared between conv_tc.cu, conv_tc2.cu and executor.cu ----
 struct TcPrepEntry {
     const float* w;   // parameter, spconv layout [C_out, K, C_in]
     void* img;        // bf16 UMMA image, K * cin * cout elements
     int cin, cout, K;
     int mode;         // 0 forward image, 1 dgrad image
     int mirror;       // dgrad: kernel offsets mirrored (submanifold table re-used as its own transpose)
-    int layout;       // 0: round-1 core-matrix image (tc_scatter_kernel, legacy gather kernel); 1: swizzled + padded to 16 (conv_tc2.cu)
+    int layout;       // 0: core-matrix image of the scatter dgrad (tc_scatter_kernel); 1: swizzled + padded to 16 (conv_tc2.cu)
     int first;        // element prefix (filled by tc_prep_images)
 };
 static constexpr int TC_PREP_MAX = 64;
@@ -171,27 +171,25 @@ struct TcPrepTable {
     int n, total;
 };
 int tc_prep_images(TcPrepTable& t, cudaStream_t stream);
+// ---- conv_tc.cu (tensor-core scatter dgrad of many-to-one tables) ----
+static inline bool tc_scatter_ch_ok(int c) { return c == 16 || c == 32 || c == 64; }
 int tc_scatter_with_image(int kc, int nr, const void* dout_bf16, const void* wimg, const int32_t* nbr, float* din, int n_out,
                           int K, int* err, cudaStream_t stream);
-int tc_conv_with_image(int kc, int nr, const void* in_bf16, const void* wimg, const int32_t* nbr, long long pitch, float* out,
-                       int n_rows, const int* n_dev, int K, double* bn_sums, int* err, cudaStream_t stream, const float* addend,
-                       int* tile_counter = nullptr, int flags = 0);   // flags: bit 0 sparse offsets (strided dgrad), bit 1 early tables
-bool tc_conv_ch_ok(int c);
-// ---- conv_tc2.cu (persistent tensor-core conv) ----
-extern int g_tc_variant;
+// ---- conv_tc2.cu (persistent tensor-core conv: forward and gather dgrad) ----
+int num_sms();   // of the current device
 size_t tc_image_bytes(int cin, int cout, int K, int layout);
 bool tc2_ch_ok(int c);
 int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_t* nbr, long long pitch, float* out, int n_rows,
              const int* n_dev, int K, double* bn_sums, int* err, cudaStream_t stream, const float* addend,
-             int* tile_counter = nullptr, int sparse_k = 0);
+             int* tile_counter = nullptr, int flags = 0);   // flags: bit 0 sparse offsets (strided dgrad), bit 1 early tables
 
-// ---- wgrad_tc3.cu (half-tile-stage variant of the persistent wgrad, A/B) ----
-extern int g_wgrad_variant;
+// ---- wgrad_tc3.cu (persistent tensor-core wgrad) ----
+extern int g_wgrad3_ctas;
 int tc3_wgrad(int cin, int cout, const void* in_bf16, const void* dout_bf16, const int32_t* nbr, long long pitch, float* scratch,
-              int n_rows, const int* n_dev, int K, int* err, cudaStream_t stream, int* tile_counter);
-// ---- wgrad_tc2.cu (persistent tensor-core wgrad) ----
+              int n_rows, const int* n_dev, int K, int* err, cudaStream_t stream, int* tile_counter, int max_ctas);
+int wgrad3_passes(int cin, int cout, int K);
 struct WgradFinEntry {
-    const float* scratch;   // [K][cin][cout] accumulated by tc2_wgrad
+    const float* scratch;   // [K][cin][cout] accumulated by tc3_wgrad
     float* dw;              // parameter layout [cout][K][cin]
     int cin, cout, K, first;
 };
@@ -201,8 +199,5 @@ struct WgradFinTable {
     int n, total;
 };
 int wgrad_finalize(WgradFinTable& t, cudaStream_t stream);
-int tc2_wgrad(int cin, int cout, const void* in_bf16, const void* dout_bf16, const int32_t* nbr, long long pitch, float* scratch,
-              int n_rows, const int* n_dev, int K, int* err, cudaStream_t stream, int* tile_counter);
-int wgrad2_passes(int cin, int cout, int K);
 
 }  // namespace vc

@@ -1,56 +1,16 @@
-// bf16 tensor-core sparse convolution (forward and dgrad) — wgmma, sm_90a.
+// bf16 tensor-core sparse convolution, per-operator C ABI — wgmma, sm_90a.
 //
-// Same output-stationary tiling as conv_f32.cu (one CTA = 128 output rows, loop over the kernel offsets that
-// touch the tile), but the inner [128 x C_in] x [C_in x C_out] contraction of every offset runs on the tensor cores:
-//   * operands are bf16.  The gathered neighbour rows land in shared memory through 16-byte cp.async chunks
-//     (zero-fill for missing neighbours) directly in the GMMA canonical K-major, no-swizzle layout
-//     (8-row x 16-byte core matrices: chunk (r, c) at ((r/8)*C/8 + c)*128 + (r%8)*16), the weight slice of the
-//     offset is a pre-formatted image copied linearly — no register staging, no re-layout pass;
-//   * a consumer warpgroup issues 2 x C_in/16 `wgmma.mma_async` (two m64 row blocks, N=C_out, K=16) per offset,
-//     accumulating all offsets of the tile in registers (fp32); once the MMAs of a stage have completed
-//     (wgmma.wait_group) one thread frees it on an mbarrier; a ring of TC_STAGES operand stages keeps the next gather
-//     in flight behind the MMA;
-//   * epilogue: accumulator registers -> smem -> coalesced fp32 stores + per-tile BN sums.
-// Replaces spconv `ops.indice_conv` behind spconv_backbone.py:89,92-93,113,563-564 in the bf16 (benchmark)
-// precision mode; the fp32 kernels in conv_f32.cu stay the 1e-4 parity path.
-// Algorithmic bytes per launch (e=2 for the gathered operand, 4 for the fp32 output):
-//   N_in*C_in*2 + N_out*C_out*4 + P*8 + K*C_in*C_out*2;  FLOPs 2*P*C_in*C_out.
+//   * vc_cast_f32_bf16: the f32 -> bf16 cast of the gathered operand;
+//   * vc_conv_fwd_tc / vc_conv_dgrad_tc: build the weight image of the call and run the persistent gather-GEMM kernel of
+//     conv_tc2.cu (the plan executor calls that kernel directly with images it prepares once per step);
+//   * vc_conv_dgrad_scatter_tc: the input gradient of a many-to-one table (tc_scatter_kernel below), which has no gather form.
+// Replaces spconv `ops.indice_conv` / `indice_conv_backward` behind spconv_backbone.py:89,92-93,113,563-564 in the bf16
+// (benchmark) precision mode; the fp32 kernels in conv_f32.cu stay the 1e-4 parity path.
 #include <cuda_bf16.h>
 
 #include "tc_common.cuh"
 
 namespace vc {
-
-#ifdef VC_TC_TRACE
-// debug build only (profiles/trace_tc.py): per-CTA SM-clock timestamps of the pipeline events of the first CTAs
-__device__ long long* g_trace = nullptr;
-#define VC_TRACE(slot) do { if (g_trace && blockIdx.x < 64) g_trace[blockIdx.x * 64 + (slot)] = clock64(); } while (0)
-#else
-#define VC_TRACE(slot) do { } while (0)
-#endif
-
-#ifndef VC_TC_NPW
-#define VC_TC_NPW 4
-#endif
-static constexpr int TC_NPW = VC_TC_NPW;               // gather-producer warps (4 or 8)
-static constexpr int TC_PRODUCERS = 32 * TC_NPW;
-static constexpr int TC_THREADS = TC_PRODUCERS + 128;  // + the last four warps: the MMA warpgroup
-#ifndef VC_TC_STAGES
-// ring depth: a shallow ring leaves shared memory for more CTAs per SM, and CTA-level parallelism hides the gather latency
-#define VC_TC_STAGES 2
-#endif
-static constexpr int TC_STAGES = VC_TC_STAGES;
-static constexpr int TC_LAG = TC_STAGES - 1;   // stages a producer thread keeps in flight before it signals `full`
-template <int KC, int NR>
-struct TcCfg {
-    static constexpr int CPR = KC / 8;                       // 16-byte chunks per gathered row
-    static constexpr int A_BYTES = TCM * KC * 2;
-    static constexpr int B_BYTES = NR * KC * 2;
-    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int EPI_BYTES = TCM * (NR + 1) * 4;     // epilogue staging, aliases the stage ring
-    static constexpr int RING_BYTES = TC_STAGES * STAGE_BYTES > EPI_BYTES ? TC_STAGES * STAGE_BYTES : EPI_BYTES;
-    static constexpr size_t smem(int K) { return (size_t)RING_BYTES + (size_t)K * TCM * 4; }
-};
 
 // f32 -> bf16 cast of a feature matrix (the gathered operand)
 __global__ void cast_bf16_kernel(const float4* __restrict__ in, uint2* __restrict__ out, size_t n4) {
@@ -66,238 +26,14 @@ __global__ void cast_bf16_kernel(const float4* __restrict__ in, uint2* __restric
     }
 }
 
-// Warp-specialised: warps 0-3 are gather producers (each owns 32 rows of the tile and streams its 16-byte chunks of
-// every stage with cp.async, then signals the stage's `full` mbarrier), warps 4-7 are the MMA warpgroup
-// (wait full -> fence.proxy.async -> 2 x C_in/16 wgmma -> once they completed, arrive on the stage's `empty` mbarrier).
-// No block-wide barrier inside the main loop; the ring is TC_STAGES deep.
+// operands of the scatter kernel in the GMMA canonical K-major, no-swizzle layout: 8-row x 16-byte core matrices, chunk
+// (r, c) of a [rows x KC] matrix at ((r/8)*KC/8 + c)*128 + (r%8)*16 (weight-image layout 0 of tc_prep_images)
 template <int KC, int NR>
-__global__ void __launch_bounds__(TC_THREADS)
-tc_gather_gemm_kernel(const __nv_bfloat16* __restrict__ in, const __nv_bfloat16* __restrict__ wimg,
-                      const int32_t* __restrict__ nbr, float* out, int n_out, int K, double* __restrict__ bn_sums,
-                      int* __restrict__ err, const float* addend) {
-    // addend (may be NULL, may alias `out`): a [n_out, NR] fp32 matrix added to the result in the epilogue — the plan
-    // executor's gradient accumulation (an earlier contribution to the same feature slot) without a separate add kernel
-    using C = TcCfg<KC, NR>;
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* ring = smem_raw;                                          // [stages][A | B]
-    int* nbr_s = reinterpret_cast<int*>(smem_raw + C::RING_BYTES);           // [K][128]
-    __shared__ __align__(8) uint64_t full_bar[TC_STAGES];
-    __shared__ __align__(8) uint64_t empty_bar[TC_STAGES];
-    __shared__ int klist[MAXK_TC];
-    __shared__ unsigned kmask;
-    __shared__ float red[4][2][NR];
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int base = blockIdx.x * TCM;
-    if (tid == 0) VC_TRACE(0);
-
-    if (tid == 0) {
-        VC_TRACE(1);
-#pragma unroll
-        for (int s = 0; s < TC_STAGES; ++s) {
-            mbar_init(&full_bar[s], TC_PRODUCERS + 1);   // 128 gather threads (cp.async arrive) + 1 expect_tx arrive (TMA)
-            mbar_init(&empty_bar[s], 1);                  // MMA warpgroup, after its wgmma.wait_group
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        kmask = 0u;
-    }
-    // on-chip set-up above overlaps the previous kernel's tail (PDL); everything below reads global memory
-    pdl_wait();
-    pdl_launch_dependents();
-    // stage the tile's slice of the neighbour table
-    stage_nbr_tile<TC_THREADS, 24>(nbr, n_out, 0, K, base, nbr_s);   // all of a thread's loads in one round trip
-    __syncthreads();
-    for (int k = warp; k < K; k += TC_THREADS / 32) {
-        bool any = false;
-#pragma unroll
-        for (int j = 0; j < TCM / 32; ++j) any |= nbr_s[k * TCM + j * 32 + lane] >= 0;
-        if (__any_sync(0xffffffffu, any) && lane == 0) atomicOr(&kmask, 1u << k);
-    }
-    __syncthreads();
-    const unsigned km = kmask;
-    const int nk = __popc(km);
-    if (tid == 0) {
-        int c = 0;
-        for (int k = 0; k < K; ++k)
-            if (km >> k & 1u) klist[c++] = k;
-    }
-    __syncthreads();
-
-    bool ok = true;
-    if (tid == 0) { VC_TRACE(2); VC_TRACE(63); }
-    const int t = tid - TC_PRODUCERS;                    // thread of the MMA warpgroup
-    float acc[2][NR / 2];                                // rows [0, 64) and [64, 128)
-#pragma unroll
-    for (int j = 0; j < NR / 2; ++j) acc[0][j] = acc[1][j] = 0.f;
-#ifdef VC_TC_TRACE
-    if (tid == 0 && g_trace && blockIdx.x < 64) g_trace[blockIdx.x * 64 + 62] = nk;
-#endif
-    if (nk > 0) {
-        if (warp < TC_NPW) {
-            // ---------------- gather producers ----------------
-            // per warp instruction 8 rows x (up to) 4 chunks: conflict-free smem writes, full 32-byte sectors
-            constexpr int CW = C::CPR < 4 ? C::CPR : 4;
-            constexpr int RPI = 8 * (4 / CW);
-            constexpr int RPW = TCM / TC_NPW;             // rows per producer warp
-            constexpr int NIT = RPW / RPI, NCG = C::CPR / CW;
-            static_assert(RPW % RPI == 0, "producer warp rows must be a multiple of the rows per instruction");
-            const int rl = lane & 7, xq = lane >> 3;
-            const int c_sub = xq % CW, r_sub = xq / CW;
-            // everything that does not depend on the stage is computed once: the rows this thread gathers, their chunk
-            // offsets inside a stage image, the shared-space base address
-            int rows[NIT];
-            uint32_t dst_off[NIT][NCG];
-#pragma unroll
-            for (int it = 0; it < NIT; ++it) {
-                const int r = warp * RPW + it * RPI + r_sub * 8 + rl;
-                rows[it] = r;
-#pragma unroll
-                for (int cg = 0; cg < NCG; ++cg) dst_off[it][cg] = (uint32_t)(((r >> 3) * C::CPR + cg * CW + c_sub) * 128 + (r & 7) * 16);
-            }
-            const uint32_t ring_s = smem_u32(ring);
-            for (int t = 0; t < nk; ++t) {
-                const int st = t % TC_STAGES;
-                const int k = klist[t];
-                int src[NIT];
-#pragma unroll
-                for (int it = 0; it < NIT; ++it) src[it] = nbr_s[k * TCM + rows[it]];     // independent loads first
-                if (t >= TC_STAGES) ok &= mbar_wait(&empty_bar[st], (uint32_t)((t / TC_STAGES - 1) & 1), err);
-                const uint32_t a_s = ring_s + st * C::STAGE_BYTES;
-                unsigned char* B = ring + st * C::STAGE_BYTES + C::A_BYTES;
-#pragma unroll
-                for (int it = 0; it < NIT; ++it) {
-                    const __nv_bfloat16* srow = in + (size_t)(src[it] < 0 ? 0 : src[it]) * KC + c_sub * 8;
-#pragma unroll
-                    for (int cg = 0; cg < NCG; ++cg) cp_async16_s(a_s + dst_off[it][cg], srow + cg * CW * 8, src[it] >= 0);
-                }
-                if (tid == 0) {
-                    // the offset's weight image: ONE bulk (TMA-engine) copy, completion counted in bytes on full[st]
-                    const unsigned char* wsrc = reinterpret_cast<const unsigned char*>(wimg) + (size_t)k * C::B_BYTES;
-                    const uint32_t bar = smem_u32(&full_bar[st]);
-                    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"((uint32_t)C::B_BYTES)
-                                 : "memory");
-                    asm volatile(
-                        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                            smem_u32(B)),
-                        "l"(wsrc), "r"((uint32_t)C::B_BYTES), "r"(bar)
-                        : "memory");
-                }
-                // Signal `full` with a LAG of TC_LAG stages: commit this stage's copies as one cp.async group, then wait only
-                // until the group issued TC_LAG stages ago has landed and arrive for THAT stage.  (Arriving for the
-                // current stage with cp.async.mbarrier.arrive.noinc measured as one memory round trip per stage: the
-                // producer did not run ahead.  This keeps TC_LAG+1 stages of gathers in flight per thread.)
-                cp_async_commit();
-                if (t >= TC_LAG) {
-                    cp_async_wait<TC_LAG>();
-                    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&full_bar[(t - TC_LAG) % TC_STAGES]))
-                                 : "memory");
-                }
-            }
-            cp_async_wait<0>();
-            for (int t = (nk > TC_LAG ? nk - TC_LAG : 0); t < nk; ++t)
-                asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&full_bar[t % TC_STAGES])) : "memory");
-        } else {
-            // ---------------- MMA warpgroup ----------------
-            // A stage is released as soon as its OWN MMAs have completed.  (Releasing it after the next stage's MMAs were
-            // issued would need full[t+1], which the producers signal TC_LAG stages late, after waiting for empty[t]: a cycle.)
-            for (int tt = 0; tt < nk; ++tt) {
-                const int st = tt % TC_STAGES;
-                ok &= mbar_wait(&full_bar[st], (uint32_t)((tt / TC_STAGES) & 1), err);
-                if (t == 0 && tt < 27) VC_TRACE(4 + tt);
-                fence_async_smem();     // generic-proxy (cp.async) writes -> visible to the tensor core's async proxy
-                wg_fence();
-                const uint32_t a0 = smem_u32(ring + st * C::STAGE_BYTES);
-                const uint32_t b0 = a0 + C::A_BYTES;
-#pragma unroll
-                for (int m = 0; m < KC / 16; ++m) {
-                    const uint64_t bd = gmma_desc(b0 + m * 256, 128, C::CPR * 128, 0);
-#pragma unroll
-                    for (int h = 0; h < 2; ++h)
-                        wgmma_bf16<NR, 0, 0>(acc[h], gmma_desc(a0 + h * 8 * C::CPR * 128 + m * 256, 128, C::CPR * 128, 0), bd,
-                                             (tt > 0 || m > 0) ? 1u : 0u);
-                }
-                wg_commit();
-                wg_wait<0>();
-                if (t == 0) mbar_arrive(&empty_bar[st]);
-            }
-            wg_fence_acc(acc[0]);
-            wg_fence_acc(acc[1]);
-            if (t == 0) VC_TRACE(40);
-        }
-    }
-    __syncthreads();    // every MMA has completed: the ring can be reused as epilogue staging
-
-    float* stg = reinterpret_cast<float*>(ring);    // [128][NR+1]
-    if (t >= 0) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-            for (int j = 0; j < NR / 2; ++j) stg[(64 * h + wg_row(j, t)) * (NR + 1) + wg_col(j, t)] = acc[h][j];
-    }
-    __syncthreads();
-    // coalesced fp32 stores: consecutive threads -> consecutive float4 of the [128, NR] tile
-    for (int q = tid; q < TCM * NR / 4; q += TC_THREADS) {
-        const int r = q / (NR / 4), c4 = q % (NR / 4);
-        if (base + r < n_out) {
-            const float* s = stg + r * (NR + 1) + c4 * 4;
-            float4 v = make_float4(s[0], s[1], s[2], s[3]);
-            const size_t o = (size_t)(base + r) * NR + c4 * 4;
-            if (addend != nullptr) {       // same element read and written by this thread only: aliasing `out` is safe
-                const float4 a = *reinterpret_cast<const float4*>(addend + o);
-                v.x += a.x; v.y += a.y; v.z += a.z; v.w += a.w;
-            }
-            *reinterpret_cast<float4*>(out + o) = v;
-        }
-    }
-    if (bn_sums != nullptr) {
-        // column sums over the tile's valid rows: thread (ch, quarter) sums 32 rows
-        const int rows_valid = min(TCM, n_out - base);
-        for (int idx = tid; idx < NR * 4; idx += TC_THREADS) {
-            const int ch = idx % NR, qd = idx / NR;
-            float s = 0.f, q2 = 0.f;
-            for (int r = qd * 32; r < min(qd * 32 + 32, rows_valid); ++r) {
-                float x = stg[r * (NR + 1) + ch];
-                s += x;
-                q2 = fmaf(x, x, q2);
-            }
-            red[qd][0][ch] = s;
-            red[qd][1][ch] = q2;
-        }
-        __syncthreads();
-        for (int idx = tid; idx < 2 * NR; idx += TC_THREADS) {
-            const int which = idx / NR, ch = idx % NR;
-            atomicAdd(bn_sums + which * NR + ch,
-                      (double)(red[0][which][ch] + red[1][which][ch] + red[2][which][ch] + red[3][which][ch]));
-        }
-    }
-    if (tid == 0) VC_TRACE(41);
-    (void)ok;
-}
-
-template <int KC, int NR>
-static int launch_tc(const __nv_bfloat16* in, const __nv_bfloat16* wimg, const int32_t* nbr, float* out, int n_out, int K,
-                     double* bn_sums, int* err, cudaStream_t stream, const float* addend = nullptr) {
-    size_t smem = TcCfg<KC, NR>::smem(K);
-    auto kern = tc_gather_gemm_kernel<KC, NR>;
-    VC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    VC_LAUNCH_CHAIN(kern, dim3(cdiv(n_out, TCM)), dim3(TC_THREADS), smem, stream, in, wimg, nbr, out, n_out, K, bn_sums, err,
-                    addend);
-    return VC_OK;
-}
-
-static bool tc_ch_ok(int c) { return c == 16 || c == 32 || c == 64; }
-
-static int dispatch_tc(int kc, int nr, const __nv_bfloat16* in, const __nv_bfloat16* wimg, const int32_t* nbr, float* out,
-                       int n_out, int K, double* bn_sums, int* err, cudaStream_t stream, const float* addend = nullptr) {
-#define VC_TC_CASE(A, B) \
-    if (kc == A && nr == B) return launch_tc<A, B>(in, wimg, nbr, out, n_out, K, bn_sums, err, stream, addend);
-    VC_TC_CASE(16, 16) VC_TC_CASE(16, 32) VC_TC_CASE(16, 64)
-    VC_TC_CASE(32, 16) VC_TC_CASE(32, 32) VC_TC_CASE(32, 64)
-    VC_TC_CASE(64, 16) VC_TC_CASE(64, 32) VC_TC_CASE(64, 64)
-#undef VC_TC_CASE
-    set_error("tensor-core conv: unsupported channel pair (%d, %d), need 16/32/64", kc, nr);
-    return VC_ERR_UNSUPPORTED;
-}
+struct TcCfg {
+    static constexpr int CPR = KC / 8;                       // 16-byte chunks per row
+    static constexpr int A_BYTES = TCM * KC * 2;             // the dout tile
+    static constexpr int B_BYTES = NR * KC * 2;              // one offset's weight image
+};
 
 // ------------------------------------------------------------------------------------------------
 // dgrad of a MANY-TO-ONE table (the image branch: several rows share a pixel, so the transposed relation is not a
@@ -385,7 +121,7 @@ static int launch_tc_scatter(const __nv_bfloat16* dout, const __nv_bfloat16* wim
     return VC_OK;
 }
 
-// kc = C_out (reduction), nr = C_in (gradient channels); wimg = the K dgrad images (prep mode 1, no mirror)
+// kc = C_out (reduction), nr = C_in (gradient channels); wimg = the K dgrad images (prep mode 1, layout 0, no mirror)
 int tc_scatter_with_image(int kc, int nr, const void* dout_bf16, const void* wimg, const int32_t* nbr, float* din, int n_out,
                           int K, int* err, cudaStream_t stream) {
     if (n_out == 0) return VC_OK;
@@ -400,25 +136,6 @@ int tc_scatter_with_image(int kc, int nr, const void* dout_bf16, const void* wim
     set_error("tensor-core scatter dgrad: unsupported channel pair (%d, %d), need 16/32/64", kc, nr);
     return VC_ERR_UNSUPPORTED;
 }
-
-// ---- entry point for the plan executor (executor.cu) and the per-operator C ABI: pre-built weight images ----
-// variant 1 (default): the persistent kernel of conv_tc2.cu (swizzled images, C = 8 supported, optional device row count);
-// variant 0: the round-1 kernel above (core-matrix images, C >= 16, host row count, dense table pitch)
-int tc_conv_with_image(int kc, int nr, const void* in_bf16, const void* wimg, const int32_t* nbr, long long pitch, float* out,
-                       int n_rows, const int* n_dev, int K, double* bn_sums, int* err, cudaStream_t stream, const float* addend,
-                       int* tile_counter, int sparse_k) {
-    if (n_rows == 0) return VC_OK;
-    if (g_tc_variant == 1)
-        return tc2_conv(kc, nr, in_bf16, wimg, nbr, pitch, out, n_rows, n_dev, K, bn_sums, err, stream, addend, tile_counter, sparse_k);
-    if (n_dev != nullptr || pitch != n_rows) {
-        set_error("round-1 tensor-core conv kernel needs a host row count and a dense table");
-        return VC_ERR_UNSUPPORTED;
-    }
-    return dispatch_tc(kc, nr, (const __nv_bfloat16*)in_bf16, (const __nv_bfloat16*)wimg, nbr, out, n_rows, K, bn_sums, err,
-                       stream, addend);
-}
-
-bool tc_conv_ch_ok(int c) { return g_tc_variant == 1 ? tc2_ch_ok(c) : tc_ch_ok(c); }
 
 }  // namespace vc
 
@@ -450,7 +167,7 @@ static int tc_one_image(const float* w, void* img, int cin, int cout, int K, int
 static int tc_common(const void* feats_bf16, const float* w, const int32_t* nbr, float* out, int n_rows, int cin, int cout,
                      int K, int mode, int mirror, double* bn_sums, void* ws, size_t ws_bytes, int32_t* err, cudaStream_t stream) {
     VC_CHECK_ARG(n_rows >= 0 && K >= 1 && K <= MAXK_TC, "bad n=%d or K=%d", n_rows, K);
-    if (!tc_conv_ch_ok(cin) || !tc_conv_ch_ok(cout)) {
+    if (!tc2_ch_ok(cin) || !tc2_ch_ok(cout)) {
         set_error("tensor-core conv: unsupported channels cin=%d cout=%d", cin, cout);
         return VC_ERR_UNSUPPORTED;
     }
@@ -460,11 +177,11 @@ static int tc_common(const void* feats_bf16, const float* w, const int32_t* nbr,
         set_error("tensor-core conv workspace %zu < %zu", ws_bytes, vc_conv_tc_ws_bytes(cin, cout, K));
         return VC_ERR_WORKSPACE;
     }
-    int rc = tc_one_image(w, ws, cin, cout, K, mode, mirror, g_tc_variant, stream);
+    int rc = tc_one_image(w, ws, cin, cout, K, mode, mirror, 1, stream);
     if (rc) return rc;
     int kc = mode == 0 ? cin : cout, nr = mode == 0 ? cout : cin;
-    return tc_conv_with_image(kc, nr, feats_bf16, ws, nbr, n_rows, out, n_rows, nullptr, K, bn_sums, err, stream, nullptr, nullptr,
-                              (mode == 1 && !mirror) ? 1 : 0);
+    return tc2_conv(kc, nr, feats_bf16, ws, nbr, n_rows, out, n_rows, nullptr, K, bn_sums, err, stream, nullptr, nullptr,
+                    (mode == 1 && !mirror) ? 1 : 0);
 }
 
 extern "C" int vc_conv_fwd_tc(const void* in_bf16, const float* w, const int32_t* nbr, float* out, int n_out, int cin,
@@ -479,7 +196,7 @@ extern "C" int vc_conv_dgrad_scatter_tc(const void* dout_bf16, const float* w, c
                                         vc_stream_t stream_) {
     cudaStream_t stream = (cudaStream_t)stream_;
     VC_CHECK_ARG(n_out >= 0 && K >= 1 && K <= MAXK_TC, "bad n=%d or K=%d", n_out, K);
-    if (!tc_ch_ok(cin) || !tc_ch_ok(cout)) {
+    if (!tc_scatter_ch_ok(cin) || !tc_scatter_ch_ok(cout)) {
         set_error("tensor-core scatter dgrad: unsupported channels cin=%d cout=%d (need 16/32/64)", cin, cout);
         return VC_ERR_UNSUPPORTED;
     }
@@ -500,363 +217,3 @@ extern "C" int vc_conv_dgrad_tc(const void* dout_bf16, const float* w, const int
     return tc_common(dout_bf16, w, nbr_t, din, n_in, cin, cout, K, 1, mirror, nullptr, ws, ws_bytes, err_flag,
                      (cudaStream_t)stream_);
 }
-
-// ================================================================================================
-// wgrad on tensor cores.
-//   dW[k] (C_in x C_out) = sum over output rows o of  in[nbr[k,o], :]^T  (x)  dout[o, :]
-// Output-stationary again: for one tile of 128 output rows the dout tile B [128 x C_out] is the SAME operand
-// for every kernel offset, and the gathered tile A_k [128 x C_in] is exactly the forward kernel's operand.
-// Both are used MN-major (the reduction runs over the 128 rows), which is the same core-matrix image as the
-// forward K-major gather — so no transpose anywhere.  G = 128/C_in offsets are stacked along the MMA M
-// dimension (rows of D = (offset j, channel ci)), 2 x 8 MMAs (two m64 row blocks, K=16 rows each) per group and tile;
-// every CTA keeps its pass's accumulators (<= 64 / C_out groups) in registers across ALL the tiles it owns (persistent
-// CTAs, one per SM) and writes one fp32 partial at the end; partials are summed in a fixed order.
-// ================================================================================================
-namespace vc {
-
-static constexpr int WG_THREADS = 128;   // one warpgroup: gather + MMA + epilogue
-
-template <int CI, int CO>
-struct WgTc {
-    static constexpr int CPR = CI / 8, CPO = CO / 8;
-    static constexpr int G = 128 / CI;                 // offsets stacked along M
-    static constexpr int A_STAGE = 16 * 2048;          // [16 row groups][16 slots][8 rows][16 B]
-    static constexpr int B_BYTES = TCM * CO * 2;
-    static constexpr int STAGES = 3;
-    static constexpr int MAX_GROUPS = 64 / CO;         // accumulator registers per thread: 64
-    static constexpr size_t smem(int kcount) { return (size_t)STAGES * A_STAGE + B_BYTES + 2 * (size_t)kcount * TCM * 4; }
-};
-
-template <int CI, int CO>
-__global__ void __launch_bounds__(WG_THREADS)
-tc_wgrad_kernel(const __nv_bfloat16* __restrict__ in, const __nv_bfloat16* __restrict__ dout,
-                const int32_t* __restrict__ nbr, float* __restrict__ partial, int n_out, int K, int groups_per_pass,
-                int* __restrict__ err) {
-    using C = WgTc<CI, CO>;
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* ring = smem_raw;
-    unsigned char* Bt = smem_raw + C::STAGES * C::A_STAGE;
-    int* nbr_buf = reinterpret_cast<int*>(Bt + C::B_BYTES);   // [2][k_count][128]: current tile / prefetched next tile
-    __shared__ __align__(8) uint64_t stage_done[C::STAGES];
-    __shared__ __align__(8) uint64_t tile_done;
-    __shared__ unsigned gmask_s;
-    __shared__ int glist[32];
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int n_groups_total = (K + C::G - 1) / C::G;
-    const int g_begin = blockIdx.y * groups_per_pass;
-    const int g_count = min(groups_per_pass, n_groups_total - g_begin);
-    const int k_begin = g_begin * C::G;
-    const int k_count = min(g_count * C::G, K - k_begin);
-    const int n_tiles = (n_out + TCM - 1) / TCM;
-
-    if (tid == 0) {
-        for (int s = 0; s < C::STAGES; ++s) mbar_init(&stage_done[s], 1);
-        mbar_init(&tile_done, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-
-    const int rl = lane & 7, xq = lane >> 3;   // 8 rows x 4 consecutive slots per warp instruction
-    unsigned it = 0;          // stage uses so far (ring position; same value in every thread)
-    unsigned tiles_done = 0;  // tiles that issued at least one MMA group
-    bool ok = true;
-    float acc[C::MAX_GROUPS][2][CO / 2];      // group, m64 row block
-#pragma unroll
-    for (int gg = 0; gg < C::MAX_GROUPS; ++gg)
-#pragma unroll
-        for (int j = 0; j < CO / 2; ++j) acc[gg][0][j] = acc[gg][1][j] = 0.f;
-
-    // neighbour-table slice of a tile: thread `tid` owns row base+tid for every offset of this pass (coalesced per
-    // offset).  The NEXT tile's slice is loaded into registers at the top of the current tile and parked in the
-    // other smem buffer at its end, so no tile ever waits for its table (it was 43 % of this kernel's stall samples).
-    int nv[MAXK_TC];
-    auto load_nbr_regs = [&](int tile_) {
-        const int row = tile_ * TCM + tid;
-#pragma unroll
-        for (int j = 0; j < MAXK_TC; ++j)
-            nv[j] = (j < k_count && tile_ < n_tiles && row < n_out) ? __ldg(nbr + (size_t)(k_begin + j) * n_out + row) : -1;
-    };
-    auto park_nbr_regs = [&](int* dst) {
-#pragma unroll
-        for (int j = 0; j < MAXK_TC; ++j)
-            if (j < k_count) dst[j * TCM + tid] = nv[j];
-    };
-    int cur = 0;
-    load_nbr_regs(blockIdx.x);
-    park_nbr_regs(nbr_buf);
-    __syncthreads();
-
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        const int base = tile * TCM;
-        int* nbr_s = nbr_buf + cur * k_count * TCM;
-        int* nbr_next = nbr_buf + (cur ^ 1) * k_count * TCM;
-        load_nbr_regs(tile + gridDim.x);             // in flight while this tile is processed
-        // previous tile's MMAs still read Bt: wait for them before overwriting it
-        if (tiles_done > 0) ok &= mbar_wait(&tile_done, (tiles_done - 1) & 1u, err);
-        if (tid == 0) gmask_s = 0u;
-        // dout tile, image [r/8][CPO][r%8][16 B]
-        for (int q = tid; q < TCM * C::CPO; q += WG_THREADS) {
-            int r = (q / (8 * C::CPO)) * 8 + (q & 7), c = (q >> 3) % C::CPO;
-            bool v = base + r < n_out;
-            cp_async16(Bt + ((r >> 3) * C::CPO + c) * 128 + (r & 7) * 16, dout + (size_t)(v ? base + r : 0) * CO + c * 8, v);
-        }
-        cp_async_commit();
-        __syncthreads();
-        for (int g = warp; g < g_count; g += WG_THREADS / 32) {
-            bool any = false;
-            for (int j = 0; j < C::G; ++j) {
-                int kk = g * C::G + j;
-                if (kk < k_count) {
-#pragma unroll
-                    for (int q = 0; q < TCM / 32; ++q) any |= nbr_s[kk * TCM + q * 32 + lane] >= 0;
-                }
-            }
-            if (__any_sync(0xffffffffu, any) && lane == 0) atomicOr(&gmask_s, 1u << g);
-        }
-        __syncthreads();
-        const unsigned gm = gmask_s;
-        const int ng = __popc(gm);
-        if (tid == 0) {
-            int c = 0;
-            for (int g = 0; g < g_count; ++g)
-                if (gm >> g & 1u) glist[c++] = g;
-        }
-        __syncthreads();
-        if (ng == 0) {
-            cp_async_wait<0>();
-            park_nbr_regs(nbr_next);
-            cur ^= 1;
-            __syncthreads();
-            continue;
-        }
-
-        auto issue_group = [&](int t, unsigned use) {
-            const int g = glist[t];
-            const uint32_t a_s = smem_u32(ring + (use % C::STAGES) * C::A_STAGE);
-            int src[4][4];
-#pragma unroll
-            for (int sg = 0; sg < 4; ++sg) {                    // 16 slots = 4 x 4; independent table reads first
-                const int kk = g * C::G + (sg * 4 + xq) / C::CPR;
-#pragma unroll
-                for (int itr = 0; itr < 4; ++itr)
-                    src[itr][sg] = (kk < k_count) ? nbr_s[kk * TCM + warp * 32 + itr * 8 + rl] : -1;
-            }
-#pragma unroll
-            for (int itr = 0; itr < 4; ++itr) {                 // 4 x 8 rows per warp
-                const int r = warp * 32 + itr * 8 + rl;
-#pragma unroll
-                for (int sg = 0; sg < 4; ++sg) {
-                    const int slot = sg * 4 + xq;
-                    const int sv = src[itr][sg];
-                    cp_async16_s(a_s + (uint32_t)(((r >> 3) * 16 + slot) * 128 + (r & 7) * 16),
-                                 in + (size_t)(sv < 0 ? 0 : sv) * CI + (slot % C::CPR) * 8, sv >= 0);
-                }
-            }
-        };
-
-        // software pipeline over the active groups of this tile (ring positions continue across tiles)
-        const unsigned it0 = it;
-        for (int t = 0; t < C::STAGES - 1; ++t) {
-            if (t < ng) {
-                unsigned use = it0 + t;
-                if (use >= (unsigned)C::STAGES) ok &= mbar_wait(&stage_done[use % C::STAGES], ((use / C::STAGES) - 1) & 1u, err);
-                issue_group(t, use);
-            }
-            cp_async_commit();
-        }
-        for (int t = 0; t < ng; ++t) {
-            const int tn = t + C::STAGES - 1;
-            if (tn < ng) {
-                unsigned use = it0 + tn;
-                if (use >= (unsigned)C::STAGES) ok &= mbar_wait(&stage_done[use % C::STAGES], ((use / C::STAGES) - 1) & 1u, err);
-                issue_group(tn, use);
-            }
-            cp_async_commit();
-            cp_async_wait<C::STAGES - 1>();      // group t (and, on t == 0, the dout tile) has landed
-            fence_async_smem();
-            __syncthreads();
-            {
-                const unsigned use = it0 + t;
-                const int g = glist[t];
-                const uint32_t a0 = smem_u32(ring + (use % C::STAGES) * C::A_STAGE);
-                const uint32_t b0 = smem_u32(Bt);
-                wg_fence();
-                // both operands MN-major, no swizzle: LBO = between core matrices along K, SBO = along M / N
-#pragma unroll
-                for (int gg = 0; gg < C::MAX_GROUPS; ++gg) {
-                    if (gg == g) {
-#pragma unroll
-                        for (int s = 0; s < 8; ++s) {   // 16 rows (two 8-row groups) per MMA
-                            const uint64_t bd = gmma_desc(b0 + s * 2 * C::CPO * 128, C::CPO * 128, 128, 0);
-#pragma unroll
-                            for (int h = 0; h < 2; ++h)
-                                wgmma_bf16<CO, 1, 1>(acc[gg][h], gmma_desc(a0 + s * 2 * 2048 + h * 1024, 2048, 128, 0), bd, 1u);
-                        }
-                    }
-                }
-                wg_commit();
-                wg_wait<0>();
-                if (tid == 0) {
-                    mbar_arrive(&stage_done[use % C::STAGES]);
-                    if (t == ng - 1) mbar_arrive(&tile_done);
-                }
-            }
-        }
-        it = it0 + ng;
-        ++tiles_done;
-        park_nbr_regs(nbr_next);    // nbr_next was last read while tile-1's gathers were issued: free since then
-        cur ^= 1;
-        __syncthreads();
-    }
-    if (tiles_done > 0) ok &= mbar_wait(&tile_done, (tiles_done - 1) & 1u, err);
-    cp_async_wait<0>();
-#pragma unroll
-    for (int gg = 0; gg < C::MAX_GROUPS; ++gg) {
-        wg_fence_acc(acc[gg][0]);
-        wg_fence_acc(acc[gg][1]);
-    }
-    // epilogue: accumulator row = (offset j, channel ci) of the group, column = C_out
-    float* mine = partial + (size_t)blockIdx.x * K * CI * CO;
-#pragma unroll
-    for (int gg = 0; gg < C::MAX_GROUPS; ++gg) {
-        if (gg >= g_count) break;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-#pragma unroll
-            for (int j = 0; j < CO / 2; j += 2) {
-                const int m = 64 * h + wg_row(j, tid);
-                const int kk = gg * C::G + m / CI, ci = m % CI;
-                if (kk < k_count)
-                    *reinterpret_cast<float2*>(mine + ((size_t)(k_begin + kk) * CI + ci) * CO + wg_col(j, tid)) =
-                        make_float2(acc[gg][h][j], acc[gg][h][j + 1]);
-            }
-        }
-    }
-    (void)ok;
-}
-
-// fixed-order sum of the per-CTA partials; threads index the PARTIAL layout [k][ci][co] so every one of the R reads
-// is coalesced, the single (transposing) write goes to the parameter layout [co][k][ci]
-__global__ void __launch_bounds__(256) wgrad_tc_reduce_kernel(const float* __restrict__ partial, float* __restrict__ dw,
-                                                              int R, int K, int cin, int cout) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    int total = K * cin * cout;
-    if (i >= total) return;
-    int co = i % cout, ci = (i / cout) % cin, k = i / (cout * cin);
-    float v0 = 0.f, v1 = 0.f, v2 = 0.f, v3 = 0.f;
-    int r = 0;
-    for (; r + 4 <= R; r += 4) {
-        v0 += __ldg(partial + (size_t)(r + 0) * total + i);
-        v1 += __ldg(partial + (size_t)(r + 1) * total + i);
-        v2 += __ldg(partial + (size_t)(r + 2) * total + i);
-        v3 += __ldg(partial + (size_t)(r + 3) * total + i);
-    }
-    for (; r < R; ++r) v0 += __ldg(partial + (size_t)r * total + i);
-    dw[((size_t)co * K + k) * cin + ci] = (v0 + v1) + (v2 + v3);
-}
-
-// Background mode (vc_conv_wgrad_tc_config): wgrad runs on its own stream next to the BN-backward / dgrad chain.  Its
-// persistent CTAs then (a) number fewer than the SMs and (b) pad their dynamic shared memory so that no gather-GEMM CTA
-// fits beside them for the whole lifetime of the persistent CTA.  The chain keeps the remaining SMs to itself.
-static int g_wgrad_ctas = 0;          // 0: one CTA per SM of the current device
-static int g_wgrad_smem_floor = 0;
-
-static int wgrad_tc_grid(int n_out) {
-    int cap = g_wgrad_ctas;
-    if (cap <= 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&cap, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || cap <= 0) cap = 132;
-    }
-    int tiles = (n_out + TCM - 1) / TCM;
-    return tiles < cap ? (tiles < 1 ? 1 : tiles) : cap;
-}
-
-template <int CI, int CO>
-static int launch_wgrad_tc(const __nv_bfloat16* in, const __nv_bfloat16* dout, const int32_t* nbr, float* partial, int n_out,
-                           int K, int* err, cudaStream_t stream) {
-    using C = WgTc<CI, CO>;
-    int n_groups = (K + C::G - 1) / C::G;
-    int gpp = n_groups < C::MAX_GROUPS ? n_groups : C::MAX_GROUPS;
-    int passes = (n_groups + gpp - 1) / gpp;
-    gpp = (n_groups + passes - 1) / passes;       // balance the passes
-    int kcount = gpp * C::G < K ? gpp * C::G : K;
-    size_t smem = C::smem(kcount);
-    if (smem < (size_t)g_wgrad_smem_floor) smem = (size_t)g_wgrad_smem_floor;
-    auto kern = tc_wgrad_kernel<CI, CO>;
-    VC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<dim3(wgrad_tc_grid(n_out), passes), WG_THREADS, smem, stream>>>(in, dout, nbr, partial, n_out, K, gpp, err);
-    VC_LAUNCH_CHECK();
-    return VC_OK;
-}
-
-}  // namespace vc
-
-extern "C" int vc_conv_wgrad_tc_config(int max_ctas, int smem_floor_bytes) {
-    VC_CHECK_ARG(max_ctas >= 0 && max_ctas <= 1024 && smem_floor_bytes >= 0 && smem_floor_bytes <= 227 * 1024,
-                 "wgrad config out of range (ctas %d, smem floor %d)", max_ctas, smem_floor_bytes);
-    vc::g_wgrad_ctas = max_ctas;
-    vc::g_wgrad_smem_floor = smem_floor_bytes;
-    return VC_OK;
-}
-
-extern "C" size_t vc_conv_wgrad_tc_ws_bytes(int n_out, int cin, int cout, int K) {
-    // round-1 kernel: one [K, cin, cout] partial per CTA; persistent kernel (variant 1): one scratch image + 2 tile counters
-    const size_t v0 = (size_t)vc::wgrad_tc_grid(n_out) * K * cin * cout * sizeof(float);
-    const size_t v1 = (size_t)K * cin * cout * sizeof(float) + 64;
-    return v0 > v1 ? v0 : v1;
-}
-
-extern "C" int vc_conv_wgrad_tc(const void* in_bf16, const void* dout_bf16, const int32_t* nbr, float* dw, int n_out,
-                                int cin, int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag,
-                                vc_stream_t stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
-    VC_CHECK_ARG(n_out >= 0 && K >= 1 && K <= MAXK_TC && dw, "bad arguments");
-    if (!tc_conv_ch_ok(cin) || !tc_conv_ch_ok(cout)) {
-        set_error("tensor-core wgrad: unsupported channels cin=%d cout=%d", cin, cout);
-        return VC_ERR_UNSUPPORTED;
-    }
-    if (n_out == 0) {
-        VC_CUDA(cudaMemsetAsync(dw, 0, (size_t)K * cin * cout * 4, stream));
-        return VC_OK;
-    }
-    VC_CHECK_ARG(in_bf16 && dout_bf16 && nbr && ws, "null pointer");
-    if (ws_bytes < vc_conv_wgrad_tc_ws_bytes(n_out, cin, cout, K)) {
-        set_error("tensor-core wgrad workspace %zu < %zu", ws_bytes, vc_conv_wgrad_tc_ws_bytes(n_out, cin, cout, K));
-        return VC_ERR_WORKSPACE;
-    }
-    if (g_tc_variant == 1) {
-        // persistent kernel (wgrad_tc2.cu): accumulate into a zeroed scratch image, then one transposing pass
-        const size_t wbytes = (size_t)K * cin * cout * sizeof(float);
-        VC_CUDA(cudaMemsetAsync(ws, 0, wbytes + 64, stream));
-        int rc1 = tc2_wgrad(cin, cout, in_bf16, dout_bf16, nbr, n_out, (float*)ws, n_out, nullptr, K, err_flag, stream,
-                            reinterpret_cast<int*>((char*)ws + wbytes));
-        if (rc1) return rc1;
-        WgradFinTable T;
-        T.n = 1;
-        T.e[0].scratch = (const float*)ws; T.e[0].dw = dw; T.e[0].cin = cin; T.e[0].cout = cout; T.e[0].K = K; T.e[0].first = 0;
-        return wgrad_finalize(T, stream);
-    }
-    float* partial = (float*)ws;
-    const __nv_bfloat16* a = (const __nv_bfloat16*)in_bf16;
-    const __nv_bfloat16* b = (const __nv_bfloat16*)dout_bf16;
-    int rc = VC_ERR_UNSUPPORTED;
-#define VC_WG_CASE(A, B) \
-    if (cin == A && cout == B) rc = launch_wgrad_tc<A, B>(a, b, nbr, partial, n_out, K, err_flag, stream);
-    VC_WG_CASE(16, 16) VC_WG_CASE(16, 32) VC_WG_CASE(16, 64)
-    VC_WG_CASE(32, 16) VC_WG_CASE(32, 32) VC_WG_CASE(32, 64)
-    VC_WG_CASE(64, 16) VC_WG_CASE(64, 32) VC_WG_CASE(64, 64)
-#undef VC_WG_CASE
-    if (rc) return rc;
-    int total = K * cin * cout;
-    wgrad_tc_reduce_kernel<<<cdiv(total, 256), 256, 0, stream>>>(partial, dw, wgrad_tc_grid(n_out), K, cin, cout);
-    VC_LAUNCH_CHECK();
-    return VC_OK;
-}
-
-#ifdef VC_TC_TRACE
-extern "C" int vc_debug_set_trace(long long* buf) {
-    return cudaMemcpyToSymbol(vc::g_trace, &buf, sizeof(buf)) == cudaSuccess ? 0 : -2;
-}
-#endif

@@ -1,9 +1,9 @@
-// bf16 tensor-core sparse convolution, forward and dgrad — PERSISTENT variant (round 2), wgmma, sm_90a.
+// bf16 tensor-core sparse convolution, forward and gather dgrad — persistent gather-GEMM, wgmma, sm_90a.
 //
-// Same contraction as conv_tc.cu (output-stationary 128-row tiles, per kernel offset one [128 x C_in] x [C_in x C_out]
-// product accumulating in fp32).  A launch of the round-1 kernel was one wave of short-lived CTAs, each a chain of <= 27
-// dependent {table read -> gather round trip -> MMA} links on a 2-deep ring.  Here CTAs live for the whole launch, claim
-// tiles from a counter and run a warp-specialised pipeline (DESIGN.md section 4 has the account).
+// Output-stationary 128-row tiles, per kernel offset one [128 x C_in] x [C_in x C_out] product accumulating in fp32.
+// A launch of one short-lived CTA per tile (round 1) was one wave of CTAs, each a chain of <= 27 dependent {table read ->
+// gather round trip -> MMA} links on a 2-deep ring.  Here CTAs live for the whole launch, claim tiles from a counter and
+// run a warp-specialised pipeline (DESIGN.md section 4 has the account).
 // TWO CTAs per SM by default (<= 111 KB shared memory each; one CTA with the whole SM where a two-stage ring would not fit),
 // 448 threads per CTA:
 //   warps 0-7   two consumer warpgroups, one per 64-row half of the tile: wait for a ring stage, issue its wgmma.mma_async
@@ -30,15 +30,20 @@
 
 namespace vc {
 
-int g_tc_variant = 1;   // 1: this kernel; 0: the round-1 kernel (conv_tc.cu) — vc_set_tc_variant, A/B runs only
+int num_sms() {
+    static int sms = 0;
+    if (sms == 0) {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
+    }
+    return sms;
+}
 
 namespace {
 
 #ifndef VC_P_GROUPS
 #define VC_P_GROUPS 1            // producer groups of 8 warps; consecutive ring stages go to consecutive groups (1: two CTAs fit an SM)
-#endif
-#ifndef VC_P_SKIP
-#define VC_P_SKIP 1              // 1: missing neighbours cost a shared-memory zero store, not a (zero-fill) cp.async
 #endif
 constexpr int P_CONS_WARPS = 8;                                 // two consumer warpgroups
 constexpr int P_CONS_THREADS = 32 * P_CONS_WARPS;
@@ -152,7 +157,7 @@ __global__ void __launch_bounds__(P_THREADS, P_GROUPS == 1 ? 2 : 1) tc_conv_pers
         for (int s = 0; s < S; ++s) {
             // every producer thread (cp.async.mbarrier.arrive.noinc: fires when its copies of the stage have landed) + one release
             // arrive per producer warp for its zero stores [+ the weight warp's expect_tx]
-            mbar_init(&full_bar[s], 32 * P_PROD_WARPS + (VC_P_SKIP ? P_PROD_WARPS : 0) + (wres ? 0 : 1));
+            mbar_init(&full_bar[s], 32 * P_PROD_WARPS + P_PROD_WARPS + (wres ? 0 : 1));
             mbar_init(&empty_bar[s], 2);                       // one arrive per consumer warpgroup
         }
         for (int b = 0; b < P_NTB; ++b) {
@@ -337,11 +342,7 @@ __global__ void __launch_bounds__(P_THREADS, P_GROUPS == 1 ? 2 : 1) tc_conv_pers
                     for (int g = 0; g < C::G; ++g) {
 #pragma unroll
                         const int kk = g < cnt ? (a.scan_k ? klist_s[tb][t0 + g] : t0 + g) : 0;
-#ifdef VC_DBG_NO_TBL
-                        for (int i = 0; i < NIT; ++i) src[g][i] = g < cnt ? rows[i] + (int)((uintptr_t)tbl & 1) + 0 * kk : -1;
-#else
                         for (int i = 0; i < NIT; ++i) src[g][i] = g < cnt ? tbl[kk * TCM + rows[i]] : -1;
-#endif
                     }
                     if (wr > 0) P_WAIT(&empty_bar[s], (uint32_t)((wr - 1) & 1), 0x112);
                     if (leader) P_CLOCK(7, tr3);                                  // phase 1: ring slot free
@@ -356,30 +357,17 @@ __global__ void __launch_bounds__(P_THREADS, P_GROUPS == 1 ? 2 : 1) tc_conv_pers
                                 const __nv_bfloat16* srow = a.in + (size_t)(v ? src[g][i] : 0) * a.in_c + c_sub * 8;
 #pragma unroll
                                 for (int cg = 0; cg < NCG; ++cg) {
-                                    const bool vc = v && ch_ok[cg];
-#if defined(VC_DBG_NO_COPY) && defined(VC_DBG_NO_ZERO)
-                                    (void)vc; (void)srow;
-#elif defined(VC_DBG_NO_COPY)
-                                    if (!vc) sts_zero16(a_s + dst_off[i][cg]);
-#elif defined(VC_DBG_LINEAR_DST)
-                                    if (vc) cp_async16_s(a_s + (uint32_t)((rows[i] * C::CPR + cg * CW + c_sub) * 16), srow + cg * CW * 8, true);
+                                    // a missing neighbour costs a shared-memory zero store, not a zero-fill cp.async
+                                    if (v && ch_ok[cg]) cp_async16_s(a_s + dst_off[i][cg], srow + cg * CW * 8, true);
                                     else sts_zero16(a_s + dst_off[i][cg]);
-#elif VC_P_SKIP
-                                    if (vc) cp_async16_s(a_s + dst_off[i][cg], srow + cg * CW * 8, true);
-                                    else sts_zero16(a_s + dst_off[i][cg]);
-#else
-                                    cp_async16_s(a_s + dst_off[i][cg], vc ? srow + cg * CW * 8 : a.in, vc);
-#endif
                                 }
                             }
                         }
                     }
                     if (leader) P_CLOCK(7, tr3);                                  // phase 2: copies issued
                     cp_async_arrive_noinc(&full_bar[s]);       // fires when this thread's copies of the stage have landed
-#if VC_P_SKIP
                     __syncwarp();
                     if (lane == 0) mbar_arrive(&full_bar[s]);  // release: publishes the warp's zero stores
-#endif
                     if (leader) P_CLOCK(7, tr3);                                  // phase 3: stage signalled
                     if (leader) P_TRACE(1, tr);
                 }
@@ -573,16 +561,6 @@ __device__ __forceinline__ size_t img_off(int k, int n, int kk, int NRp) {
     return (size_t)k * NRp * ROWB + swz_off<ROWB>(n, kk >> 3) + (size_t)(kk & 7) * 2;
 }
 
-int num_sms() {
-    static int sms = 0;
-    if (sms == 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
-    }
-    return sms;
-}
-
 #ifndef VC_P_MIN_STAGES2
 #define VC_P_MIN_STAGES2 2       // two CTAs per SM are used when each still gets a ring of at least this many stages
 #endif
@@ -672,7 +650,7 @@ __global__ void __launch_bounds__(256) prep_weights_tc_batch_kernel(TcPrepTable 
         }
     }
     const __nv_bfloat16 b = __float2bfloat16_rn(v);
-    if (e.layout == 0) {      // round-1 image: 8-row x 16-byte core matrices, no swizzle (tc_scatter_kernel, legacy gather kernel)
+    if (e.layout == 0) {      // 8-row x 16-byte core matrices, no swizzle (tc_scatter_kernel)
         const size_t off = (size_t)k * NRr * KCc + ((size_t)((n >> 3) * (KCc >> 3) + (kk >> 3)) * 64) + (n & 7) * 8 + (kk & 7);
         reinterpret_cast<__nv_bfloat16*>(e.img)[off] = b;
     } else {
@@ -705,7 +683,7 @@ bool tc2_ch_ok(int c) { return c == 8 || c == 16 || c == 32 || c == 64; }
 // (layout 1).  n_dev (optional) overrides n_rows on the device; n_rows is then the capacity the grid is sized for.
 int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_t* nbr, long long pitch, float* out,
              int n_rows, const int* n_dev, int K, double* bn_sums, int* err, cudaStream_t stream, const float* addend,
-             int* tile_counter, int sparse_k) {
+             int* tile_counter, int flags) {
     if (n_rows == 0) return VC_OK;
     if (!tc2_ch_ok(kc) || !tc2_ch_ok(nr) || K < 1 || K > MAXK_TC) {
         set_error("tensor-core conv: unsupported shape (%d -> %d channels, K=%d)", kc, nr, K);
@@ -714,7 +692,7 @@ int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_
     PArgs a;
     a.in = (const __nv_bfloat16*)in_bf16; a.in_c = kc; a.wimg = (const unsigned char*)wimg; a.nbr = nbr; a.pitch = pitch;
     a.out = out; a.out_c = nr; a.addend = addend; a.bn_sums = bn_sums; a.n_dev = n_dev; a.n_host = n_rows; a.tile_counter = tile_counter;
-    a.K = K; a.S = 0; a.w_resident = 0; a.ntb_alloc = P_NTB; a.scan_k = sparse_k & 1; a.early_tables = (sparse_k >> 1) & 1;
+    a.K = K; a.S = 0; a.w_resident = 0; a.ntb_alloc = P_NTB; a.scan_k = flags & 1; a.early_tables = (flags >> 1) & 1;
     a.err = err;
     const int kcp = tc_pad16(kc), nrp = tc_pad16(nr);
 #define VC_P_CASE(A, B) \
@@ -741,7 +719,6 @@ extern "C" int vc_conv_tc2_config(int ctas_per_sm) {
 }
 
 extern "C" int vc_set_tc_variant(int variant) {
-    VC_CHECK_ARG(variant == 0 || variant == 1, "tensor-core conv variant must be 0 (round-1 kernel) or 1 (persistent)");
-    vc::g_tc_variant = variant;
+    VC_CHECK_ARG(variant == 1, "tensor-core conv variant must be 1 (the persistent kernel is the only one)");
     return VC_OK;
 }

@@ -62,7 +62,7 @@ struct Layer {
     int* tile_ctr;         // [CTR_PER_LAYER] tile-scheduler counters of the persistent kernels (forward, dgrad, wgrad passes), zeroed with the sums
     float* wscratch;       // [K][cin][cout] fp32 accumulator of the persistent wgrad kernel (zeroed with the sums), or NULL
     void *wimg_fwd, *wimg_dgrad;
-    int in_slot, out_slot, rb, use_tc, use_tc_w, cin, cout, need_dgrad;   // use_tc: conv fwd / gather dgrad; use_tc_w: wgrad / scatter dgrad
+    int in_slot, out_slot, rb, use_tc, use_tc_scatter, cin, cout, need_dgrad;   // use_tc: conv fwd / gather dgrad / wgrad
 };
 struct State {
     uint64_t magic;
@@ -185,8 +185,6 @@ int launch_add(const float* a, const float* b, float* c, size_t n, cudaStream_t 
     VC_LAUNCH_CHAIN(add_kernel, dim3(ew_grid(n / 4)), dim3(256), 0, st, (const float4*)a, (const float4*)b, (float4*)c, n / 4);
     return VC_OK;
 }
-
-bool tc_ok(int c) { return c == 16 || c == 32 || c == 64; }
 
 struct Ctx {
     const int32_t* oi;
@@ -391,7 +389,7 @@ extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_o
             const int* o = C.op(i);
             sums_doubles += 4 * (size_t)o[F_COUT];
             ++n_cbr;
-            if (training && precision == 1 && g_tc_variant == 1 && tc2_ch_ok(o[F_CIN]) && tc2_ch_ok(o[F_COUT]))
+            if (training && precision == 1 && tc2_ch_ok(o[F_CIN]) && tc2_ch_ok(o[F_COUT]))
                 wg_floats += ((size_t)rb_K[o[F_C]] * o[F_CIN] * o[F_COUT] + 63) / 64 * 64;
         }
     const size_t zero_bytes = sums_doubles * 8 + n_cbr * CTR_PER_LAYER * sizeof(int) + wg_floats * 4;
@@ -409,13 +407,13 @@ extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_o
         Layer& L = S->layer[o[F_LAYER]];
         L.cin = o[F_CIN]; L.cout = o[F_COUT]; L.in_slot = o[F_A]; L.out_slot = o[F_B]; L.rb = o[F_C];
         L.need_dgrad = o[F_X0];
-        L.use_tc = precision == 1 && tc_conv_ch_ok(L.cin) && tc_conv_ch_ok(L.cout);
-        L.use_tc_w = precision == 1 && tc_ok(L.cin) && tc_ok(L.cout);
+        L.use_tc = precision == 1 && tc2_ch_ok(L.cin) && tc2_ch_ok(L.cout);
+        L.use_tc_scatter = precision == 1 && tc_scatter_ch_ok(L.cin) && tc_scatter_ch_ok(L.cout);
         L.sums = sums_all + sums_cur;
         sums_cur += 4 * (size_t)L.cout;
         L.tile_ctr = ctr_all + CTR_PER_LAYER * ctr_cur++;
         L.wscratch = nullptr;
-        if (training && precision == 1 && g_tc_variant == 1 && tc2_ch_ok(L.cin) && tc2_ch_ok(L.cout)) {
+        if (training && L.use_tc) {
             L.wscratch = wg_all + wg_cur;
             wg_cur += ((size_t)rb_K[L.rb] * L.cin * L.cout + 63) / 64 * 64;
         }
@@ -430,11 +428,11 @@ extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_o
             if (!L.use_tc) continue;
             const int K = rb_K[L.rb];
             // dgrad image: mirrored for a submanifold table used as its own transpose, plain for a strided conv's
-            // nbr_bwd table and for the many-to-one image-branch table (tensor-core scatter, round-1 image layout)
+            // nbr_bwd table and for the many-to-one image-branch table (tensor-core scatter, image layout 0)
             const bool many_to_one = rb_subm[L.rb] && !rb_unique[L.rb];
-            const bool dgrad_tc = training && L.need_dgrad && (!many_to_one || L.use_tc_w);
+            const bool dgrad_tc = training && L.need_dgrad && (!many_to_one || L.use_tc_scatter);
             for (int mode = 0; mode < (dgrad_tc ? 2 : 1); ++mode) {
-                const int layout = (mode == 1 && many_to_one) ? 0 : g_tc_variant;
+                const int layout = (mode == 1 && many_to_one) ? 0 : 1;
                 VC_ALLOC(img, void*, tc_image_bytes(L.cin, L.cout, K, layout));
                 (mode == 0 ? L.wimg_fwd : L.wimg_dgrad) = img;
                 if (T.n == TC_PREP_MAX) {
@@ -629,8 +627,8 @@ extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_o
                     // (flag bit 1: the rulebook was built on another stream and joined by an event, so the kernel may load its first
                     //  table slices before its griddepcontrol.wait — conv_tc2.cu)
                     if (do_feat)
-                        VC_TRY(tc_conv_with_image(L.cin, L.cout, X.bf16, L.wimg_fwd, R.nbr, R.n_out, x, R.n_out, R.n_out_dev, R.K, sums, C.err, st,
-                                                  nullptr, L.tile_ctr, (phase == 2 || C.st[R.prod] != C.st[s]) ? 2 : 0));
+                        VC_TRY(tc2_conv(L.cin, L.cout, X.bf16, L.wimg_fwd, R.nbr, R.n_out, x, R.n_out, R.n_out_dev, R.K, sums, C.err, st,
+                                        nullptr, L.tile_ctr, (phase == 2 || C.st[R.prod] != C.st[s]) ? 2 : 0));
                 } else {
                     const size_t wsb = vc_conv_ws_bytes(L.cin, L.cout, R.K);
                     VC_ALLOC(ws, void*, wsb);
@@ -758,6 +756,8 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
     const int training = S->training;
     WgradFinTable fin;          // persistent wgrad kernels accumulate into scratch images; ONE transposing launch at the end
     fin.n = 0;
+    // wgrad CTAs: half the SMs by default, so that a CTA of the dgrad chain fits beside each (DESIGN.md section 4)
+    const int wgrad_ctas = g_wgrad3_ctas > 0 ? g_wgrad3_ctas : (num_sms() + 1) / 2;
 
     for (int i = 0; i < MAX_F; ++i) { S->f[i].grad = nullptr; S->f[i].grad_state = G_EMPTY; }
     for (int i = 0; i < n_pub; ++i) {
@@ -823,19 +823,14 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
         }
         if (L.wscratch != nullptr) {
             Timed t(6, li, wst);
-            VC_TRY((g_wgrad_variant ? tc3_wgrad : tc2_wgrad)(L.cin, L.cout, X.bf16, dxb, R.nbr, R.n_out, L.wscratch, R.n_out, R.n_out_dev,
-                                                              R.K, C.err, wst, L.tile_ctr + 2));
+            VC_TRY(tc3_wgrad(L.cin, L.cout, X.bf16, dxb, R.nbr, R.n_out, L.wscratch, R.n_out, R.n_out_dev, R.K, C.err, wst,
+                             L.tile_ctr + 2, wgrad_ctas));
             if (fin.n == WGRAD_FIN_MAX) {
                 VC_TRY(wgrad_finalize(fin, wst));
                 fin.n = 0;
             }
             WgradFinEntry& fe = fin.e[fin.n++];
             fe.scratch = L.wscratch; fe.dw = dw; fe.cin = L.cin; fe.cout = L.cout; fe.K = R.K; fe.first = 0;
-        } else if (L.use_tc_w) {
-            const size_t wsb = vc_conv_wgrad_tc_ws_bytes(R.n_out, L.cin, L.cout, R.K);
-            VC_ALLOC(ws, void*, wsb);
-            Timed t(6, li, wst);
-            VC_TRY(vc_conv_wgrad_tc(X.bf16, dxb, R.nbr, dw, R.n_out, L.cin, L.cout, R.K, ws, wsb, C.err, wst));
         } else {
             const size_t wsb = vc_conv_wgrad_ws_bytes(R.n_out, L.cin, L.cout, R.K);
             VC_ALLOC(ws, void*, wsb);
@@ -845,7 +840,7 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
         if (two) last_w_ev = record_on(C, 1);
         // dgrad
         if (!L.need_dgrad || L.in_slot == 0) continue;
-        if (R.subm && !R.unique && L.use_tc_w && L.wimg_dgrad) {
+        if (R.subm && !R.unique && L.use_tc_scatter && L.wimg_dgrad) {
             VC_TRY(contribute_scatter(C, X, st, [&](float* dst) -> int {
                 Timed t(7, li, st);
                 return tc_scatter_with_image(L.cout, L.cin, dxb, L.wimg_dgrad, R.nbr, dst, R.n_out, R.K, C.err, st);
@@ -861,8 +856,8 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
             const int32_t* table = R.subm ? R.nbr : R.nbr_bwd;
             VC_TRY(contribute_fused(C, X, [&](float* dst, const float* addend) -> int {
                 Timed t(3, li, st);
-                return tc_conv_with_image(L.cout, L.cin, dxb, L.wimg_dgrad, table, R.n_in, dst, R.n_in, R.n_in_dev, R.K, nullptr, C.err, st,
-                                          addend, L.tile_ctr + 1, (R.subm ? 0 : 1) | 2);      // (tables from the forward call: early loads allowed)
+                return tc2_conv(L.cout, L.cin, dxb, L.wimg_dgrad, table, R.n_in, dst, R.n_in, R.n_in_dev, R.K, nullptr, C.err, st,
+                                addend, L.tile_ctr + 1, (R.subm ? 0 : 1) | 2);      // (tables from the forward call: early loads allowed)
             }));
         } else {
             const size_t wsb = vc_conv_ws_bytes(L.cin, L.cout, R.K);

@@ -1,4 +1,4 @@
-// wgmma / mbarrier helpers shared by the tensor-core kernels (conv_tc.cu, conv_tc2.cu, wgrad_tc2.cu, wgrad_tc3.cu) — sm_90a.
+// wgmma / mbarrier helpers shared by the tensor-core kernels (conv_tc.cu, conv_tc2.cu, wgrad_tc3.cu) — sm_90a.
 #pragma once
 #include <cuda_bf16.h>
 
@@ -217,7 +217,7 @@ __device__ __forceinline__ void red_add_v2(float* p, float a, float b) {
     asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
 }
 
-// ---- weight-gradient consumers (wgrad_tc2.cu, wgrad_tc3.cu) ---------------------------------------------------------------
+// ---- weight-gradient consumers (wgrad_tc3.cu) ---------------------------------------------------------------------------
 // D[(offset j, channel ci), co] += sum over rows of in[nbr[k, row], ci] * dout[row, co]: the gathered tiles and the dout tile are
 // both used MN-major (the reduction runs over the rows).  A group = 128 / CI kernel offsets stacked along M; warpgroup wg
 // owns M rows [64 wg, 64 wg + 64), i.e. starts 64 / CI gathered tiles into the stage.  acc[g] is group g of the pass; a group

@@ -1,36 +1,34 @@
-// Weight gradient of the sparse convolutions on tensor cores — HALF-TILE-STAGE variant of wgrad_tc2.cu (A/B: vc_conv_wgrad_tc3_config):
-// ring stages of 64 rows (16 KB), <= 111 KB shared memory and 416 threads per CTA, so that a wgrad CTA and a dgrad CTA of the main
-// stream can share an SM.  wgmma, sm_90a.
+// Weight gradient of the sparse convolutions on tensor cores — persistent, wgmma, sm_90a.
 //
 //   dW[k] (C_in x C_out) = sum over output rows o of  in[nbr[k,o], :]^T (x) dout[o, :]
 //
-// Same machinery as the persistent forward kernel (conv_tc2.cu): one CTA per SM walks 128-row output tiles (dynamic tile
-// counter), a loader warp stages the tile's neighbour-table slice (L2 prefetch several tiles ahead, cp.async into a
-// 2-deep shared ring), 4 producer warps gather the rows with 16-byte cp.async into 32/64/128-byte-swizzled tiles, two
-// consumer warpgroups (64 accumulator rows each) issue the MMAs.  What differs:
+// Ring stages of 64 rows (16 KB), <= 111 KB shared memory and 416 threads per CTA, so that a wgrad CTA and a dgrad CTA of the
+// main stream can share an SM: the plan executor runs this kernel on its own stream beside the dgrad chain.
+// Same machinery as the persistent forward kernel (conv_tc2.cu): persistent CTAs walk 128-row output tiles (dynamic tile
+// counter), a loader warp stages the tile's neighbour-table slice (cp.async into a 2-deep shared ring), 4 producer warps
+// gather the rows with 16-byte cp.async into 32/64/128-byte-swizzled tiles, two consumer warpgroups (64 accumulator rows
+// each) issue the MMAs.  What differs:
 //   * the gathered tile is used MN-MAJOR (the reduction runs over the 128 rows): the row-major swizzled tile the forward
 //     kernel builds is exactly the canonical Major-MN layout, and G = 128 / C_in kernel offsets are stacked along the MMA
 //     M dimension through the descriptor's leading-byte offset (one ring stage = G half tiles);
 //   * the second operand is the tile of dout itself (contiguous rows, loaded once per tile, double buffered);
 //   * the accumulators of the pass's offset groups (<= 64 / C_out, 32 registers per thread: two CTAs fit an SM) stay
-//     resident in registers across all tiles of the CTA (more groups: more passes, blockIdx.y); at the end each CTA adds its [K, C_in, C_out] partial into ONE fp32 scratch image with 8-byte vector reductions.  Round 1
-//     wrote 128 full partials per layer and re-read them in a second kernel (218 MB + 218 MB per step for 1.7 MB of
-//     gradients); here the reduction traffic is (#CTAs x gradient size) of L2 atomics and the only extra launch per STEP
-//     is the transposing finalize of all layers (wgrad_finalize_kernel).
-//   * C = 8 layers run with channels padded to 16 (zero-filled by the gather), so stage 1 no longer needs the fp32 kernel.
+//     resident in registers across all tiles of the CTA (more groups: more passes, blockIdx.y); at the end each CTA adds
+//     its [K, C_in, C_out] partial into ONE fp32 scratch image with 8-byte vector reductions.  Per-CTA partials re-read by a
+//     second kernel (round 1) cost 218 MB + 218 MB per step for 1.7 MB of gradients; here the reduction traffic is
+//     (#CTAs x gradient size) of L2 atomics and the only extra launch per STEP is the transposing finalize of all layers
+//     (wgrad_finalize_kernel).  The order of those reductions depends on scheduling: results vary in the last bits.
+//   * C = 8 layers run with channels padded to 16 (zero-filled by the gather).
 // Replaces spconv `ops.indice_conv_backward` (filter gradient) behind spconv_backbone.py:89,92-93,113,563-564.
 // Algorithmic bytes per launch: (N_in*C_in + N_out*C_out)*2 + P*8 + K*C_in*C_out*4;  FLOPs 2*P*C_in*C_out.
 #include "tc_common.cuh"
 
 namespace vc {
 
-int g_wgrad_variant = 1;    // plan executor: 1 = this file (default), 0 = wgrad_tc2.cu (one CTA per SM, 32 KB stages)
+int g_wgrad3_ctas = 0;      // CTA cap of the plan executor's launches (vc_conv_wgrad_tc3_config); 0 = half the SMs
 
 namespace {
 
-#ifndef VC_P_SKIP
-#define VC_P_SKIP 1              // 1: missing neighbours cost a shared-memory zero store, not a (zero-fill) cp.async
-#endif
 // Two CTAs per SM (like conv_tc2.cu: a CTA that leaves half the SM free can share it with the dgrad kernels of the main
 // stream).  A ring stage is HALF a tile (64 rows) of the GW offsets of one accumulator group: 16 KB; the two producer groups
 // (2 warps each) own the two halves.
@@ -107,7 +105,7 @@ __global__ void __launch_bounds__(W_THREADS, 2) tc_wgrad_half_kernel(const WArgs
         for (int s = 0; s < S; ++s) {
             // every producer thread of the stage's group (cp.async.mbarrier.arrive.noinc: fires when the thread's copies have
             // landed) + one release arrive per warp for its zero stores
-            mbar_init(&full_bar[s], 32 * W_GROUP_WARPS + (VC_P_SKIP ? W_GROUP_WARPS : 0));
+            mbar_init(&full_bar[s], 32 * W_GROUP_WARPS + W_GROUP_WARPS);
             mbar_init(&empty_bar[s], 2);                       // one arrive per consumer warpgroup
         }
         for (int b = 0; b < W_NTB; ++b) {
@@ -275,21 +273,15 @@ __global__ void __launch_bounds__(W_THREADS, 2) tc_wgrad_half_kernel(const WArgs
                             const __nv_bfloat16* srow = a.in + (size_t)(v ? src[j][i] : 0) * a.in_c + c_sub * 8;
 #pragma unroll
                             for (int cg = 0; cg < NCG; ++cg) {
-                                const bool vc = v && ch_ok[cg];
-#if VC_P_SKIP
-                                if (vc) cp_async16_s(a_s + dst_off[i][cg], srow + cg * CW * 8, true);
+                                // a missing neighbour costs a shared-memory zero store, not a zero-fill cp.async
+                                if (v && ch_ok[cg]) cp_async16_s(a_s + dst_off[i][cg], srow + cg * CW * 8, true);
                                 else w_sts_zero16(a_s + dst_off[i][cg]);
-#else
-                                cp_async16_s(a_s + dst_off[i][cg], vc ? srow + cg * CW * 8 : a.in, vc);
-#endif
                             }
                         }
                     }
                     cp_async_arrive_noinc(&full_bar[s]);
-#if VC_P_SKIP
                     __syncwarp();
                     if (lane == 0) mbar_arrive(&full_bar[s]);     // release: publishes the warp's zero stores
-#endif
                 }
                 if (++turn == W_GROUPS) turn = 0;
                 if (++s == S) {
@@ -356,22 +348,8 @@ done:
     __syncthreads();
 }
 
-int g_wgrad3_ctas = 0;      // CTA cap; 0 = half the SMs: the kernel runs on its own stream BESIDE the main stream's dgrad (a CTA of
-                            // each fits an SM) and fewer CTAs halve the [K,C_in,C_out] reduction traffic.  Measured on an H100 80GB
-                            // HBM3 at 700 W, graph step: 66 CTAs 4.36 ms/step, 132 CTAs 4.45, 33 CTAs 4.71 (wgrad_tc2: 4.58)
-
-int wg_num_sms() {
-    static int sms = 0;
-    if (sms == 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
-    }
-    return sms;
-}
-
 template <int CI, int CO>
-int launch_wgrad3(const WArgs& a0, int n_cap, cudaStream_t stream) {
+int launch_wgrad3(const WArgs& a0, int n_cap, int max_ctas, cudaStream_t stream) {
     using C = WCfg2<CI, CO>;
     WArgs a = a0;
     const int n_groups = (a.K + C::GW - 1) / C::GW;
@@ -396,17 +374,17 @@ int launch_wgrad3(const WArgs& a0, int n_cap, cudaStream_t stream) {
         attr_done = true;
     }
     const int tiles = cdiv(n_cap, TCM);
-    int cap = g_wgrad3_ctas > 0 ? g_wgrad3_ctas : (wg_num_sms() + 1) / 2;
-    const int grid = tiles < cap ? (tiles < 1 ? 1 : tiles) : cap;
+    const int grid = tiles < max_ctas ? (tiles < 1 ? 1 : tiles) : max_ctas;
     VC_LAUNCH_CHAIN(kern, dim3(grid, passes), dim3(W_THREADS), smem, stream, a);
     return VC_OK;
 }
 
 }  // namespace
 
-// scratch: [K][cin][cout] fp32, ZERO on entry (the kernel accumulates); tile_counter: `wgrad3_passes(cin, cout, K)` ints, zero
+// scratch: [K][cin][cout] fp32, ZERO on entry (the kernel accumulates); tile_counter: `wgrad3_passes(cin, cout, K)` ints, zero;
+// at most max_ctas CTAs per pass
 int tc3_wgrad(int cin, int cout, const void* in_bf16, const void* dout_bf16, const int32_t* nbr, long long pitch, float* scratch,
-              int n_rows, const int* n_dev, int K, int* err, cudaStream_t stream, int* tile_counter) {
+              int n_rows, const int* n_dev, int K, int* err, cudaStream_t stream, int* tile_counter, int max_ctas) {
     if (n_rows == 0) return VC_OK;
     if (!tc2_ch_ok(cin) || !tc2_ch_ok(cout) || K < 1 || K > MAXK_TC) {
         set_error("tensor-core wgrad: unsupported shape (%d -> %d channels, K=%d)", cin, cout, K);
@@ -418,7 +396,7 @@ int tc3_wgrad(int cin, int cout, const void* in_bf16, const void* dout_bf16, con
     a.groups_per_pass = 0; a.err = err;
     const int ci = tc_pad16(cin), co = tc_pad16(cout);
 #define VC_W_CASE(A, B) \
-    if (ci == A && co == B) return launch_wgrad3<A, B>(a, n_rows, stream);
+    if (ci == A && co == B) return launch_wgrad3<A, B>(a, n_rows, max_ctas, stream);
     VC_W_CASE(16, 16) VC_W_CASE(16, 32) VC_W_CASE(16, 64)
     VC_W_CASE(32, 16) VC_W_CASE(32, 32) VC_W_CASE(32, 64)
     VC_W_CASE(64, 16) VC_W_CASE(64, 32) VC_W_CASE(64, 64)
@@ -433,12 +411,80 @@ int wgrad3_passes(int cin, int cout, int K) {
     return (n_groups + max_groups - 1) / max_groups;
 }
 
+// scratch [K][cin][cout] (one per layer) -> parameter layout dW [cout][K][cin], every layer of a step in ONE launch
+__global__ void __launch_bounds__(256) wgrad_finalize_kernel(WgradFinTable t) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= t.total) return;
+    int lo = 0, hi = t.n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (t.e[mid].first <= i) lo = mid; else hi = mid - 1;
+    }
+    const WgradFinEntry& e = t.e[lo];
+    const int j = i - e.first;                       // index in the parameter layout: coalesced writes
+    const int ci = j % e.cin, k = (j / e.cin) % e.K, co = j / (e.cin * e.K);
+    e.dw[j] = __ldg(e.scratch + ((size_t)k * e.cin + ci) * e.cout + co);
+}
+
+int wgrad_finalize(WgradFinTable& t, cudaStream_t stream) {
+    if (t.n == 0) return VC_OK;
+    int total = 0;
+    for (int i = 0; i < t.n; ++i) {
+        t.e[i].first = total;
+        total += t.e[i].K * t.e[i].cin * t.e[i].cout;
+    }
+    t.total = total;
+    wgrad_finalize_kernel<<<cdiv(total, 256), 256, 0, stream>>>(t);
+    VC_LAUNCH_CHECK();
+    return VC_OK;
+}
+
 }  // namespace vc
 
+using namespace vc;
+
 extern "C" int vc_conv_wgrad_tc3_config(int variant, int max_ctas) {
-    VC_CHECK_ARG(variant == 0 || variant == 1, "wgrad variant must be 0 (one CTA per SM, 32 KB stages) or 1 (half-tile stages, <= 111 KB)");
+    VC_CHECK_ARG(variant == 1, "wgrad variant must be 1 (the half-tile-stage kernel is the only one)");
     VC_CHECK_ARG(max_ctas >= 0 && max_ctas <= 1024, "wgrad CTA cap out of range (%d)", max_ctas);
-    vc::g_wgrad_variant = variant;
-    vc::g_wgrad3_ctas = max_ctas;
+    g_wgrad3_ctas = max_ctas;
     return VC_OK;
+}
+
+extern "C" size_t vc_conv_wgrad_tc_ws_bytes(int n_out, int cin, int cout, int K) {
+    // the scratch image all CTAs accumulate into (whatever n_out), then one tile counter per pass
+    const size_t passes = tc2_ch_ok(cin) && tc2_ch_ok(cout) && K >= 1 ? (size_t)wgrad3_passes(cin, cout, K) : 0;
+    const size_t bytes = (size_t)K * cin * cout * sizeof(float) + passes * sizeof(int);
+    return (bytes + 255) & ~(size_t)255;
+}
+
+extern "C" int vc_conv_wgrad_tc(const void* in_bf16, const void* dout_bf16, const int32_t* nbr, float* dw, int n_out,
+                                int cin, int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag,
+                                vc_stream_t stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    VC_CHECK_ARG(n_out >= 0 && K >= 1 && K <= MAXK_TC && dw, "bad arguments");
+    if (!tc2_ch_ok(cin) || !tc2_ch_ok(cout)) {
+        set_error("tensor-core wgrad: unsupported channels cin=%d cout=%d", cin, cout);
+        return VC_ERR_UNSUPPORTED;
+    }
+    if (n_out == 0) {
+        VC_CUDA(cudaMemsetAsync(dw, 0, (size_t)K * cin * cout * 4, stream));
+        return VC_OK;
+    }
+    VC_CHECK_ARG(in_bf16 && dout_bf16 && nbr && ws, "null pointer");
+    const size_t need = vc_conv_wgrad_tc_ws_bytes(n_out, cin, cout, K);
+    if (ws_bytes < need) {
+        set_error("tensor-core wgrad workspace %zu < %zu", ws_bytes, need);
+        return VC_ERR_WORKSPACE;
+    }
+    // accumulate into a zeroed scratch image, then one transposing pass
+    const size_t wbytes = (size_t)K * cin * cout * sizeof(float);
+    VC_CUDA(cudaMemsetAsync(ws, 0, need, stream));
+    // alone on its stream the kernel measured fastest with one CTA per SM (DESIGN.md section 4)
+    int rc = tc3_wgrad(cin, cout, in_bf16, dout_bf16, nbr, n_out, (float*)ws, n_out, nullptr, K, err_flag, stream,
+                       reinterpret_cast<int*>((char*)ws + wbytes), num_sms());
+    if (rc) return rc;
+    WgradFinTable T;
+    T.n = 1;
+    T.e[0].scratch = (const float*)ws; T.e[0].dw = dw; T.e[0].cin = cin; T.e[0].cout = cout; T.e[0].K = K; T.e[0].first = 0;
+    return wgrad_finalize(T, stream);
 }

@@ -21,25 +21,18 @@ from ._lib import check
 ENABLED = os.environ.get('VIRCONV_EXECUTOR', '1') != '0'
 TWO_STREAMS = os.environ.get('VIRCONV_EXEC_STREAMS', '3') != '1'
 THREE_STREAMS = os.environ.get('VIRCONV_EXEC_STREAMS', '3') == '3'
-# weight gradients on their own stream next to the BN-backward / dgrad chain (vc_exec_backward's wgrad_stream), with the
-# wgrad CTAs limited to WGRAD_CTAS SMs they keep to themselves (vc_conv_wgrad_tc_config)
-# (the shared-memory floor that keeps gather CTAs off the wgrad SMs is off by default)
+# weight gradients on their own stream next to the BN-backward / dgrad chain (vc_exec_backward's wgrad_stream)
 WGRAD_STREAM = os.environ.get('VIRCONV_WGRAD_STREAM', '1') != '0'
-WGRAD_CTAS = int(os.environ.get('VIRCONV_WGRAD_CTAS', '128'))     # (round-1 wgrad kernel only; not re-measured on H100)
-WGRAD_SMEM_KB = int(os.environ.get('VIRCONV_WGRAD_SMEM_KB', '0'))
 _WSTREAM = {}
-_WCFG = [None]
 
 
 def _wgrad_stream(device):
+    if not WGRAD_STREAM:
+        return None
     key = (device.type, device.index)
     if key not in _WSTREAM:
         _WSTREAM[key] = torch.cuda.Stream(device=device)
-    cfg = (WGRAD_CTAS, WGRAD_SMEM_KB * 1024) if WGRAD_STREAM else (0, 0)      # 0: one CTA per SM
-    if _WCFG[0] != cfg:
-        check(_lib.load().vc_conv_wgrad_tc_config(*cfg), 'vc_conv_wgrad_tc_config')
-        _WCFG[0] = cfg
-    return _WSTREAM[key] if WGRAD_STREAM else None
+    return _WSTREAM[key]
 
 
 TIMING = False                     # bench.py's roofline pass: per-launch events around the conv kernels

@@ -198,13 +198,13 @@ def tc_error_flag(device):
 
 
 def tc_supported(cin, cout):
-    """Channel pairs of the tensor-core wgrad / scatter-dgrad kernels."""
+    """Channel pairs of the tensor-core scatter-dgrad kernel (`tc_scatter_ch_ok`, csrc/common.cuh)."""
     return cin in (16, 32, 64) and cout in (16, 32, 64)
 
 
 def tc_conv_supported(cin, cout):
-    """Channel pairs of the tensor-core conv forward / gather-dgrad kernel (persistent kernel, csrc/conv_tc2.cu): the
-    C = 8 layers run with K and N padded to 16 (zero-filled by the gather / the weight image)."""
+    """Channel pairs of the tensor-core conv forward / gather-dgrad / wgrad kernels (csrc/conv_tc2.cu, csrc/wgrad_tc3.cu):
+    the C = 8 layers run with K and N padded to 16 (zero-filled by the gather / the weight image)."""
     return cin in (8, 16, 32, 64) and cout in (8, 16, 32, 64)
 
 
