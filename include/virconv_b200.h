@@ -403,6 +403,52 @@ int vc_roi_targets(const float* rois, const float* roi_scores, const int64_t* ro
                    int32_t* status, void* ws, size_t ws_bytes, vc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Training losses of the detector heads with their gradients, whose rules csrc/head_losses.cu states.  No host read;
+ * graph-capturable; losses and gradients are bit-identical run to run (fixed-order float64 sums, no float atomics).
+ *   vc_rpn_loss  <- AnchorHeadTemplate.get_loss (anchor_head_template.py:178-333; OD_LOSS off, WeightedSmoothL1Loss,
+ *                   one head, 7 codes): cls_preds [B, N, n_cls], box_preds [B, N, 7], dir_cls_preds [B, N, n_bins] or
+ *                   NULL (no direction term), labels [B, N] int32, reg_targets [B, N, 7], anchors [N, 7] (shared by all
+ *                   scenes; read only for the direction target), all fp32 contiguous; alpha / gamma of the focal loss,
+ *                   beta of the smooth-L1, code_weights HOST [7], the cls / loc / dir loss weights, DIR_OFFSET ->
+ *                   losses [4] fp32 = (cls, loc, dir, total) as the reference's tb values; g_cls / g_box / g_dir = d total
+ *                   / d each prediction (shapes of the inputs), every element written.  ws >= vc_rpn_loss_ws_bytes(B, N).
+ *                   A memset and two launches.
+ *   vc_rcnn_loss <- RoIHeadTemplate.get_loss (roi_head_template.py:161-291; CLS_LOSS BinaryCrossEntropy, REG_LOSS
+ *                   smooth-l1): K <= VC_RCNN_MAX_BRANCHES branches from a HOST table, each n rows of rcnn_cls [n, 1],
+ *                   rcnn_reg [n, 7], its targets rois [n, ldr], gt_of_rois (canonical) / gt_of_rois_src [n, ldg],
+ *                   reg_valid_mask int64 [n], rcnn_cls_labels fp32 [n], and a weight; several branches may share one
+ *                   target set.  corner != 0: CORNER_LOSS_REGULARIZATION.  -> losses [K * 4 + 1] fp32 = per branch
+ *                   (cls, reg, corner, bb), then the weighted total (the reference's rcnn_loss); g_cls [n] / g_reg [n, 7]
+ *                   per branch = d total / d rcnn_cls / rcnn_reg, every element written.  The table is copied into the
+ *                   launch's parameters: no host-to-device copy.  ws >= vc_rcnn_loss_ws_bytes(K).  A memset and one
+ *                   launch (one CTA per branch).
+ * ---------------------------------------------------------------------------------------------- */
+#define VC_RCNN_MAX_BRANCHES 18
+typedef struct vc_rcnn_branch {
+    const float* rcnn_cls;
+    const float* rcnn_reg;
+    const float* rois;
+    const float* gt_of_rois;
+    const float* gt_of_rois_src;
+    const int64_t* reg_valid_mask;
+    const float* rcnn_cls_labels;
+    float* g_cls;
+    float* g_reg;
+    int n, ldr, ldg;
+    float weight;
+} vc_rcnn_branch;
+size_t vc_rpn_loss_ws_bytes(int B, int N);
+int vc_rpn_loss(const float* cls_preds, const float* box_preds, const float* dir_cls_preds, const int32_t* labels,
+                const float* reg_targets, const float* anchors, int B, int N, int n_cls, int n_bins, double alpha,
+                double gamma, double beta, const double* code_weights /*host[7]*/, double cls_weight, double loc_weight,
+                double dir_weight, double dir_offset, float* losses, float* g_cls, float* g_box, float* g_dir, void* ws,
+                size_t ws_bytes, vc_stream_t stream);
+size_t vc_rcnn_loss_ws_bytes(int K);
+int vc_rcnn_loss(const vc_rcnn_branch* branches /*host[K]*/, int K, double beta, const double* code_weights /*host[7]*/,
+                 double cls_weight, double reg_weight, double corner_weight, int corner, float* losses, void* ws,
+                 size_t ws_bytes, vc_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Plan executor: a whole backbone forward / backward in ONE call.  Replaces the Python layer loop of
  * `VirConvL8x.forward` (spconv_backbone.py:609-699), `NRConvBlock.forward` (:207-229) and the two streams of
  * `VirConv8x.forward` (:339-535) together with autograd's reverse walk over them: the host side of ~100 operator

@@ -85,6 +85,11 @@ SIGNATURES = {
     'vc_roi_targets_ws_bytes': (_Z, [_I, _I, _I]),
     'vc_roi_targets': (_I, [_P, _P, _P, _I, _I, _I, _P, _I, _I, _I, _HOSTD, _HOSTD, _HOSTD, _D, _HOSTD, _HOSTD, _I, _I, _I,
                             _D, _P, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _Z, _P]),
+    'vc_rpn_loss_ws_bytes': (_Z, [_I, _I]),
+    'vc_rpn_loss': (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _D, _D, _D, _HOSTD, _D, _D, _D, _D, _P, _P, _P, _P, _P, _Z,
+                         _P]),
+    'vc_rcnn_loss_ws_bytes': (_Z, [_I]),
+    'vc_rcnn_loss': (_I, [_P, _I, _D, _HOSTD, _D, _D, _D, _I, _P, _P, _Z, _P]),
     'vc_exec_state_bytes': (_Z, []),
     'vc_exec_forward': (_I, [_P, _P, _I, _P, _P, _I, _P, _I, _P, _I, _HOST, _I, _P, _I, _I, _I, _P, _Z, _P, _P, _P, _Z, _P, _P, _I,
                              _P, _P, _P, _P]),

@@ -25,9 +25,12 @@ FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-line
 # kernels do (the equality tests of the target assignment compare those values)
 # roi_targets.cu: no contraction, so that the 3-D IoU it takes from box_geom.cuh is bit for bit vc_boxes_iou3d's and its
 # labels round as torch's elementwise kernels do
+# head_losses.cu: no contraction, so that each float64 operation of the losses and their gradients rounds once, as the
+# float64 restatement in oracle/head_losses.py does
 FILE_FLAGS = {'iou3d_nms.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
               'anchor_targets.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
-              'roi_targets.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off']}
+              'roi_targets.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
+              'head_losses.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off']}
 
 
 def flags_for(src):

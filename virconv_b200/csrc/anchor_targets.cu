@@ -47,6 +47,7 @@
 // bit those of pass 1, and writes every output.  Both passes trim and classify the GT rows themselves (rule 1).
 #include <math.h>
 
+#include "box_coder.cuh"
 #include "common.cuh"
 
 namespace vc {
@@ -156,20 +157,6 @@ __global__ void __launch_bounds__(AT_THREADS) at_colmax_kernel(AtParams p) {
     }
 }
 
-// ResidualCoder.encode_torch (rule 4)
-__device__ __forceinline__ void encode(const float* __restrict__ g, const float* __restrict__ a, float* t) {
-    const float dxa = fmaxf(a[3], 1e-5f), dya = fmaxf(a[4], 1e-5f), dza = fmaxf(a[5], 1e-5f);
-    const float dxg = fmaxf(g[3], 1e-5f), dyg = fmaxf(g[4], 1e-5f), dzg = fmaxf(g[5], 1e-5f);
-    const float diag = sqrtf(dxa * dxa + dya * dya);
-    t[0] = (g[0] - a[0]) / diag;
-    t[1] = (g[1] - a[1]) / diag;
-    t[2] = (g[2] - a[2]) / dza;
-    t[3] = logf(dxg / dxa);
-    t[4] = logf(dyg / dya);
-    t[5] = logf(dzg / dza);
-    t[6] = g[6] - a[6];
-}
-
 __global__ void __launch_bounds__(AT_THREADS) at_assign_kernel(AtParams p) {
     __shared__ SceneGt s;
     const int b = blockIdx.y;
@@ -201,7 +188,7 @@ __global__ void __launch_bounds__(AT_THREADS) at_assign_kernel(AtParams p) {
         const int cls = s.cls[arg];
         label = forced ? cls : best < p.unmatched[set] ? 0 : best >= p.matched[set] ? cls : -1;
         gi = best;
-        if (label > 0) encode(p.gt + ((size_t)b * p.M + arg) * p.ld, anc, t);
+        if (label > 0) residual_encode(p.gt + ((size_t)b * p.M + arg) * p.ld, anc, t);   // rule 4
     }
     p.labels[o] = label;
     p.gt_ious[o] = gi;

@@ -30,6 +30,9 @@ device versions (virconv_b200.anchor_targets): the RPN's anchor mask and target 
 With `use_fused_roi_targets` the `ProposalTargetLayer` the RoI heads build (looked up in roi_head_template, which imports
 the name at module level, and in its own module) and `RoIHeadTemplate.assign_targets` are this package's device versions
 (virconv_b200.roi_targets): the RCNN's RoI sampling, labels and canonical transform in one call without a host read.
+With `use_fused_losses` `AnchorHeadTemplate.get_loss` and `RoIHeadTemplate.get_loss` are this package's drop-in methods
+(virconv_b200.head_losses): the RPN and RCNN training losses and their gradients in one kernel call each, without a host
+read apart from the one copy of the tb values.
 """
 from __future__ import annotations
 
@@ -220,7 +223,7 @@ def _points_in_boxes_cpu(boxes, points, point_indices):
 
 
 def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=False, use_fused_rpn_targets=False,
-            use_fused_roi_targets=False):
+            use_fused_roi_targets=False, use_fused_losses=False):
     """Register everything listed in the module docstring.  `reference_root`: put that checkout first on sys.path."""
     if reference_root is not None and reference_root not in sys.path:
         sys.path.insert(0, reference_root)
@@ -305,4 +308,10 @@ def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=F
         if rht.assign_targets is not roi_targets.assign_targets:
             roi_targets._reference_assign_targets = rht.assign_targets
         rht.assign_targets = roi_targets.assign_targets
+    if use_fused_losses:
+        from . import head_losses
+        aht = importlib.import_module('pcdet.models.dense_heads.anchor_head_template').AnchorHeadTemplate
+        aht.get_loss = head_losses.anchor_head_get_loss
+        rht = importlib.import_module('pcdet.models.roi_heads.roi_head_template').RoIHeadTemplate
+        rht.get_loss = head_losses.roi_head_get_loss
     return True
