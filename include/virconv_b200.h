@@ -251,6 +251,15 @@ int vc_dense_bwd_f32(const float* dout, const int32_t* indices, int n, int c, in
 int vc_cat2_f32(const float* a, const float* b, float* out, void* out_bf16 /*may be NULL*/, int n, int ca, int cb,
                 vc_stream_t stream);
 
+/* Mean over the valid rows of a [cap_rows, c] fp32 matrix (c % 4 == 0): n_dev (device int32[1], may be NULL: all cap_rows
+ * rows) is the row count.  Deterministic: float64 partials added in a fixed order that depends on (cap_rows, c) only.
+ * ws >= vc_masked_mean_ws_bytes().  The backward writes the whole [cap_rows, c] gradient: g / (n*c) on the first n rows,
+ * zeros on the rest (g: device float32[1]). */
+size_t vc_masked_mean_ws_bytes(void);
+int vc_masked_mean_f32(const float* x, long long cap_rows, int c, const int32_t* n_dev, float* out /*device [1]*/, void* ws,
+                       size_t ws_bytes, vc_stream_t stream);
+int vc_masked_mean_bwd_f32(const float* g, long long cap_rows, int c, const int32_t* n_dev, float* dx, vc_stream_t stream);
+
 /* Row gather for StVD layer discard (spconv_backbone.py:134-147): out[r] = in[rows[r]]. */
 int vc_gather_rows(const void* in, const int32_t* rows, void* out, int n_rows, int row_bytes, vc_stream_t stream);
 

@@ -60,6 +60,9 @@ SIGNATURES = {
     'vc_voxelize_mean': (_I, [_P, _I, _I, _I, _HOSTF, _HOSTF, _I, _I, _I, _P, _P, _P, _P, _P, _P, _Z, _P]),
     'vc_voxel2pinds': (_I, [_P, _I, _I, _I, _HOST, _P, _P]),
     'vc_cat2_f32': (_I, [_P, _P, _P, _P, _I, _I, _I, _P]),
+    'vc_masked_mean_ws_bytes': (_Z, []),
+    'vc_masked_mean_f32': (_I, [_P, ctypes.c_longlong, _I, _P, _P, _P, _Z, _P]),
+    'vc_masked_mean_bwd_f32': (_I, [_P, ctypes.c_longlong, _I, _P, _P, _P]),
     'vc_gather_rows': (_I, [_P, _P, _P, _I, _I, _P]),
     'vc_stvd_ws_bytes': (_Z, [_I]),
     'vc_stvd_partition': (_I, [_P, _I, _I, _I, ctypes.c_double, _P, _P, _Z, _P]),

@@ -174,19 +174,24 @@ int tc_prep_images(TcPrepTable& t, cudaStream_t stream);
 // ---- conv_tc.cu (tensor-core scatter dgrad of many-to-one tables) ----
 static inline bool tc_scatter_ch_ok(int c) { return c == 16 || c == 32 || c == 64; }
 int tc_scatter_with_image(int kc, int nr, const void* dout_bf16, const void* wimg, const int32_t* nbr, float* din, int n_out,
-                          int K, int* err, cudaStream_t stream);
+                          int K, int* err, cudaStream_t stream, int din_ld = 0);   // din_ld: row pitch of din (0: nr)
+// fp32 scatter dgrad (vc_conv_dgrad_scatter_f32) into a din of row pitch din_ld (>= cin, multiple of 4)
+int conv_dgrad_scatter_f32_ld(const float* dout, const float* w, const int32_t* nbr, float* din, int din_ld, int n_out, int cin,
+                              int cout, int K, void* ws, size_t ws_bytes, cudaStream_t stream);
 // ---- conv_tc2.cu (persistent tensor-core conv: forward and gather dgrad) ----
 int num_sms();   // of the current device
 size_t tc_image_bytes(int cin, int cout, int K, int layout);
 bool tc2_ch_ok(int c);
 int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_t* nbr, long long pitch, float* out, int n_rows,
              const int* n_dev, int K, double* bn_sums, int* err, cudaStream_t stream, const float* addend,
-             int* tile_counter = nullptr, int flags = 0);   // flags: bit 0 sparse offsets (strided dgrad), bit 1 early tables
+             int* tile_counter = nullptr, int flags = 0,   // flags: bit 0 sparse offsets (strided dgrad), bit 1 early tables
+             int in_ld = 0);                               // row pitch of in_bf16 (0: kc)
 
 // ---- wgrad_tc3.cu (persistent tensor-core wgrad) ----
 extern int g_wgrad3_ctas;
 int tc3_wgrad(int cin, int cout, const void* in_bf16, const void* dout_bf16, const int32_t* nbr, long long pitch, float* scratch,
-              int n_rows, const int* n_dev, int K, int* err, cudaStream_t stream, int* tile_counter, int max_ctas);
+              int n_rows, const int* n_dev, int K, int* err, cudaStream_t stream, int* tile_counter, int max_ctas,
+              int in_ld = 0);   // row pitch of in_bf16 (0: cin)
 int wgrad3_passes(int cin, int cout, int K);
 struct WgradFinEntry {
     const float* scratch;   // [K][cin][cout] accumulated by tc3_wgrad

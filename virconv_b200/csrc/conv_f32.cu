@@ -212,11 +212,11 @@ gather_gemm_kernel(const float* __restrict__ in, const float* __restrict__ wt, c
     }
 }
 
-// din[nbr[k,o], :] += dout[o, :] @ wt[k]     (many-to-one tables: float atomics)
+// din[nbr[k,o], :] += dout[o, :] @ wt[k]     (many-to-one tables: float atomics; din row pitch out_ld)
 template <int CI, int CO>
 __global__ void __launch_bounds__(NTHREADS, 2)
 scatter_gemm_kernel(const float* __restrict__ in, const float* __restrict__ wt, const int32_t* __restrict__ nbr,
-                    float* __restrict__ out, int n_rows, int K) {
+                    float* __restrict__ out, int out_ld, int n_rows, int K) {
     using C = Cfg<CI, CO>;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float* As = reinterpret_cast<float*>(smem_raw);         // [TM][AS]  rows of `in` (contiguous tile)
@@ -261,7 +261,7 @@ scatter_gemm_kernel(const float* __restrict__ in, const float* __restrict__ wt, 
         for (int r = 0; r < C::RT; ++r) {
             int dst = nbr_s[k * TM + row0 + r];
             if (dst >= 0) {
-                float* p = out + (size_t)dst * CO + tx * 4;
+                float* p = out + (size_t)dst * out_ld + tx * 4;
                 // one 16-byte vector reduction (sm_90+) instead of four scalar atomics: a quarter of the L2 atomic operations
                 asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(acc[r][0]), "f"(acc[r][1]),
                              "f"(acc[r][2]), "f"(acc[r][3])
@@ -401,12 +401,12 @@ static int launch_gather(const float* in, const float* wt, const int32_t* nbr, f
     return VC_OK;
 }
 template <int CI, int CO>
-static int launch_scatter(const float* in, const float* wt, const int32_t* nbr, float* out, int n_rows, int K,
+static int launch_scatter(const float* in, const float* wt, const int32_t* nbr, float* out, int out_ld, int n_rows, int K,
                           cudaStream_t stream) {
     size_t smem = Cfg<CI, CO>::smem_scatter(K);
     auto kern = scatter_gemm_kernel<CI, CO>;
     VC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    VC_LAUNCH_CHAIN(kern, dim3(cdiv(n_rows, TM)), dim3(NTHREADS), smem, stream, in, wt, nbr, out, n_rows, K);
+    VC_LAUNCH_CHAIN(kern, dim3(cdiv(n_rows, TM)), dim3(NTHREADS), smem, stream, in, wt, nbr, out, out_ld, n_rows, K);
     return VC_OK;
 }
 template <int CI, int CO>
@@ -502,16 +502,21 @@ extern "C" int vc_conv_dgrad_f32(const float* dout, const float* w, const int32_
     });
 }
 
-extern "C" int vc_conv_dgrad_scatter_f32(const float* dout, const float* w, const int32_t* nbr, float* din, int n_out,
-                                         int cin, int cout, int K, void* ws, size_t ws_bytes, vc_stream_t stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
+int vc::conv_dgrad_scatter_f32_ld(const float* dout, const float* w, const int32_t* nbr, float* din, int din_ld, int n_out,
+                                  int cin, int cout, int K, void* ws, size_t ws_bytes, cudaStream_t stream) {
     int rc = check_conv_args(n_out, cin, cout, K, dout, w, nbr, din, ws, ws_bytes);
     if (rc || n_out == 0) return rc;
+    VC_CHECK_ARG(din_ld >= cin && din_ld % 4 == 0, "scatter dgrad: row pitch %d for %d channels", din_ld, cin);
     float* wt = (float*)ws;
     if ((rc = prep(w, wt, cin, cout, K, 1, 0, stream))) return rc;
     return dispatch(cout, cin, [&](auto ci, auto co) {
-        return launch_scatter<decltype(ci)::value, decltype(co)::value>(dout, wt, nbr, din, n_out, K, stream);
+        return launch_scatter<decltype(ci)::value, decltype(co)::value>(dout, wt, nbr, din, din_ld, n_out, K, stream);
     });
+}
+
+extern "C" int vc_conv_dgrad_scatter_f32(const float* dout, const float* w, const int32_t* nbr, float* din, int n_out,
+                                         int cin, int cout, int K, void* ws, size_t ws_bytes, vc_stream_t stream_) {
+    return vc::conv_dgrad_scatter_f32_ld(dout, w, nbr, din, cin, n_out, cin, cout, K, ws, ws_bytes, (cudaStream_t)stream_);
 }
 
 extern "C" size_t vc_conv_wgrad_ws_bytes(int n_out, int cin, int cout, int K) {

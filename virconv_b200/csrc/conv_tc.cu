@@ -47,7 +47,7 @@ struct TcCfg {
 template <int KC, int NR>
 __global__ void __launch_bounds__(128)
 tc_scatter_kernel(const __nv_bfloat16* __restrict__ dout, const __nv_bfloat16* __restrict__ wimg,
-                  const int32_t* __restrict__ nbr, float* __restrict__ din, int n_out, int K, int* __restrict__ err) {
+                  const int32_t* __restrict__ nbr, float* __restrict__ din, int din_ld, int n_out, int K, int* __restrict__ err) {
     using C = TcCfg<KC, NR>;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char* A = smem_raw;                               // [128 x KC] bf16, GMMA K-major core-matrix image
@@ -103,7 +103,7 @@ tc_scatter_kernel(const __nv_bfloat16* __restrict__ dout, const __nv_bfloat16* _
 #pragma unroll
             for (int j = 0; j < NR / 2; j += 2) {
                 const int dst = nbr_s[k * TCM + 64 * h + wg_row(j, tid)];
-                if (dst >= 0) red_add_v2(din + (size_t)dst * NR + wg_col(j, tid), acc[h][j], acc[h][j + 1]);
+                if (dst >= 0) red_add_v2(din + (size_t)dst * din_ld + wg_col(j, tid), acc[h][j], acc[h][j + 1]);
             }
         }
     }
@@ -111,24 +111,29 @@ tc_scatter_kernel(const __nv_bfloat16* __restrict__ dout, const __nv_bfloat16* _
 }
 
 template <int KC, int NR>
-static int launch_tc_scatter(const __nv_bfloat16* dout, const __nv_bfloat16* wimg, const int32_t* nbr, float* din, int n_out,
-                             int K, int* err, cudaStream_t stream) {
+static int launch_tc_scatter(const __nv_bfloat16* dout, const __nv_bfloat16* wimg, const int32_t* nbr, float* din, int din_ld,
+                             int n_out, int K, int* err, cudaStream_t stream) {
     size_t smem = (size_t)TcCfg<KC, NR>::A_BYTES + (size_t)K * TcCfg<KC, NR>::B_BYTES + (size_t)K * TCM * 4;
     auto kern = tc_scatter_kernel<KC, NR>;
     VC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<cdiv(n_out, TCM), 128, smem, stream>>>(dout, wimg, nbr, din, n_out, K, err);
+    kern<<<cdiv(n_out, TCM), 128, smem, stream>>>(dout, wimg, nbr, din, din_ld, n_out, K, err);
     VC_LAUNCH_CHECK();
     return VC_OK;
 }
 
 // kc = C_out (reduction), nr = C_in (gradient channels); wimg = the K dgrad images (prep mode 1, layout 0, no mirror)
 int tc_scatter_with_image(int kc, int nr, const void* dout_bf16, const void* wimg, const int32_t* nbr, float* din, int n_out,
-                          int K, int* err, cudaStream_t stream) {
+                          int K, int* err, cudaStream_t stream, int din_ld) {
     if (n_out == 0) return VC_OK;
+    if (din_ld == 0) din_ld = nr;
+    if (din_ld < nr || din_ld % 2 != 0) {
+        set_error("tensor-core scatter dgrad: row pitch %d for %d channels", din_ld, nr);
+        return VC_ERR_INVALID;
+    }
     const __nv_bfloat16* a = (const __nv_bfloat16*)dout_bf16;
     const __nv_bfloat16* b = (const __nv_bfloat16*)wimg;
 #define VC_TS_CASE(A, B) \
-    if (kc == A && nr == B) return launch_tc_scatter<A, B>(a, b, nbr, din, n_out, K, err, stream);
+    if (kc == A && nr == B) return launch_tc_scatter<A, B>(a, b, nbr, din, din_ld, n_out, K, err, stream);
     VC_TS_CASE(16, 16) VC_TS_CASE(16, 32) VC_TS_CASE(16, 64)
     VC_TS_CASE(32, 16) VC_TS_CASE(32, 32) VC_TS_CASE(32, 64)
     VC_TS_CASE(64, 16) VC_TS_CASE(64, 32) VC_TS_CASE(64, 64)

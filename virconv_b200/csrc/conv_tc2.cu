@@ -69,8 +69,9 @@ struct PCfg {
 };
 
 struct PArgs {
-    const __nv_bfloat16* in;   // gathered operand rows, row pitch in_c elements
+    const __nv_bfloat16* in;   // gathered operand rows, row pitch in_ld elements
     int in_c;                  // real channels of a row (8 or KC)
+    int in_ld;                 // row pitch (>= in_c: the rows may be a column slice of a wider matrix)
     const unsigned char* wimg; // K swizzled [NR][KC] images
     const int32_t* nbr;        // [K][pitch]
     long long pitch;
@@ -354,7 +355,7 @@ __global__ void __launch_bounds__(P_THREADS, P_GROUPS == 1 ? 2 : 1) tc_conv_pers
 #pragma unroll
                             for (int i = 0; i < NIT; ++i) {
                                 const bool v = src[g][i] >= 0;
-                                const __nv_bfloat16* srow = a.in + (size_t)(v ? src[g][i] : 0) * a.in_c + c_sub * 8;
+                                const __nv_bfloat16* srow = a.in + (size_t)(v ? src[g][i] : 0) * a.in_ld + c_sub * 8;
 #pragma unroll
                                 for (int cg = 0; cg < NCG; ++cg) {
                                     // a missing neighbour costs a shared-memory zero store, not a zero-fill cp.async
@@ -683,14 +684,19 @@ bool tc2_ch_ok(int c) { return c == 8 || c == 16 || c == 32 || c == 64; }
 // (layout 1).  n_dev (optional) overrides n_rows on the device; n_rows is then the capacity the grid is sized for.
 int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_t* nbr, long long pitch, float* out,
              int n_rows, const int* n_dev, int K, double* bn_sums, int* err, cudaStream_t stream, const float* addend,
-             int* tile_counter, int flags) {
+             int* tile_counter, int flags, int in_ld) {
     if (n_rows == 0) return VC_OK;
     if (!tc2_ch_ok(kc) || !tc2_ch_ok(nr) || K < 1 || K > MAXK_TC) {
         set_error("tensor-core conv: unsupported shape (%d -> %d channels, K=%d)", kc, nr, K);
         return VC_ERR_UNSUPPORTED;
     }
     PArgs a;
-    a.in = (const __nv_bfloat16*)in_bf16; a.in_c = kc; a.wimg = (const unsigned char*)wimg; a.nbr = nbr; a.pitch = pitch;
+    if (in_ld == 0) in_ld = kc;
+    if (in_ld < kc || in_ld % 8 != 0) {
+        set_error("tensor-core conv: row pitch %d for %d channels", in_ld, kc);
+        return VC_ERR_INVALID;
+    }
+    a.in = (const __nv_bfloat16*)in_bf16; a.in_c = kc; a.in_ld = in_ld; a.wimg = (const unsigned char*)wimg; a.nbr = nbr; a.pitch = pitch;
     a.out = out; a.out_c = nr; a.addend = addend; a.bn_sums = bn_sums; a.n_dev = n_dev; a.n_host = n_rows; a.tile_counter = tile_counter;
     a.K = K; a.S = 0; a.w_resident = 0; a.ntb_alloc = P_NTB; a.scan_k = flags & 1; a.early_tables = (flags >> 1) & 1;
     a.err = err;

@@ -43,11 +43,13 @@ struct ISet {
     int prod;
 };
 struct FSlot {
-    float* f32;
+    float* f32;            // NULL where no reader needs fp32 (the bf16 kernels read the shadow)
     void* bf16;
-    float* grad;
+    float* grad;           // [rows, c], row pitch gld
     const int* n_dev;      // static mode (see ISet)
-    int rows, c, grad_state, ev, prod;
+    int rows, c, ld;       // ld: row pitch of f32 / bf16 (> c: a column slice of an in-place concat)
+    int gld;               // row pitch of grad (> c: a column slice of the concat's gradient; only scatter dgrads and BN read it)
+    int grad_state, ev, prod;
 };
 struct RBk {
     int32_t *nbr, *nbr_bwd, *pair_num;
@@ -366,7 +368,7 @@ extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_o
 
     S->iset[0].idx = const_cast<int32_t*>(idx0); S->iset[0].n = n0; S->iset[0].ndim = 3; S->iset[0].n_dev = n0_dev;
     for (int d = 0; d < 3; ++d) S->iset[0].shape[d] = shape0[d];
-    S->f[0].f32 = const_cast<float*>(feats0); S->f[0].rows = n0; S->f[0].c = c0; S->f[0].n_dev = n0_dev;
+    S->f[0].f32 = const_cast<float*>(feats0); S->f[0].rows = n0; S->f[0].c = c0; S->f[0].ld = c0; S->f[0].n_dev = n0_dev;
 
     // rulebook meta known from the plan alone (needed to choose the dgrad weight images)
     int rb_subm[MAX_RB] = {0}, rb_unique[MAX_RB] = {0}, rb_K[MAX_RB] = {0};
@@ -378,6 +380,42 @@ extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_o
             rb_K[o[F_C]] = K;
             rb_subm[o[F_C]] = o[F_KIND] == OP_SUBM_RB;
             rb_unique[o[F_C]] = o[F_KIND] == OP_CONV_RB ? 1 : o[F_X0];
+        }
+    }
+
+    // Which feature slots need an fp32 copy: published ones (x1 of the producing op), the input of a layer without the
+    // tensor-core forward + wgrad pair (fp32 conv or fp32 wgrad), and the fp32 precision mode.  Everything else is read as
+    // bf16 only, so its fp32 copy is not written.  A concat whose inputs need no fp32 copy of their own is built in place:
+    // the BN-apply of each input layer writes its column slice of the concat (fp32 if the concat needs it, and bf16), and
+    // the concat op launches nothing.
+    bool need_f32[MAX_F] = {false};
+    int slot_c[MAX_F] = {0}, cat_out[MAX_F], cat_col[MAX_F] = {0};
+    bool cat_inplace[MAX_OPS] = {false};
+    for (int i = 0; i < MAX_F; ++i) cat_out[i] = -1;
+    slot_c[0] = c0;
+    need_f32[0] = true;
+    for (int i = 0; i < n_ops; ++i) {
+        const int* o = C.op(i);
+        if (o[F_KIND] == OP_CBR) {
+            slot_c[o[F_B]] = o[F_COUT];
+            const bool tc = precision == 1 && tc2_ch_ok(o[F_CIN]) && tc2_ch_ok(o[F_COUT]);
+            if (precision == 0 || o[F_X1]) need_f32[o[F_B]] = true;
+            if (!(training && tc)) need_f32[o[F_A]] = true;
+        } else if (o[F_KIND] == OP_CAT) {
+            slot_c[o[F_C]] = slot_c[o[F_A]] + slot_c[o[F_B]];
+            if (precision == 0 || o[F_X1]) need_f32[o[F_C]] = true;
+        }
+    }
+    for (int i = 0; i < n_ops; ++i) {
+        const int* o = C.op(i);
+        if (o[F_KIND] != OP_CAT) continue;
+        const int a = o[F_A], b = o[F_B];
+        cat_inplace[i] = precision == 1 && a != 0 && b != 0 && a != b && !need_f32[a] && !need_f32[b] && cat_out[a] < 0 && cat_out[b] < 0;
+        if (cat_inplace[i]) {
+            cat_out[a] = cat_out[b] = o[F_C];
+            cat_col[b] = slot_c[a];
+        } else {
+            need_f32[a] = need_f32[b] = true;
         }
     }
 
@@ -602,23 +640,46 @@ extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_o
                 FSlot& X = S->f[L.in_slot];
                 FSlot& Y = S->f[L.out_slot];
                 RBk& R = S->rb[L.rb];
-                VC_CHECK_ARG(X.f32 && R.nbr && X.c == L.cin && X.rows == R.n_in, "op %d: input slot / rulebook mismatch (rows %d vs %d, c %d vs %d)",
-                             i, X.rows, R.n_in, X.c, L.cin);
+                VC_CHECK_ARG((X.f32 || X.bf16) && R.nbr && X.c == L.cin && X.rows == R.n_in,
+                             "op %d: input slot / rulebook mismatch (rows %d vs %d, c %d vs %d)", i, X.rows, R.n_in, X.c, L.cin);
                 VC_TRY(wait_for(C, R.ev, R.prod, s));
                 VC_TRY(wait_for(C, X.ev, X.prod, s));
                 const size_t elems = (size_t)R.n_out * L.cout;
                 VC_ALLOC(x, float*, elems * 4);
-                VC_ALLOC(y, float*, elems * 4);
                 VC_ALLOC(stats, float*, (size_t)4 * L.cout * 4);
+                float* y = nullptr;
                 void* yb = nullptr;
-                if (precision == 1) {
-                    VC_ALLOC(yb_, void*, elems * 2);
-                    yb = yb_;
+                int y_ld = L.cout;
+                if (cat_out[L.out_slot] >= 0) {   // a column slice of an in-place concat (allocated by its first input)
+                    FSlot& O = S->f[cat_out[L.out_slot]];
+                    if (O.bf16 == nullptr) {
+                        O.rows = R.n_out; O.c = O.ld = slot_c[cat_out[L.out_slot]];
+                        if (need_f32[cat_out[L.out_slot]]) {
+                            VC_ALLOC(of_, float*, (size_t)O.rows * O.c * 4);
+                            O.f32 = of_;
+                        }
+                        VC_ALLOC(ob_, void*, (size_t)O.rows * O.c * 2);
+                        O.bf16 = ob_;
+                    }
+                    VC_CHECK_ARG(O.rows == R.n_out, "op %d: concat inputs with different row counts", i);
+                    y_ld = O.ld;
+                    if (O.f32) y = O.f32 + cat_col[L.out_slot];
+                    yb = (__nv_bfloat16*)O.bf16 + cat_col[L.out_slot];
+                } else {
+                    if (need_f32[L.out_slot]) {
+                        VC_ALLOC(y_, float*, elems * 4);
+                        y = y_;
+                    }
+                    if (precision == 1) {
+                        VC_ALLOC(yb_, void*, elems * 2);
+                        yb = yb_;
+                    }
                 }
                 L.x = x; L.y = y; L.stats = stats;
                 double* sums = training ? L.sums : nullptr;
                 if (L.use_tc && R.n_out > 0) {
                     if (!X.bf16) {   // no producer wrote a shadow (network input): cast once
+                        VC_CHECK_ARG(X.ld == X.c, "op %d: no bf16 copy of a strided input", i);
                         VC_ALLOC(xb, void*, (size_t)X.rows * X.c * 2);
                         if (do_feat) VC_TRY(vc_cast_f32_bf16(X.f32, xb, (long long)X.rows * X.c, st));
                         X.bf16 = xb;
@@ -628,18 +689,19 @@ extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_o
                     //  table slices before its griddepcontrol.wait — conv_tc2.cu)
                     if (do_feat)
                         VC_TRY(tc2_conv(L.cin, L.cout, X.bf16, L.wimg_fwd, R.nbr, R.n_out, x, R.n_out, R.n_out_dev, R.K, sums, C.err, st,
-                                        nullptr, L.tile_ctr, (phase == 2 || C.st[R.prod] != C.st[s]) ? 2 : 0));
+                                        nullptr, L.tile_ctr, (phase == 2 || C.st[R.prod] != C.st[s]) ? 2 : 0, X.ld));
                 } else {
                     const size_t wsb = vc_conv_ws_bytes(L.cin, L.cout, R.K);
                     VC_ALLOC(ws, void*, wsb);
+                    VC_CHECK_ARG(X.f32 && X.ld == X.c, "op %d: the fp32 conv needs a dense fp32 input", i);
                     Timed t(0, li, st);
                     if (do_feat) VC_TRY(vc_conv_fwd_f32(X.f32, C.P<const float>(li, P_W), R.nbr, x, R.n_out, L.cin, L.cout, R.K, sums, ws, wsb, st));
                 }
                 if (do_feat)
                     VC_TRY(bn_apply_relu_dev(x, L.sums, R.n_out, R.n_out_dev, L.cout, C.P<const float>(li, P_GAMMA), C.P<const float>(li, P_BETA),
                                              C.P<float>(li, P_RM), C.P<float>(li, P_RV), C.P<long long>(li, P_NBT), C.lf[2 * li + 1],
-                                             C.lf[2 * li], training, y, L.cout, yb, L.cout, stats, 1, is_static, st));
-                Y.f32 = y; Y.bf16 = yb; Y.rows = R.n_out; Y.c = L.cout; Y.prod = s; Y.n_dev = R.n_out_dev;
+                                             C.lf[2 * li], training, y, y_ld, yb, y_ld, stats, 1, is_static, st));
+                Y.f32 = y; Y.bf16 = yb; Y.rows = R.n_out; Y.c = L.cout; Y.ld = y_ld; Y.prod = s; Y.n_dev = R.n_out_dev;
                 Y.ev = side_ev(s);
                 break;
             }
@@ -647,9 +709,16 @@ extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_o
                 FSlot& Aa = S->f[o[F_A]];
                 FSlot& Bb = S->f[o[F_B]];
                 FSlot& O = S->f[o[F_C]];
-                VC_CHECK_ARG(Aa.f32 && Bb.f32 && Aa.rows == Bb.rows, "op %d: concat inputs not built / row mismatch", i);
                 VC_TRY(wait_for(C, Aa.ev, Aa.prod, s));
                 VC_TRY(wait_for(C, Bb.ev, Bb.prod, s));
+                if (cat_inplace[i]) {   // both halves are already written (OP_CBR): nothing to launch
+                    VC_CHECK_ARG(Aa.bf16 && Bb.bf16 && Aa.rows == Bb.rows && O.bf16, "op %d: concat inputs not built / row mismatch", i);
+                    O.prod = s; O.n_dev = Aa.n_dev;
+                    O.ev = side_ev(s);
+                    break;
+                }
+                VC_CHECK_ARG(Aa.f32 && Bb.f32 && Aa.ld == Aa.c && Bb.ld == Bb.c && Aa.rows == Bb.rows,
+                             "op %d: concat inputs not built / row mismatch", i);
                 const size_t elems = (size_t)Aa.rows * (Aa.c + Bb.c);
                 VC_ALLOC(out, float*, elems * 4);
                 void* ob = nullptr;
@@ -658,7 +727,7 @@ extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_o
                     ob = ob_;
                 }
                 if (do_feat) VC_TRY(cat2_dev(Aa.f32, Bb.f32, out, ob, Aa.rows, Aa.n_dev, Aa.c, Bb.c, st));
-                O.f32 = out; O.bf16 = ob; O.rows = Aa.rows; O.c = Aa.c + Bb.c; O.prod = s; O.n_dev = Aa.n_dev;
+                O.f32 = out; O.bf16 = ob; O.rows = Aa.rows; O.c = O.ld = Aa.c + Bb.c; O.prod = s; O.n_dev = Aa.n_dev;
                 O.ev = side_ev(s);
                 break;
             }
@@ -678,6 +747,7 @@ namespace {
 template <class W>
 int contribute(Ctx& C, FSlot& F, cudaStream_t st, W&& write) {
     const size_t n = (size_t)F.rows * F.c;
+    VC_CHECK_ARG(F.gld == F.c, "a column slice of a gradient cannot take this contribution");
     if (F.grad_state == G_EMPTY) {
         VC_ALLOC(buf, float*, n * 4);
         VC_TRY(write(buf));
@@ -701,6 +771,7 @@ int contribute(Ctx& C, FSlot& F, cudaStream_t st, W&& write) {
 template <class W>
 int contribute_fused(Ctx& C, FSlot& F, W&& write) {
     const size_t n = (size_t)F.rows * F.c;
+    VC_CHECK_ARG(F.gld == F.c, "a column slice of a gradient cannot take this contribution");
     if (F.grad_state == G_OWN) {
         VC_TRY(write(F.grad, (const float*)F.grad));
     } else {
@@ -712,8 +783,9 @@ int contribute_fused(Ctx& C, FSlot& F, W&& write) {
     return VC_OK;
 }
 
-// contribution by a kernel that ACCUMULATES with atomics (the scatter dgrads): `scatter(dst)` adds into dst, which must
-// hold the sum so far — zeros, a copy of the outside gradient, or the slot's own buffer (then nothing is staged at all)
+// contribution by a kernel that ACCUMULATES with atomics (the scatter dgrads): `scatter(dst, ld)` adds into dst (row pitch
+// ld), which must hold the sum so far — zeros, a copy of the outside gradient, or the slot's own buffer (then nothing is
+// staged at all; it may be a column slice of the concat's gradient)
 template <class W>
 int contribute_scatter(Ctx& C, FSlot& F, cudaStream_t st, W&& scatter) {
     const size_t n = (size_t)F.rows * F.c;
@@ -724,9 +796,10 @@ int contribute_scatter(Ctx& C, FSlot& F, cudaStream_t st, W&& scatter) {
         else
             VC_CUDA(cudaMemsetAsync(buf, 0, n * 4, st));
         F.grad = buf;
+        F.gld = F.c;
         F.grad_state = G_OWN;
     }
-    return scatter(F.grad);
+    return scatter(F.grad, F.gld);
 }
 
 }  // namespace
@@ -759,7 +832,7 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
     // wgrad CTAs: half the SMs by default, so that a CTA of the dgrad chain fits beside each (DESIGN.md section 4)
     const int wgrad_ctas = g_wgrad3_ctas > 0 ? g_wgrad3_ctas : (num_sms() + 1) / 2;
 
-    for (int i = 0; i < MAX_F; ++i) { S->f[i].grad = nullptr; S->f[i].grad_state = G_EMPTY; }
+    for (int i = 0; i < MAX_F; ++i) { S->f[i].grad = nullptr; S->f[i].gld = S->f[i].c; S->f[i].grad_state = G_EMPTY; }
     for (int i = 0; i < n_pub; ++i) {
         VC_CHECK_ARG(pub_slots[i] > 0 && pub_slots[i] < MAX_F, "published slot id");
         if (ext_grads[i]) {
@@ -777,6 +850,15 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
             FSlot& Bb = S->f[o[F_B]];
             FSlot& O = S->f[o[F_C]];
             if (O.grad_state == G_EMPTY) continue;
+            VC_CHECK_ARG(O.gld == O.c, "op %d: the gradient of a concat is a slice itself", i);
+            if (S->precision == 1 && O.grad_state == G_OWN && Aa.grad_state == G_EMPTY && Bb.grad_state == G_EMPTY) {
+                // the inputs' gradients are the two column slices of the concat's own buffer: nothing is split or copied.
+                // Their readers take a row pitch: BN backward, and the scatter dgrad of the image branch, which adds into
+                // the first input's slice in place (nothing reads the concat's gradient after this op)
+                Aa.grad = O.grad; Aa.gld = O.c; Aa.grad_state = G_OWN;
+                Bb.grad = O.grad + Aa.c; Bb.gld = O.c; Bb.grad_state = G_OWN;
+                continue;
+            }
             float *da, *db;
             const float *a_add = nullptr, *b_add = nullptr;
             if (Aa.grad_state == G_OWN) { da = Aa.grad; a_add = Aa.grad; }
@@ -787,8 +869,8 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
                 VC_LAUNCH_CHAIN(cat2_bwd_kernel, dim3(ew_grid((size_t)O.rows * O.c / 4)), dim3(256), 0, st, (const float4*)O.grad,
                                 O.rows, Aa.c / 4, Bb.c / 4, (float4*)da, (const float4*)a_add, (float4*)db, (const float4*)b_add);
             }
-            Aa.grad = da; Aa.grad_state = G_OWN;
-            Bb.grad = db; Bb.grad_state = G_OWN;
+            Aa.grad = da; Aa.gld = Aa.c; Aa.grad_state = G_OWN;
+            Bb.grad = db; Bb.gld = Bb.c; Bb.grad_state = G_OWN;
             continue;
         }
         if (o[F_KIND] != OP_CBR) continue;
@@ -808,13 +890,20 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
             continue;
         }
         const size_t elems = (size_t)R.n_out * L.cout;
-        VC_ALLOC(dx, float*, elems * 4);
+        // the fp32 input gradient is read by the fp32 wgrad and the fp32 dgrads only (the tensor-core ones read dxb)
+        const bool dgrad = L.need_dgrad && L.in_slot != 0;
+        const bool tc_dgrad = L.wimg_dgrad && ((R.subm && !R.unique) ? L.use_tc_scatter : L.use_tc);
+        float* dx = nullptr;
+        if (L.wscratch == nullptr || (dgrad && !tc_dgrad)) {
+            VC_ALLOC(t, float*, elems * 4);
+            dx = t;
+        }
         void* dxb = nullptr;
         if (S->precision == 1) {
             VC_ALLOC(t, void*, elems * 2);
             dxb = t;
         }
-        VC_TRY(bn_relu_bwd_dev(Y.grad, L.cout, L.x, C.P<const float>(li, P_GAMMA), L.stats, dx, dxb, dgamma, dbeta, R.n_out, R.n_out_dev,
+        VC_TRY(bn_relu_bwd_dev(Y.grad, Y.gld, L.x, C.P<const float>(li, P_GAMMA), L.stats, dx, dxb, dgamma, dbeta, R.n_out, R.n_out_dev,
                                L.cout, training, L.sums + 2 * L.cout, S->is_static, st));
         // wgrad (needs dx / its bf16 shadow: ordered after the BN backward through an event when on its own stream)
         if (two) {
@@ -824,7 +913,7 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
         if (L.wscratch != nullptr) {
             Timed t(6, li, wst);
             VC_TRY(tc3_wgrad(L.cin, L.cout, X.bf16, dxb, R.nbr, R.n_out, L.wscratch, R.n_out, R.n_out_dev, R.K, C.err, wst,
-                             L.tile_ctr + 2, wgrad_ctas));
+                             L.tile_ctr + 2, wgrad_ctas, X.ld));
             if (fin.n == WGRAD_FIN_MAX) {
                 VC_TRY(wgrad_finalize(fin, wst));
                 fin.n = 0;
@@ -834,23 +923,24 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
         } else {
             const size_t wsb = vc_conv_wgrad_ws_bytes(R.n_out, L.cin, L.cout, R.K);
             VC_ALLOC(ws, void*, wsb);
+            VC_CHECK_ARG(X.f32 && X.ld == X.c, "layer %d: the fp32 wgrad needs a dense fp32 input", li);
             Timed t(5, li, wst);
             VC_TRY(vc_conv_wgrad_f32(X.f32, dx, R.nbr, dw, R.n_out, L.cin, L.cout, R.K, ws, wsb, wst));
         }
         if (two) last_w_ev = record_on(C, 1);
         // dgrad
-        if (!L.need_dgrad || L.in_slot == 0) continue;
+        if (!dgrad) continue;
         if (R.subm && !R.unique && L.use_tc_scatter && L.wimg_dgrad) {
-            VC_TRY(contribute_scatter(C, X, st, [&](float* dst) -> int {
+            VC_TRY(contribute_scatter(C, X, st, [&](float* dst, int ld) -> int {
                 Timed t(7, li, st);
-                return tc_scatter_with_image(L.cout, L.cin, dxb, L.wimg_dgrad, R.nbr, dst, R.n_out, R.K, C.err, st);
+                return tc_scatter_with_image(L.cout, L.cin, dxb, L.wimg_dgrad, R.nbr, dst, R.n_out, R.K, C.err, st, ld);
             }));
         } else if (R.subm && !R.unique) {
             const size_t wsb = vc_conv_ws_bytes(L.cin, L.cout, R.K);
             VC_ALLOC(ws, void*, wsb);
-            VC_TRY(contribute_scatter(C, X, st, [&](float* dst) -> int {
+            VC_TRY(contribute_scatter(C, X, st, [&](float* dst, int ld) -> int {
                 Timed t(4, li, st);
-                return vc_conv_dgrad_scatter_f32(dx, C.P<const float>(li, P_W), R.nbr, dst, R.n_out, L.cin, L.cout, R.K, ws, wsb, st);
+                return conv_dgrad_scatter_f32_ld(dx, C.P<const float>(li, P_W), R.nbr, dst, ld, R.n_out, L.cin, L.cout, R.K, ws, wsb, st);
             }));
         } else if (L.use_tc && L.wimg_dgrad) {
             const int32_t* table = R.subm ? R.nbr : R.nbr_bwd;

@@ -131,9 +131,99 @@ __global__ void cat2_kernel(const float4* __restrict__ a, const float4* __restri
     }
 }
 
+// mean of the first n rows of a [cap, c] matrix: float64 per-thread sums over float4s in a fixed grid-stride order, a
+// fixed-order block reduction, and the last CTA (atomic ticket) adds the CTA partials — all its threads, each over a fixed
+// subset, then the same block reduction — so the result depends on the grid size only, never on timing.
+constexpr int MM_THREADS = 256;
+
+__device__ __forceinline__ double mm_block_sum(double s, double* warp_s) {   // valid in thread 0
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_down_sync(0xffffffffu, s, o);
+    if ((threadIdx.x & 31) == 0) warp_s[threadIdx.x >> 5] = s;
+    __syncthreads();
+    double b = 0.0;
+    if (threadIdx.x == 0)
+        for (int w = 0; w < MM_THREADS / 32; ++w) b += warp_s[w];
+    return b;
+}
+
+__global__ void __launch_bounds__(MM_THREADS) masked_mean_kernel(const float4* __restrict__ x, long long cap_rows,
+                                                                 const int* __restrict__ n_dev, int c4, double* part,
+                                                                 unsigned* ticket, float* out) {
+    const long long n = n_dev != nullptr ? min(cap_rows, (long long)max(__ldg(n_dev), 0)) : cap_rows;
+    const long long total4 = n * c4;
+    const long long stride = (long long)gridDim.x * MM_THREADS;
+    long long i = (long long)blockIdx.x * MM_THREADS + threadIdx.x;
+    double s = 0.0;
+    for (; i + 3 * stride < total4; i += 4 * stride) {   // four loads in flight per thread
+        float4 v[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) v[u] = x[i + u * stride];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) s += ((double)v[u].x + (double)v[u].y) + ((double)v[u].z + (double)v[u].w);
+    }
+    for (; i < total4; i += stride) {
+        const float4 v = x[i];
+        s += ((double)v.x + (double)v.y) + ((double)v.z + (double)v.w);
+    }
+    __shared__ double warp_s[MM_THREADS / 32];
+    __shared__ bool last;
+    const double b = mm_block_sum(s, warp_s);
+    if (threadIdx.x == 0) {
+        part[blockIdx.x] = b;
+        __threadfence();
+        last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    double t = 0.0;
+    for (unsigned k = threadIdx.x; k < gridDim.x; k += MM_THREADS) t += __ldcg(part + k);
+    t = mm_block_sum(t, warp_s);
+    if (threadIdx.x == 0) *out = (float)(t / (double)(n * c4 * 4));   // (no rows: 0/0 = NaN, as torch's mean of an empty tensor)
+}
+
+// gradient of that mean: dx[r, :] = g / (n*c) for r < n, 0 for the rows [n, cap)
+__global__ void __launch_bounds__(MM_THREADS) masked_mean_bwd_kernel(const float* __restrict__ g, long long cap_rows,
+                                                                     const int* __restrict__ n_dev, int c4, float4* __restrict__ dx) {
+    const long long n = n_dev != nullptr ? min(cap_rows, (long long)max(__ldg(n_dev), 0)) : cap_rows;
+    const float v = __fdiv_rn(__ldg(g), (float)(n * c4 * 4));
+    const float4 val = make_float4(v, v, v, v), zero = make_float4(0.f, 0.f, 0.f, 0.f);
+    const long long live4 = n * c4, total4 = cap_rows * c4;
+    for (long long i = (long long)blockIdx.x * MM_THREADS + threadIdx.x; i < total4; i += (long long)gridDim.x * MM_THREADS)
+        dx[i] = i < live4 ? val : zero;
+}
+
+int mm_grid(long long cap_rows, int c) {   // a function of the capacity only: the reduction order of a shape is fixed
+    const long long b = cdiv(cap_rows * c / 4, (long long)MM_THREADS * 8);
+    return (int)(b < 1 ? 1 : (b > 4 * 132 ? 4 * 132 : b));
+}
+
 }  // namespace vc
 
 using namespace vc;
+
+extern "C" size_t vc_masked_mean_ws_bytes(void) { return 256 + 4 * 132 * sizeof(double); }
+
+extern "C" int vc_masked_mean_f32(const float* x, long long cap_rows, int c, const int32_t* n_dev, float* out, void* ws,
+                                  size_t ws_bytes, vc_stream_t stream_) {
+    VC_CHECK_ARG(cap_rows >= 0 && c > 0 && c % 4 == 0, "masked mean: bad shape [%lld, %d]", cap_rows, c);
+    VC_CHECK_ARG(x && out && ws && ws_bytes >= vc_masked_mean_ws_bytes(), "masked mean: null pointer / workspace too small");
+    VC_CUDA(cudaMemsetAsync(ws, 0, sizeof(unsigned), (cudaStream_t)stream_));   // the ticket
+    masked_mean_kernel<<<mm_grid(cap_rows, c), MM_THREADS, 0, (cudaStream_t)stream_>>>(
+        (const float4*)x, cap_rows, n_dev, c / 4, (double*)((char*)ws + 256), (unsigned*)ws, out);
+    VC_LAUNCH_CHECK();
+    return VC_OK;
+}
+
+extern "C" int vc_masked_mean_bwd_f32(const float* g, long long cap_rows, int c, const int32_t* n_dev, float* dx,
+                                      vc_stream_t stream_) {
+    VC_CHECK_ARG(cap_rows >= 0 && c > 0 && c % 4 == 0, "masked mean: bad shape [%lld, %d]", cap_rows, c);
+    VC_CHECK_ARG(g && (dx || cap_rows == 0), "masked mean: null pointer");
+    if (cap_rows == 0) return VC_OK;
+    masked_mean_bwd_kernel<<<mm_grid(cap_rows, c), MM_THREADS, 0, (cudaStream_t)stream_>>>(g, cap_rows, n_dev, c / 4, (float4*)dx);
+    VC_LAUNCH_CHECK();
+    return VC_OK;
+}
 
 int vc::cat2_dev(const float* a, const float* b, float* out, void* out_bf16, int n, const int* n_dev, int ca, int cb,
                  cudaStream_t stream) {

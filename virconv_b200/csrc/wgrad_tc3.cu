@@ -55,8 +55,9 @@ struct WCfg2 {
 };
 
 struct WArgs {
-    const __nv_bfloat16* in;    // [n_in, in_c] gathered rows
+    const __nv_bfloat16* in;    // [n_in, in_ld] gathered rows
     int in_c;                   // real channels (8 or CI)
+    int in_ld;                  // row pitch (>= in_c: the rows may be a column slice of a wider matrix)
     const __nv_bfloat16* dout;  // [n_out, out_c]
     int out_c;                  // real channels (8 or CO)
     const int32_t* nbr;         // [K][pitch]
@@ -270,7 +271,7 @@ __global__ void __launch_bounds__(W_THREADS, 2) tc_wgrad_half_kernel(const WArgs
 #pragma unroll
                         for (int i = 0; i < NIT; ++i) {
                             const bool v = src[j][i] >= 0;
-                            const __nv_bfloat16* srow = a.in + (size_t)(v ? src[j][i] : 0) * a.in_c + c_sub * 8;
+                            const __nv_bfloat16* srow = a.in + (size_t)(v ? src[j][i] : 0) * a.in_ld + c_sub * 8;
 #pragma unroll
                             for (int cg = 0; cg < NCG; ++cg) {
                                 // a missing neighbour costs a shared-memory zero store, not a zero-fill cp.async
@@ -384,14 +385,19 @@ int launch_wgrad3(const WArgs& a0, int n_cap, int max_ctas, cudaStream_t stream)
 // scratch: [K][cin][cout] fp32, ZERO on entry (the kernel accumulates); tile_counter: `wgrad3_passes(cin, cout, K)` ints, zero;
 // at most max_ctas CTAs per pass
 int tc3_wgrad(int cin, int cout, const void* in_bf16, const void* dout_bf16, const int32_t* nbr, long long pitch, float* scratch,
-              int n_rows, const int* n_dev, int K, int* err, cudaStream_t stream, int* tile_counter, int max_ctas) {
+              int n_rows, const int* n_dev, int K, int* err, cudaStream_t stream, int* tile_counter, int max_ctas, int in_ld) {
     if (n_rows == 0) return VC_OK;
     if (!tc2_ch_ok(cin) || !tc2_ch_ok(cout) || K < 1 || K > MAXK_TC) {
         set_error("tensor-core wgrad: unsupported shape (%d -> %d channels, K=%d)", cin, cout, K);
         return VC_ERR_UNSUPPORTED;
     }
     WArgs a;
-    a.in = (const __nv_bfloat16*)in_bf16; a.in_c = cin; a.dout = (const __nv_bfloat16*)dout_bf16; a.out_c = cout; a.nbr = nbr;
+    if (in_ld == 0) in_ld = cin;
+    if (in_ld < cin || in_ld % 8 != 0) {
+        set_error("tensor-core wgrad: row pitch %d for %d channels", in_ld, cin);
+        return VC_ERR_INVALID;
+    }
+    a.in = (const __nv_bfloat16*)in_bf16; a.in_c = cin; a.in_ld = in_ld; a.dout = (const __nv_bfloat16*)dout_bf16; a.out_c = cout; a.nbr = nbr;
     a.pitch = pitch; a.scratch = scratch; a.n_dev = n_dev; a.n_host = n_rows; a.tile_counter = tile_counter; a.K = K; a.S = 0;
     a.groups_per_pass = 0; a.err = err;
     const int ci = tc_pad16(cin), co = tc_pad16(cout);

@@ -132,7 +132,13 @@ class Plan:
         return out
 
     def publish(self, name, f_slot, iset):
+        """The op producing `f_slot` is marked (x1 = 1): its fp32 output is read outside the plan.  The executor writes fp32
+        activations only where such a reader exists; the bf16 kernels read the bf16 shadow."""
         self.published.append((name, f_slot, iset))
+        for row in self.rows_i:
+            if (row[0] == OP_CBR and row[3] == f_slot) or (row[0] == OP_CAT and row[4] == f_slot):
+                row[22] = 1
+        self._final = None
 
     def finalize(self):
         if self._final is None:

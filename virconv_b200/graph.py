@@ -24,11 +24,38 @@ import torch
 from . import _lib, executor, ops
 
 
+class _MaskedMean(torch.autograd.Function):
+    """One library kernel each way (vc_masked_mean_f32 / _bwd_f32): the backward writes the contiguous [N, C] gradient the
+    plan executor consumes, so nothing downstream has to expand or copy it."""
+
+    @staticmethod
+    def forward(ctx, features, num_rows):
+        ops._require_cuda(features, num_rows)
+        assert features.dtype == torch.float32 and features.dim() == 2, (features.dtype, features.shape)
+        assert num_rows is None or (num_rows.dtype == torch.int32 and num_rows.numel() == 1)
+        lib = _lib.load()
+        x = features.contiguous()
+        out = torch.empty((), dtype=torch.float32, device=x.device)
+        ws = torch.empty(lib.vc_masked_mean_ws_bytes(), dtype=torch.uint8, device=x.device)
+        _lib.check(lib.vc_masked_mean_f32(ops._p(x), x.shape[0], x.shape[1], ops._p(num_rows), ops._p(out), ops._p(ws), ws.numel(),
+                                          ops._stream()), 'vc_masked_mean_f32')
+        ctx.shape, ctx.num_rows = x.shape, num_rows
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        lib = _lib.load()
+        g = g.contiguous()
+        dx = torch.empty(ctx.shape, dtype=torch.float32, device=g.device)
+        _lib.check(lib.vc_masked_mean_bwd_f32(ops._p(g), ctx.shape[0], ctx.shape[1], ops._p(ctx.num_rows), ops._p(dx), ops._stream()),
+                   'vc_masked_mean_bwd_f32')
+        return dx, None
+
+
 def masked_mean(t):
-    """Mean over the valid rows of a published tensor: static mode (zero tail, device row count) or exact mode."""
-    if getattr(t, 'num_rows', None) is None:
-        return t.features.mean()
-    return t.features.sum() / (t.num_rows.to(torch.float32) * t.features.shape[1]).squeeze(0)
+    """Mean over the valid rows of a published tensor: static mode (zero tail, device row count `num_rows`) or exact mode
+    (every row)."""
+    return _MaskedMean.apply(t.features, getattr(t, 'num_rows', None))
 
 
 class GraphedStep:
