@@ -470,7 +470,8 @@ int vc_rcnn_loss(const vc_rcnn_branch* branches /*host[K]*/, int K, double beta,
  *               4 CBR       features a, rulebook c -> features b            conv + BatchNorm1d + ReLU of layer [20]
  *                                                                            ([18] cin, [19] cout, [21] = input needs grad)
  *               5 CAT       features a, features b -> features c            channel concat
- *     [1] stream (0 main: feature ops, 1 side: index ops)   [2..4] a, b, c   [5] ndim   [6..8] kernel size
+ *     [1] stream (0 main: feature ops, 1 side: index ops, 2 second side stream: the image branch's index ops)
+ *     [2..4] a, b, c   [5] ndim   [6..8] kernel size
  *     [9..11] stride   [12..14] padding   [15..17] dilation
  *   layer_ptrs [n_layers, 9] uint64: weight, gamma, beta, running_mean, running_var, num_batches_tracked, then the
  *   caller's gradient buffers d_weight, d_gamma, d_beta (written by vc_exec_backward); layer_f [n_layers, 2] = eps, momentum.
@@ -480,7 +481,8 @@ int vc_rcnn_loss(const vc_rcnn_branch* branches /*host[K]*/, int K, double beta,
  * addresses and row counts that vc_exec_backward and vc_exec_query read; the library keeps nothing else between calls
  * (apart from a pool of CUDA events for cross-stream ordering).  `pinned_host`: >= 16 int32 of page-locked host memory
  * for the row-count read-backs.  precision 0 = fp32 kernels, 1 = bf16 tensor-core kernels where channels allow.
- * Index ops run on side_stream (may be NULL = single stream); on return every later use of main_stream is ordered
+ * Index ops run on side_stream (may be NULL = single stream), those of stream 2 on side2_stream (may be NULL: then on
+ * side_stream); on return every later use of main_stream is ordered
  * after all of the step's work.  side_waits_main != 0: the side stream first waits for everything already queued on
  * main_stream (always safe).  0: the caller guarantees idx0 / proj_params are valid in side_stream order and that the
  * arena may be written from side_stream right away (e.g. it was allocated there) — the index ops of this step then
@@ -492,12 +494,16 @@ int vc_rcnn_loss(const vc_rcnn_branch* branches /*host[K]*/, int K, double beta,
  * (vc_exec_query(state, 2, id)[6] = its address), published buffers have capacity rows with a zero / -1 tail, and a row
  * count that does not fit its capacity is clamped and reported as max() into *overflow_flag (device int32; zero it
  * before the step, re-run with larger capacities when it is non-zero afterwards).  Use side_waits_main = 1 under capture.
+ * flags: bits 8-9 = phase (static mode only).  0 enqueues the whole forward, 1 ONLY the index operators (rulebooks,
+ * projections), 2 ONLY the feature operators (weight images, conv + BN + ReLU, concat) over the arena phase 1 filled: call
+ * both with the same arguments, so they allocate the same addresses and leave the same state (graph.PipelinedStep runs
+ * the index phase of step t+1 beside the feature phase of step t).  Other bits are ignored (callers pass bit 0 = 1).
  * ---------------------------------------------------------------------------------------------- */
 size_t vc_exec_state_bytes(void);
 int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_ops, const uint64_t* layer_ptrs, const float* layer_f,
                     int n_layers, const float* feats0, int c0, const int32_t* idx0, int n0, const int32_t* shape0 /*host[3]*/,
                     int batch_size, const float* proj_params /*device [B,28], may be NULL without INDEX2UV ops*/,
-                    int training, int precision, int want_pair_num, void* arena, size_t arena_bytes,
+                    int training, int precision, int flags, void* arena, size_t arena_bytes,
                     int32_t* pinned_host, int32_t* err_flag, void* state, size_t state_bytes, vc_stream_t main_stream,
                     vc_stream_t side_stream, int side_waits_main, const int32_t* caps /*host, may be NULL*/,
                     const int32_t* n0_dev /*device, NULL = exact mode*/, int32_t* overflow_flag /*device*/,
@@ -512,11 +518,12 @@ int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_ops, const 
                      size_t arena_bytes, int32_t* err_flag, void* state, vc_stream_t stream, vc_stream_t wgrad_stream);
 /* Read a state blob.  what 0: out[0] = arena bytes in use;  1 (feature slot id): f32 ptr, bf16 ptr, rows, c;
  * 2 (index set): idx ptr, n, ndim, shape[3];  3 (rulebook): nbr, nbr_bwd, pair_num ptrs, K, n_in, n_out, subm, unique;
- * 4 (layer): x ptr, y ptr, stats ptr, use_tc, rulebook id, in slot, out slot.  out: >= 8 int64 (host). */
+ * 4 (layer): x ptr, y ptr, stats ptr, forward runs on the tensor cores, rulebook id, in slot, out slot.  out: >= 8 int64
+ * (host). */
 int vc_exec_query(const void* state, int what, int id, long long* out);
 /* Optional per-launch timing of the conv kernels (bench.py's roofline pass): vc_exec_timing(1) clears and arms it,
  * vc_exec_timing_read synchronises and returns up to max_records (ms, [kind, layer]) records; kind 0 fwd f32, 1 fwd tc,
- * 2 dgrad f32, 3 dgrad tc, 4 dgrad scatter, 5 wgrad f32, 6 wgrad tc. */
+ * 2 dgrad f32, 3 dgrad tc, 4 dgrad scatter f32, 5 wgrad f32, 6 wgrad tc, 7 dgrad scatter tc. */
 int vc_exec_timing(int enable);
 int vc_exec_timing_read(float* ms_out, int32_t* kind_layer_out, int max_records);
 

@@ -58,13 +58,18 @@ struct RBk {
 };
 constexpr int CTR_PER_LAYER = 16;  // forward, dgrad, up to 14 wgrad passes (C_in = C_out = 64, K = 27: 14 groups, one per pass in wgrad_tc3)
 
+// conv launches of a layer; the values are the timing records' kinds (vc_exec_timing_read, executor.KIND_NAMES)
+enum ConvKind : int { K_NONE = -1 /* no input gradient */, K_FWD_F32 = 0, K_FWD_TC = 1, K_DGRAD_F32 = 2, K_DGRAD_TC = 3,
+                      K_DGRAD_SCATTER_F32 = 4, K_WGRAD_F32 = 5, K_WGRAD_TC = 6, K_DGRAD_SCATTER_TC = 7 };
+
 struct Layer {
     float *x, *y, *stats;
     double* sums;          // [4*cout]: forward sums, backward sums
     int* tile_ctr;         // [CTR_PER_LAYER] tile-scheduler counters of the persistent kernels (forward, dgrad, wgrad passes), zeroed with the sums
     float* wscratch;       // [K][cin][cout] fp32 accumulator of the persistent wgrad kernel (zeroed with the sums), or NULL
     void *wimg_fwd, *wimg_dgrad;
-    int in_slot, out_slot, rb, use_tc, use_tc_scatter, cin, cout, need_dgrad;   // use_tc: conv fwd / gather dgrad / wgrad
+    int in_slot, out_slot, rb, cin, cout;
+    ConvKind fwd, dgrad, wgrad;   // chosen by choose_kernels
 };
 struct State {
     uint64_t magic;
@@ -95,7 +100,7 @@ struct Arena {
 // library-owned event pool (cross-stream ordering only; timing disabled).  An event may be re-recorded as soon as the
 // wait on its previous recording has been ENQUEUED, so a small round-robin pool is enough.
 constexpr int EV_POOL = 512;   // > the events of one forward / backward call: the cursor restarts at every call
-// (process-wide, not thread_local: autograd runs backward on its own thread; one process drives one device)
+// (process-wide, not per thread: autograd runs backward on its own thread; one process drives one device)
 cudaEvent_t g_ev[EV_POOL];
 int g_ev_dev = -1, g_ev_next = 0;
 
@@ -114,7 +119,7 @@ int ev_init() {
 // optional per-kernel timing (bench.py's roofline pass): event pairs around the conv launches
 struct TimeRec {
     cudaEvent_t a, b;
-    int kind, layer;   // kind: 0 conv fwd f32, 1 conv fwd tc, 2 dgrad f32, 3 dgrad tc, 4 dgrad scatter, 5 wgrad f32, 6 wgrad tc, 7 scatter tc
+    int kind, layer;   // kind: a ConvKind
 };
 constexpr int T_MAX = 4096;
 TimeRec g_t[T_MAX];
@@ -254,6 +259,310 @@ int check_plan(const int32_t* oi, int n_ops, int n_layers) {
     return VC_OK;
 }
 
+// the one place that decides which conv kernels a layer runs (the tensor-core backward only in a BN-training step)
+void choose_kernels(Layer& L, int precision, int training, int need_dgrad, const RBk& R) {
+    const bool tc = precision == 1 && tc2_ch_ok(L.cin) && tc2_ch_ok(L.cout);
+    const bool tc_bwd = tc && training;
+    L.fwd = tc ? K_FWD_TC : K_FWD_F32;
+    L.wgrad = tc_bwd ? K_WGRAD_TC : K_WGRAD_F32;
+    if (!need_dgrad || L.in_slot == 0)
+        L.dgrad = K_NONE;
+    else if (R.subm && !R.unique)   // many-to-one table (the image branch's projected pixels collide): atomic scatter
+        L.dgrad = tc_bwd && tc_scatter_ch_ok(L.cin) && tc_scatter_ch_ok(L.cout) ? K_DGRAD_SCATTER_TC : K_DGRAD_SCATTER_F32;
+    else
+        L.dgrad = tc_bwd ? K_DGRAD_TC : K_DGRAD_F32;
+}
+
+// fp32 accumulator of the tensor-core wgrad, padded to 64 floats
+size_t wgrad_acc_floats(const Layer& L, int K) { return L.wgrad == K_WGRAD_TC ? ((size_t)K * L.cin * L.cout + 63) / 64 * 64 : 0; }
+
+// what the forward shares between its planning pass and its per-op enqueue functions (value-initialised)
+struct FwdCtx : Ctx {
+    // derived from the plan alone by plan_step, before any CUDA call: both phases of a phased step derive the same, so they
+    // agree on every arena address (rulebook meta and layer kinds go straight into the State)
+    int slot_c[MAX_F], cat_out[MAX_F], cat_col[MAX_F];   // cat_out: the in-place concat a slot is a column slice of, or -1
+    bool need_f32[MAX_F], cat_inplace[MAX_OPS];
+    size_t sums_doubles, n_cbr, wg_floats;               // the zeroed region: BN sums, tile counters, wgrad accumulators
+    const float* proj;
+    const int32_t* caps;
+    int32_t *overflow, *pinned;
+    int n_syncs, last_ev[3] = {-1, -1, -1};   // last_ev: latest event of each side stream (joined into main at the end)
+    bool do_idx, do_feat, two;   // do_idx / do_feat: enqueue the index / feature operators (both unless phased)
+    // per strided conv op: the workspace its count, indices and tables phases share; done: count and indices are enqueued
+    struct { void* ws; size_t wsb; bool done; } chain[MAX_OPS];
+    template <class T>
+    void produced(T& r, int s) {   // r was written on stream s: consumers on the other streams wait for r.ev
+        r.prod = s;
+        r.ev = s == 0 ? -1 : (last_ev[s] = record_on(*this, s));
+    }
+};
+
+// Which feature slots need an fp32 copy: published ones (x1 of the producing op), the input of a layer without the
+// tensor-core forward + wgrad pair (fp32 conv or fp32 wgrad), and the fp32 precision mode.  Everything else is read as
+// bf16 only, so its fp32 copy is not written.  A concat whose inputs need no fp32 copy of their own is built in place:
+// the BN-apply of each input layer writes its column slice of the concat (fp32 if the concat needs it, and bf16), and
+// the concat op launches nothing.
+void plan_step(FwdCtx& C, int c0, int precision, int training) {
+    for (int i = 0; i < MAX_F; ++i) C.cat_out[i] = -1;
+    C.slot_c[0] = c0;
+    C.need_f32[0] = true;
+    for (int i = 0; i < C.n_ops; ++i) {
+        const int* o = C.op(i);
+        if (o[F_KIND] == OP_SUBM_RB || o[F_KIND] == OP_CONV_RB) {
+            RBk& R = C.S->rb[o[F_C]];
+            R.K = 1;
+            for (int d = 0; d < o[F_NDIM]; ++d) R.K *= o[F_KS + d];
+            R.subm = o[F_KIND] == OP_SUBM_RB;
+            R.unique = R.subm ? o[F_X0] : 1;
+        } else if (o[F_KIND] == OP_CBR) {
+            Layer& L = C.S->layer[o[F_LAYER]];
+            L.cin = o[F_CIN]; L.cout = o[F_COUT]; L.in_slot = o[F_A]; L.out_slot = o[F_B]; L.rb = o[F_C];
+            choose_kernels(L, precision, training, o[F_X0], C.S->rb[L.rb]);
+            C.slot_c[L.out_slot] = L.cout;
+            if (precision == 0 || o[F_X1]) C.need_f32[L.out_slot] = true;
+            if (L.fwd == K_FWD_F32 || L.wgrad == K_WGRAD_F32) C.need_f32[L.in_slot] = true;
+            C.sums_doubles += 4 * (size_t)L.cout;
+            ++C.n_cbr;
+            C.wg_floats += wgrad_acc_floats(L, C.S->rb[L.rb].K);
+        } else if (o[F_KIND] == OP_CAT) {
+            C.slot_c[o[F_C]] = C.slot_c[o[F_A]] + C.slot_c[o[F_B]];
+            if (precision == 0 || o[F_X1]) C.need_f32[o[F_C]] = true;
+        }
+    }
+    for (int i = 0; i < C.n_ops; ++i) {
+        const int* o = C.op(i);
+        if (o[F_KIND] != OP_CAT) continue;
+        const int a = o[F_A], b = o[F_B];
+        C.cat_inplace[i] = precision == 1 && a != 0 && b != 0 && a != b && !C.need_f32[a] && !C.need_f32[b] && C.cat_out[a] < 0 &&
+                           C.cat_out[b] < 0;
+        if (C.cat_inplace[i]) {
+            C.cat_out[a] = C.cat_out[b] = o[F_C];
+            C.cat_col[b] = C.slot_c[a];
+        } else {
+            C.need_f32[a] = C.need_f32[b] = true;
+        }
+    }
+}
+
+// one function per op kind: op i (plan row o), enqueued on stream s
+int fwd_subm_rb(FwdCtx& C, int i, const int* o, int s) {
+    ISet& I = C.S->iset[o[F_A]];
+    RBk& R = C.S->rb[o[F_C]];
+    VC_CHECK_ARG(I.idx && I.ndim == o[F_NDIM], "op %d: index set %d not built / wrong ndim", i, o[F_A]);
+    VC_TRY(wait_for(C, I.ev, I.prod, s));
+    R.n_in = R.n_out = I.n;
+    R.n_in_dev = R.n_out_dev = I.n_dev;
+    VC_ALLOC(nbr, int32_t*, (size_t)R.K * I.n * 4);
+    VC_ALLOC(pn, int32_t*, (size_t)R.K * 4);
+    R.nbr = nbr; R.pair_num = pn;
+    const size_t wsb = vc_subm_rulebook_ws_bytes(I.n);
+    VC_ALLOC(ws, void*, wsb);
+    if (C.do_idx)
+        VC_TRY(subm_rulebook_dev(I.idx, I.n, I.n_dev, I.ndim, C.S->batch_size, I.shape, o + F_KS, o + F_DL, R.nbr, R.pair_num, ws, wsb,
+                                 C.st[s]));
+    C.produced(R, s);
+    return VC_OK;
+}
+
+// count + row-count read-back + output indices of strided conv op j (its input index set must exist)
+int fwd_conv_count(FwdCtx& C, int j) {
+    const int* o = C.op(j);
+    const int s = C.two ? o[F_STREAM] : 0;
+    cudaStream_t st = C.st[s];
+    ISet& I = C.S->iset[o[F_A]];
+    ISet& O = C.S->iset[o[F_B]];
+    RBk& R = C.S->rb[o[F_C]];
+    VC_CHECK_ARG(I.ndim == o[F_NDIM], "op %d: index set %d has the wrong ndim", j, o[F_A]);
+    VC_TRY(wait_for(C, I.ev, I.prod, s));
+    int32_t oshape[3] = {0, 0, 0};
+    VC_TRY(vc_conv_out_shape(I.ndim, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL, oshape));
+    const size_t wsb = vc_conv_rulebook_ws_bytes(I.ndim, C.S->batch_size, oshape);
+    VC_ALLOC(ws, void*, wsb);
+    VC_ALLOC(n_dev, int32_t*, 4);
+    int n_out;
+    if (C.S->is_static) {
+        n_out = C.caps[o[F_B]];
+        VC_CHECK_ARG(n_out > 0, "op %d: static mode needs a capacity for index set %d", j, o[F_B]);
+        if (C.do_idx)
+            VC_TRY(conv_rulebook_count_dev(I.idx, I.n, I.n_dev, I.ndim, C.S->batch_size, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL,
+                                           n_dev, n_out, C.overflow, ws, wsb, st));
+    } else {
+        VC_TRY(conv_rulebook_count_dev(I.idx, I.n, nullptr, I.ndim, C.S->batch_size, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL,
+                                       n_dev, 0, nullptr, ws, wsb, st));
+        VC_CUDA(cudaMemcpyAsync(C.pinned + (C.n_syncs & 7), n_dev, 4, cudaMemcpyDeviceToHost, st));
+        // the tensor-core kernels' pipeline-timeout flag rides along with the first read-back of a step (it reports on the
+        // kernels of EARLIER steps: a wedged mbarrier wait must not go unnoticed in production — ADVICE r1)
+        if (C.n_syncs == 0 && C.err != nullptr) VC_CUDA(cudaMemcpyAsync(C.pinned + 15, C.err, 4, cudaMemcpyDeviceToHost, st));
+        VC_CUDA(cudaStreamSynchronize(st));        // the one data-dependent size per strided conv
+        n_out = C.pinned[C.n_syncs & 7];
+        if (C.n_syncs == 0 && C.err != nullptr && C.pinned[15] != 0) {
+            set_error("a tensor-core kernel's pipeline wait timed out in an earlier step (error flag %d): its results are invalid",
+                      C.pinned[15]);
+            return VC_ERR_PIPELINE;
+        }
+        ++C.n_syncs;
+    }
+    R.n_in = I.n; R.n_out = n_out;
+    R.n_in_dev = I.n_dev; R.n_out_dev = C.S->is_static ? n_dev : nullptr;
+    O.n = n_out; O.ndim = I.ndim; O.n_dev = R.n_out_dev;
+    for (int d = 0; d < 3; ++d) O.shape[d] = oshape[d];
+    VC_ALLOC(oidx, int32_t*, (size_t)(n_out > 0 ? n_out : 1) * (1 + I.ndim) * 4);
+    O.idx = oidx;
+    if (C.S->is_static && C.do_idx) VC_CUDA(cudaMemsetAsync(oidx, 0xFF, (size_t)n_out * (1 + I.ndim) * 4, st));   // defined tail (-1) for the published indices
+    if (C.do_idx)
+        VC_TRY(conv_rulebook_fill_phases(I.idx, I.n, I.n_dev, I.ndim, C.S->batch_size, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL,
+                                         n_out, O.idx, nullptr, nullptr, nullptr, ws, wsb, st, 1));
+    C.produced(O, s);
+    C.chain[j] = {ws, wsb, true};
+    return VC_OK;
+}
+
+int fwd_conv_rb(FwdCtx& C, int i, const int* o, int s) {
+    // First strided conv reached: run the count -> (host reads the row count) -> emit-indices chain of EVERY strided conv of
+    // the plan now, back to back.  Each link only needs the previous link's output indices, and it is the only part of the
+    // forward the host has to wait for; the neighbour tables, submanifold rulebooks and projections queue up behind it
+    // without further synchronisation.
+    if (!C.chain[i].done) {
+        if (C.S->is_static) {
+            // no host read to wait for: keep the natural order (count -> indices -> tables per stage), so the tables of an
+            // early stage are not queued behind the counting kernels of all later ones
+            VC_TRY(fwd_conv_count(C, i));
+        } else {
+            for (int j = i; j < C.n_ops; ++j)
+                if (C.op(j)[F_KIND] == OP_CONV_RB && C.S->iset[C.op(j)[F_A]].idx) VC_TRY(fwd_conv_count(C, j));
+        }
+    }
+    VC_CHECK_ARG(C.chain[i].done, "op %d: index set %d not built", i, o[F_A]);
+    ISet& I = C.S->iset[o[F_A]];
+    ISet& O = C.S->iset[o[F_B]];
+    RBk& R = C.S->rb[o[F_C]];
+    VC_TRY(wait_for(C, I.ev, I.prod, s));
+    VC_TRY(wait_for(C, O.ev, O.prod, s));
+    VC_ALLOC(nbr, int32_t*, (size_t)R.K * (R.n_out > 0 ? R.n_out : 1) * 4);
+    VC_ALLOC(nbr_bwd, int32_t*, (size_t)R.K * I.n * 4);
+    VC_ALLOC(pn, int32_t*, (size_t)R.K * 4);
+    R.nbr = nbr; R.nbr_bwd = nbr_bwd; R.pair_num = pn;
+    if (C.do_idx)
+        VC_TRY(conv_rulebook_fill_phases(I.idx, I.n, I.n_dev, I.ndim, C.S->batch_size, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL,
+                                         R.n_out, O.idx, R.nbr, R.nbr_bwd, R.pair_num, C.chain[i].ws, C.chain[i].wsb, C.st[s], 2));
+    C.produced(R, s);
+    return VC_OK;
+}
+
+int fwd_index2uv(FwdCtx& C, int i, const int* o, int s) {
+    ISet& I = C.S->iset[o[F_A]];
+    ISet& O = C.S->iset[o[F_B]];
+    VC_CHECK_ARG(I.idx && I.ndim == 3 && C.proj, "op %d: index2uv needs a built 3-D index set and projection params", i);
+    VC_TRY(wait_for(C, I.ev, I.prod, s));
+    VC_ALLOC(uv, int32_t*, (size_t)I.n * 3 * 4);
+    O.idx = uv; O.n = I.n; O.ndim = 2; O.shape[0] = o[F_KS]; O.shape[1] = o[F_KS + 1]; O.shape[2] = 0; O.n_dev = I.n_dev;
+    if (C.do_idx)
+        VC_TRY(index2uv_dev(I.idx, I.n, I.n_dev, C.S->batch_size, C.proj, C.of + (size_t)i * OPF, o[F_X0], o[F_X1], o[F_X2], uv, C.st[s]));
+    C.produced(O, s);
+    return VC_OK;
+}
+
+int fwd_cbr(FwdCtx& C, int i, const int* o, int s) {
+    State* S = C.S;
+    cudaStream_t st = C.st[s];
+    const int li = o[F_LAYER];
+    Layer& L = S->layer[li];
+    FSlot& X = S->f[L.in_slot];
+    FSlot& Y = S->f[L.out_slot];
+    RBk& R = S->rb[L.rb];
+    VC_CHECK_ARG((X.f32 || X.bf16) && R.nbr && X.c == L.cin && X.rows == R.n_in,
+                 "op %d: input slot / rulebook mismatch (rows %d vs %d, c %d vs %d)", i, X.rows, R.n_in, X.c, L.cin);
+    VC_TRY(wait_for(C, R.ev, R.prod, s));
+    VC_TRY(wait_for(C, X.ev, X.prod, s));
+    const size_t elems = (size_t)R.n_out * L.cout;
+    VC_ALLOC(x, float*, elems * 4);
+    VC_ALLOC(stats, float*, (size_t)4 * L.cout * 4);
+    float* y = nullptr;
+    void* yb = nullptr;
+    int y_ld = L.cout;
+    const int cat = C.cat_out[L.out_slot];
+    if (cat >= 0) {   // a column slice of an in-place concat (allocated by its first input)
+        FSlot& O = S->f[cat];
+        if (O.bf16 == nullptr) {
+            O.rows = R.n_out; O.c = O.ld = C.slot_c[cat];
+            if (C.need_f32[cat]) {
+                VC_ALLOC(of_, float*, (size_t)O.rows * O.c * 4);
+                O.f32 = of_;
+            }
+            VC_ALLOC(ob_, void*, (size_t)O.rows * O.c * 2);
+            O.bf16 = ob_;
+        }
+        VC_CHECK_ARG(O.rows == R.n_out, "op %d: concat inputs with different row counts", i);
+        y_ld = O.ld;
+        if (O.f32) y = O.f32 + C.cat_col[L.out_slot];
+        yb = (__nv_bfloat16*)O.bf16 + C.cat_col[L.out_slot];
+    } else {
+        if (C.need_f32[L.out_slot]) {
+            VC_ALLOC(y_, float*, elems * 4);
+            y = y_;
+        }
+        if (S->precision == 1) {
+            VC_ALLOC(yb_, void*, elems * 2);
+            yb = yb_;
+        }
+    }
+    L.x = x; L.y = y; L.stats = stats;
+    double* sums = S->training ? L.sums : nullptr;
+    if (L.fwd == K_FWD_TC && R.n_out > 0) {
+        if (!X.bf16) {   // no producer wrote a shadow (network input): cast once
+            VC_CHECK_ARG(X.ld == X.c, "op %d: no bf16 copy of a strided input", i);
+            VC_ALLOC(xb, void*, (size_t)X.rows * X.c * 2);
+            if (C.do_feat) VC_TRY(vc_cast_f32_bf16(X.f32, xb, (long long)X.rows * X.c, st));
+            X.bf16 = xb;
+        }
+        Timed t(K_FWD_TC, li, st);
+        // (flag bit 1: the rulebook was built on another stream and joined by an event, or by an earlier call, so the kernel
+        //  may load its first table slices before its griddepcontrol.wait — conv_tc2.cu)
+        if (C.do_feat)
+            VC_TRY(tc2_conv(L.cin, L.cout, X.bf16, L.wimg_fwd, R.nbr, R.n_out, x, R.n_out, R.n_out_dev, R.K, sums, C.err, st, nullptr,
+                            L.tile_ctr, (!C.do_idx || C.st[R.prod] != C.st[s]) ? 2 : 0, X.ld));
+    } else {   // (also a tensor-core layer without output rows)
+        const size_t wsb = vc_conv_ws_bytes(L.cin, L.cout, R.K);
+        VC_ALLOC(ws, void*, wsb);
+        VC_CHECK_ARG(X.f32 && X.ld == X.c, "op %d: the fp32 conv needs a dense fp32 input", i);
+        Timed t(K_FWD_F32, li, st);
+        if (C.do_feat) VC_TRY(vc_conv_fwd_f32(X.f32, C.P<const float>(li, P_W), R.nbr, x, R.n_out, L.cin, L.cout, R.K, sums, ws, wsb, st));
+    }
+    if (C.do_feat)
+        VC_TRY(bn_apply_relu_dev(x, L.sums, R.n_out, R.n_out_dev, L.cout, C.P<const float>(li, P_GAMMA), C.P<const float>(li, P_BETA),
+                                 C.P<float>(li, P_RM), C.P<float>(li, P_RV), C.P<long long>(li, P_NBT), C.lf[2 * li + 1], C.lf[2 * li],
+                                 S->training, y, y_ld, yb, y_ld, stats, 1, C.S->is_static, st));
+    Y.f32 = y; Y.bf16 = yb; Y.rows = R.n_out; Y.c = L.cout; Y.ld = y_ld; Y.n_dev = R.n_out_dev;
+    C.produced(Y, s);
+    return VC_OK;
+}
+
+int fwd_cat(FwdCtx& C, int i, const int* o, int s) {
+    FSlot& Aa = C.S->f[o[F_A]];
+    FSlot& Bb = C.S->f[o[F_B]];
+    FSlot& O = C.S->f[o[F_C]];
+    VC_TRY(wait_for(C, Aa.ev, Aa.prod, s));
+    VC_TRY(wait_for(C, Bb.ev, Bb.prod, s));
+    if (C.cat_inplace[i]) {   // both halves are already written (fwd_cbr): nothing to launch
+        VC_CHECK_ARG(Aa.bf16 && Bb.bf16 && Aa.rows == Bb.rows && O.bf16, "op %d: concat inputs not built / row mismatch", i);
+    } else {
+        VC_CHECK_ARG(Aa.f32 && Bb.f32 && Aa.ld == Aa.c && Bb.ld == Bb.c && Aa.rows == Bb.rows,
+                     "op %d: concat inputs not built / row mismatch", i);
+        const size_t elems = (size_t)Aa.rows * (Aa.c + Bb.c);
+        VC_ALLOC(out, float*, elems * 4);
+        void* ob = nullptr;
+        if (C.S->precision == 1) {
+            VC_ALLOC(ob_, void*, elems * 2);
+            ob = ob_;
+        }
+        if (C.do_feat) VC_TRY(cat2_dev(Aa.f32, Bb.f32, out, ob, Aa.rows, Aa.n_dev, Aa.c, Bb.c, C.st[s]));
+        O.f32 = out; O.bf16 = ob; O.rows = Aa.rows; O.c = O.ld = Aa.c + Bb.c;
+    }
+    O.n_dev = Aa.n_dev;
+    C.produced(O, s);
+    return VC_OK;
+}
+
 }  // namespace
 }  // namespace vc
 
@@ -313,7 +622,7 @@ extern "C" int vc_exec_query(const void* state, int what, int id, long long* out
             VC_CHECK_ARG(id >= 0 && id < MAX_L, "layer id");
             const Layer& l = S->layer[id];
             out[0] = (long long)(uintptr_t)l.x; out[1] = (long long)(uintptr_t)l.y; out[2] = (long long)(uintptr_t)l.stats;
-            out[3] = l.use_tc; out[4] = l.rb; out[5] = l.in_slot; out[6] = l.out_slot;
+            out[3] = l.fwd == K_FWD_TC; out[4] = l.rb; out[5] = l.in_slot; out[6] = l.out_slot;
             return VC_OK;
         }
     }
@@ -324,30 +633,21 @@ extern "C" int vc_exec_query(const void* state, int what, int id, long long* out
 extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_ops, const uint64_t* layer_ptrs,
                                const float* layer_f, int n_layers, const float* feats0, int c0, const int32_t* idx0, int n0,
                                const int32_t* shape0, int batch_size, const float* proj_params, int training, int precision,
-                               int want_pair_num, void* arena, size_t arena_bytes, int32_t* pinned_host, int32_t* err_flag,
+                               int flags, void* arena, size_t arena_bytes, int32_t* pinned_host, int32_t* err_flag,
                                void* state, size_t state_bytes, vc_stream_t main_stream, vc_stream_t side_stream,
                                int side_waits_main, const int32_t* caps, const int32_t* n0_dev, int32_t* overflow_flag,
                                vc_stream_t side2_stream) {
-    // Static mode (n0_dev != NULL; CUDA-graph capturable: no host read of a device value, every buffer sized from host-side
-    // capacities): n0 is the capacity of the input buffers, *n0_dev the number of valid rows, caps[i] the row capacity of
-    // index set i (the strided convs' outputs); every data-dependent row count stays in device memory, kernels clamp to the
-    // capacities and report an overflow through *overflow_flag (the largest row count that did not fit).
+    // static mode and phased execution: include/virconv_b200.h.  Both phases walk the whole plan with the same
+    // deterministic bump allocation, so they agree on every address and leave the same state blob.
     const bool is_static = n0_dev != nullptr;
     VC_CHECK_ARG(!is_static || (caps && overflow_flag), "static mode needs capacities and an overflow flag");
-    // Phased execution (static mode only; bits 8-9 of want_pair_num): 1 = enqueue ONLY the index operators (voxel -> rulebooks,
-    // projection), 2 = ONLY the feature operators (weight images, conv + BN + ReLU, concat).  Both phases walk the whole plan with
-    // the same deterministic bump allocation, so they agree on every address and leave the same state blob: graph.GraphedStep
-    // captures them as two graphs and runs the index graph of step t+1 beside the feature graph of step t.
-    const int phase = (want_pair_num >> 8) & 3;
-    want_pair_num &= 0xff;
+    const int phase = (flags >> 8) & 3;
     VC_CHECK_ARG(phase == 0 || (is_static && phase <= 2), "phased execution needs static mode");
-    const bool do_idx = phase != 2, do_feat = phase != 1;
     VC_TRY(check_plan(ops_i, n_ops, n_layers));
     VC_CHECK_ARG(state && state_bytes >= sizeof(State), "state blob too small (%zu < %zu)", state_bytes, sizeof(State));
     VC_CHECK_ARG(feats0 && idx0 && n0 > 0 && shape0 && batch_size > 0 && arena && pinned_host && ops_f && layer_ptrs && layer_f,
                  "null / empty argument");
     VC_CHECK_ARG(precision == 0 || precision == 1, "precision must be 0 (fp32) or 1 (bf16)");
-    VC_TRY(ev_init());
     State* S = new (state) State();
     memset(S, 0, sizeof(State));
     S->n_ops = n_ops; S->n_layers = n_layers; S->training = training; S->precision = precision; S->batch_size = batch_size;
@@ -355,386 +655,88 @@ extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_o
     for (int i = 0; i < MAX_I; ++i) S->iset[i].ev = -1;
     for (int i = 0; i < MAX_F; ++i) S->f[i].ev = -1;
     for (int i = 0; i < MAX_RB; ++i) S->rb[i].ev = -1;
+    S->iset[0].idx = const_cast<int32_t*>(idx0); S->iset[0].n = n0; S->iset[0].ndim = 3; S->iset[0].n_dev = n0_dev;
+    for (int d = 0; d < 3; ++d) S->iset[0].shape[d] = shape0[d];
+    S->f[0].f32 = const_cast<float*>(feats0); S->f[0].rows = n0; S->f[0].c = c0; S->f[0].ld = c0; S->f[0].n_dev = n0_dev;
 
-    Ctx C;
+    FwdCtx C = {};
     C.oi = ops_i; C.of = ops_f; C.n_ops = n_ops; C.lp = layer_ptrs; C.lf = layer_f; C.n_layers = n_layers; C.S = S;
     C.A = Arena{(char*)arena, arena_bytes, 0, false};
     C.st[0] = (cudaStream_t)main_stream;
     C.st[1] = side_stream ? (cudaStream_t)side_stream : (cudaStream_t)main_stream;
     C.st[2] = (side_stream && side2_stream) ? (cudaStream_t)side2_stream : C.st[1];   // image-branch index ops (index2uv + 2-D rulebooks)
     C.err = err_flag;
-    const bool two = C.st[0] != C.st[1];
+    C.proj = proj_params; C.caps = caps; C.overflow = overflow_flag; C.pinned = pinned_host;
+    C.do_idx = phase != 2; C.do_feat = phase != 1; C.two = C.st[0] != C.st[1];
+    plan_step(C, c0, precision, training);
+
+    VC_TRY(ev_init());
     g_ev_next = 0;
-
-    S->iset[0].idx = const_cast<int32_t*>(idx0); S->iset[0].n = n0; S->iset[0].ndim = 3; S->iset[0].n_dev = n0_dev;
-    for (int d = 0; d < 3; ++d) S->iset[0].shape[d] = shape0[d];
-    S->f[0].f32 = const_cast<float*>(feats0); S->f[0].rows = n0; S->f[0].c = c0; S->f[0].ld = c0; S->f[0].n_dev = n0_dev;
-
-    // rulebook meta known from the plan alone (needed to choose the dgrad weight images)
-    int rb_subm[MAX_RB] = {0}, rb_unique[MAX_RB] = {0}, rb_K[MAX_RB] = {0};
-    for (int i = 0; i < n_ops; ++i) {
-        const int* o = C.op(i);
-        if (o[F_KIND] == OP_SUBM_RB || o[F_KIND] == OP_CONV_RB) {
-            int K = 1;
-            for (int d = 0; d < o[F_NDIM]; ++d) K *= o[F_KS + d];
-            rb_K[o[F_C]] = K;
-            rb_subm[o[F_C]] = o[F_KIND] == OP_SUBM_RB;
-            rb_unique[o[F_C]] = o[F_KIND] == OP_CONV_RB ? 1 : o[F_X0];
-        }
-    }
-
-    // Which feature slots need an fp32 copy: published ones (x1 of the producing op), the input of a layer without the
-    // tensor-core forward + wgrad pair (fp32 conv or fp32 wgrad), and the fp32 precision mode.  Everything else is read as
-    // bf16 only, so its fp32 copy is not written.  A concat whose inputs need no fp32 copy of their own is built in place:
-    // the BN-apply of each input layer writes its column slice of the concat (fp32 if the concat needs it, and bf16), and
-    // the concat op launches nothing.
-    bool need_f32[MAX_F] = {false};
-    int slot_c[MAX_F] = {0}, cat_out[MAX_F], cat_col[MAX_F] = {0};
-    bool cat_inplace[MAX_OPS] = {false};
-    for (int i = 0; i < MAX_F; ++i) cat_out[i] = -1;
-    slot_c[0] = c0;
-    need_f32[0] = true;
-    for (int i = 0; i < n_ops; ++i) {
-        const int* o = C.op(i);
-        if (o[F_KIND] == OP_CBR) {
-            slot_c[o[F_B]] = o[F_COUT];
-            const bool tc = precision == 1 && tc2_ch_ok(o[F_CIN]) && tc2_ch_ok(o[F_COUT]);
-            if (precision == 0 || o[F_X1]) need_f32[o[F_B]] = true;
-            if (!(training && tc)) need_f32[o[F_A]] = true;
-        } else if (o[F_KIND] == OP_CAT) {
-            slot_c[o[F_C]] = slot_c[o[F_A]] + slot_c[o[F_B]];
-            if (precision == 0 || o[F_X1]) need_f32[o[F_C]] = true;
-        }
-    }
-    for (int i = 0; i < n_ops; ++i) {
-        const int* o = C.op(i);
-        if (o[F_KIND] != OP_CAT) continue;
-        const int a = o[F_A], b = o[F_B];
-        cat_inplace[i] = precision == 1 && a != 0 && b != 0 && a != b && !need_f32[a] && !need_f32[b] && cat_out[a] < 0 && cat_out[b] < 0;
-        if (cat_inplace[i]) {
-            cat_out[a] = cat_out[b] = o[F_C];
-            cat_col[b] = slot_c[a];
-        } else {
-            need_f32[a] = need_f32[b] = true;
-        }
-    }
-
     // BatchNorm accumulators + tile-scheduler counters (+ the wgrad accumulators of a training step) of every layer: one
     // region, one memset
-    size_t sums_doubles = 0, n_cbr = 0, wg_floats = 0;
-    for (int i = 0; i < n_ops; ++i)
-        if (C.op(i)[F_KIND] == OP_CBR) {
-            const int* o = C.op(i);
-            sums_doubles += 4 * (size_t)o[F_COUT];
-            ++n_cbr;
-            if (training && precision == 1 && tc2_ch_ok(o[F_CIN]) && tc2_ch_ok(o[F_COUT]))
-                wg_floats += ((size_t)rb_K[o[F_C]] * o[F_CIN] * o[F_COUT] + 63) / 64 * 64;
-        }
-    const size_t zero_bytes = sums_doubles * 8 + n_cbr * CTR_PER_LAYER * sizeof(int) + wg_floats * 4;
+    const size_t zero_bytes = C.sums_doubles * 8 + C.n_cbr * CTR_PER_LAYER * sizeof(int) + C.wg_floats * 4;
     VC_ALLOC(sums_all, double*, zero_bytes);
-    int* ctr_all = reinterpret_cast<int*>(sums_all + sums_doubles);
-    float* wg_all = reinterpret_cast<float*>(ctr_all + n_cbr * CTR_PER_LAYER);
-    if (zero_bytes && do_feat) VC_CUDA(cudaMemsetAsync(sums_all, 0, zero_bytes, C.st[0]));
-    size_t wg_cur = 0;
-    size_t sums_cur = 0, ctr_cur = 0;
+    int* ctr_all = reinterpret_cast<int*>(sums_all + C.sums_doubles);
+    float* wg_all = reinterpret_cast<float*>(ctr_all + C.n_cbr * CTR_PER_LAYER);
+    if (zero_bytes && C.do_feat) VC_CUDA(cudaMemsetAsync(sums_all, 0, zero_bytes, C.st[0]));
 
     // tensor-core weight images of every layer, one launch
+    TcPrepTable T;
+    T.n = 0;
     for (int i = 0; i < n_ops; ++i) {
         const int* o = C.op(i);
         if (o[F_KIND] != OP_CBR) continue;
         Layer& L = S->layer[o[F_LAYER]];
-        L.cin = o[F_CIN]; L.cout = o[F_COUT]; L.in_slot = o[F_A]; L.out_slot = o[F_B]; L.rb = o[F_C];
-        L.need_dgrad = o[F_X0];
-        L.use_tc = precision == 1 && tc2_ch_ok(L.cin) && tc2_ch_ok(L.cout);
-        L.use_tc_scatter = precision == 1 && tc_scatter_ch_ok(L.cin) && tc_scatter_ch_ok(L.cout);
-        L.sums = sums_all + sums_cur;
-        sums_cur += 4 * (size_t)L.cout;
-        L.tile_ctr = ctr_all + CTR_PER_LAYER * ctr_cur++;
-        L.wscratch = nullptr;
-        if (training && L.use_tc) {
-            L.wscratch = wg_all + wg_cur;
-            wg_cur += ((size_t)rb_K[L.rb] * L.cin * L.cout + 63) / 64 * 64;
-        }
-    }
-    if (precision == 1) {
-        TcPrepTable T;
-        T.n = 0;
-        for (int i = 0; i < n_ops; ++i) {
-            const int* o = C.op(i);
-            if (o[F_KIND] != OP_CBR) continue;
-            Layer& L = S->layer[o[F_LAYER]];
-            if (!L.use_tc) continue;
-            const int K = rb_K[L.rb];
-            // dgrad image: mirrored for a submanifold table used as its own transpose, plain for a strided conv's
-            // nbr_bwd table and for the many-to-one image-branch table (tensor-core scatter, image layout 0)
-            const bool many_to_one = rb_subm[L.rb] && !rb_unique[L.rb];
-            const bool dgrad_tc = training && L.need_dgrad && (!many_to_one || L.use_tc_scatter);
-            for (int mode = 0; mode < (dgrad_tc ? 2 : 1); ++mode) {
-                const int layout = (mode == 1 && many_to_one) ? 0 : 1;
-                VC_ALLOC(img, void*, tc_image_bytes(L.cin, L.cout, K, layout));
-                (mode == 0 ? L.wimg_fwd : L.wimg_dgrad) = img;
-                if (T.n == TC_PREP_MAX) {
-                    if (do_feat) VC_TRY(tc_prep_images(T, C.st[0]));
-                    T.n = 0;
-                }
-                TcPrepEntry& e = T.e[T.n++];
-                e.w = C.P<const float>(o[F_LAYER], P_W); e.img = img; e.cin = L.cin; e.cout = L.cout; e.K = K; e.mode = mode;
-                e.mirror = mode == 1 && rb_subm[L.rb] && !many_to_one;
-                e.layout = layout;
+        const RBk& R = S->rb[L.rb];
+        L.sums = sums_all;
+        sums_all += 4 * (size_t)L.cout;
+        L.tile_ctr = ctr_all;
+        ctr_all += CTR_PER_LAYER;
+        L.wscratch = L.wgrad == K_WGRAD_TC ? wg_all : nullptr;
+        wg_all += wgrad_acc_floats(L, R.K);
+        // dgrad image: mirrored for a submanifold table used as its own transpose, plain for a strided conv's nbr_bwd table
+        // (gather dgrad), layout 0 for the many-to-one image-branch table (tensor-core scatter)
+        const int n_img = L.fwd != K_FWD_TC ? 0 : (L.dgrad == K_DGRAD_TC || L.dgrad == K_DGRAD_SCATTER_TC) ? 2 : 1;
+        for (int mode = 0; mode < n_img; ++mode) {
+            const int layout = (mode == 1 && L.dgrad == K_DGRAD_SCATTER_TC) ? 0 : 1;
+            VC_ALLOC(img, void*, tc_image_bytes(L.cin, L.cout, R.K, layout));
+            (mode == 0 ? L.wimg_fwd : L.wimg_dgrad) = img;
+            if (T.n == TC_PREP_MAX) {
+                if (C.do_feat) VC_TRY(tc_prep_images(T, C.st[0]));
+                T.n = 0;
             }
+            TcPrepEntry& e = T.e[T.n++];
+            e.w = C.P<const float>(o[F_LAYER], P_W); e.img = img; e.cin = L.cin; e.cout = L.cout; e.K = R.K; e.mode = mode;
+            e.mirror = mode == 1 && L.dgrad == K_DGRAD_TC && R.subm;
+            e.layout = layout;
         }
-        if (do_feat) VC_TRY(tc_prep_images(T, C.st[0]));
     }
+    if (C.do_feat) VC_TRY(tc_prep_images(T, C.st[0]));
 
     // the side stream starts after everything already queued on main (the caller's inputs) — unless the caller vouches
     // that idx0 / proj_params are already valid for the side stream and the arena is safe to write from it
     // (side_waits_main = 0): the index pipeline of this step then overlaps whatever main is still running (the
     // previous step's backward)
-    if (two && side_waits_main) {
+    if (C.two && side_waits_main) {
         int e = record_on(C, 0);
         if (e >= 0) {
             VC_CUDA(cudaStreamWaitEvent(C.st[1], g_ev[e], 0));
             if (C.st[2] != C.st[1]) VC_CUDA(cudaStreamWaitEvent(C.st[2], g_ev[e], 0));
         }
     }
-    int last_ev[3] = {-1, -1, -1};     // latest event of each side stream (joined into main at the end)
-    auto side_ev = [&](int s_) -> int {
-        if (s_ == 0) return -1;
-        return last_ev[s_] = record_on(C, s_);
-    };
-    int n_syncs = 0;
-    static thread_local void* chain_ws[MAX_OPS];
-    static thread_local size_t chain_wsb[MAX_OPS];
-    static thread_local bool chain_done[MAX_OPS];
-    for (int i = 0; i < n_ops; ++i) chain_done[i] = false;
-    // count + row-count read-back + output indices of strided conv op j (its input index set must exist)
-    auto count_emit = [&](int j) -> int {
-        const int* o = C.op(j);
-        const int s = two ? o[F_STREAM] : 0;
-        cudaStream_t st = C.st[s];
-        ISet& I = S->iset[o[F_A]];
-        ISet& O = S->iset[o[F_B]];
-        RBk& R = S->rb[o[F_C]];
-        VC_CHECK_ARG(I.ndim == o[F_NDIM], "op %d: index set %d has the wrong ndim", j, o[F_A]);
-        VC_TRY(wait_for(C, I.ev, I.prod, s));
-        int32_t oshape[3] = {0, 0, 0};
-        VC_TRY(vc_conv_out_shape(I.ndim, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL, oshape));
-        const size_t wsb = vc_conv_rulebook_ws_bytes(I.ndim, batch_size, oshape);
-        VC_ALLOC(ws, void*, wsb);
-        VC_ALLOC(n_dev, int32_t*, 4);
-        int n_out;
-        if (is_static) {
-            n_out = caps[o[F_B]];
-            VC_CHECK_ARG(n_out > 0, "op %d: static mode needs a capacity for index set %d", j, o[F_B]);
-            if (do_idx)
-                VC_TRY(conv_rulebook_count_dev(I.idx, I.n, I.n_dev, I.ndim, batch_size, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL,
-                                               n_dev, n_out, overflow_flag, ws, wsb, st));
-        } else {
-            VC_TRY(conv_rulebook_count_dev(I.idx, I.n, nullptr, I.ndim, batch_size, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL,
-                                           n_dev, 0, nullptr, ws, wsb, st));
-            VC_CUDA(cudaMemcpyAsync(pinned_host + (n_syncs & 7), n_dev, 4, cudaMemcpyDeviceToHost, st));
-            // the tensor-core kernels' pipeline-timeout flag rides along with the first read-back of a step (it reports on the
-            // kernels of EARLIER steps: a wedged mbarrier wait must not go unnoticed in production — ADVICE r1)
-            if (n_syncs == 0 && C.err != nullptr) VC_CUDA(cudaMemcpyAsync(pinned_host + 15, C.err, 4, cudaMemcpyDeviceToHost, st));
-            VC_CUDA(cudaStreamSynchronize(st));        // the one data-dependent size per strided conv
-            n_out = pinned_host[n_syncs & 7];
-            if (n_syncs == 0 && C.err != nullptr && pinned_host[15] != 0) {
-                set_error("a tensor-core kernel's pipeline wait timed out in an earlier step (error flag %d): its results are invalid",
-                          pinned_host[15]);
-                return VC_ERR_PIPELINE;
-            }
-            ++n_syncs;
-        }
-        R.K = rb_K[o[F_C]]; R.n_in = I.n; R.n_out = n_out; R.subm = 0; R.unique = 1;
-        R.n_in_dev = I.n_dev; R.n_out_dev = is_static ? n_dev : nullptr;
-        O.n = n_out; O.ndim = I.ndim; O.n_dev = R.n_out_dev;
-        for (int d = 0; d < 3; ++d) O.shape[d] = oshape[d];
-        VC_ALLOC(oidx, int32_t*, (size_t)(n_out > 0 ? n_out : 1) * (1 + I.ndim) * 4);
-        O.idx = oidx;
-        if (is_static && do_idx) VC_CUDA(cudaMemsetAsync(oidx, 0xFF, (size_t)n_out * (1 + I.ndim) * 4, st));   // defined tail (-1) for the published indices
-        if (do_idx)
-            VC_TRY(conv_rulebook_fill_phases(I.idx, I.n, I.n_dev, I.ndim, batch_size, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL, n_out, O.idx,
-                                             nullptr, nullptr, nullptr, ws, wsb, st, 1));
-        O.prod = s;
-        O.ev = side_ev(s);
-        chain_ws[j] = ws; chain_wsb[j] = wsb; chain_done[j] = true;
-        return VC_OK;
-    };
-
     for (int i = 0; i < n_ops; ++i) {
         const int* o = C.op(i);
-        const float* fo = C.of + (size_t)i * OPF;
-        const int s = two ? o[F_STREAM] : 0;
-        cudaStream_t st = C.st[s];
+        const int s = C.two ? o[F_STREAM] : 0;
         switch (o[F_KIND]) {
-            case OP_SUBM_RB: {
-                ISet& I = S->iset[o[F_A]];
-                RBk& R = S->rb[o[F_C]];
-                VC_CHECK_ARG(I.idx && I.ndim == o[F_NDIM], "op %d: index set %d not built / wrong ndim", i, o[F_A]);
-                VC_TRY(wait_for(C, I.ev, I.prod, s));
-                R.K = rb_K[o[F_C]]; R.n_in = R.n_out = I.n; R.subm = 1; R.unique = o[F_X0];
-                R.n_in_dev = R.n_out_dev = I.n_dev;
-                VC_ALLOC(nbr, int32_t*, (size_t)R.K * I.n * 4);
-                R.nbr = nbr;
-                if (want_pair_num) {
-                    VC_ALLOC(pn, int32_t*, (size_t)R.K * 4);
-                    R.pair_num = pn;
-                }
-                const size_t wsb = vc_subm_rulebook_ws_bytes(I.n);
-                VC_ALLOC(ws, void*, wsb);
-                if (do_idx) VC_TRY(subm_rulebook_dev(I.idx, I.n, I.n_dev, I.ndim, batch_size, I.shape, o + F_KS, o + F_DL, R.nbr, R.pair_num, ws, wsb, st));
-                R.prod = s;
-                R.ev = side_ev(s);
-                break;
-            }
-            case OP_CONV_RB: {
-                // First strided conv reached: run the count -> (host reads the row count) -> emit-indices chain of EVERY
-                // strided conv of the plan now, back to back.  Each link only needs the previous link's output indices,
-                // and it is the only part of the forward the host has to wait for; the neighbour tables, submanifold
-                // rulebooks and projections queue up behind it without further synchronisation.
-                if (!chain_done[i]) {
-                    if (is_static) {
-                        // no host read to wait for: keep the natural order (count -> indices -> tables per stage), so the
-                        // tables of an early stage are not queued behind the counting kernels of all later ones
-                        VC_TRY(count_emit(i));
-                    } else {
-                        for (int j = i; j < n_ops; ++j)
-                            if (C.op(j)[F_KIND] == OP_CONV_RB && S->iset[C.op(j)[F_A]].idx) VC_TRY(count_emit(j));
-                    }
-                }
-                VC_CHECK_ARG(chain_done[i], "op %d: index set %d not built", i, o[F_A]);
-                ISet& I = S->iset[o[F_A]];
-                ISet& O = S->iset[o[F_B]];
-                RBk& R = S->rb[o[F_C]];
-                VC_TRY(wait_for(C, I.ev, I.prod, s));
-                VC_TRY(wait_for(C, O.ev, O.prod, s));
-                VC_ALLOC(nbr, int32_t*, (size_t)R.K * (R.n_out > 0 ? R.n_out : 1) * 4);
-                VC_ALLOC(nbr_bwd, int32_t*, (size_t)R.K * I.n * 4);
-                R.nbr = nbr; R.nbr_bwd = nbr_bwd;
-                if (want_pair_num) {
-                    VC_ALLOC(pn, int32_t*, (size_t)R.K * 4);
-                    R.pair_num = pn;
-                }
-                if (do_idx)
-                    VC_TRY(conv_rulebook_fill_phases(I.idx, I.n, I.n_dev, I.ndim, batch_size, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL,
-                                                     R.n_out, O.idx, R.nbr, R.nbr_bwd, R.pair_num, chain_ws[i], chain_wsb[i], st, 2));
-                R.prod = s;
-                R.ev = side_ev(s);
-                break;
-            }
-            case OP_INDEX2UV: {
-                ISet& I = S->iset[o[F_A]];
-                ISet& O = S->iset[o[F_B]];
-                VC_CHECK_ARG(I.idx && I.ndim == 3 && proj_params, "op %d: index2uv needs a built 3-D index set and projection params", i);
-                VC_TRY(wait_for(C, I.ev, I.prod, s));
-                VC_ALLOC(uv, int32_t*, (size_t)I.n * 3 * 4);
-                O.idx = uv; O.n = I.n; O.ndim = 2; O.shape[0] = o[F_KS]; O.shape[1] = o[F_KS + 1]; O.shape[2] = 0; O.n_dev = I.n_dev;
-                if (do_idx) VC_TRY(index2uv_dev(I.idx, I.n, I.n_dev, batch_size, proj_params, fo, o[F_X0], o[F_X1], o[F_X2], uv, st));
-                O.prod = s;
-                O.ev = side_ev(s);
-                break;
-            }
-            case OP_CBR: {
-                const int li = o[F_LAYER];
-                Layer& L = S->layer[li];
-                FSlot& X = S->f[L.in_slot];
-                FSlot& Y = S->f[L.out_slot];
-                RBk& R = S->rb[L.rb];
-                VC_CHECK_ARG((X.f32 || X.bf16) && R.nbr && X.c == L.cin && X.rows == R.n_in,
-                             "op %d: input slot / rulebook mismatch (rows %d vs %d, c %d vs %d)", i, X.rows, R.n_in, X.c, L.cin);
-                VC_TRY(wait_for(C, R.ev, R.prod, s));
-                VC_TRY(wait_for(C, X.ev, X.prod, s));
-                const size_t elems = (size_t)R.n_out * L.cout;
-                VC_ALLOC(x, float*, elems * 4);
-                VC_ALLOC(stats, float*, (size_t)4 * L.cout * 4);
-                float* y = nullptr;
-                void* yb = nullptr;
-                int y_ld = L.cout;
-                if (cat_out[L.out_slot] >= 0) {   // a column slice of an in-place concat (allocated by its first input)
-                    FSlot& O = S->f[cat_out[L.out_slot]];
-                    if (O.bf16 == nullptr) {
-                        O.rows = R.n_out; O.c = O.ld = slot_c[cat_out[L.out_slot]];
-                        if (need_f32[cat_out[L.out_slot]]) {
-                            VC_ALLOC(of_, float*, (size_t)O.rows * O.c * 4);
-                            O.f32 = of_;
-                        }
-                        VC_ALLOC(ob_, void*, (size_t)O.rows * O.c * 2);
-                        O.bf16 = ob_;
-                    }
-                    VC_CHECK_ARG(O.rows == R.n_out, "op %d: concat inputs with different row counts", i);
-                    y_ld = O.ld;
-                    if (O.f32) y = O.f32 + cat_col[L.out_slot];
-                    yb = (__nv_bfloat16*)O.bf16 + cat_col[L.out_slot];
-                } else {
-                    if (need_f32[L.out_slot]) {
-                        VC_ALLOC(y_, float*, elems * 4);
-                        y = y_;
-                    }
-                    if (precision == 1) {
-                        VC_ALLOC(yb_, void*, elems * 2);
-                        yb = yb_;
-                    }
-                }
-                L.x = x; L.y = y; L.stats = stats;
-                double* sums = training ? L.sums : nullptr;
-                if (L.use_tc && R.n_out > 0) {
-                    if (!X.bf16) {   // no producer wrote a shadow (network input): cast once
-                        VC_CHECK_ARG(X.ld == X.c, "op %d: no bf16 copy of a strided input", i);
-                        VC_ALLOC(xb, void*, (size_t)X.rows * X.c * 2);
-                        if (do_feat) VC_TRY(vc_cast_f32_bf16(X.f32, xb, (long long)X.rows * X.c, st));
-                        X.bf16 = xb;
-                    }
-                    Timed t(1, li, st);
-                    // (flag bit 1: the rulebook was built on another stream and joined by an event, so the kernel may load its first
-                    //  table slices before its griddepcontrol.wait — conv_tc2.cu)
-                    if (do_feat)
-                        VC_TRY(tc2_conv(L.cin, L.cout, X.bf16, L.wimg_fwd, R.nbr, R.n_out, x, R.n_out, R.n_out_dev, R.K, sums, C.err, st,
-                                        nullptr, L.tile_ctr, (phase == 2 || C.st[R.prod] != C.st[s]) ? 2 : 0, X.ld));
-                } else {
-                    const size_t wsb = vc_conv_ws_bytes(L.cin, L.cout, R.K);
-                    VC_ALLOC(ws, void*, wsb);
-                    VC_CHECK_ARG(X.f32 && X.ld == X.c, "op %d: the fp32 conv needs a dense fp32 input", i);
-                    Timed t(0, li, st);
-                    if (do_feat) VC_TRY(vc_conv_fwd_f32(X.f32, C.P<const float>(li, P_W), R.nbr, x, R.n_out, L.cin, L.cout, R.K, sums, ws, wsb, st));
-                }
-                if (do_feat)
-                    VC_TRY(bn_apply_relu_dev(x, L.sums, R.n_out, R.n_out_dev, L.cout, C.P<const float>(li, P_GAMMA), C.P<const float>(li, P_BETA),
-                                             C.P<float>(li, P_RM), C.P<float>(li, P_RV), C.P<long long>(li, P_NBT), C.lf[2 * li + 1],
-                                             C.lf[2 * li], training, y, y_ld, yb, y_ld, stats, 1, is_static, st));
-                Y.f32 = y; Y.bf16 = yb; Y.rows = R.n_out; Y.c = L.cout; Y.ld = y_ld; Y.prod = s; Y.n_dev = R.n_out_dev;
-                Y.ev = side_ev(s);
-                break;
-            }
-            case OP_CAT: {
-                FSlot& Aa = S->f[o[F_A]];
-                FSlot& Bb = S->f[o[F_B]];
-                FSlot& O = S->f[o[F_C]];
-                VC_TRY(wait_for(C, Aa.ev, Aa.prod, s));
-                VC_TRY(wait_for(C, Bb.ev, Bb.prod, s));
-                if (cat_inplace[i]) {   // both halves are already written (OP_CBR): nothing to launch
-                    VC_CHECK_ARG(Aa.bf16 && Bb.bf16 && Aa.rows == Bb.rows && O.bf16, "op %d: concat inputs not built / row mismatch", i);
-                    O.prod = s; O.n_dev = Aa.n_dev;
-                    O.ev = side_ev(s);
-                    break;
-                }
-                VC_CHECK_ARG(Aa.f32 && Bb.f32 && Aa.ld == Aa.c && Bb.ld == Bb.c && Aa.rows == Bb.rows,
-                             "op %d: concat inputs not built / row mismatch", i);
-                const size_t elems = (size_t)Aa.rows * (Aa.c + Bb.c);
-                VC_ALLOC(out, float*, elems * 4);
-                void* ob = nullptr;
-                if (precision == 1) {
-                    VC_ALLOC(ob_, void*, elems * 2);
-                    ob = ob_;
-                }
-                if (do_feat) VC_TRY(cat2_dev(Aa.f32, Bb.f32, out, ob, Aa.rows, Aa.n_dev, Aa.c, Bb.c, st));
-                O.f32 = out; O.bf16 = ob; O.rows = Aa.rows; O.c = O.ld = Aa.c + Bb.c; O.prod = s; O.n_dev = Aa.n_dev;
-                O.ev = side_ev(s);
-                break;
-            }
+            case OP_SUBM_RB: VC_TRY(fwd_subm_rb(C, i, o, s)); break;
+            case OP_CONV_RB: VC_TRY(fwd_conv_rb(C, i, o, s)); break;
+            case OP_INDEX2UV: VC_TRY(fwd_index2uv(C, i, o, s)); break;
+            case OP_CBR: VC_TRY(fwd_cbr(C, i, o, s)); break;
+            case OP_CAT: VC_TRY(fwd_cat(C, i, o, s)); break;
         }
     }
-    for (int s_ = 1; s_ <= 2; ++s_)
-        if (two && last_ev[s_] >= 0) VC_CUDA(cudaStreamWaitEvent(C.st[0], g_ev[last_ev[s_]], 0));   // join
+    for (int s = 1; s <= 2; ++s)
+        if (C.two && C.last_ev[s] >= 0) VC_CUDA(cudaStreamWaitEvent(C.st[0], g_ev[C.last_ev[s]], 0));   // join
     S->used = C.A.used;
     S->magic = STATE_MAGIC;
     return VC_OK;
@@ -891,10 +893,8 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
         }
         const size_t elems = (size_t)R.n_out * L.cout;
         // the fp32 input gradient is read by the fp32 wgrad and the fp32 dgrads only (the tensor-core ones read dxb)
-        const bool dgrad = L.need_dgrad && L.in_slot != 0;
-        const bool tc_dgrad = L.wimg_dgrad && ((R.subm && !R.unique) ? L.use_tc_scatter : L.use_tc);
         float* dx = nullptr;
-        if (L.wscratch == nullptr || (dgrad && !tc_dgrad)) {
+        if (L.wgrad == K_WGRAD_F32 || L.dgrad == K_DGRAD_F32 || L.dgrad == K_DGRAD_SCATTER_F32) {
             VC_ALLOC(t, float*, elems * 4);
             dx = t;
         }
@@ -910,8 +910,8 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
             int e = record_on(C, 0);
             if (e >= 0) VC_CUDA(cudaStreamWaitEvent(wst, g_ev[e], 0));
         }
-        if (L.wscratch != nullptr) {
-            Timed t(6, li, wst);
+        if (L.wgrad == K_WGRAD_TC) {
+            Timed t(L.wgrad, li, wst);
             VC_TRY(tc3_wgrad(L.cin, L.cout, X.bf16, dxb, R.nbr, R.n_out, L.wscratch, R.n_out, R.n_out_dev, R.K, C.err, wst,
                              L.tile_ctr + 2, wgrad_ctas, X.ld));
             if (fin.n == WGRAD_FIN_MAX) {
@@ -924,40 +924,46 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
             const size_t wsb = vc_conv_wgrad_ws_bytes(R.n_out, L.cin, L.cout, R.K);
             VC_ALLOC(ws, void*, wsb);
             VC_CHECK_ARG(X.f32 && X.ld == X.c, "layer %d: the fp32 wgrad needs a dense fp32 input", li);
-            Timed t(5, li, wst);
+            Timed t(L.wgrad, li, wst);
             VC_TRY(vc_conv_wgrad_f32(X.f32, dx, R.nbr, dw, R.n_out, L.cin, L.cout, R.K, ws, wsb, wst));
         }
         if (two) last_w_ev = record_on(C, 1);
         // dgrad
-        if (!dgrad) continue;
-        if (R.subm && !R.unique && L.use_tc_scatter && L.wimg_dgrad) {
-            VC_TRY(contribute_scatter(C, X, st, [&](float* dst, int ld) -> int {
-                Timed t(7, li, st);
-                return tc_scatter_with_image(L.cout, L.cin, dxb, L.wimg_dgrad, R.nbr, dst, R.n_out, R.K, C.err, st, ld);
-            }));
-        } else if (R.subm && !R.unique) {
-            const size_t wsb = vc_conv_ws_bytes(L.cin, L.cout, R.K);
-            VC_ALLOC(ws, void*, wsb);
-            VC_TRY(contribute_scatter(C, X, st, [&](float* dst, int ld) -> int {
-                Timed t(4, li, st);
-                return conv_dgrad_scatter_f32_ld(dx, C.P<const float>(li, P_W), R.nbr, dst, ld, R.n_out, L.cin, L.cout, R.K, ws, wsb, st);
-            }));
-        } else if (L.use_tc && L.wimg_dgrad) {
-            const int32_t* table = R.subm ? R.nbr : R.nbr_bwd;
-            VC_TRY(contribute_fused(C, X, [&](float* dst, const float* addend) -> int {
-                Timed t(3, li, st);
-                return tc2_conv(L.cout, L.cin, dxb, L.wimg_dgrad, table, R.n_in, dst, R.n_in, R.n_in_dev, R.K, nullptr, C.err, st,
-                                addend, L.tile_ctr + 1, (R.subm ? 0 : 1) | 2);      // (tables from the forward call: early loads allowed)
-            }));
-        } else {
-            const size_t wsb = vc_conv_ws_bytes(L.cin, L.cout, R.K);
-            VC_ALLOC(ws, void*, wsb);
-            const int32_t* table = R.subm ? R.nbr : R.nbr_bwd;
-            VC_TRY(contribute(C, X, st, [&](float* dst) -> int {
-                Timed t(2, li, st);
-                return vc_conv_dgrad_f32(dx, C.P<const float>(li, P_W), table, dst, R.n_in, L.cin, L.cout, R.K, R.subm ? 1 : 0, ws, wsb,
-                                         st);
-            }));
+        const int32_t* table = R.subm ? R.nbr : R.nbr_bwd;
+        const size_t wsb = vc_conv_ws_bytes(L.cin, L.cout, R.K);
+        void* ws = nullptr;   // the fp32 dgrads' workspace
+        if (L.dgrad == K_DGRAD_F32 || L.dgrad == K_DGRAD_SCATTER_F32) {
+            VC_ALLOC(t, void*, wsb);
+            ws = t;
+        }
+        switch (L.dgrad) {
+            case K_DGRAD_SCATTER_TC:
+                VC_TRY(contribute_scatter(C, X, st, [&](float* dst, int ld) -> int {
+                    Timed t(L.dgrad, li, st);
+                    return tc_scatter_with_image(L.cout, L.cin, dxb, L.wimg_dgrad, R.nbr, dst, R.n_out, R.K, C.err, st, ld);
+                }));
+                break;
+            case K_DGRAD_SCATTER_F32:
+                VC_TRY(contribute_scatter(C, X, st, [&](float* dst, int ld) -> int {
+                    Timed t(L.dgrad, li, st);
+                    return conv_dgrad_scatter_f32_ld(dx, C.P<const float>(li, P_W), R.nbr, dst, ld, R.n_out, L.cin, L.cout, R.K, ws, wsb, st);
+                }));
+                break;
+            case K_DGRAD_TC:
+                VC_TRY(contribute_fused(C, X, [&](float* dst, const float* addend) -> int {
+                    Timed t(L.dgrad, li, st);
+                    return tc2_conv(L.cout, L.cin, dxb, L.wimg_dgrad, table, R.n_in, dst, R.n_in, R.n_in_dev, R.K, nullptr, C.err, st,
+                                    addend, L.tile_ctr + 1, (R.subm ? 0 : 1) | 2);      // (tables from the forward call: early loads allowed)
+                }));
+                break;
+            case K_DGRAD_F32:
+                VC_TRY(contribute(C, X, st, [&](float* dst) -> int {
+                    Timed t(L.dgrad, li, st);
+                    return vc_conv_dgrad_f32(dx, C.P<const float>(li, P_W), table, dst, R.n_in, L.cin, L.cout, R.K, R.subm ? 1 : 0, ws,
+                                             wsb, st);
+                }));
+                break;
+            default: break;   // K_NONE
         }
     }
     if (fin.n > 0) {

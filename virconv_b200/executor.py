@@ -41,6 +41,7 @@ LAST_RUN = None                    # the most recent forward's record while TIMI
 OP_SUBM_RB, OP_CONV_RB, OP_INDEX2UV, OP_CBR, OP_CAT = 1, 2, 3, 4, 5
 VC_ERR_WORKSPACE = -3
 OPI, OPF, PCOLS = 24, 8, 9
+# the timing records' kinds: enum ConvKind of csrc/executor.cu
 KIND_NAMES = {0: 'conv_fwd', 1: 'conv_fwd_tc', 2: 'conv_dgrad', 3: 'conv_dgrad_tc', 4: 'conv_dgrad_scatter',
               5: 'conv_wgrad', 6: 'conv_wgrad_tc', 7: 'conv_dgrad_scatter_tc'}
 
@@ -442,32 +443,46 @@ class StaticSpec:
         return self._arr
 
 
+def _index_streams(dev, inputs_ready=False):
+    """(side, side2) index streams of vc_exec_forward, None to share the previous one.  No side2 (image branch) with
+    `inputs_ready`: the index streams then do not wait for main, and the arena is registered with ONE side stream."""
+    side = ops.side(dev).stream if TWO_STREAMS else None
+    return side, (ops.side2(dev) if (side is not None and THREE_STREAMS and not inputs_ready) else None)
+
+
+def _exec_forward(plan, feats, coords, spatial_shape, batch_size, proj, training, precision, static, arena, side, side2,
+                  side_waits_main):
+    """One vc_exec_forward call (only one phase where static.phase says so) -> (return code, state blob)."""
+    oi, of, lf, _, _ = plan.finalize()
+    tab, lib, dev = _layer_ptrs(plan), _lib.load(), feats.device
+    state = np.zeros(lib.vc_exec_state_bytes(), dtype=np.uint8)
+    return lib.vc_exec_forward(
+        oi.ctypes.data, of.ctypes.data, oi.shape[0], tab.ctypes.data, lf.ctypes.data, len(plan.layers), feats.data_ptr(),
+        feats.shape[1], coords.data_ptr(), feats.shape[0], _lib.host_i32(spatial_shape), int(batch_size),
+        proj.data_ptr() if proj is not None else None, int(training), int(precision == 'bf16'),
+        1 | ((static.phase if static is not None else 0) << 8), arena.data_ptr(), arena.numel(), _pinned(dev).data_ptr(),
+        ops.tc_error_flag(dev).data_ptr(), state.ctypes.data, state.size, ops._stream(),
+        side.cuda_stream if side is not None else None, int(side_waits_main),
+        static.caps_array().ctypes.data if static is not None else None, static.n_dev.data_ptr() if static is not None else None,
+        static.overflow.data_ptr() if static is not None else None, side2.cuda_stream if side2 is not None else None), state
+
+
 class PlanFn(torch.autograd.Function):
     """forward: (features of the published slots..., ) ; backward: gradients of every layer's weight / gamma / beta."""
 
     @staticmethod
     def forward(ctx, plan, holder, feats, coords, spatial_shape, batch_size, proj, training, precision, inputs_ready, static,
                 with_bwd, *params):
-        lib = _lib.load()
         ctx.set_materialize_grads(False)     # published tensors the loss does not touch arrive as None, not as zeros
         dev = feats.device
-        oi, of, lf, sizes, offs = plan.finalize()
         feats = feats.contiguous()
         n0 = feats.shape[0]
-        main = ops._stream()
-        side_obj = ops.side(dev).stream if TWO_STREAMS else None
-        side = side_obj.cuda_stream if side_obj is not None else None
-        # second index stream (image-branch projection + 2-D rulebooks).  Only where the call's own fork / join orders it
-        # (static mode, or inputs the side streams must wait for anyway): with `inputs_ready` the index streams do not wait
-        # for main, and the arena / coordinate tensors are only registered with ONE side stream
-        side2_obj = ops.side2(dev) if (side_obj is not None and THREE_STREAMS and not inputs_ready) else None
-        side2 = side2_obj.cuda_stream if side2_obj is not None else None
+        side_obj, side2_obj = _index_streams(dev, inputs_ready)
         inflight = None
         if static is not None:
             inputs_ready = False             # under capture the side stream must fork from the capturing stream
         else:
             inflight = _throttle(plan, dev)
-        tab = _layer_ptrs(plan)
         for attempt in range(3):
             nbytes = _arena_bytes(plan, n0, dev, with_bwd)
             if static is not None and static.arena is not None:
@@ -485,17 +500,8 @@ class PlanFn(torch.autograd.Function):
                 arena.record_stream(torch.cuda.current_stream(dev))
             else:
                 arena = _alloc_arena(plan, nbytes, dev, None)
-            state = np.zeros(lib.vc_exec_state_bytes(), dtype=np.uint8)
-            rc = lib.vc_exec_forward(oi.ctypes.data, of.ctypes.data, oi.shape[0], tab.ctypes.data, lf.ctypes.data, len(plan.layers),
-                                     feats.data_ptr(), feats.shape[1], coords.data_ptr(), n0, _lib.host_i32(spatial_shape),
-                                     int(batch_size), proj.data_ptr() if proj is not None else None, int(training),
-                                     int(precision == 'bf16'), 1 | ((static.phase if static is not None else 0) << 8), arena.data_ptr(),
-                                     arena.numel(),
-                                     _pinned(dev).data_ptr(), ops.tc_error_flag(dev).data_ptr(), state.ctypes.data, state.size,
-                                     main, side, 0 if (inputs_ready and side is not None) else 1,
-                                     static.caps_array().ctypes.data if static is not None else None,
-                                     static.n_dev.data_ptr() if static is not None else None,
-                                     static.overflow.data_ptr() if static is not None else None, side2)
+            rc, state = _exec_forward(plan, feats, coords, spatial_shape, batch_size, proj, training, precision, static, arena,
+                                      side_obj, side2_obj, side_waits_main=not (inputs_ready and side_obj is not None))
             if rc != VC_ERR_WORKSPACE:
                 break
             # too small (first use of a plan on an unusually dense batch): the call is restartable — nothing it enqueued is
@@ -555,20 +561,8 @@ def run_index(plan, feats, coords_i32, spatial_shape, batch_size, proj, training
     `static.arena`; `run_plan` with `static.phase == 2` later enqueues the feature operators over the same arena."""
     ops._require_cuda(feats, coords_i32)
     assert static is not None and static.arena is not None and static.phase == 1
-    lib = _lib.load()
-    dev = feats.device
-    oi, of, lf, sizes, offs = plan.finalize()
-    tab = _layer_ptrs(plan)
-    side_obj = ops.side(dev).stream if TWO_STREAMS else None
-    side2_obj = ops.side2(dev) if (side_obj is not None and THREE_STREAMS) else None
-    state = np.zeros(lib.vc_exec_state_bytes(), dtype=np.uint8)
-    rc = lib.vc_exec_forward(oi.ctypes.data, of.ctypes.data, oi.shape[0], tab.ctypes.data, lf.ctypes.data, len(plan.layers),
-                             feats.data_ptr(), feats.shape[1], coords_i32.data_ptr(), feats.shape[0], _lib.host_i32(spatial_shape),
-                             int(batch_size), proj.data_ptr(), int(training), int(precision == 'bf16'), 1 | (1 << 8),
-                             static.arena.data_ptr(), static.arena.numel(), _pinned(dev).data_ptr(), ops.tc_error_flag(dev).data_ptr(),
-                             state.ctypes.data, state.size, ops._stream(), side_obj.cuda_stream if side_obj is not None else None, 1,
-                             static.caps_array().ctypes.data, static.n_dev.data_ptr(), static.overflow.data_ptr(),
-                             side2_obj.cuda_stream if side2_obj is not None else None)
+    rc, _ = _exec_forward(plan, feats, coords_i32, spatial_shape, batch_size, proj, training, precision, static, static.arena,
+                          *_index_streams(feats.device), side_waits_main=True)
     check(rc, 'vc_exec_forward (index phase)')
 
 
