@@ -235,6 +235,18 @@ int vc_stvd_partition(const float* points, int n, int c, int bin_num, double max
 int vc_stvd_gather(const float* points, int n, int c, const int32_t* segs /*host*/, int n_seg, const int32_t* sel_dev,
                    float* out /*[n_out, c]*/, int n_out, void* ws, size_t ws_bytes, vc_stream_t stream);
 
+/* StVD layer discard (`layer_voxel_discard`, spconv_backbone.py:134-147) with the subset drawn on the device, no host read
+ * (graph-capturable), csrc/stvd_layer.cu.  Over n rows (n_dev != NULL: *n_dev valid rows of a capacity-n buffer) at discard
+ * site `site`: k = int(n_valid * (1 - rate)) evaluated in float64; the kept rows are the k rows with the smallest (u_i, i),
+ * u_i = keys[i] (keys != NULL, uint32) or word 0 of Philox4x32-10 with counter (i, site, 0, 0) and key
+ * (seed & 0xffffffff, seed >> 32), seed = *seed_dev (int64).  -> keep [n] = the kept rows in ascending order, tail -1;
+ * *kept_dev = k; pos [n] (may be NULL) = a row's position in keep or -1.  The same result on every run.
+ * ws >= vc_stvd_layer_keep_ws_bytes(n).  A memset and seven launches. */
+size_t vc_stvd_layer_keep_ws_bytes(int cap);
+int vc_stvd_layer_keep(const uint32_t* keys /*may be NULL*/, const int64_t* seed_dev /*may be NULL with keys*/, int site, int n,
+                       const int32_t* n_dev /*may be NULL*/, double rate, int32_t* keep, int32_t* kept_dev /*[1]*/,
+                       int32_t* pos /*may be NULL*/, void* ws, size_t ws_bytes, vc_stream_t stream);
+
 /* `generate_voxel2pinds` (pcdet/utils/spconv_utils.py:13-21): dense [B, *spatial_shape] int32 map voxel -> row, -1 where
  * empty (the RoI head's look-up table, ted_head.py:527,625). */
 int vc_voxel2pinds(const int32_t* indices, int n, int ndim, int batch_size, const int32_t* spatial_shape, int32_t* out,
@@ -470,6 +482,10 @@ int vc_rcnn_loss(const vc_rcnn_branch* branches /*host[K]*/, int K, double beta,
  *               4 CBR       features a, rulebook c -> features b            conv + BatchNorm1d + ReLU of layer [20]
  *                                                                            ([18] cin, [19] cout, [21] = input needs grad)
  *               5 CAT       features a, features b -> features c            channel concat
+ *               6 DISCARD   index set a, features [18] -> index set b, features [19]   StVD layer discard at site c
+ *                                                                            (vc_stvd_layer_keep: selection and index gather
+ *                                                                            on the index stream, feature gather on main;
+ *                                                                            [6],[7] = float64 rate, low / high 32 bits)
  *     [1] stream (0 main: feature ops, 1 side: index ops, 2 second side stream: the image branch's index ops)
  *     [2..4] a, b, c   [5] ndim   [6..8] kernel size
  *     [9..11] stride   [12..14] padding   [15..17] dilation
@@ -508,6 +524,16 @@ int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_ops, const u
                     vc_stream_t side_stream, int side_waits_main, const int32_t* caps /*host, may be NULL*/,
                     const int32_t* n0_dev /*device, NULL = exact mode*/, int32_t* overflow_flag /*device*/,
                     vc_stream_t side2_stream /*may be NULL: ops planned for stream 2 (image branch) then share side_stream*/);
+/* vc_exec_forward plus the seed of the plan's DISCARD ops (device int64[1], read on the index stream); vc_exec_forward is
+ * this call with rng_seed_dev = NULL, which a plan with a DISCARD op rejects.  In exact mode a discard that keeps no row
+ * fails (VC_ERR_INVALID, naming the site); in static mode its output set has the input's capacity. */
+int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, int n_ops, const uint64_t* layer_ptrs, const float* layer_f,
+                           int n_layers, const float* feats0, int c0, const int32_t* idx0, int n0, const int32_t* shape0,
+                           int batch_size, const float* proj_params, int training, int precision, int flags, void* arena,
+                           size_t arena_bytes, int32_t* pinned_host, int32_t* err_flag, void* state, size_t state_bytes,
+                           vc_stream_t main_stream, vc_stream_t side_stream, int side_waits_main, const int32_t* caps,
+                           const int32_t* n0_dev, int32_t* overflow_flag, vc_stream_t side2_stream,
+                           const int64_t* rng_seed_dev /*may be NULL without DISCARD ops*/);
 /* Reverse walk.  pub_slots [n_pub]: feature slots whose gradients come from outside (the published tensors), ext_grads
  * [n_pub]: device pointers to those gradients ([rows, c] fp32 contiguous, read only) or 0.  Writes d_weight / d_gamma /
  * d_beta of every layer (zeros where nothing flowed back).  Same arena as the forward (it continues allocating).
@@ -518,7 +544,8 @@ int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_ops, const 
                      size_t arena_bytes, int32_t* err_flag, void* state, vc_stream_t stream, vc_stream_t wgrad_stream);
 /* Read a state blob.  what 0: out[0] = arena bytes in use;  1 (feature slot id): f32 ptr, bf16 ptr, rows, c;
  * 2 (index set): idx ptr, n, ndim, shape[3];  3 (rulebook): nbr, nbr_bwd, pair_num ptrs, K, n_in, n_out, subm, unique;
- * 4 (layer): x ptr, y ptr, stats ptr, forward runs on the tensor cores, rulebook id, in slot, out slot.  out: >= 8 int64
+ * 4 (layer): x ptr, y ptr, stats ptr, forward runs on the tensor cores, rulebook id, in slot, out slot;  5 (op index of a
+ * DISCARD): keep ptr, kept rows (exact mode; static mode: the capacity), kept_dev ptr, n_in, site.  out: >= 8 int64
  * (host). */
 int vc_exec_query(const void* state, int what, int id, long long* out);
 /* Optional per-launch timing of the conv kernels (bench.py's roofline pass): vc_exec_timing(1) clears and arms it,

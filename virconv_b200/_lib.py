@@ -67,6 +67,8 @@ SIGNATURES = {
     'vc_stvd_ws_bytes': (_Z, [_I]),
     'vc_stvd_partition': (_I, [_P, _I, _I, _I, ctypes.c_double, _P, _P, _Z, _P]),
     'vc_stvd_gather': (_I, [_P, _I, _I, _HOST, _I, _P, _P, _I, _P, _Z, _P]),
+    'vc_stvd_layer_keep_ws_bytes': (_Z, [_I]),
+    'vc_stvd_layer_keep': (_I, [_P, _P, _I, _I, _P, _D, _P, _P, _P, _P, _Z, _P]),
     'vc_voxel_query': (_I, [_I, _I, _I, _I, _I, _F, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     'vc_group_points': (_I, [_I, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
     'vc_group_points_grad': (_I, [_I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
@@ -96,6 +98,8 @@ SIGNATURES = {
     'vc_exec_state_bytes': (_Z, []),
     'vc_exec_forward': (_I, [_P, _P, _I, _P, _P, _I, _P, _I, _P, _I, _HOST, _I, _P, _I, _I, _I, _P, _Z, _P, _P, _P, _Z, _P, _P, _I,
                              _P, _P, _P, _P]),
+    'vc_exec_forward_seeded': (_I, [_P, _P, _I, _P, _P, _I, _P, _I, _P, _I, _HOST, _I, _P, _I, _I, _I, _P, _Z, _P, _P, _P, _Z, _P, _P,
+                                    _I, _P, _P, _P, _P, _P]),
     'vc_exec_backward': (_I, [_P, _P, _I, _P, _P, _I, _P, _P, _I, _P, _Z, _P, _P, _P, _P]),
     'vc_exec_query': (_I, [_P, _I, _I, _P]),
     'vc_exec_timing': (_I, [_I]),

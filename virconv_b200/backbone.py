@@ -11,7 +11,12 @@ layer_voxel_discard :134-147.  Differences that do not change results:
     indexing, :61-78); its per-sample matrices are built once per forward;
   * StVD layer discard: `discard_mode='spconv2_compat'` reproduces the reference under spconv 2.x, where
     `layer_voxel_discard` returns None after rebinding a local and the caller's tensor is unchanged
-    (SURVEY §5 note) — i.e. no discard; `discard_mode='paper'` really drops rows, order-preserving.
+    (SURVEY §5 note) — i.e. no discard; `discard_mode='paper'` really drops rows, order-preserving.  Where the kept rows
+    are drawn: `discard_rng='numpy'` (default) from the global numpy stream on the host, as the reference under
+    `set_random_seed`, on the per-operator module path; `discard_rng='device'` on the GPU inside the plan executor
+    (csrc/stvd_layer.cu: a uniformly random k-subset of the same size, from one int64 seed per forward drawn with
+    torch's CUDA generator, or `batch_dict['stvd_seed']`), which a CUDA graph can capture.  Either way the applied lists
+    can be fed back through `batch_dict['stvd_keep_rows']`; the device draw records them in `batch_dict['stvd_kept_rows']`.
 """
 from __future__ import annotations
 
@@ -124,6 +129,19 @@ def plan_nrconv(plan, block, f, iset, proj_stride):
     return plan.cat(d3, d2), iset
 
 
+def _published_tensors(run, res, names, coords0, shape0, batch_size):
+    """The named results of a plan run; tensors over index sets of one group (executor.Plan.iset_group) share one lazy
+    indice_dict."""
+    plan, dicts, out = run.plan, {}, []
+    sets = {name: iset for name, _, iset in plan.published}
+    for name in names:
+        g = plan.iset_group[sets[name]]
+        if g not in dicts:
+            dicts[g] = executor.LazyIndiceDict(run, coords0, shape0, g)
+        out.append(_published_tensor(res, name, batch_size, dicts[g]))
+    return tuple(out)
+
+
 def _published_tensor(res, name, batch_size, indice_dict):
     f, idx, shape, fb, cnt = res[name]
     t = spconv.SparseConvTensor(f, idx, shape, batch_size, indice_dict=indice_dict)
@@ -139,8 +157,27 @@ def stvd_keep_rows(n, rate, rng=np.random):
     return np.sort(keep)
 
 
+_I64 = torch.iinfo(torch.int64)
+
+
+def stvd_seed(batch_dict, device):
+    """The draw behind one forward's device-side layer discards: batch_dict['stvd_seed'] (int64 device tensor) when given,
+    else one int64 from torch's CUDA generator on the current stream — fresh on every replay of a captured graph, repeated
+    under torch.manual_seed."""
+    seed = batch_dict.get('stvd_seed')
+    if seed is None:
+        return torch.randint(_I64.min, _I64.max, (1,), dtype=torch.int64, device=device)
+    assert torch.is_tensor(seed) and seed.dtype == torch.int64 and seed.device == device and seed.numel() == 1, \
+        "batch_dict['stvd_seed'] must be one int64 on the model's device"
+    return seed.reshape(1)
+
+
 def discard_rows(t, keep_rows):
-    rows = torch.as_tensor(np.ascontiguousarray(keep_rows), dtype=torch.int32).to(t.features.device)
+    if torch.is_tensor(keep_rows):      # a list the device draw recorded (static mode: capacity-sized, count in .num_rows)
+        n = getattr(keep_rows, 'num_rows', None)
+        rows = (keep_rows if n is None else keep_rows[:int(n)]).to(device=t.features.device, dtype=torch.int32).contiguous()
+    else:
+        rows = torch.as_tensor(np.ascontiguousarray(keep_rows), dtype=torch.int32).to(t.features.device)
     feats = ops.GatherRowsFn.apply(t.features, rows)
     idx = ops.gather_rows(spconv._as_i32(t.indices), rows)
     return spconv.SparseConvTensor(feats, idx, t.spatial_shape, t.batch_size)
@@ -150,7 +187,7 @@ class VirConvL8x(nn.Module):
     """VirConv-L backbone (fused LiDAR + virtual stream), spconv_backbone.py:538-699."""
 
     def __init__(self, model_cfg, input_channels, grid_size, discard_mode='spconv2_compat', precision='fp32',
-                 **kwargs):
+                 discard_rng='numpy', **kwargs):
         super().__init__()
         self.model_cfg = model_cfg
         self.return_num_features_as_dict = _cfg_get(model_cfg, 'RETURN_NUM_FEATURES_AS_DICT', False)
@@ -158,7 +195,8 @@ class VirConvL8x(nn.Module):
         self.layer_discard_rate = _cfg_get(model_cfg, 'LAYER_DISCARD_RATE', 0.0)
         num_filters = list(_cfg_get(model_cfg, 'NUM_FILTERS', [16, 32, 64, 64]))
         assert discard_mode in ('spconv2_compat', 'paper')
-        self.discard_mode = discard_mode
+        assert discard_rng in ('numpy', 'device')
+        self.discard_mode, self.discard_rng = discard_mode, discard_rng
         norm_fn = partial(nn.BatchNorm1d, eps=1e-3, momentum=0.01)
         gs = [int(g) for g in grid_size]
         self.sparse_shape = [gs[2] + 1, gs[1], gs[0]]            # grid_size[::-1] + [1, 0, 0]   (:552)
@@ -184,28 +222,40 @@ class VirConvL8x(nn.Module):
         keep = given[layer] if given is not None else stvd_keep_rows(t.features.shape[0], self.layer_discard_rate)
         return discard_rows(t, keep)
 
+    def _discarding(self):
+        return self.training and self.discard_mode == 'paper' and self.layer_discard_rate != 0
+
+    def _device_discard(self):
+        return self._discarding() and self.discard_rng == 'device'
+
     # -- native plan (csrc/executor.cu): the whole forward / backward in one C-ABI call each -------------------
     def _plan(self):
-        if getattr(self, '_plan_cache', None) is None:
+        """The plan of the current mode: with the three layer discards (sites 0-2, after vir_conv1..3) in a device-drawn
+        paper-mode training forward, without them otherwise; both are cached."""
+        stvd = self._device_discard()
+        attr = '_plan_stvd_cache' if stvd else '_plan_cache'
+        if getattr(self, attr, None) is None:
             plan = executor.Plan(self.vir_conv1.d3_conv1[0].in_channels)
             f, iset = 0, 0
             for i, (blk, s) in enumerate(zip((self.vir_conv1, self.vir_conv2, self.vir_conv3, self.vir_conv4), (1, 2, 4, 8))):
                 f, iset = plan_nrconv(plan, blk, f, iset, s)
+                if stvd and i < 3:
+                    f, iset = plan.discard(f, iset, i, self.layer_discard_rate)
                 plan.publish('x_conv%d' % (i + 1), f, iset)
             conv = self.conv_out[0]
             iset, rb = plan.conv_rb(iset, 3, conv.kernel_size, conv.stride, conv.padding, conv.dilation, keys=[conv.indice_key])
             plan.publish('out', plan.cbr(f, rb, conv, self.conv_out[1], seq=self.conv_out), iset)
-            self._plan_cache = plan
-        return self._plan_cache
+            setattr(self, attr, plan)
+        return getattr(self, attr)
 
-    def _use_plan(self, feats):
+    def _use_plan(self, feats, batch_dict=None):
         if not executor.ENABLED or not feats.is_cuda or feats.shape[0] == 0 or feats.requires_grad:
             return False             # (the plan does not propagate a gradient into the voxel features; the module path does)
-        if self.training and self.discard_mode == 'paper' and self.layer_discard_rate != 0:
-            return False             # row-dropping StVD between the blocks is only on the module path
+        if self._discarding() and (self.discard_rng != 'device' or (batch_dict or {}).get('stvd_keep_rows') is not None):
+            return False             # host-drawn or caller-given kept rows: the module path
         plan = self._plan()
         if not plan.is_current():          # a sub-module was replaced after the plan was built (e.g. SyncBatchNorm conversion)
-            self._plan_cache = None
+            self._plan_cache = self._plan_stvd_cache = None
             plan = self._plan()
         if not plan.eligible():            # (checked every forward: dtype / layout / module type may change under .half(), .to())
             return False
@@ -219,11 +269,14 @@ class VirConvL8x(nn.Module):
         feature operators over it."""
         feats, coords = batch_dict['voxel_features'], batch_dict['voxel_coords']
         static = batch_dict['virconv_static']
-        assert static.phase == 1 and self._use_plan(feats)
+        assert static.phase == 1 and self._use_plan(feats, batch_dict)
         ci = spconv._as_i32(coords)
+        # (the layer discards select their rows in this phase; the feature phase gathers with the same seed)
+        seed = stvd_seed(batch_dict, feats.device) if self._device_discard() else None
         executor.run_index(self._plan(), feats, ci, self.sparse_shape, batch_dict['batch_size'], batch_dict['virconv_proj'],
-                           self.conv_out[1].training, self.conv_out[0].precision, static)
+                           self.conv_out[1].training, self.conv_out[0].precision, static, seed)
         batch_dict['virconv_ci'] = ci
+        batch_dict['virconv_stvd_seed'] = seed
         return batch_dict
 
     def forward(self, batch_dict):
@@ -238,14 +291,19 @@ class VirConvL8x(nn.Module):
             trans = batch_dict['aug_param'] if 'aug_param' in batch_dict else None
             if 'transform_param' in batch_dict:
                 trans = batch_dict['transform_param'][:, i, :]
-            if self._use_plan(feats):
+            if self._use_plan(feats, batch_dict):
                 bn_training = self.conv_out[1].training
                 # 'virconv_inputs_ready': the caller's promise that voxel_coords is resident and complete (a prefetched
                 # batch) -> the index pipeline of this step (starting with the .int() of the coordinates, :641) runs on
                 # the side stream without waiting for main, i.e. it may overlap the previous step's backward
                 side = ops.side(feats.device).stream if executor.TWO_STREAMS else None
                 static = batch_dict.get('virconv_static')
-                ready = side is not None and static is None and bool(batch_dict.get('virconv_inputs_ready', False))
+                seed = None
+                if self._device_discard():
+                    seed = batch_dict['virconv_stvd_seed'] if static is not None and static.phase == 2 else \
+                        stvd_seed(batch_dict, feats.device)
+                ready = (side is not None and static is None and seed is None
+                         and bool(batch_dict.get('virconv_inputs_ready', False)))
                 if static is not None and static.phase == 2:
                     ci = batch_dict['virconv_ci']           # (built by index_phase for this very batch)
                 elif ready and (coords.dtype != torch.int32 or not coords.is_contiguous()):
@@ -263,11 +321,12 @@ class VirConvL8x(nn.Module):
                     assert static is None, "static mode needs batch_dict['virconv_proj'] (ops.projection_params on the device)"
                     proj = ops.projection_params(calib, trans, batch_size, feats.device, side)
                 run, res = executor.run_plan(self._plan(), feats, ci, self.sparse_shape, batch_size, proj, bn_training,
-                                             self.conv_out[0].precision, inputs_ready=ready, static=static)
+                                             self.conv_out[0].precision, inputs_ready=ready, static=static, seed=seed)
                 executor.note_last_run(self, run)   # (graph.GraphedStep sizes its capacities from an exact-mode run)
-                idict = executor.LazyIndiceDict(run, ci, self.sparse_shape)
-                x1, x2, x3, x4, out = (_published_tensor(res, k, batch_size, idict)
-                                       for k in ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4', 'out'))
+                x1, x2, x3, x4, out = _published_tensors(run, res, ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4', 'out'), ci,
+                                                         self.sparse_shape, batch_size)
+                if seed is not None:
+                    batch_dict['stvd_kept_rows' + rid] = run.kept_rows()
                 batch_dict.update({
                     'encoded_spconv_tensor' + rid: out,
                     'encoded_spconv_tensor_stride' + rid: 8,
@@ -315,7 +374,8 @@ class VirConv8x(nn.Module):
     Eval mode batches the ROT_NUM transformed copies along x into one [D, H, 4W] tensor (:360,:418-432) and splits the
     published tensors afterwards."""
 
-    def __init__(self, model_cfg, input_channels, grid_size, discard_mode='spconv2_compat', precision='fp32', **kwargs):
+    def __init__(self, model_cfg, input_channels, grid_size, discard_mode='spconv2_compat', precision='fp32',
+                 discard_rng='numpy', **kwargs):
         super().__init__()
         self.model_cfg = model_cfg
         self.return_num_features_as_dict = _cfg_get(model_cfg, 'RETURN_NUM_FEATURES_AS_DICT', False)
@@ -324,7 +384,8 @@ class VirConv8x(nn.Module):
         f = list(_cfg_get(model_cfg, 'NUM_FILTERS', [16, 32, 64, 64]))
         self.mm = bool(_cfg_get(model_cfg, 'MM', False))
         assert discard_mode in ('spconv2_compat', 'paper')
-        self.discard_mode = discard_mode
+        assert discard_rng in ('numpy', 'device')
+        self.discard_mode, self.discard_rng = discard_mode, discard_rng
         norm_fn = partial(nn.BatchNorm1d, eps=1e-3, momentum=0.01)
         gs = [int(g) for g in grid_size]
         self.sparse_shape = [gs[2] + 1, gs[1], gs[0]]
@@ -378,15 +439,22 @@ class VirConv8x(nn.Module):
             self._plan_lidar_cache = plan
         return self._plan_lidar_cache
 
-    def _plan_mm(self):
-        if getattr(self, '_plan_mm_cache', None) is None:
+    def _plan_mm(self, stvd=False):
+        """Virtual-point stream (:468-535).  stvd: with the device-drawn layer discards at sites 0 (the input voxels, :489)
+        and 1-3 (after vir_conv1..3); the LiDAR stream has none in the reference."""
+        attr = '_plan_mm_stvd_cache' if stvd else '_plan_mm_cache'
+        if getattr(self, attr, None) is None:
             plan = executor.Plan(self.vir_conv1.d3_conv1[0].in_channels)
             f, iset = 0, 0
+            if stvd:
+                f, iset = plan.discard(f, iset, 0, self.layer_discard_rate)
             for i, (blk, s) in enumerate(zip((self.vir_conv1, self.vir_conv2, self.vir_conv3, self.vir_conv4), (1, 2, 4, 8))):
                 f, iset = plan_nrconv(plan, blk, f, iset, s)
+                if stvd and i < 3:
+                    f, iset = plan.discard(f, iset, i + 1, self.layer_discard_rate)
                 plan.publish('x_conv%d' % (i + 1), f, iset)
-            self._plan_mm_cache = plan
-        return self._plan_mm_cache
+            setattr(self, attr, plan)
+        return getattr(self, attr)
 
     @staticmethod
     def _plan_usable(plan, feats):
@@ -396,12 +464,12 @@ class VirConv8x(nn.Module):
         mode = plan.layers[0][1].training
         return all(bn.training == mode for _, bn in plan.layers)
 
-    def _run(self, plan, feats, coords, shape, batch_size, proj, names):
+    def _run(self, plan, feats, coords, shape, batch_size, proj, names, seed=None):
+        """-> (run record, published tensors)"""
         ci = spconv._as_i32(coords)
         run, res = executor.run_plan(plan, feats, ci, shape, batch_size, proj, plan.layers[0][1].training,
-                                     plan.layers[0][0].precision)
-        idict = executor.LazyIndiceDict(run, ci, shape)
-        return tuple(_published_tensor(res, k, batch_size, idict) for k in names)
+                                     plan.layers[0][0].precision, seed=seed)
+        return run, _published_tensors(run, res, names, ci, shape, batch_size)
 
     def _lidar_stream(self, feats, coords, shape, batch_size):
         plan = self._plan_lidar()
@@ -409,7 +477,7 @@ class VirConv8x(nn.Module):
             self._plan_lidar_cache = None
             plan = self._plan_lidar()
         if self._plan_usable(plan, feats):
-            return self._run(plan, feats, coords, shape, batch_size, None, ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4', 'out'))
+            return self._run(plan, feats, coords, shape, batch_size, None, ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4', 'out'))[1]
         x = spconv.SparseConvTensor(feats, coords.int(), shape, batch_size)
         x1 = self.conv1(self.conv_input(x))
         x2 = self.conv2(x1)
@@ -463,13 +531,18 @@ class VirConv8x(nn.Module):
                 if 'transform_param' in batch_dict:
                     trans = batch_dict['transform_param'][:, i, :]
                 discarding = self.training and self.discard_mode == 'paper' and self.layer_discard_rate != 0
-                if not self._plan_mm().is_current():
-                    self._plan_mm_cache = None
-                if not discarding and self._plan_usable(self._plan_mm(), feats):
+                # device-drawn discards run in the plan; host-drawn or caller-given kept rows on the module path
+                stvd = discarding and self.discard_rng == 'device' and batch_dict.get('stvd_keep_rows') is None
+                if not self._plan_mm(stvd).is_current():
+                    self._plan_mm_cache = self._plan_mm_stvd_cache = None
+                if (stvd or not discarding) and self._plan_usable(self._plan_mm(stvd), feats):
                     side = ops.side(feats.device).stream if executor.TWO_STREAMS else None
                     proj = ops.projection_params(calib, trans, batch_size, feats.device, side)
-                    x1, x2, x3, x4 = self._run(self._plan_mm(), feats, coords, self.sparse_shape, batch_size, proj,
-                                               ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4'))
+                    seed = stvd_seed(batch_dict, feats.device) if stvd else None
+                    run, (x1, x2, x3, x4) = self._run(self._plan_mm(stvd), feats, coords, self.sparse_shape, batch_size, proj,
+                                                      ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4'), seed)
+                    if stvd:
+                        batch_dict['stvd_kept_rows' + s] = run.kept_rows()
                     batch_dict.update({
                         'encoded_spconv_tensor_stride_mm' + s: 8,
                         'multi_scale_3d_features_mm' + s: {'x_conv1': x1, 'x_conv2': x2, 'x_conv3': x3, 'x_conv4': x4},

@@ -155,6 +155,14 @@ int cat2_dev(const float* a, const float* b, float* out, void* out_bf16, int n, 
 int index2uv_dev(const int32_t* indices, int n, const int* n_dev, int batch_size, const float* params, const float* grid,
                  int stride, int u_max, int v_max, int32_t* uv_out, cudaStream_t stream);
 
+// ---- stvd_layer.cu internals used by the plan executor (StVD layer discard) ----
+// out[r] = keep[r] >= 0 ? in[keep[r]] : 0 for r < rows (fp32 and / or bf16; either may be NULL), in [*, c] dense, c % 4 == 0
+int stvd_gather_feats_dev(const float* in, int c, const int32_t* keep, int rows, float* out, void* out_bf16, cudaStream_t st);
+// out[r] = keep[r] >= 0 ? in[keep[r]] : -1 (rows of `cols` int32)
+int stvd_gather_idx_dev(const int32_t* in, int cols, const int32_t* keep, int rows, int32_t* out, cudaStream_t st);
+// dx[i] = pos[i] >= 0 ? dy[pos[i]] : 0 for i < n_in, row pitches dy_ld / dx_ld
+int stvd_grad_dev(const float* dy, int dy_ld, int c, const int32_t* pos, int n_in, float* dx, int dx_ld, cudaStream_t st);
+
 // ---- shared between conv_tc.cu, conv_tc2.cu and executor.cu ----
 struct TcPrepEntry {
     const float* w;   // parameter, spconv layout [C_out, K, C_in]

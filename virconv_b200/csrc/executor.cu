@@ -27,7 +27,7 @@ namespace {
 
 constexpr int MAX_OPS = 256, MAX_F = 160, MAX_I = 64, MAX_RB = 64, MAX_L = 96, OPI = 24, OPF = 8;
 constexpr uint64_t STATE_MAGIC = 0x5643455845433031ULL;  // "VCEXEC01"
-enum { OP_SUBM_RB = 1, OP_CONV_RB = 2, OP_INDEX2UV = 3, OP_CBR = 4, OP_CAT = 5 };
+enum { OP_SUBM_RB = 1, OP_CONV_RB = 2, OP_INDEX2UV = 3, OP_CBR = 4, OP_CAT = 5, OP_DISCARD = 6 };
 enum { G_EMPTY = 0, G_EXT = 1, G_OWN = 2 };
 // op int fields
 enum { F_KIND = 0, F_STREAM = 1, F_A = 2, F_B = 3, F_C = 4, F_NDIM = 5, F_KS = 6, F_ST = 9, F_PD = 12, F_DL = 15, F_CIN = 18,
@@ -71,6 +71,11 @@ struct Layer {
     int in_slot, out_slot, rb, cin, cout;
     ConvKind fwd, dgrad, wgrad;   // chosen by choose_kernels
 };
+struct Disc {              // a DISCARD op (StVD layer discard): what its selection left behind
+    int32_t *keep, *pos;   // keep [n_in]: kept rows ascending, tail -1; pos [n_in]: position in keep or -1
+    int32_t* kept_dev;     // device int32[1]: number of kept rows
+    int n_in, k, site;     // k: kept rows (exact mode) or the capacity n_in (static mode)
+};
 struct State {
     uint64_t magic;
     size_t used;           // arena bytes in use after the last call
@@ -79,6 +84,7 @@ struct State {
     FSlot f[MAX_F];
     RBk rb[MAX_RB];
     Layer layer[MAX_L];
+    Disc disc[MAX_OPS];    // by op index
 };
 
 struct Arena {
@@ -239,7 +245,7 @@ int check_plan(const int32_t* oi, int n_ops, int n_layers) {
     VC_CHECK_ARG(oi && n_ops > 0 && n_ops <= MAX_OPS && n_layers >= 0 && n_layers <= MAX_L, "bad plan size");
     for (int i = 0; i < n_ops; ++i) {
         const int* o = oi + (size_t)i * OPI;
-        VC_CHECK_ARG(o[F_KIND] >= OP_SUBM_RB && o[F_KIND] <= OP_CAT, "op %d: unknown kind %d", i, o[F_KIND]);
+        VC_CHECK_ARG(o[F_KIND] >= OP_SUBM_RB && o[F_KIND] <= OP_DISCARD, "op %d: unknown kind %d", i, o[F_KIND]);
         VC_CHECK_ARG(o[F_STREAM] >= 0 && o[F_STREAM] <= 2, "op %d: bad stream", i);
         const int lim_a = (o[F_KIND] == OP_CBR || o[F_KIND] == OP_CAT) ? MAX_F : MAX_I;
         VC_CHECK_ARG(o[F_A] >= 0 && o[F_A] < lim_a, "op %d: slot a out of range", i);
@@ -252,6 +258,10 @@ int check_plan(const int32_t* oi, int n_ops, int n_layers) {
             VC_CHECK_ARG(o[F_C] >= 0 && o[F_C] < MAX_RB, "op %d: bad rulebook id", i);
         } else if (o[F_KIND] == OP_CONV_RB) {
             VC_CHECK_ARG(o[F_B] >= 0 && o[F_B] < MAX_I && o[F_C] >= 0 && o[F_C] < MAX_RB, "op %d: bad ids", i);
+        } else if (o[F_KIND] == OP_DISCARD) {
+            VC_CHECK_ARG(o[F_B] >= 0 && o[F_B] < MAX_I && o[F_C] >= 0 && o[F_CIN] >= 0 && o[F_CIN] < MAX_F && o[F_COUT] > 0 &&
+                             o[F_COUT] < MAX_F && o[F_CIN] != o[F_COUT],
+                         "op %d: bad discard ids", i);
         } else {
             VC_CHECK_ARG(o[F_B] >= 0 && o[F_B] < MAX_I, "op %d: bad index-set id", i);
         }
@@ -284,6 +294,7 @@ struct FwdCtx : Ctx {
     bool need_f32[MAX_F], cat_inplace[MAX_OPS];
     size_t sums_doubles, n_cbr, wg_floats;               // the zeroed region: BN sums, tile counters, wgrad accumulators
     const float* proj;
+    const int64_t* seed;   // of the DISCARD ops
     const int32_t* caps;
     int32_t *overflow, *pinned;
     int n_syncs, last_ev[3] = {-1, -1, -1};   // last_ev: latest event of each side stream (joined into main at the end)
@@ -327,6 +338,10 @@ void plan_step(FwdCtx& C, int c0, int precision, int training) {
         } else if (o[F_KIND] == OP_CAT) {
             C.slot_c[o[F_C]] = C.slot_c[o[F_A]] + C.slot_c[o[F_B]];
             if (precision == 0 || o[F_X1]) C.need_f32[o[F_C]] = true;
+        } else if (o[F_KIND] == OP_DISCARD) {   // the discard gathers fp32 rows (and rounds its own bf16 shadow)
+            C.slot_c[o[F_COUT]] = C.slot_c[o[F_CIN]];
+            C.need_f32[o[F_CIN]] = true;
+            if (precision == 0 || o[F_X1]) C.need_f32[o[F_COUT]] = true;
         }
     }
     for (int i = 0; i < C.n_ops; ++i) {
@@ -417,6 +432,78 @@ int fwd_conv_count(FwdCtx& C, int j) {
     return VC_OK;
 }
 
+double op_rate(const int* o) {   // the float64 rate of a DISCARD op, stored as two int32 halves
+    const uint64_t bits = (uint64_t)(uint32_t)o[F_KS] | ((uint64_t)(uint32_t)o[F_KS + 1] << 32);
+    double r;
+    memcpy(&r, &bits, 8);
+    return r;
+}
+
+// index part of DISCARD op j on the index stream: row selection (vc_stvd_layer_keep) and the kept rows' indices
+int fwd_discard_keep(FwdCtx& C, int j) {
+    const int* o = C.op(j);
+    const int s = C.two ? o[F_STREAM] : 0;
+    cudaStream_t st = C.st[s];
+    ISet& I = C.S->iset[o[F_A]];
+    ISet& O = C.S->iset[o[F_B]];
+    Disc& D = C.S->disc[j];
+    const double rate = op_rate(o);
+    VC_CHECK_ARG(I.idx, "op %d: index set %d not built", j, o[F_A]);
+    VC_CHECK_ARG(rate >= 0.0 && rate <= 1.0, "op %d: discard rate %g outside [0, 1]", j, rate);
+    VC_TRY(wait_for(C, I.ev, I.prod, s));
+    int k = I.n;   // static mode: the capacity; the kept count stays on the device
+    if (!C.S->is_static) {
+        k = (int)((double)I.n * (1.0 - rate));
+        VC_CHECK_ARG(k > 0, "StVD layer discard at site %d: %d rows at rate %g keep no row", o[F_C], I.n, rate);
+    }
+    const int cap = I.n > 0 ? I.n : 1;
+    VC_ALLOC(keep, int32_t*, (size_t)cap * 4);
+    VC_ALLOC(pos, int32_t*, (size_t)cap * 4);
+    VC_ALLOC(kept_dev, int32_t*, 4);
+    const size_t wsb = vc_stvd_layer_keep_ws_bytes(I.n);
+    VC_ALLOC(ws, void*, wsb);
+    VC_ALLOC(oidx, int32_t*, (size_t)(k > 0 ? k : 1) * (1 + I.ndim) * 4);
+    if (C.do_idx) {
+        VC_TRY(vc_stvd_layer_keep(nullptr, C.seed, o[F_C], I.n, I.n_dev, rate, keep, kept_dev, pos, ws, wsb, st));
+        VC_TRY(stvd_gather_idx_dev(I.idx, 1 + I.ndim, keep, k, oidx, st));
+    }
+    D.keep = keep; D.pos = pos; D.kept_dev = kept_dev; D.n_in = I.n; D.k = k; D.site = o[F_C];
+    O.idx = oidx; O.n = k; O.ndim = I.ndim; O.n_dev = C.S->is_static ? kept_dev : nullptr;
+    for (int d = 0; d < 3; ++d) O.shape[d] = I.shape[d];
+    C.produced(O, s);
+    C.chain[j].done = true;
+    return VC_OK;
+}
+
+// DISCARD op i: its index part (unless the strided convs' chain ran it), then the feature gather on the main stream — the
+// kept fp32 rows (the published x_conv*) and their bf16 rounding (the next down conv's operand), zero tail in static mode
+int fwd_discard(FwdCtx& C, int i, const int* o) {
+    if (!C.chain[i].done) VC_TRY(fwd_discard_keep(C, i));
+    const Disc& D = C.S->disc[i];
+    ISet& O = C.S->iset[o[F_B]];
+    FSlot& X = C.S->f[o[F_CIN]];
+    FSlot& Y = C.S->f[o[F_COUT]];
+    VC_CHECK_ARG(X.f32 && X.ld == X.c && X.rows == D.n_in, "op %d: discard input slot %d not built / rows %d vs %d", i, o[F_CIN],
+                 X.rows, D.n_in);
+    VC_TRY(wait_for(C, O.ev, O.prod, 0));
+    VC_TRY(wait_for(C, X.ev, X.prod, 0));
+    const size_t elems = (size_t)O.n * X.c;
+    float* y = nullptr;
+    void* yb = nullptr;
+    if (C.need_f32[o[F_COUT]]) {
+        VC_ALLOC(y_, float*, elems * 4);
+        y = y_;
+    }
+    if (C.S->precision == 1) {
+        VC_ALLOC(yb_, void*, elems * 2);
+        yb = yb_;
+    }
+    if (C.do_feat) VC_TRY(stvd_gather_feats_dev(X.f32, X.c, D.keep, O.n, y, yb, C.st[0]));
+    Y.f32 = y; Y.bf16 = yb; Y.rows = O.n; Y.c = Y.ld = X.c; Y.n_dev = O.n_dev;
+    C.produced(Y, 0);
+    return VC_OK;
+}
+
 int fwd_conv_rb(FwdCtx& C, int i, const int* o, int s) {
     // First strided conv reached: run the count -> (host reads the row count) -> emit-indices chain of EVERY strided conv of
     // the plan now, back to back.  Each link only needs the previous link's output indices, and it is the only part of the
@@ -428,8 +515,12 @@ int fwd_conv_rb(FwdCtx& C, int i, const int* o, int s) {
             // early stage are not queued behind the counting kernels of all later ones
             VC_TRY(fwd_conv_count(C, i));
         } else {
-            for (int j = i; j < C.n_ops; ++j)
-                if (C.op(j)[F_KIND] == OP_CONV_RB && C.S->iset[C.op(j)[F_A]].idx) VC_TRY(fwd_conv_count(C, j));
+            // (a layer discard between two strided convs selects its rows in the same chain: the next count reads them)
+            for (int j = i; j < C.n_ops; ++j) {
+                const int* oj = C.op(j);
+                if (oj[F_KIND] == OP_CONV_RB && C.S->iset[oj[F_A]].idx) VC_TRY(fwd_conv_count(C, j));
+                else if (oj[F_KIND] == OP_DISCARD && !C.chain[j].done && C.S->iset[oj[F_A]].idx) VC_TRY(fwd_discard_keep(C, j));
+            }
         }
     }
     VC_CHECK_ARG(C.chain[i].done, "op %d: index set %d not built", i, o[F_A]);
@@ -625,6 +716,13 @@ extern "C" int vc_exec_query(const void* state, int what, int id, long long* out
             out[3] = l.fwd == K_FWD_TC; out[4] = l.rb; out[5] = l.in_slot; out[6] = l.out_slot;
             return VC_OK;
         }
+        case 5: {
+            VC_CHECK_ARG(id >= 0 && id < MAX_OPS && S->disc[id].keep, "op %d is not a layer discard of this run", id);
+            const Disc& d = S->disc[id];
+            out[0] = (long long)(uintptr_t)d.keep; out[1] = d.k; out[2] = (long long)(uintptr_t)d.kept_dev; out[3] = d.n_in;
+            out[4] = d.site;
+            return VC_OK;
+        }
     }
     set_error("vc_exec_query: unknown selector %d", what);
     return VC_ERR_INVALID;
@@ -637,6 +735,19 @@ extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_o
                                void* state, size_t state_bytes, vc_stream_t main_stream, vc_stream_t side_stream,
                                int side_waits_main, const int32_t* caps, const int32_t* n0_dev, int32_t* overflow_flag,
                                vc_stream_t side2_stream) {
+    return vc_exec_forward_seeded(ops_i, ops_f, n_ops, layer_ptrs, layer_f, n_layers, feats0, c0, idx0, n0, shape0, batch_size,
+                                  proj_params, training, precision, flags, arena, arena_bytes, pinned_host, err_flag, state,
+                                  state_bytes, main_stream, side_stream, side_waits_main, caps, n0_dev, overflow_flag, side2_stream,
+                                  nullptr);
+}
+
+extern "C" int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, int n_ops, const uint64_t* layer_ptrs,
+                                      const float* layer_f, int n_layers, const float* feats0, int c0, const int32_t* idx0, int n0,
+                                      const int32_t* shape0, int batch_size, const float* proj_params, int training, int precision,
+                                      int flags, void* arena, size_t arena_bytes, int32_t* pinned_host, int32_t* err_flag,
+                                      void* state, size_t state_bytes, vc_stream_t main_stream, vc_stream_t side_stream,
+                                      int side_waits_main, const int32_t* caps, const int32_t* n0_dev, int32_t* overflow_flag,
+                                      vc_stream_t side2_stream, const int64_t* rng_seed_dev) {
     // static mode and phased execution: include/virconv_b200.h.  Both phases walk the whole plan with the same
     // deterministic bump allocation, so they agree on every address and leave the same state blob.
     const bool is_static = n0_dev != nullptr;
@@ -644,6 +755,9 @@ extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_o
     const int phase = (flags >> 8) & 3;
     VC_CHECK_ARG(phase == 0 || (is_static && phase <= 2), "phased execution needs static mode");
     VC_TRY(check_plan(ops_i, n_ops, n_layers));
+    for (int i = 0; i < n_ops; ++i)
+        VC_CHECK_ARG(ops_i[(size_t)i * OPI + F_KIND] != OP_DISCARD || rng_seed_dev,
+                     "op %d: a StVD layer discard needs a seed (vc_exec_forward_seeded with rng_seed_dev)", i);
     VC_CHECK_ARG(state && state_bytes >= sizeof(State), "state blob too small (%zu < %zu)", state_bytes, sizeof(State));
     VC_CHECK_ARG(feats0 && idx0 && n0 > 0 && shape0 && batch_size > 0 && arena && pinned_host && ops_f && layer_ptrs && layer_f,
                  "null / empty argument");
@@ -666,7 +780,7 @@ extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_o
     C.st[1] = side_stream ? (cudaStream_t)side_stream : (cudaStream_t)main_stream;
     C.st[2] = (side_stream && side2_stream) ? (cudaStream_t)side2_stream : C.st[1];   // image-branch index ops (index2uv + 2-D rulebooks)
     C.err = err_flag;
-    C.proj = proj_params; C.caps = caps; C.overflow = overflow_flag; C.pinned = pinned_host;
+    C.proj = proj_params; C.seed = rng_seed_dev; C.caps = caps; C.overflow = overflow_flag; C.pinned = pinned_host;
     C.do_idx = phase != 2; C.do_feat = phase != 1; C.two = C.st[0] != C.st[1];
     plan_step(C, c0, precision, training);
 
@@ -733,6 +847,7 @@ extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_o
             case OP_INDEX2UV: VC_TRY(fwd_index2uv(C, i, o, s)); break;
             case OP_CBR: VC_TRY(fwd_cbr(C, i, o, s)); break;
             case OP_CAT: VC_TRY(fwd_cat(C, i, o, s)); break;
+            case OP_DISCARD: VC_TRY(fwd_discard(C, i, o)); break;
         }
     }
     for (int s = 1; s <= 2; ++s)
@@ -873,6 +988,18 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
             }
             Aa.grad = da; Aa.gld = Aa.c; Aa.grad_state = G_OWN;
             Bb.grad = db; Bb.gld = Bb.c; Bb.grad_state = G_OWN;
+            continue;
+        }
+        if (o[F_KIND] == OP_DISCARD) {
+            // dense gather through pos: every input row gets its kept row's gradient or zero.  The buffer becomes the gradient
+            // of the concat that fed the discard, which the concat's backward then hands on in column slices
+            FSlot& X = S->f[o[F_CIN]];
+            FSlot& Y = S->f[o[F_COUT]];
+            if (Y.grad_state == G_EMPTY || o[F_CIN] == 0) continue;
+            VC_CHECK_ARG(X.grad_state == G_EMPTY, "op %d: the input of a layer discard has a second gradient source", i);
+            VC_ALLOC(dx, float*, (size_t)X.rows * X.c * 4);
+            VC_TRY(stvd_grad_dev(Y.grad, Y.gld, X.c, S->disc[i].pos, X.rows, dx, X.c, st));
+            X.grad = dx; X.gld = X.c; X.grad_state = G_OWN;
             continue;
         }
         if (o[F_KIND] != OP_CBR) continue;

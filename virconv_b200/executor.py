@@ -38,7 +38,7 @@ def _wgrad_stream(device):
 TIMING = False                     # bench.py's roofline pass: per-launch events around the conv kernels
 LAST_RUN = None                    # the most recent forward's record while TIMING is on (bench.py reads its row counts)
 
-OP_SUBM_RB, OP_CONV_RB, OP_INDEX2UV, OP_CBR, OP_CAT = 1, 2, 3, 4, 5
+OP_SUBM_RB, OP_CONV_RB, OP_INDEX2UV, OP_CBR, OP_CAT, OP_DISCARD = 1, 2, 3, 4, 5, 6
 VC_ERR_WORKSPACE = -3
 OPI, OPF, PCOLS = 24, 8, 9
 # the timing records' kinds: enum ConvKind of csrc/executor.cu
@@ -63,6 +63,12 @@ class Plan:
         self.f_channels = {0: in_channels}
         self.published = []           # (name, feature slot, index set)
         self.rb_keys = {}             # rulebook id -> (indice_keys, ndim, in index set, out index set)
+        self.discards = []            # (site, op index) of the StVD layer discards, in plan order
+        # index set -> group: the sets derived from one another without a layer discard in between.  A published tensor's
+        # indice_dict holds the rulebooks of its group only (a discard's output starts a new group, as the module path starts
+        # a new SparseConvTensor there), never one built over rows the tensor does not carry
+        self.iset_group = {0: 0}
+        self.no_grad = {0}            # feature slots no parameter gradient flows into (the input and discards of it)
         self._final = None
         # per-device run-time state (dies with the plan, i.e. with the model that owns it)
         self.arena_bytes = {}         # (device index, training) -> arena size handed out (monotone)
@@ -97,6 +103,7 @@ class Plan:
         self.n_rb += 1
         self.n_i += 1
         self.rb_keys[rb] = (tuple(keys), ndim, iset, out)
+        self.iset_group[out] = self.iset_group[iset]
         self._row(OP_CONV_RB, 1, a=iset, b=out, c=rb, ndim=ndim, ks=_t3(ksize, ndim, 1), st=_t3(stride, ndim, 1),
                   pd=_t3(padding, ndim, 0), dl=_t3(dilation, ndim, 1))
         return out, rb
@@ -105,6 +112,7 @@ class Plan:
                  v_max=600, image_shape=(1600, 600), stream=1):
         out = self.n_i
         self.n_i += 1
+        self.iset_group[out] = self.iset_group[iset]
         vs = np.array(voxel_size, dtype=np.float64) * stride      # same host arithmetic as ops.index2uv
         grid = [vs[0], vs[1], vs[2], pts_range[0] + vs[0] / 2, pts_range[1] + vs[1] / 2, pts_range[2] + vs[2] / 2]
         self._row(OP_INDEX2UV, stream, a=iset, b=out, ndim=3, ks=(int(image_shape[0]), int(image_shape[1]), 0), x0=int(stride),
@@ -122,7 +130,7 @@ class Plan:
         assert self.f_channels[f_in] == conv.in_channels, (self.f_channels[f_in], conv.in_channels)
         self.f_channels[out] = conv.out_channels
         self._row(OP_CBR, 0, a=f_in, b=out, c=rb, cin=conv.in_channels, cout=conv.out_channels, layer=layer,
-                  x0=int(f_in != 0))
+                  x0=int(f_in not in self.no_grad))
         return out
 
     def cat(self, fa, fb):
@@ -132,12 +140,29 @@ class Plan:
         self._row(OP_CAT, 0, a=fa, b=fb, c=out)
         return out
 
+    def discard(self, f, iset, site, rate):
+        """StVD layer discard (`layer_voxel_discard`, spconv_backbone.py:134-147) of feature slot `f` over index set `iset`
+        at discard site `site`: -> (feature slot, index set) of the kept rows.  The rate reaches the executor as float64 (two
+        int32 halves of the op row): int(n * (1 - rate)) must round as Python's does."""
+        out_f, out_i = self.n_f, self.n_i
+        self.n_f += 1
+        self.n_i += 1
+        self.f_channels[out_f] = self.f_channels[f]
+        self.iset_group[out_i] = max(self.iset_group.values()) + 1
+        if f in self.no_grad:
+            self.no_grad.add(out_f)
+        lo, hi = (int(v) for v in np.array([rate], dtype=np.float64).view(np.int32))
+        self.discards.append((int(site), len(self.rows_i)))
+        self._row(OP_DISCARD, 1, a=iset, b=out_i, c=int(site), ks=(lo, hi, 0), cin=f, cout=out_f)
+        return out_f, out_i
+
     def publish(self, name, f_slot, iset):
         """The op producing `f_slot` is marked (x1 = 1): its fp32 output is read outside the plan.  The executor writes fp32
         activations only where such a reader exists; the bf16 kernels read the bf16 shadow."""
         self.published.append((name, f_slot, iset))
         for row in self.rows_i:
-            if (row[0] == OP_CBR and row[3] == f_slot) or (row[0] == OP_CAT and row[4] == f_slot):
+            if ((row[0] == OP_CBR and row[3] == f_slot) or (row[0] == OP_CAT and row[4] == f_slot)
+                    or (row[0] == OP_DISCARD and row[19] == f_slot)):
                 row[22] = 1
         self._final = None
 
@@ -326,6 +351,18 @@ class _Run:
         p = self.query(2, iset)[6]
         return _view(self.arena, p, (1,), torch.int32) if p else None
 
+    def kept_rows(self):
+        """The rows each layer discard of this run kept, one int32 tensor per site in site order: [k] in exact mode;
+        capacity-sized with a -1 tail and the device count as `.num_rows` in static mode."""
+        out = []
+        for site, op in sorted(self.plan.discards):
+            p, k, pk, n_in, _ = self.query(5, op)[:5]
+            t = _view(self.arena, p, (k,), torch.int32)
+            if self.static is not None:
+                t.num_rows = _view(self.arena, pk, (1,), torch.int32)
+            out.append(t)
+        return out
+
     def rulebook(self, rb):
         """(nbr [K, n_out] int32, nbr_bwd or None, pair_num or None, meta dict) — tests compare these with the oracle."""
         p, pbw, ppn, K, n_in, n_out, subm, unique = self.query(3, rb)
@@ -338,19 +375,20 @@ class _Run:
 class LazyIndiceDict(dict):
     """`SparseConvTensor.indice_dict` of the tensors a plan publishes: {indice_key: ops.Rulebook} like the module path
     leaves behind (spconv caches its indice pairs there), but materialised on first access — building a dozen tensor
-    views per step for a dictionary nobody reads would be pure host overhead."""
+    views per step for a dictionary nobody reads would be pure host overhead.  `group`: the index-set group
+    (Plan.iset_group) of the tensors the dictionary belongs to."""
 
-    def __init__(self, run, coords0, shape0):
+    def __init__(self, run, coords0, shape0, group=0):
         super().__init__()
-        self._src = (run, coords0, shape0)
+        self._src = (run, coords0, shape0, group)
 
     def _fill(self):
         if self._src is None:
             return
-        run, coords0, shape0 = self._src
+        run, coords0, shape0, group = self._src
         self._src = None
         for rb, (keys, ndim, i_in, i_out) in run.plan.rb_keys.items():
-            if not keys:
+            if not keys or run.plan.iset_group[i_out] != group:
                 continue
             nbr, nbw, pn, meta = run.rulebook(rb)
             oidx, oshape = (coords0, list(shape0)) if i_out == 0 else run.indices(i_out)
@@ -451,12 +489,13 @@ def _index_streams(dev, inputs_ready=False):
 
 
 def _exec_forward(plan, feats, coords, spatial_shape, batch_size, proj, training, precision, static, arena, side, side2,
-                  side_waits_main):
-    """One vc_exec_forward call (only one phase where static.phase says so) -> (return code, state blob)."""
+                  side_waits_main, seed=None):
+    """One vc_exec_forward_seeded call (only one phase where static.phase says so) -> (return code, state blob).  seed:
+    device int64[1] of the plan's layer discards."""
     oi, of, lf, _, _ = plan.finalize()
     tab, lib, dev = _layer_ptrs(plan), _lib.load(), feats.device
     state = np.zeros(lib.vc_exec_state_bytes(), dtype=np.uint8)
-    return lib.vc_exec_forward(
+    return lib.vc_exec_forward_seeded(
         oi.ctypes.data, of.ctypes.data, oi.shape[0], tab.ctypes.data, lf.ctypes.data, len(plan.layers), feats.data_ptr(),
         feats.shape[1], coords.data_ptr(), feats.shape[0], _lib.host_i32(spatial_shape), int(batch_size),
         proj.data_ptr() if proj is not None else None, int(training), int(precision == 'bf16'),
@@ -464,7 +503,8 @@ def _exec_forward(plan, feats, coords, spatial_shape, batch_size, proj, training
         ops.tc_error_flag(dev).data_ptr(), state.ctypes.data, state.size, ops._stream(),
         side.cuda_stream if side is not None else None, int(side_waits_main),
         static.caps_array().ctypes.data if static is not None else None, static.n_dev.data_ptr() if static is not None else None,
-        static.overflow.data_ptr() if static is not None else None, side2.cuda_stream if side2 is not None else None), state
+        static.overflow.data_ptr() if static is not None else None, side2.cuda_stream if side2 is not None else None,
+        seed.data_ptr() if seed is not None else None), state
 
 
 class PlanFn(torch.autograd.Function):
@@ -472,7 +512,7 @@ class PlanFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, plan, holder, feats, coords, spatial_shape, batch_size, proj, training, precision, inputs_ready, static,
-                with_bwd, *params):
+                with_bwd, seed, *params):
         ctx.set_materialize_grads(False)     # published tensors the loss does not touch arrive as None, not as zeros
         dev = feats.device
         feats = feats.contiguous()
@@ -501,7 +541,7 @@ class PlanFn(torch.autograd.Function):
             else:
                 arena = _alloc_arena(plan, nbytes, dev, None)
             rc, state = _exec_forward(plan, feats, coords, spatial_shape, batch_size, proj, training, precision, static, arena,
-                                      side_obj, side2_obj, side_waits_main=not (inputs_ready and side_obj is not None))
+                                      side_obj, side2_obj, side_waits_main=not (inputs_ready and side_obj is not None), seed=seed)
             if rc != VC_ERR_WORKSPACE:
                 break
             # too small (first use of a plan on an unusually dense batch): the call is restartable — nothing it enqueued is
@@ -520,7 +560,7 @@ class PlanFn(torch.autograd.Function):
         if TIMING:
             global LAST_RUN
             LAST_RUN = run
-        ctx.run, ctx.feats, ctx.coords, ctx.proj = run, feats, coords, proj
+        ctx.run, ctx.feats, ctx.coords, ctx.proj, ctx.seed = run, feats, coords, proj, seed
         return tuple(run.feature(slot) for _, slot, _ in plan.published)
 
     @staticmethod
@@ -553,27 +593,30 @@ class PlanFn(torch.autograd.Function):
         run.flat_grad = flat
         views = flat.split(sizes)
         out = [v.view_as(p) for v, p in zip(views, plan.params())]
-        return (None,) * 12 + tuple(out)
+        return (None,) * 13 + tuple(out)
 
 
-def run_index(plan, feats, coords_i32, spatial_shape, batch_size, proj, training, precision, static):
+def run_index(plan, feats, coords_i32, spatial_shape, batch_size, proj, training, precision, static, seed=None):
     """Phase 1 of a phased static execution: enqueue ONLY the index operators of the plan (rulebooks, projection) into
     `static.arena`; `run_plan` with `static.phase == 2` later enqueues the feature operators over the same arena."""
     ops._require_cuda(feats, coords_i32)
     assert static is not None and static.arena is not None and static.phase == 1
     rc, _ = _exec_forward(plan, feats, coords_i32, spatial_shape, batch_size, proj, training, precision, static, static.arena,
-                          *_index_streams(feats.device), side_waits_main=True)
+                          *_index_streams(feats.device), side_waits_main=True, seed=seed)
     check(rc, 'vc_exec_forward (index phase)')
 
 
-def run_plan(plan, feats, coords_i32, spatial_shape, batch_size, proj, training, precision, inputs_ready=False, static=None):
+def run_plan(plan, feats, coords_i32, spatial_shape, batch_size, proj, training, precision, inputs_ready=False, static=None,
+             seed=None):
     """-> (run record, {name: (features, indices, spatial_shape, bf16 shadow, device row count or None)}).  `coords_i32`
     [N,4] int32 contiguous (b,z,y,x).  inputs_ready: the caller vouches that `coords_i32` and `proj` are complete in the
     SIDE stream's order (resident from an earlier step, or produced on / synchronised with ops.side(device).stream): the
     index pipeline then does not wait for the main stream and overlaps the previous step's backward.  static: a StaticSpec
-    (capacity-sized tensors, device row counts, no host synchronisation: CUDA-graph capturable)."""
+    (capacity-sized tensors, device row counts, no host synchronisation: CUDA-graph capturable).  seed: device int64[1], the
+    draw of the plan's layer discards (Plan.discard), read on the index stream after everything queued on main so far."""
     ops._require_cuda(feats, coords_i32)
     assert coords_i32.dtype == torch.int32 and coords_i32.is_contiguous()
+    inputs_ready = inputs_ready and seed is None       # (the seed is drawn on main: the index stream must wait for it)
     holder = []
     # the arena also holds what a backward saves / stages: sized for it whenever autograd will record this call
     with_bwd = bool(training) or (torch.is_grad_enabled() and (feats.requires_grad or any(p.requires_grad for p in plan.params())))
@@ -587,7 +630,7 @@ def run_plan(plan, feats, coords_i32, spatial_shape, batch_size, proj, training,
         static.param_aliases = {id(p): a for p, a in zip(params, aliases)}
         params = aliases
     outs = PlanFn.apply(plan, holder, feats, coords_i32, list(spatial_shape), batch_size, proj, training, precision,
-                        bool(inputs_ready), static, with_bwd, *params)
+                        bool(inputs_ready), static, with_bwd, seed, *params)
     run = holder[0]
     res = {}
     for (name, slot, iset), f in zip(plan.published, outs):

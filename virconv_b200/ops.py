@@ -659,6 +659,28 @@ class GatherRowsFn(torch.autograd.Function):
         return din, None
 
 
+def stvd_layer_keep(n, rate, site, seed=None, keys=None, n_dev=None, device=None):
+    """Device-drawn StVD layer discard rows (vc_stvd_layer_keep): over n rows (n_dev: device int32[1] of valid rows, n
+    the capacity), the k = int(n_valid * (1 - rate)) rows with the smallest (Philox key of (row, site) under `seed`, row),
+    or of the given uint32 `keys` (an int64 / int32 tensor holding them), ascending.  -> (keep [n] int32 with a -1 tail,
+    kept [1] int32, pos [n] int32 = position in keep or -1)."""
+    lib = _lib.load()
+    dev = torch.device(device) if device is not None else (seed if seed is not None else keys).device
+    n = int(n)
+    keep = torch.empty((n,), dtype=torch.int32, device=dev)
+    pos = torch.empty((n,), dtype=torch.int32, device=dev)
+    kept = torch.empty((1,), dtype=torch.int32, device=dev)
+    if keys is not None:
+        keys = keys.to(device=dev, dtype=torch.int64).to(torch.int32).contiguous()     # (bit pattern of the uint32 keys)
+        assert keys.numel() >= n
+    if seed is not None:
+        assert seed.dtype == torch.int64 and seed.device == dev
+    ws = _ws(lib.vc_stvd_layer_keep_ws_bytes(n), dev)
+    check(lib.vc_stvd_layer_keep(_p(keys), _p(seed), int(site), n, _p(n_dev), float(rate), _p(keep), _p(kept), _p(pos), _p(ws),
+                                 ws.numel(), _stream()), 'vc_stvd_layer_keep')
+    return keep, kept, pos
+
+
 # ------------------------------------------------------------------------------------------------
 # voxelisation + MeanVFE, voxel -> row map
 # ------------------------------------------------------------------------------------------------
