@@ -165,6 +165,48 @@ int vc_conv_wgrad_tc(const void* in_bf16, const void* dout_bf16, const int32_t* 
                      int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag, vc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Deterministic variants (the plan executor's mode under torch.use_deterministic_algorithms): no float atomics, every
+ * reduction in an order fixed by the data alone, so the results are bit-identical from run to run and for every grid
+ * size / CTA cap.
+ * ---------------------------------------------------------------------------------------------- */
+/* Conv forward (precision 0: fp32 `in`, gather_gemm_kernel; 1: bf16 `in`, the persistent tensor-core kernel) with the
+ * BatchNorm channel sums: every 128-row tile writes its float64 partial [2, cout], then the partials are added in tile
+ * order into bn_sums [2, cout] (overwritten, not accumulated).  cin, cout in {8,16,32,64}.
+ * ws >= vc_conv_fwd_det_ws_bytes(n_out, cin, cout, K). */
+size_t vc_conv_fwd_det_ws_bytes(int n_out, int cin, int cout, int K);
+int vc_conv_fwd_det(int precision, const void* in, const float* w, const int32_t* nbr, float* out, int n_out, int cin, int cout,
+                    int K, double* bn_sums, void* ws, size_t ws_bytes, int32_t* err_flag, vc_stream_t stream);
+/* vc_conv_wgrad_tc with the rows split into 32 runs of consecutive 128-row tiles (from n_out alone); a CTA claims whole
+ * runs, each run's sum goes to its own fp32 image, and the images are added in run order.  The CTA cap of
+ * vc_conv_wgrad_tc3_config applies (0: one CTA per SM).  ws >= vc_conv_wgrad_tc_det_ws_bytes(...) (32 images). */
+size_t vc_conv_wgrad_tc_det_ws_bytes(int n_out, int cin, int cout, int K);
+int vc_conv_wgrad_tc_det(const void* in_bf16, const void* dout_bf16, const int32_t* nbr, float* dw, int n_out, int cin,
+                         int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag, vc_stream_t stream);
+/* vc_bn_relu_bwd_f32 with (sum g, sum g*xhat) reduced per 512-row chunk into float64 partials (ws) and added in chunk order
+ * (vc_set_bn_fused selects one cooperative launch or two, with the same result).  ws >= vc_bn_bwd_det_ws_bytes(n, c). */
+size_t vc_bn_bwd_det_ws_bytes(int n, int c);
+int vc_bn_relu_bwd_det_f32(const float* dy, const float* x, const float* gamma, const float* stats, float* dx, void* dx_bf16,
+                           float* dgamma, float* dbeta, int n, int c, int training, void* ws, size_t ws_bytes, vc_stream_t stream);
+/* vc_subm_rulebook plus rep [n]: the lowest row at each row's own coordinate (the row itself when it lies outside the grid)
+ * — the groups of rows the many-to-one 2-D tables merge. */
+int vc_subm_rulebook_rep(const int32_t* indices, int n, int ndim, int batch_size, const int32_t* spatial_shape,
+                         const int32_t* ksize, const int32_t* dilation, int32_t* nbr, int32_t* pair_num, int32_t* rep, void* ws,
+                         size_t ws_bytes, vc_stream_t stream);
+/* Input gradient of a many-to-one submanifold table (odd kernel sizes) in gather form, OVERWRITING din [n, cin]:
+ *   din[i] = W_c^T dout[i] + [rep[i] == i] sum_{k != c} W_k^T S[p(i) - delta_k],
+ * S[p] = the sum of dout over the rows at pixel p in ascending row order — equal to vc_conv_dgrad_scatter_* up to the
+ * summation order.  The rows are grouped by rep with integer atomics, each group sorted, and the result comes from one
+ * mirrored gather dgrad over [dout; S] (fp32: gather_gemm_kernel; tc: bf16 dout and S, the persistent tensor-core kernel).
+ * n_dev (device int32, may be NULL): rows below it are valid, n is the capacity (table tail -1, din tail 0).
+ * ws >= vc_conv_dgrad_gather2d_ws_bytes(n, cin, cout, K). */
+size_t vc_conv_dgrad_gather2d_ws_bytes(int n, int cin, int cout, int K);
+int vc_conv_dgrad_gather2d_f32(const float* dout, const float* w, const int32_t* nbr, const int32_t* rep, float* din, int n,
+                               const int32_t* n_dev, int cin, int cout, int K, void* ws, size_t ws_bytes, vc_stream_t stream);
+int vc_conv_dgrad_gather2d_tc(const void* dout_bf16, const float* w, const int32_t* nbr, const int32_t* rep, float* din, int n,
+                              const int32_t* n_dev, int cin, int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag,
+                              vc_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * BatchNorm1d(eps, momentum) + ReLU over the active rows.  Replaces the `norm_fn(out_channels)`,
  * `nn.ReLU()` members of every `spconv.SparseSequential` (spconv_backbone.py:101-105, :160, :561-567).
  * ---------------------------------------------------------------------------------------------- */
@@ -513,7 +555,12 @@ int vc_rcnn_loss(const vc_rcnn_branch* branches /*host[K]*/, int K, double beta,
  * flags: bits 8-9 = phase (static mode only).  0 enqueues the whole forward, 1 ONLY the index operators (rulebooks,
  * projections), 2 ONLY the feature operators (weight images, conv + BN + ReLU, concat) over the arena phase 1 filled: call
  * both with the same arguments, so they allocate the same addresses and leave the same state (graph.PipelinedStep runs
- * the index phase of step t+1 beside the feature phase of step t).  Other bits are ignored (callers pass bit 0 = 1).
+ * the index phase of step t+1 beside the feature phase of step t).  Bit 2 = deterministic mode, recorded in the state
+ * for the backward: the BN sums of the conv forward per 128-row tile and of BN backward per 512-row chunk, the
+ * tensor-core wgrad per row run (32 images per layer), all added in a fixed order, and the many-to-one 2-D tables'
+ * input gradient in gather form (vc_conv_dgrad_gather2d_*; timing kinds 8 / 9) — published features, indices, BN
+ * running statistics and gradients are then bit-identical from run to run.  Other bits are ignored (callers pass
+ * bit 0 = 1).
  * ---------------------------------------------------------------------------------------------- */
 size_t vc_exec_state_bytes(void);
 int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_ops, const uint64_t* layer_ptrs, const float* layer_f,
@@ -542,7 +589,8 @@ int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, int n_ops, 
 int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_ops, const uint64_t* layer_ptrs, const float* layer_f,
                      int n_layers, const int32_t* pub_slots, const uint64_t* ext_grads, int n_pub, void* arena,
                      size_t arena_bytes, int32_t* err_flag, void* state, vc_stream_t stream, vc_stream_t wgrad_stream);
-/* Read a state blob.  what 0: out[0] = arena bytes in use;  1 (feature slot id): f32 ptr, bf16 ptr, rows, c;
+/* Read a state blob.  what 0: out[0] = arena bytes in use, out[1] = of them, the deterministic mode's partials, tables and
+ * operands, out[2] = deterministic mode;  1 (feature slot id): f32 ptr, bf16 ptr, rows, c;
  * 2 (index set): idx ptr, n, ndim, shape[3];  3 (rulebook): nbr, nbr_bwd, pair_num ptrs, K, n_in, n_out, subm, unique;
  * 4 (layer): x ptr, y ptr, stats ptr, forward runs on the tensor cores, rulebook id, in slot, out slot;  5 (op index of a
  * DISCARD): keep ptr, kept rows (exact mode; static mode: the capacity), kept_dev ptr, n_in, site.  out: >= 8 int64
@@ -550,7 +598,8 @@ int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_ops, const 
 int vc_exec_query(const void* state, int what, int id, long long* out);
 /* Optional per-launch timing of the conv kernels (bench.py's roofline pass): vc_exec_timing(1) clears and arms it,
  * vc_exec_timing_read synchronises and returns up to max_records (ms, [kind, layer]) records; kind 0 fwd f32, 1 fwd tc,
- * 2 dgrad f32, 3 dgrad tc, 4 dgrad scatter f32, 5 wgrad f32, 6 wgrad tc, 7 dgrad scatter tc. */
+ * 2 dgrad f32, 3 dgrad tc, 4 dgrad scatter f32, 5 wgrad f32, 6 wgrad tc, 7 dgrad scatter tc, 8 dgrad gather2d f32,
+ * 9 dgrad gather2d tc. */
 int vc_exec_timing(int enable);
 int vc_exec_timing_read(float* ms_out, int32_t* kind_layer_out, int max_records);
 

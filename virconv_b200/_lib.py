@@ -51,6 +51,16 @@ SIGNATURES = {
     'vc_conv_dgrad_scatter_tc': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _Z, _P, _P]),
     'vc_conv_wgrad_tc_ws_bytes': (_Z, [_I, _I, _I, _I]),
     'vc_conv_wgrad_tc': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _Z, _P, _P]),
+    'vc_conv_fwd_det_ws_bytes': (_Z, [_I, _I, _I, _I]),
+    'vc_conv_fwd_det': (_I, [_I, _P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _P, _P]),
+    'vc_conv_wgrad_tc_det_ws_bytes': (_Z, [_I, _I, _I, _I]),
+    'vc_conv_wgrad_tc_det': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _Z, _P, _P]),
+    'vc_bn_bwd_det_ws_bytes': (_Z, [_I, _I]),
+    'vc_bn_relu_bwd_det_f32': (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _Z, _P]),
+    'vc_subm_rulebook_rep': (_I, [_P, _I, _I, _I, _HOST, _HOST, _HOST, _P, _P, _P, _P, _Z, _P]),
+    'vc_conv_dgrad_gather2d_ws_bytes': (_Z, [_I, _I, _I, _I]),
+    'vc_conv_dgrad_gather2d_f32': (_I, [_P, _P, _P, _P, _P, _I, _P, _I, _I, _I, _P, _Z, _P]),
+    'vc_conv_dgrad_gather2d_tc': (_I, [_P, _P, _P, _P, _P, _I, _P, _I, _I, _I, _P, _Z, _P, _P]),
     'vc_bn_apply_relu_f32': (_I, [_P, _P, _I, _I, _P, _P, _P, _P, _P, _F, _F, _I, _P, _P, _P, _I, _P]),
     'vc_bn_relu_bwd_f32': (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _P]),
     'vc_index2uv': (_I, [_P, _I, _I, _P, _HOSTF, _I, _I, _I, _P, _P]),

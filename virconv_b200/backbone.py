@@ -20,9 +20,11 @@ layer_voxel_discard :134-147.  Differences that do not change results:
 """
 from __future__ import annotations
 
+import warnings
 from functools import partial
 
 import numpy as np
+
 import torch
 import torch.nn as nn
 
@@ -334,6 +336,9 @@ class VirConvL8x(nn.Module):
                     'multi_scale_3d_strides' + rid: {'x_conv1': 1, 'x_conv2': 2, 'x_conv3': 4, 'x_conv4': 8},
                 })
                 continue
+            _module_path_under_determinism(_module_path_reason(
+                feats, self._plan() if executor.ENABLED and feats.is_cuda else None,
+                self._discarding() and (self.discard_rng != 'device' or batch_dict.get('stvd_keep_rows') is not None)))
             proj = ops.projection_params(calib, trans, batch_size, feats.device)
             x = spconv.SparseConvTensor(feats, coords.int(), self.sparse_shape, batch_size)
 
@@ -353,6 +358,36 @@ class VirConvL8x(nn.Module):
                 'multi_scale_3d_strides' + rid: {'x_conv1': 1, 'x_conv2': 2, 'x_conv3': 4, 'x_conv4': 8},
             })
         return batch_dict
+
+
+def _module_path_under_determinism(reason):
+    """torch.use_deterministic_algorithms(True) and a forward that takes the per-operator module path, whose scatter
+    dgrads, weight gradients and BatchNorm sums use float atomics: torch's contract for an operation without a
+    deterministic implementation — raise, or warn under warn_only=True."""
+    if not torch.are_deterministic_algorithms_enabled():
+        return
+    msg = ('VirConv backbone: the per-operator module path (%s) has no deterministic implementation; the plan executor '
+           'has one' % reason)
+    if torch.is_deterministic_algorithms_warn_only_enabled():
+        warnings.warn(msg)
+    else:
+        raise RuntimeError(msg)
+
+
+def _module_path_reason(feats, plan=None, discard=False):
+    if not executor.ENABLED:
+        return 'VIRCONV_EXECUTOR=0'
+    if not feats.is_cuda:
+        return 'features not on a CUDA device'
+    if feats.shape[0] == 0:
+        return 'no input voxels'
+    if feats.requires_grad:
+        return 'gradient into the voxel features'
+    if discard:
+        return 'host-drawn or caller-given StVD layer discard'
+    if plan is not None and not plan.eligible():
+        return 'SyncBatchNorm, momentum=None, bias or a non-fp32 module'
+    return 'BatchNorm layers in mixed train / eval modes'
 
 
 def decompose_tensor(t, i, batch_size):
@@ -478,6 +513,7 @@ class VirConv8x(nn.Module):
             plan = self._plan_lidar()
         if self._plan_usable(plan, feats):
             return self._run(plan, feats, coords, shape, batch_size, None, ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4', 'out'))[1]
+        _module_path_under_determinism(_module_path_reason(feats, plan))
         x = spconv.SparseConvTensor(feats, coords.int(), shape, batch_size)
         x1 = self.conv1(self.conv_input(x))
         x2 = self.conv2(x1)
@@ -548,6 +584,7 @@ class VirConv8x(nn.Module):
                         'multi_scale_3d_features_mm' + s: {'x_conv1': x1, 'x_conv2': x2, 'x_conv3': x3, 'x_conv4': x4},
                         'multi_scale_3d_strides' + s: dict(strides)})
                     continue
+                _module_path_under_determinism(_module_path_reason(feats, self._plan_mm(stvd), discarding and not stvd))
                 proj = ops.projection_params(calib, trans, batch_size, feats.device)
                 x = spconv.SparseConvTensor(feats, coords.int(), self.sparse_shape, batch_size)
                 x = self._maybe_discard(x, batch_dict, 0)              # VirConv8x also discards the input voxels (:489-490)

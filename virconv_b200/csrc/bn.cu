@@ -108,16 +108,110 @@ __global__ void __launch_bounds__(256) bn_apply_relu_kernel(
     }
 }
 
+// ---- deterministic mode (torch.use_deterministic_algorithms): fixed-order float64 reductions ------------------------------
+// Partials are keyed by a unit of work that does not depend on the launch (a conv's 128-row tile, a BN_DET_ROWS chunk of
+// rows); they are summed in that unit's order, so the result is bit-identical for every grid size and every schedule.
+
+// sums[j] = sum over parts p < n_parts of part[p][j], j < 2c: one block per column, thread t takes parts t, t + 256, ...
+// in ascending order, then a fixed tree.  n_parts = cdiv(rows, rows_per_part), rows from n_dev when given.
+__global__ void __launch_bounds__(256) bn_sums_reduce_kernel(const double* __restrict__ part, int cap_rows, const int* __restrict__ n_dev,
+                                                             int rows_per_part, int c, double* __restrict__ sums) {
+    __shared__ double red[256];
+    pdl_wait();
+    pdl_launch_dependents();
+    const int rows = n_dev != nullptr ? min(cap_rows, __ldg(n_dev)) : cap_rows;
+    const int n_parts = (rows + rows_per_part - 1) / rows_per_part;
+    const int j = blockIdx.x;
+    double v = 0.0;
+    for (int p = threadIdx.x; p < n_parts; p += 256) v += part[(size_t)p * 2 * c + j];
+    red[threadIdx.x] = v;
+    __syncthreads();
+    for (int s = 128; s > 0; s >>= 1) {
+        if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) sums[j] = red[0];
+}
+
+// BN backward, deterministic: chunk ch = rows [ch * BN_DET_ROWS, ...) -> part[ch][2][c] = (sum g, sum g*xhat) in float64.
+// Thread (cg, rl) takes rows rl, rl + rowlanes, ... of the chunk; the row lanes are added in lane order.  Needs
+// rowlanes * 2 * c floats of shared memory (shf) and a __syncthreads-uniform call.
+__device__ __forceinline__ void bn_bwd_chunk_partials(const float4* __restrict__ dy, int dy_ld4, const float4* __restrict__ x,
+                                                      const float* __restrict__ stats, int n, int c, double* __restrict__ part,
+                                                      float* shf) {
+    const int c4 = c / 4, cg = threadIdx.x % c4, rl = threadIdx.x / c4, rowlanes = blockDim.x / c4;
+    const float4 sc = reinterpret_cast<const float4*>(stats)[cg];
+    const float4 sh = reinterpret_cast<const float4*>(stats + c)[cg];
+    const float4 m = reinterpret_cast<const float4*>(stats + 2 * c)[cg];
+    const float4 is = reinterpret_cast<const float4*>(stats + 3 * c)[cg];
+    const int n_chunks = (n + BN_DET_ROWS - 1) / BN_DET_ROWS;
+    for (int chk = blockIdx.x; chk < n_chunks; chk += gridDim.x) {
+        const int end = min(n, (chk + 1) * BN_DET_ROWS);
+        float s[4] = {0, 0, 0, 0}, q[4] = {0, 0, 0, 0};
+        for (int row = chk * BN_DET_ROWS + rl; row < end; row += rowlanes) {
+            const size_t i = (size_t)row * c4 + cg;
+            float4 g = dy[(size_t)row * dy_ld4 + cg], xx = x[i];
+            g.x = fmaf(xx.x, sc.x, sh.x) > 0.f ? g.x : 0.f; g.y = fmaf(xx.y, sc.y, sh.y) > 0.f ? g.y : 0.f;
+            g.z = fmaf(xx.z, sc.z, sh.z) > 0.f ? g.z : 0.f; g.w = fmaf(xx.w, sc.w, sh.w) > 0.f ? g.w : 0.f;
+            s[0] += g.x; s[1] += g.y; s[2] += g.z; s[3] += g.w;
+            q[0] = fmaf(g.x, (xx.x - m.x) * is.x, q[0]); q[1] = fmaf(g.y, (xx.y - m.y) * is.y, q[1]);
+            q[2] = fmaf(g.z, (xx.z - m.z) * is.z, q[2]); q[3] = fmaf(g.w, (xx.w - m.w) * is.w, q[3]);
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            shf[(rl * 2 + 0) * c + cg * 4 + j] = s[j];
+            shf[(rl * 2 + 1) * c + cg * 4 + j] = q[j];
+        }
+        __syncthreads();
+        if (threadIdx.x < 2 * c) {
+            const int which = threadIdx.x / c, ch = threadIdx.x % c;
+            double v = 0.0;
+            for (int l = 0; l < rowlanes; ++l) v += (double)shf[(l * 2 + which) * c + ch];
+            part[(size_t)chk * 2 * c + which * c + ch] = v;
+        }
+        __syncthreads();
+    }
+}
+
+// (S, Q) of every channel from the chunk partials, the same in every block: thread t adds chunks sub, sub + nsub, ... of
+// column t % 2c (sub = t / 2c), the subs are then added in order.  dsh: 256 doubles of shared memory.  Returns through
+// S_out / Q_out for threads < c.
+__device__ __forceinline__ void bn_bwd_sum_partials(const double* __restrict__ part, int n, int c, double* dsh, double& S_out,
+                                                    double& Q_out) {
+    const int n_chunks = (n + BN_DET_ROWS - 1) / BN_DET_ROWS;
+    const int cols = 2 * c, nsub = blockDim.x / cols;
+    const int col = threadIdx.x % cols, sub = threadIdx.x / cols;
+    double v = 0.0;
+    if (sub < nsub)
+        for (int chk = sub; chk < n_chunks; chk += nsub) v += __ldcg(part + (size_t)chk * cols + col);
+    dsh[threadIdx.x] = v;
+    __syncthreads();
+    if (threadIdx.x < c) {
+        double S = 0.0, Q = 0.0;
+        for (int u = 0; u < nsub; ++u) {
+            S += dsh[u * cols + threadIdx.x];
+            Q += dsh[u * cols + c + threadIdx.x];
+        }
+        S_out = S;
+        Q_out = Q;
+    }
+    __syncthreads();
+}
+
 // backward pass 1: sum g and sum g*xhat over rows, g = dy*(y>0); block partial -> float64 atomics on bsums [2, c]
 // (the ReLU mask is recomputed from x with the forward's own scale / shift and fmaf: bit-identical to testing y > 0,
 //  so the activation itself is not read again; dy may be a column slice of a wider matrix: row pitch dy_ld4 float4)
 __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const float4* __restrict__ dy, int dy_ld4, const float4* __restrict__ x,
                                                             const float* __restrict__ stats, int n, const int* __restrict__ n_dev,
-                                                            int c, double* __restrict__ bsums) {
+                                                            int c, double* __restrict__ bsums, double* __restrict__ part) {
     extern __shared__ float shf[];  // [rowlanes][2][c]
     pdl_wait();
     pdl_launch_dependents();
     if (n_dev != nullptr) n = min(n, __ldg(n_dev));
+    if (part != nullptr) {          // deterministic: per-chunk partials, summed by the apply kernel
+        bn_bwd_chunk_partials(dy, dy_ld4, x, stats, n, c, part, shf);
+        return;
+    }
     const int c4 = c / 4;
     const int cg = threadIdx.x % c4, rl = threadIdx.x / c4, rowlanes = blockDim.x / c4;
     const float4 sc = reinterpret_cast<const float4*>(stats)[cg];
@@ -155,7 +249,8 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const float4* __restr
                                                            const double* __restrict__ bsums, int n_rows,
                                                            const int* __restrict__ n_dev, int c, int training,
                                                            float4* __restrict__ dx, uint2* __restrict__ dx_bf16,
-                                                           float* __restrict__ dgamma, float* __restrict__ dbeta, int tail_zero) {
+                                                           float* __restrict__ dgamma, float* __restrict__ dbeta, int tail_zero,
+                                                           const double* __restrict__ part) {
     pdl_wait();                 // bsums from the reduce kernel
     pdl_launch_dependents();
     const int cap_rows = n_rows;
@@ -166,9 +261,15 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const float4* __restr
     const size_t stride = (size_t)gridDim.x * blockDim.x;
     const int cg = (int)(i0 % c4);
     __shared__ float a_s[128], b_s[128], d_s[128];
+    __shared__ double dsh[256];
+    double S = 0.0, Q = 0.0;
+    if (part != nullptr) bn_bwd_sum_partials(part, n_rows, c, dsh, S, Q);
     if (threadIdx.x < c) {
         const int ch = threadIdx.x;
-        const double S = bsums[ch], Q = bsums[c + ch];
+        if (part == nullptr) {
+            S = bsums[ch];
+            Q = bsums[c + ch];
+        }
         const float mean = stats[2 * c + ch], invstd = stats[3 * c + ch];
         const float gi = gamma[ch] * invstd;
         if (training) {
@@ -223,12 +324,15 @@ __global__ void __launch_bounds__(256) bn_bwd_fused_kernel(const float4* __restr
                                                            const float* __restrict__ gamma, const float* __restrict__ stats,
                                                            double* __restrict__ bsums, int n_rows, const int* __restrict__ n_dev, int c,
                                                            int training, float4* __restrict__ dx, uint2* __restrict__ dx_bf16,
-                                                           float* __restrict__ dgamma, float* __restrict__ dbeta, int tail_zero) {
+                                                           float* __restrict__ dgamma, float* __restrict__ dbeta, int tail_zero,
+                                                           double* __restrict__ part) {
     extern __shared__ float shf[];  // [rowlanes][2][c]
     const int cap_rows = n_rows;
     if (n_dev != nullptr) n_rows = min(n_rows, __ldg(n_dev));
     const int c4 = c / 4;
-    {
+    if (part != nullptr) {          // deterministic: per-chunk partials, summed in chunk order after the barrier
+        bn_bwd_chunk_partials(dy, dy_ld4, x, stats, n_rows, c, part, shf);
+    } else {
         const int cg = threadIdx.x % c4, rl = threadIdx.x / c4, rowlanes = blockDim.x / c4;
         const float4 sc = reinterpret_cast<const float4*>(stats)[cg];
         const float4 sh = reinterpret_cast<const float4*>(stats + c)[cg];
@@ -267,9 +371,14 @@ __global__ void __launch_bounds__(256) bn_bwd_fused_kernel(const float4* __restr
     float* b_s = shf + 128;
     float* d_s = shf + 256;
     __syncthreads();
+    double S = 0.0, Q = 0.0;
+    if (part != nullptr) bn_bwd_sum_partials(part, n_rows, c, reinterpret_cast<double*>(shf + 512), S, Q);
     if (threadIdx.x < c) {
         const int ch = threadIdx.x;
-        const double S = __ldcg(bsums + ch), Q = __ldcg(bsums + c + ch);
+        if (part == nullptr) {
+            S = __ldcg(bsums + ch);
+            Q = __ldcg(bsums + c + ch);
+        }
         const float mean = stats[2 * c + ch], invstd = stats[3 * c + ch];
         const float gi = gamma[ch] * invstd;
         if (training) {
@@ -349,7 +458,7 @@ int vc::bn_apply_relu_dev(const float* x, const double* sums, int n_rows, const 
 
 int vc::bn_relu_bwd_dev(const float* dy, int dy_ld, const float* x, const float* gamma, const float* stats, float* dx,
                         void* dx_bf16, float* dgamma, float* dbeta, int n, const int* n_dev, int c, int training,
-                        double* bsums, int tail_zero, cudaStream_t stream) {
+                        double* bsums, int tail_zero, cudaStream_t stream, double* part) {
     VC_CHECK_ARG(c_ok(c) && n >= 0, "bad args n=%d c=%d", n, c);
     VC_CHECK_ARG(dgamma && dbeta && bsums && stats && gamma, "null pointer");
     VC_CHECK_ARG(dy_ld % 4 == 0 && dy_ld >= c, "bad gradient pitch");
@@ -367,14 +476,15 @@ int vc::bn_relu_bwd_dev(const float* dy, int dy_ld, const float* x, const float*
         const int c4 = c / 4, rowlanes = 256 / c4;
         int blocks = (n + rowlanes - 1) / rowlanes;
         if (blocks > max_blocks) blocks = max_blocks;
-        const size_t smem = (size_t)rowlanes * 2 * c * sizeof(float) < 3 * 128 * sizeof(float) ? 3 * 128 * sizeof(float)
-                                                                                               : (size_t)rowlanes * 2 * c * sizeof(float);
+        // (>= 512 floats + 256 doubles: the apply phase's coefficients and, in deterministic mode, the partial sums)
+        const size_t smem = (size_t)rowlanes * 2 * c * sizeof(float) < 4096 ? 4096 : (size_t)rowlanes * 2 * c * sizeof(float);
         const float4* dy4 = (const float4*)dy;
         const float4* x4 = (const float4*)x;
         int dy_ld4 = dy_ld / 4;
         float4* dx4 = (float4*)dx;
         uint2* dxb = (uint2*)dx_bf16;
-        void* args[] = {&dy4, &dy_ld4, &x4, &gamma, &stats, &bsums, &n, &n_dev, &c, &training, &dx4, &dxb, &dgamma, &dbeta, &tail_zero};
+        void* args[] = {&dy4, &dy_ld4, &x4, &gamma, &stats, &bsums, &n, &n_dev, &c, &training, &dx4, &dxb, &dgamma, &dbeta, &tail_zero,
+                        &part};
         const cudaError_t ce = cudaLaunchCooperativeKernel((const void*)bn_bwd_fused_kernel, dim3(blocks), dim3(256), args, smem, stream);
         if (ce == cudaSuccess) {
             vc::count_launch();
@@ -392,11 +502,11 @@ int vc::bn_relu_bwd_dev(const float* dy, int dy_ld, const float* x, const float*
         if (blocks > 296) blocks = 296;
         size_t smem = (size_t)rowlanes * 2 * c * sizeof(float);
         VC_LAUNCH_CHAIN(bn_bwd_reduce_kernel, dim3(blocks), dim3(256), smem, stream, (const float4*)dy, dy_ld / 4, (const float4*)x,
-                        stats, n, n_dev, c, bsums);
+                        stats, n, n_dev, c, bsums, part);
     }
     VC_LAUNCH_CHAIN(bn_bwd_apply_kernel, dim3(ew_blocks((size_t)n * c / 4)), dim3(256), 0, stream, (const float4*)dy, dy_ld / 4,
                     (const float4*)x, gamma, stats, bsums, n, n_dev, c, training, (float4*)dx, (uint2*)dx_bf16, dgamma, dbeta,
-                    tail_zero);
+                    tail_zero, (const double*)part);
     return VC_OK;
 }
 
@@ -417,6 +527,26 @@ extern "C" int vc_bn_relu_bwd_f32(const float* dy, const float* x, const float* 
     VC_CHECK_ARG(n == 0 || dx, "null pointer");
     return vc::bn_relu_bwd_dev(dy, c, x, gamma, stats, dx, dx_bf16, dgamma, dbeta, n, nullptr, c, training, bsums, 0,
                                (cudaStream_t)stream_);
+}
+
+int vc::bn_sums_reduce_dev(const double* part, int cap_rows, const int* n_dev, int rows_per_part, int c, double* sums,
+                           cudaStream_t stream) {
+    VC_CHECK_ARG(c_ok(c) && cap_rows >= 0 && rows_per_part > 0 && part && sums, "bad bn sums args");
+    VC_LAUNCH_CHAIN(bn_sums_reduce_kernel, dim3(2 * c), dim3(256), 0, stream, part, cap_rows, n_dev, rows_per_part, c, sums);
+    return VC_OK;
+}
+
+extern "C" size_t vc_bn_bwd_det_ws_bytes(int n, int c) {
+    return (size_t)((n + BN_DET_ROWS - 1) / BN_DET_ROWS) * 2 * (c > 0 ? c : 0) * sizeof(double);
+}
+
+extern "C" int vc_bn_relu_bwd_det_f32(const float* dy, const float* x, const float* gamma, const float* stats, float* dx,
+                                      void* dx_bf16, float* dgamma, float* dbeta, int n, int c, int training, void* ws,
+                                      size_t ws_bytes, vc_stream_t stream_) {
+    VC_CHECK_ARG(n == 0 || dx || dx_bf16, "null pointer");
+    VC_CHECK_ARG(ws && ws_bytes >= vc_bn_bwd_det_ws_bytes(n, c), "deterministic BN backward workspace too small");
+    return vc::bn_relu_bwd_dev(dy, c, x, gamma, stats, dx, dx_bf16, dgamma, dbeta, n, nullptr, c, training, (double*)ws, 0,
+                               (cudaStream_t)stream_, (double*)ws);
 }
 
 extern "C" int vc_set_bn_fused(int enable) {

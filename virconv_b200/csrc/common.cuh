@@ -133,7 +133,7 @@ static inline cudaError_t launch_chain(void (*kern)(KP...), dim3 grid, dim3 bloc
 // `n_dev` (optional): the row count lives in device memory and `n` / `n_out` are capacities (static mode, graph capturable)
 int subm_rulebook_dev(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size, const int32_t* spatial_shape,
                       const int32_t* ksize, const int32_t* dilation, int32_t* nbr, int32_t* pair_num, void* ws, size_t ws_bytes,
-                      cudaStream_t stream);
+                      cudaStream_t stream, int32_t* rep = nullptr);   // rep (optional): [n] lowest row at each row's coordinate
 int conv_rulebook_count_dev(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size,
                             const int32_t* spatial_shape, const int32_t* ksize, const int32_t* stride, const int32_t* padding,
                             const int32_t* dilation, int32_t* n_out_dev, int cap_out, int* overflow, void* ws, size_t ws_bytes,
@@ -148,9 +148,14 @@ int bn_apply_relu_dev(const float* x, const double* sums, int n_rows, const int*
                       const float* beta, float* running_mean, float* running_var, long long* num_batches_tracked, float momentum,
                       float eps, int training, float* y, int y_ld, void* y_bf16, int yb_ld, float* stats_out, int relu,
                       int tail_zero, cudaStream_t stream);
+// part (deterministic mode, else NULL): [cdiv(n, BN_DET_ROWS), 2, c] float64 chunk partials, summed in chunk order
 int bn_relu_bwd_dev(const float* dy, int dy_ld, const float* x, const float* gamma, const float* stats, float* dx, void* dx_bf16,
                     float* dgamma, float* dbeta, int n, const int* n_dev, int c, int training, double* bsums, int tail_zero,
-                    cudaStream_t stream);
+                    cudaStream_t stream, double* part = nullptr);
+// deterministic BN sums: sums [2, c] = the per-part partials part [cdiv(rows, rows_per_part), 2, c] added in part order
+int bn_sums_reduce_dev(const double* part, int cap_rows, const int* n_dev, int rows_per_part, int c, double* sums,
+                       cudaStream_t stream);
+static constexpr int BN_DET_ROWS = 512;   // rows per chunk of the deterministic BN backward reduction
 int cat2_dev(const float* a, const float* b, float* out, void* out_bf16, int n, const int* n_dev, int ca, int cb, cudaStream_t stream);
 int index2uv_dev(const int32_t* indices, int n, const int* n_dev, int batch_size, const float* params, const float* grid,
                  int stride, int u_max, int v_max, int32_t* uv_out, cudaStream_t stream);
@@ -186,6 +191,21 @@ int tc_scatter_with_image(int kc, int nr, const void* dout_bf16, const void* wim
 // fp32 scatter dgrad (vc_conv_dgrad_scatter_f32) into a din of row pitch din_ld (>= cin, multiple of 4)
 int conv_dgrad_scatter_f32_ld(const float* dout, const float* w, const int32_t* nbr, float* din, int din_ld, int n_out, int cin,
                               int cout, int K, void* ws, size_t ws_bytes, cudaStream_t stream);
+// ---- gather2d.cu (deterministic input gradient of the many-to-one 2-D tables) ----
+// Groups of rows sharing a coordinate, from rep (vc_subm_rulebook_rep), and the gather table over U = [dout; S] (2 cap rows):
+// nbr_g[centre][i] = i, nbr_g[k][i] = cap + nbr[k][i] for a representative i (rep[i] == i), else -1.
+struct G2Prep {
+    int32_t *nbr_g, *cnt, *off, *rows, *cur, *tot;   // cnt / off / rows: the rows of representative r's group, ascending
+};
+size_t gather2d_prep_bytes(int cap, int K);
+G2Prep gather2d_carve(void* ws, int cap, int K);
+int gather2d_prep_dev(const int32_t* nbr, const int32_t* rep, int K, int cap, const int* n_dev, const G2Prep& P, cudaStream_t st);
+// U rows [cap + r] = sum of g over group r in ascending row order (fp32 sums; g fp32 or bf16, out fp32 and / or bf16)
+int gather2d_sum_dev(const float* g, const void* g_bf16, int c, const G2Prep& P, int cap, const int* n_dev, float* u,
+                     void* u_bf16, cudaStream_t st);
+// dst[r, :] (row pitch ld) += src[r, :] (dense [cap, c]) for r below the row count
+int add_rows_ld_dev(float* dst, int ld, const float* src, int cap, const int* n_dev, int c, cudaStream_t st);
+
 // ---- conv_tc2.cu (persistent tensor-core conv: forward and gather dgrad) ----
 int num_sms();   // of the current device
 size_t tc_image_bytes(int cin, int cout, int K, int layout);
@@ -193,18 +213,28 @@ bool tc2_ch_ok(int c);
 int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_t* nbr, long long pitch, float* out, int n_rows,
              const int* n_dev, int K, double* bn_sums, int* err, cudaStream_t stream, const float* addend,
              int* tile_counter = nullptr, int flags = 0,   // flags: bit 0 sparse offsets (strided dgrad), bit 1 early tables
-             int in_ld = 0);                               // row pitch of in_bf16 (0: kc)
+             int in_ld = 0,                                // row pitch of in_bf16 (0: kc)
+             double* bn_part = nullptr);                   // deterministic BN sums: [tiles, 2, nr] per 128-row tile (bn_sums NULL)
+// fp32 gather conv forward (vc_conv_fwd_f32) whose BN channel sums go to bn_part [tiles, 2, cout] per 128-row tile instead
+int conv_fwd_f32_part(const float* in, const float* w, const int32_t* nbr, float* out, int n_out, int cin, int cout, int K,
+                      double* bn_part, void* ws, size_t ws_bytes, cudaStream_t stream);
 
 // ---- wgrad_tc3.cu (persistent tensor-core wgrad) ----
 extern int g_wgrad3_ctas;
+// det_chunks > 0 (deterministic mode): scratch holds det_chunks partial images [det_chunks][K][cin][cout], zero on entry; the
+// 128-row tiles are split into det_chunks runs of consecutive tiles (from the row count alone), a CTA claims whole runs and
+// writes each run's sum into its own image, so the result does not depend on the grid or the schedule
 int tc3_wgrad(int cin, int cout, const void* in_bf16, const void* dout_bf16, const int32_t* nbr, long long pitch, float* scratch,
               int n_rows, const int* n_dev, int K, int* err, cudaStream_t stream, int* tile_counter, int max_ctas,
-              int in_ld = 0);   // row pitch of in_bf16 (0: cin)
+              int in_ld = 0,    // row pitch of in_bf16 (0: cin)
+              int det_chunks = 0);
+static constexpr int WGRAD_DET_CHUNKS = 32;
 int wgrad3_passes(int cin, int cout, int K);
 struct WgradFinEntry {
-    const float* scratch;   // [K][cin][cout] accumulated by tc3_wgrad
+    const float* scratch;   // [n_part][K][cin][cout] accumulated by tc3_wgrad
     float* dw;              // parameter layout [cout][K][cin]
     int cin, cout, K, first;
+    int n_part;             // partial images added in order (1, or WGRAD_DET_CHUNKS in deterministic mode)
 };
 static constexpr int WGRAD_FIN_MAX = 64;
 struct WgradFinTable {

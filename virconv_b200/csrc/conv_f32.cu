@@ -17,6 +17,7 @@
 namespace vc {
 
 static constexpr int TM = VC_TILE_ROWS;
+static constexpr int TCM_ROWS = 128;
 static constexpr int NTHREADS = 256;
 static constexpr int MAXK = 32;
 
@@ -128,7 +129,7 @@ __device__ __forceinline__ void tile_mac(const float* As, const float* Ws, int r
 template <int CI, int CO>
 __global__ void __launch_bounds__(NTHREADS, (Cfg<CI, CO>::RT >= 8) ? 2 : 3)
 gather_gemm_kernel(const float* __restrict__ in, const float* __restrict__ wt, const int32_t* __restrict__ nbr,
-                   float* __restrict__ out, int n_out, int K, double* __restrict__ bn_sums) {
+                   float* __restrict__ out, int n_out, int K, double* __restrict__ bn_sums, double* __restrict__ bn_part) {
     using C = Cfg<CI, CO>;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     float* As = reinterpret_cast<float*>(smem_raw);         // [2][TM][AS]
@@ -185,7 +186,7 @@ gather_gemm_kernel(const float* __restrict__ in, const float* __restrict__ wt, c
             }
         }
     }
-    if (bn_sums != nullptr) {  // tile's channel sums for the BatchNorm that follows -> float64 accumulator [2, CO]
+    if (bn_sums != nullptr || bn_part != nullptr) {  // tile's channel sums for the BatchNorm that follows -> float64 [2, CO]
 #pragma unroll
         for (int off = C::NCG; off < 32; off <<= 1) {
 #pragma unroll
@@ -207,7 +208,10 @@ gather_gemm_kernel(const float* __restrict__ in, const float* __restrict__ wt, c
             float v = 0.f;
 #pragma unroll
             for (int w = 0; w < NTHREADS / 32; ++w) v += red[w][which][ch];
-            atomicAdd(bn_sums + which * CO + ch, (double)v);
+            if (bn_part != nullptr)   // deterministic mode: one partial per tile, added in tile order by bn_sums_reduce_dev
+                bn_part[((size_t)blockIdx.x * 2 + which) * CO + ch] = (double)v;
+            else
+                atomicAdd(bn_sums + which * CO + ch, (double)v);
         }
     }
 }
@@ -393,11 +397,11 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ partial, float* __
 
 template <int CI, int CO>
 static int launch_gather(const float* in, const float* wt, const int32_t* nbr, float* out, int n_out, int K,
-                         double* bn_sums, cudaStream_t stream) {
+                         double* bn_sums, cudaStream_t stream, double* bn_part = nullptr) {
     size_t smem = Cfg<CI, CO>::smem_gather(K);
     auto kern = gather_gemm_kernel<CI, CO>;
     VC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    VC_LAUNCH_CHAIN(kern, dim3(cdiv(n_out, TM)), dim3(NTHREADS), smem, stream, in, wt, nbr, out, n_out, K, bn_sums);
+    VC_LAUNCH_CHAIN(kern, dim3(cdiv(n_out, TM)), dim3(NTHREADS), smem, stream, in, wt, nbr, out, n_out, K, bn_sums, bn_part);
     return VC_OK;
 }
 template <int CI, int CO>
@@ -487,6 +491,19 @@ extern "C" int vc_conv_fwd_f32(const float* in, const float* w, const int32_t* n
     if ((rc = prep(w, wt, cin, cout, K, 0, 0, stream))) return rc;
     return dispatch(cin, cout, [&](auto ci, auto co) {
         return launch_gather<decltype(ci)::value, decltype(co)::value>(in, wt, nbr, out, n_out, K, bn_sums, stream);
+    });
+}
+
+int vc::conv_fwd_f32_part(const float* in, const float* w, const int32_t* nbr, float* out, int n_out, int cin, int cout, int K,
+                          double* bn_part, void* ws, size_t ws_bytes, cudaStream_t stream) {
+    static_assert(TM == TCM_ROWS, "BN partials are per 128-row tile in both conv kernels");
+    int rc = check_conv_args(n_out, cin, cout, K, in, w, nbr, out, ws, ws_bytes);
+    if (rc || n_out == 0) return rc;
+    VC_CHECK_ARG(bn_part, "null pointer");
+    float* wt = (float*)ws;
+    if ((rc = prep(w, wt, cin, cout, K, 0, 0, stream))) return rc;
+    return dispatch(cin, cout, [&](auto ci, auto co) {
+        return launch_gather<decltype(ci)::value, decltype(co)::value>(in, wt, nbr, out, n_out, K, nullptr, stream, bn_part);
     });
 }
 

@@ -195,6 +195,46 @@ extern "C" int vc_conv_fwd_tc(const void* in_bf16, const float* w, const int32_t
     return tc_common(in_bf16, w, nbr, out, n_out, cin, cout, K, 0, 0, bn_sums, ws, ws_bytes, err_flag, (cudaStream_t)stream_);
 }
 
+static size_t det_w_bytes(int cin, int cout, int K) {
+    const size_t a = vc_conv_ws_bytes(cin, cout, K), b = vc_conv_tc_ws_bytes(cin, cout, K);
+    return ((a > b ? a : b) + 255) & ~(size_t)255;
+}
+
+extern "C" size_t vc_conv_fwd_det_ws_bytes(int n_out, int cin, int cout, int K) {
+    if (n_out < 0 || cin <= 0 || cout <= 0 || K < 1) return 0;
+    return det_w_bytes(cin, cout, K) + (size_t)cdiv(n_out > 0 ? n_out : 1, TCM) * 2 * cout * sizeof(double);
+}
+
+extern "C" int vc_conv_fwd_det(int precision, const void* in, const float* w, const int32_t* nbr, float* out, int n_out, int cin,
+                               int cout, int K, double* bn_sums, void* ws, size_t ws_bytes, int32_t* err_flag, vc_stream_t stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    VC_CHECK_ARG(precision == 0 || precision == 1, "precision must be 0 (fp32) or 1 (bf16)");
+    VC_CHECK_ARG(n_out >= 0 && K >= 1 && K <= MAXK_TC, "bad n=%d or K=%d", n_out, K);
+    if (!tc2_ch_ok(cin) || !tc2_ch_ok(cout)) {
+        set_error("unsupported channels cin=%d cout=%d (need 8/16/32/64)", cin, cout);
+        return VC_ERR_UNSUPPORTED;
+    }
+    if (n_out == 0) return VC_OK;
+    VC_CHECK_ARG(in && w && nbr && out && bn_sums && ws, "null pointer");
+    if (ws_bytes < vc_conv_fwd_det_ws_bytes(n_out, cin, cout, K)) {
+        set_error("deterministic conv workspace %zu < %zu", ws_bytes, vc_conv_fwd_det_ws_bytes(n_out, cin, cout, K));
+        return VC_ERR_WORKSPACE;
+    }
+    const size_t wb = det_w_bytes(cin, cout, K);
+    double* part = reinterpret_cast<double*>((char*)ws + wb);
+    int rc;
+    if (precision == 0) {
+        rc = conv_fwd_f32_part((const float*)in, w, nbr, out, n_out, cin, cout, K, part, ws, wb, stream);
+    } else {
+        rc = tc_one_image(w, ws, cin, cout, K, 0, 0, 1, stream);
+        if (!rc)
+            rc = tc2_conv(cin, cout, in, ws, nbr, n_out, out, n_out, nullptr, K, nullptr, err_flag, stream, nullptr, nullptr, 0, 0,
+                          part);
+    }
+    if (rc) return rc;
+    return bn_sums_reduce_dev(part, n_out, nullptr, TCM, cout, bn_sums, stream);
+}
+
 /* din[nbr[k,o], :] += dout[o, :] @ w[:, k, :] on tensor cores (many-to-one tables; din zeroed by the caller) */
 extern "C" int vc_conv_dgrad_scatter_tc(const void* dout_bf16, const float* w, const int32_t* nbr, float* din, int n_out,
                                         int cin, int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag,

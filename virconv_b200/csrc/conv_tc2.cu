@@ -79,6 +79,7 @@ struct PArgs {
     int out_c;                 // real output channels (8 or NR)
     const float* addend;       // optional [n, out_c], may alias out
     double* bn_sums;           // optional [2, out_c]
+    double* bn_part;           // optional [tiles, 2, out_c]: deterministic BN sums, one float64 partial per tile (bn_sums NULL)
     const int* n_dev;          // optional device row count (n_host is then the capacity of the buffers)
     int n_host;
     int* tile_counter;         // optional (zeroed by the caller): dynamic tile scheduling; NULL: tile = blockIdx.x + i * gridDim.x
@@ -515,7 +516,7 @@ __global__ void __launch_bounds__(P_THREADS, P_GROUPS == 1 ? 2 : 1) tc_conv_pers
                         *reinterpret_cast<float4*>(a.out + o) = v;
                     }
                 }
-                if (a.bn_sums != nullptr) {
+                if (a.bn_sums != nullptr || a.bn_part != nullptr) {
                     const int rows_valid = max(0, min(64, n - hbase));
                     float ts = 0.f, tq = 0.f;
                     for (int rr = rg; rr < rows_valid; rr += n_rg) {
@@ -525,6 +526,21 @@ __global__ void __launch_bounds__(P_THREADS, P_GROUPS == 1 ? 2 : 1) tc_conv_pers
                     }
                     bs += (double)ts;
                     bq += (double)tq;
+                }
+                named_bar_sync(1, P_CONS_THREADS);
+            }
+            if (a.bn_part != nullptr) {
+                // deterministic mode: this tile's sums (row groups added in order) to its own slot; the caller adds the
+                // tiles in tile order (bn_sums_reduce_dev)
+                red_s[0][e] = bs;
+                red_s[1][e] = bq;
+                bs = bq = 0.0;
+                named_bar_sync(1, P_CONS_THREADS);
+                if (e < 2 * oc) {
+                    const int which = e / oc, c = e % oc;
+                    double v = 0.0;
+                    for (int g = 0; g < n_rg; ++g) v += red_s[which][g * oc + c];
+                    a.bn_part[((size_t)tile * 2 + which) * oc + c] = v;
                 }
                 named_bar_sync(1, P_CONS_THREADS);
             }
@@ -684,7 +700,7 @@ bool tc2_ch_ok(int c) { return c == 8 || c == 16 || c == 32 || c == 64; }
 // (layout 1).  n_dev (optional) overrides n_rows on the device; n_rows is then the capacity the grid is sized for.
 int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_t* nbr, long long pitch, float* out,
              int n_rows, const int* n_dev, int K, double* bn_sums, int* err, cudaStream_t stream, const float* addend,
-             int* tile_counter, int flags, int in_ld) {
+             int* tile_counter, int flags, int in_ld, double* bn_part) {
     if (n_rows == 0) return VC_OK;
     if (!tc2_ch_ok(kc) || !tc2_ch_ok(nr) || K < 1 || K > MAXK_TC) {
         set_error("tensor-core conv: unsupported shape (%d -> %d channels, K=%d)", kc, nr, K);
@@ -697,7 +713,7 @@ int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_
         return VC_ERR_INVALID;
     }
     a.in = (const __nv_bfloat16*)in_bf16; a.in_c = kc; a.in_ld = in_ld; a.wimg = (const unsigned char*)wimg; a.nbr = nbr; a.pitch = pitch;
-    a.out = out; a.out_c = nr; a.addend = addend; a.bn_sums = bn_sums; a.n_dev = n_dev; a.n_host = n_rows; a.tile_counter = tile_counter;
+    a.out = out; a.out_c = nr; a.addend = addend; a.bn_sums = bn_part ? nullptr : bn_sums; a.bn_part = bn_part; a.n_dev = n_dev; a.n_host = n_rows; a.tile_counter = tile_counter;
     a.K = K; a.S = 0; a.w_resident = 0; a.ntb_alloc = P_NTB; a.scan_k = flags & 1; a.early_tables = (flags >> 1) & 1;
     a.err = err;
     const int kcp = tc_pad16(kc), nrp = tc_pad16(nr);

@@ -55,12 +55,14 @@ struct RBk {
     int32_t *nbr, *nbr_bwd, *pair_num;
     const int *n_in_dev, *n_out_dev;   // static mode (see ISet); table pitches are n_out (nbr) and n_in (nbr_bwd)
     int K, n_in, n_out, subm, unique, ev, prod;
+    G2Prep g2;             // deterministic mode, many-to-one table: the gather-form dgrad's groups and table (gather2d.cu)
 };
 constexpr int CTR_PER_LAYER = 16;  // forward, dgrad, up to 14 wgrad passes (C_in = C_out = 64, K = 27: 14 groups, one per pass in wgrad_tc3)
 
 // conv launches of a layer; the values are the timing records' kinds (vc_exec_timing_read, executor.KIND_NAMES)
 enum ConvKind : int { K_NONE = -1 /* no input gradient */, K_FWD_F32 = 0, K_FWD_TC = 1, K_DGRAD_F32 = 2, K_DGRAD_TC = 3,
-                      K_DGRAD_SCATTER_F32 = 4, K_WGRAD_F32 = 5, K_WGRAD_TC = 6, K_DGRAD_SCATTER_TC = 7 };
+                      K_DGRAD_SCATTER_F32 = 4, K_WGRAD_F32 = 5, K_WGRAD_TC = 6, K_DGRAD_SCATTER_TC = 7,
+                      K_DGRAD_GATHER2D_F32 = 8, K_DGRAD_GATHER2D_TC = 9 };
 
 struct Layer {
     float *x, *y, *stats;
@@ -80,6 +82,8 @@ struct State {
     uint64_t magic;
     size_t used;           // arena bytes in use after the last call
     int n_ops, n_layers, training, precision, batch_size, is_static;
+    int deterministic;     // flags bit 2 of the forward: fixed-order reductions, no float atomics (the backward follows it)
+    size_t det_bytes;      // arena bytes of the deterministic mode's partials, tables and operands (vc_exec_query 0)
     ISet iset[MAX_I];
     FSlot f[MAX_F];
     RBk rb[MAX_RB];
@@ -269,22 +273,27 @@ int check_plan(const int32_t* oi, int n_ops, int n_layers) {
     return VC_OK;
 }
 
-// the one place that decides which conv kernels a layer runs (the tensor-core backward only in a BN-training step)
-void choose_kernels(Layer& L, int precision, int training, int need_dgrad, const RBk& R) {
+// the one place that decides which conv kernels a layer runs (the tensor-core backward only in a BN-training step; in the
+// deterministic mode the many-to-one tables take the gather-form dgrad instead of the atomic scatter)
+void choose_kernels(Layer& L, int precision, int training, int need_dgrad, const RBk& R, int det) {
     const bool tc = precision == 1 && tc2_ch_ok(L.cin) && tc2_ch_ok(L.cout);
     const bool tc_bwd = tc && training;
     L.fwd = tc ? K_FWD_TC : K_FWD_F32;
     L.wgrad = tc_bwd ? K_WGRAD_TC : K_WGRAD_F32;
     if (!need_dgrad || L.in_slot == 0)
         L.dgrad = K_NONE;
+    else if (R.subm && !R.unique && det)
+        L.dgrad = tc_bwd ? K_DGRAD_GATHER2D_TC : K_DGRAD_GATHER2D_F32;
     else if (R.subm && !R.unique)   // many-to-one table (the image branch's projected pixels collide): atomic scatter
         L.dgrad = tc_bwd && tc_scatter_ch_ok(L.cin) && tc_scatter_ch_ok(L.cout) ? K_DGRAD_SCATTER_TC : K_DGRAD_SCATTER_F32;
     else
         L.dgrad = tc_bwd ? K_DGRAD_TC : K_DGRAD_F32;
 }
 
-// fp32 accumulator of the tensor-core wgrad, padded to 64 floats
-size_t wgrad_acc_floats(const Layer& L, int K) { return L.wgrad == K_WGRAD_TC ? ((size_t)K * L.cin * L.cout + 63) / 64 * 64 : 0; }
+// fp32 accumulator of the tensor-core wgrad (deterministic mode: one image per row chunk), padded to 64 floats
+size_t wgrad_acc_floats(const Layer& L, int K, int det) {
+    return L.wgrad == K_WGRAD_TC ? ((size_t)(det ? WGRAD_DET_CHUNKS : 1) * K * L.cin * L.cout + 63) / 64 * 64 : 0;
+}
 
 // what the forward shares between its planning pass and its per-op enqueue functions (value-initialised)
 struct FwdCtx : Ctx {
@@ -328,13 +337,13 @@ void plan_step(FwdCtx& C, int c0, int precision, int training) {
         } else if (o[F_KIND] == OP_CBR) {
             Layer& L = C.S->layer[o[F_LAYER]];
             L.cin = o[F_CIN]; L.cout = o[F_COUT]; L.in_slot = o[F_A]; L.out_slot = o[F_B]; L.rb = o[F_C];
-            choose_kernels(L, precision, training, o[F_X0], C.S->rb[L.rb]);
+            choose_kernels(L, precision, training, o[F_X0], C.S->rb[L.rb], C.S->deterministic);
             C.slot_c[L.out_slot] = L.cout;
             if (precision == 0 || o[F_X1]) C.need_f32[L.out_slot] = true;
             if (L.fwd == K_FWD_F32 || L.wgrad == K_WGRAD_F32) C.need_f32[L.in_slot] = true;
             C.sums_doubles += 4 * (size_t)L.cout;
             ++C.n_cbr;
-            C.wg_floats += wgrad_acc_floats(L, C.S->rb[L.rb].K);
+            C.wg_floats += wgrad_acc_floats(L, C.S->rb[L.rb].K, C.S->deterministic);
         } else if (o[F_KIND] == OP_CAT) {
             C.slot_c[o[F_C]] = C.slot_c[o[F_A]] + C.slot_c[o[F_B]];
             if (precision == 0 || o[F_X1]) C.need_f32[o[F_C]] = true;
@@ -372,9 +381,19 @@ int fwd_subm_rb(FwdCtx& C, int i, const int* o, int s) {
     R.nbr = nbr; R.pair_num = pn;
     const size_t wsb = vc_subm_rulebook_ws_bytes(I.n);
     VC_ALLOC(ws, void*, wsb);
-    if (C.do_idx)
+    int32_t* rep = nullptr;
+    if (C.S->deterministic && !R.unique && I.n > 0) {   // the gather-form dgrad's row groups and table (gather2d.cu)
+        const size_t gb = ((size_t)I.n + 63) / 64 * 256 + gather2d_prep_bytes(I.n, R.K);
+        VC_ALLOC(g2ws, int32_t*, gb);
+        rep = g2ws;
+        R.g2 = gather2d_carve(g2ws + ((size_t)I.n + 63) / 64 * 64, I.n, R.K);
+        C.S->det_bytes += gb;
+    }
+    if (C.do_idx) {
         VC_TRY(subm_rulebook_dev(I.idx, I.n, I.n_dev, I.ndim, C.S->batch_size, I.shape, o + F_KS, o + F_DL, R.nbr, R.pair_num, ws, wsb,
-                                 C.st[s]));
+                                 C.st[s], rep));
+        if (rep) VC_TRY(gather2d_prep_dev(R.nbr, rep, R.K, I.n, I.n_dev, R.g2, C.st[s]));
+    }
     C.produced(R, s);
     return VC_OK;
 }
@@ -599,6 +618,13 @@ int fwd_cbr(FwdCtx& C, int i, const int* o, int s) {
     }
     L.x = x; L.y = y; L.stats = stats;
     double* sums = S->training ? L.sums : nullptr;
+    double* part = nullptr;   // deterministic mode: the conv's BN sums per 128-row tile, added in tile order below
+    if (sums && S->deterministic) {
+        const size_t pb = (size_t)cdiv(R.n_out > 0 ? R.n_out : 1, VC_TILE_ROWS) * 2 * L.cout * 8;
+        VC_ALLOC(p_, double*, pb);
+        part = p_;
+        S->det_bytes += pb;
+    }
     if (L.fwd == K_FWD_TC && R.n_out > 0) {
         if (!X.bf16) {   // no producer wrote a shadow (network input): cast once
             VC_CHECK_ARG(X.ld == X.c, "op %d: no bf16 copy of a strided input", i);
@@ -611,14 +637,18 @@ int fwd_cbr(FwdCtx& C, int i, const int* o, int s) {
         //  may load its first table slices before its griddepcontrol.wait — conv_tc2.cu)
         if (C.do_feat)
             VC_TRY(tc2_conv(L.cin, L.cout, X.bf16, L.wimg_fwd, R.nbr, R.n_out, x, R.n_out, R.n_out_dev, R.K, sums, C.err, st, nullptr,
-                            L.tile_ctr, (!C.do_idx || C.st[R.prod] != C.st[s]) ? 2 : 0, X.ld));
+                            L.tile_ctr, (!C.do_idx || C.st[R.prod] != C.st[s]) ? 2 : 0, X.ld, part));
     } else {   // (also a tensor-core layer without output rows)
         const size_t wsb = vc_conv_ws_bytes(L.cin, L.cout, R.K);
         VC_ALLOC(ws, void*, wsb);
         VC_CHECK_ARG(X.f32 && X.ld == X.c, "op %d: the fp32 conv needs a dense fp32 input", i);
         Timed t(K_FWD_F32, li, st);
-        if (C.do_feat) VC_TRY(vc_conv_fwd_f32(X.f32, C.P<const float>(li, P_W), R.nbr, x, R.n_out, L.cin, L.cout, R.K, sums, ws, wsb, st));
+        if (C.do_feat && part)
+            VC_TRY(conv_fwd_f32_part(X.f32, C.P<const float>(li, P_W), R.nbr, x, R.n_out, L.cin, L.cout, R.K, part, ws, wsb, st));
+        else if (C.do_feat)
+            VC_TRY(vc_conv_fwd_f32(X.f32, C.P<const float>(li, P_W), R.nbr, x, R.n_out, L.cin, L.cout, R.K, sums, ws, wsb, st));
     }
+    if (C.do_feat && part && R.n_out > 0) VC_TRY(bn_sums_reduce_dev(part, R.n_out, R.n_out_dev, VC_TILE_ROWS, L.cout, L.sums, st));
     if (C.do_feat)
         VC_TRY(bn_apply_relu_dev(x, L.sums, R.n_out, R.n_out_dev, L.cout, C.P<const float>(li, P_GAMMA), C.P<const float>(li, P_BETA),
                                  C.P<float>(li, P_RM), C.P<float>(li, P_RV), C.P<long long>(li, P_NBT), C.lf[2 * li + 1], C.lf[2 * li],
@@ -687,6 +717,8 @@ extern "C" int vc_exec_query(const void* state, int what, int id, long long* out
     switch (what) {
         case 0:
             out[0] = (long long)S->used;
+            out[1] = (long long)S->det_bytes;
+            out[2] = S->deterministic;
             return VC_OK;
         case 1: {
             VC_CHECK_ARG(id >= 0 && id < MAX_F, "slot id");
@@ -766,6 +798,7 @@ extern "C" int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, 
     memset(S, 0, sizeof(State));
     S->n_ops = n_ops; S->n_layers = n_layers; S->training = training; S->precision = precision; S->batch_size = batch_size;
     S->is_static = is_static;
+    S->deterministic = (flags >> 2) & 1;
     for (int i = 0; i < MAX_I; ++i) S->iset[i].ev = -1;
     for (int i = 0; i < MAX_F; ++i) S->f[i].ev = -1;
     for (int i = 0; i < MAX_RB; ++i) S->rb[i].ev = -1;
@@ -807,10 +840,13 @@ extern "C" int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, 
         L.tile_ctr = ctr_all;
         ctr_all += CTR_PER_LAYER;
         L.wscratch = L.wgrad == K_WGRAD_TC ? wg_all : nullptr;
-        wg_all += wgrad_acc_floats(L, R.K);
+        wg_all += wgrad_acc_floats(L, R.K, S->deterministic);
+        if (L.wscratch && S->deterministic) S->det_bytes += (wgrad_acc_floats(L, R.K, 1) - wgrad_acc_floats(L, R.K, 0)) * 4;
         // dgrad image: mirrored for a submanifold table used as its own transpose, plain for a strided conv's nbr_bwd table
         // (gather dgrad), layout 0 for the many-to-one image-branch table (tensor-core scatter)
-        const int n_img = L.fwd != K_FWD_TC ? 0 : (L.dgrad == K_DGRAD_TC || L.dgrad == K_DGRAD_SCATTER_TC) ? 2 : 1;
+        const int n_img = L.fwd != K_FWD_TC                                                                   ? 0
+                          : (L.dgrad == K_DGRAD_TC || L.dgrad == K_DGRAD_SCATTER_TC || L.dgrad == K_DGRAD_GATHER2D_TC) ? 2
+                                                                                                                      : 1;
         for (int mode = 0; mode < n_img; ++mode) {
             const int layout = (mode == 1 && L.dgrad == K_DGRAD_SCATTER_TC) ? 0 : 1;
             VC_ALLOC(img, void*, tc_image_bytes(L.cin, L.cout, R.K, layout));
@@ -821,7 +857,7 @@ extern "C" int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, 
             }
             TcPrepEntry& e = T.e[T.n++];
             e.w = C.P<const float>(o[F_LAYER], P_W); e.img = img; e.cin = L.cin; e.cout = L.cout; e.K = R.K; e.mode = mode;
-            e.mirror = mode == 1 && L.dgrad == K_DGRAD_TC && R.subm;
+            e.mirror = mode == 1 && ((L.dgrad == K_DGRAD_TC && R.subm) || L.dgrad == K_DGRAD_GATHER2D_TC);
             e.layout = layout;
         }
     }
@@ -1020,18 +1056,27 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
         }
         const size_t elems = (size_t)R.n_out * L.cout;
         // the fp32 input gradient is read by the fp32 wgrad and the fp32 dgrads only (the tensor-core ones read dxb)
+        // (gather-form dgrad: dx / dxb are the first half of its operand U = [dout; S], 2 n_out rows)
+        const bool g2 = L.dgrad == K_DGRAD_GATHER2D_F32 || L.dgrad == K_DGRAD_GATHER2D_TC;
         float* dx = nullptr;
-        if (L.wgrad == K_WGRAD_F32 || L.dgrad == K_DGRAD_F32 || L.dgrad == K_DGRAD_SCATTER_F32) {
-            VC_ALLOC(t, float*, elems * 4);
+        if (L.wgrad == K_WGRAD_F32 || L.dgrad == K_DGRAD_F32 || L.dgrad == K_DGRAD_SCATTER_F32 || L.dgrad == K_DGRAD_GATHER2D_F32) {
+            VC_ALLOC(t, float*, elems * 4 * (L.dgrad == K_DGRAD_GATHER2D_F32 ? 2 : 1));
             dx = t;
         }
         void* dxb = nullptr;
         if (S->precision == 1) {
-            VC_ALLOC(t, void*, elems * 2);
+            VC_ALLOC(t, void*, elems * 2 * (L.dgrad == K_DGRAD_GATHER2D_TC ? 2 : 1));
             dxb = t;
         }
+        double* bpart = nullptr;   // deterministic mode: BN backward partials per BN_DET_ROWS chunk, added in chunk order
+        if (S->deterministic) {
+            const size_t pb = (size_t)cdiv(R.n_out, BN_DET_ROWS) * 2 * L.cout * 8;
+            VC_ALLOC(t, double*, pb);
+            bpart = t;
+            S->det_bytes += pb + (g2 ? elems * (L.dgrad == K_DGRAD_GATHER2D_TC ? 2 : 4) : 0);
+        }
         VC_TRY(bn_relu_bwd_dev(Y.grad, Y.gld, L.x, C.P<const float>(li, P_GAMMA), L.stats, dx, dxb, dgamma, dbeta, R.n_out, R.n_out_dev,
-                               L.cout, training, L.sums + 2 * L.cout, S->is_static, st));
+                               L.cout, training, L.sums + 2 * L.cout, S->is_static, st, bpart));
         // wgrad (needs dx / its bf16 shadow: ordered after the BN backward through an event when on its own stream)
         if (two) {
             int e = record_on(C, 0);
@@ -1040,13 +1085,14 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
         if (L.wgrad == K_WGRAD_TC) {
             Timed t(L.wgrad, li, wst);
             VC_TRY(tc3_wgrad(L.cin, L.cout, X.bf16, dxb, R.nbr, R.n_out, L.wscratch, R.n_out, R.n_out_dev, R.K, C.err, wst,
-                             L.tile_ctr + 2, wgrad_ctas, X.ld));
+                             L.tile_ctr + 2, wgrad_ctas, X.ld, S->deterministic ? WGRAD_DET_CHUNKS : 0));
             if (fin.n == WGRAD_FIN_MAX) {
                 VC_TRY(wgrad_finalize(fin, wst));
                 fin.n = 0;
             }
             WgradFinEntry& fe = fin.e[fin.n++];
             fe.scratch = L.wscratch; fe.dw = dw; fe.cin = L.cin; fe.cout = L.cout; fe.K = R.K; fe.first = 0;
+            fe.n_part = S->deterministic ? WGRAD_DET_CHUNKS : 1;
         } else {
             const size_t wsb = vc_conv_wgrad_ws_bytes(R.n_out, L.cin, L.cout, R.K);
             VC_ALLOC(ws, void*, wsb);
@@ -1059,7 +1105,7 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
         const int32_t* table = R.subm ? R.nbr : R.nbr_bwd;
         const size_t wsb = vc_conv_ws_bytes(L.cin, L.cout, R.K);
         void* ws = nullptr;   // the fp32 dgrads' workspace
-        if (L.dgrad == K_DGRAD_F32 || L.dgrad == K_DGRAD_SCATTER_F32) {
+        if (L.dgrad == K_DGRAD_F32 || L.dgrad == K_DGRAD_SCATTER_F32 || L.dgrad == K_DGRAD_GATHER2D_F32) {
             VC_ALLOC(t, void*, wsb);
             ws = t;
         }
@@ -1074,6 +1120,26 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
                 VC_TRY(contribute_scatter(C, X, st, [&](float* dst, int ld) -> int {
                     Timed t(L.dgrad, li, st);
                     return conv_dgrad_scatter_f32_ld(dx, C.P<const float>(li, P_W), R.nbr, dst, ld, R.n_out, L.cin, L.cout, R.K, ws, wsb, st);
+                }));
+                break;
+            case K_DGRAD_GATHER2D_TC:
+            case K_DGRAD_GATHER2D_F32:
+                // S into U's second half, one mirrored gather dgrad over the group table, then added into the slot's gradient
+                // (which may be a column slice of the concat's gradient: row pitch ld)
+                VC_TRY(contribute_scatter(C, X, st, [&](float* dst, int ld) -> int {
+                    const bool tc = L.dgrad == K_DGRAD_GATHER2D_TC;
+                    VC_ALLOC(tmp, float*, (size_t)R.n_in * L.cin * 4);
+                    S->det_bytes += (size_t)R.n_in * L.cin * 4;
+                    Timed t(L.dgrad, li, st);
+                    VC_TRY(gather2d_sum_dev(tc ? nullptr : dx, tc ? dxb : nullptr, L.cout, R.g2, R.n_in, R.n_in_dev, tc ? nullptr : dx,
+                                            tc ? dxb : nullptr, st));
+                    if (tc)
+                        VC_TRY(tc2_conv(L.cout, L.cin, dxb, L.wimg_dgrad, R.g2.nbr_g, R.n_in, tmp, R.n_in, R.n_in_dev, R.K, nullptr, C.err,
+                                        st, nullptr, L.tile_ctr + 1, 2));
+                    else
+                        VC_TRY(vc_conv_dgrad_f32(dx, C.P<const float>(li, P_W), R.g2.nbr_g, tmp, R.n_in, L.cin, L.cout, R.K, 1, ws, wsb,
+                                                 st));
+                    return add_rows_ld_dev(dst, ld, tmp, R.n_in, R.n_in_dev, L.cin, st);
                 }));
                 break;
             case K_DGRAD_TC:

@@ -94,7 +94,7 @@ __global__ void __launch_bounds__(256) subm_probe_kernel(const int32_t* __restri
                                                          const int* __restrict__ n_dev, Geom g,
                                                          const unsigned long long* __restrict__ table,
                                                          uint32_t mask, int32_t* __restrict__ nbr,
-                                                         int32_t* __restrict__ pair_num) {
+                                                         int32_t* __restrict__ pair_num, int32_t* __restrict__ rep) {
     __shared__ int cnt;
     const int pitch = n;                  // table rows are [K][capacity]
     if (n_dev != nullptr) n = min(n, __ldg(n_dev));
@@ -108,6 +108,17 @@ __global__ void __launch_bounds__(256) subm_probe_kernel(const int32_t* __restri
         for (int d = 0; d < g.ndim; ++d) centre = centre * g.ksize[d] + g.ksize[d] / 2;
         if (k == centre) {
             res = row;  // identity (spconv Native: out = features @ W[centre])
+            if (rep != nullptr) {   // the lowest row at this row's own coordinate (the row itself when it is outside the grid)
+                int b, c[VC_MAX_NDIM];
+                load_index(idx, row, g.ndim, b, c);
+                int r = row;
+                if (index_ok(g, b, c)) {
+                    unsigned long long key = (unsigned long long)b;
+                    for (int d = 0; d < g.ndim; ++d) key = key * (unsigned long long)g.shape[d] + (unsigned long long)c[d];
+                    r = hash_lookup(table, mask, key);
+                }
+                rep[row] = r;
+            }
         } else {
             int b, c[VC_MAX_NDIM];
             load_index(idx, row, g.ndim, b, c);
@@ -125,6 +136,7 @@ __global__ void __launch_bounds__(256) subm_probe_kernel(const int32_t* __restri
         nbr[(size_t)k * pitch + row] = res;
     } else if (row < pitch) {
         nbr[(size_t)k * pitch + row] = -1;    // static mode: rows between the count and the capacity have no neighbours
+        if (rep != nullptr && blockIdx.y == 0) rep[row] = -1;
     }
     unsigned m = __ballot_sync(0xffffffffu, res >= 0);
     if ((threadIdx.x & 31) == 0 && m) atomicAdd(&cnt, __popc(m));
@@ -381,7 +393,7 @@ extern "C" size_t vc_subm_rulebook_ws_bytes(int n) { return (size_t)table_slots(
 
 int vc::subm_rulebook_dev(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size,
                           const int32_t* spatial_shape, const int32_t* ksize, const int32_t* dilation, int32_t* nbr,
-                          int32_t* pair_num, void* ws, size_t ws_bytes, cudaStream_t stream) {
+                          int32_t* pair_num, void* ws, size_t ws_bytes, cudaStream_t stream, int32_t* rep) {
     Geom g;
     int rc = make_geom(g, ndim, batch_size, spatial_shape, ksize, nullptr, nullptr, dilation);
     if (rc) return rc;
@@ -401,7 +413,7 @@ int vc::subm_rulebook_dev(const int32_t* indices, int n, const int* n_dev, int n
     VC_CUDA(cudaMemsetAsync(table, 0xFF, (size_t)slots * 8, stream));
     hash_insert_kernel<<<cdiv(n, 256), 256, 0, stream>>>(indices, n, n_dev, g, table, slots - 1);
     VC_LAUNCH_CHECK();
-    subm_probe_kernel<<<dim3(cdiv(n, 256), g.K), 256, 0, stream>>>(indices, n, n_dev, g, table, slots - 1, nbr, pair_num);
+    subm_probe_kernel<<<dim3(cdiv(n, 256), g.K), 256, 0, stream>>>(indices, n, n_dev, g, table, slots - 1, nbr, pair_num, rep);
     VC_LAUNCH_CHECK();
     return VC_OK;
 }
@@ -411,6 +423,14 @@ extern "C" int vc_subm_rulebook(const int32_t* indices, int n, int ndim, int bat
                                 void* ws, size_t ws_bytes, vc_stream_t stream_) {
     return vc::subm_rulebook_dev(indices, n, nullptr, ndim, batch_size, spatial_shape, ksize, dilation, nbr, pair_num, ws, ws_bytes,
                                  (cudaStream_t)stream_);
+}
+
+extern "C" int vc_subm_rulebook_rep(const int32_t* indices, int n, int ndim, int batch_size, const int32_t* spatial_shape,
+                                    const int32_t* ksize, const int32_t* dilation, int32_t* nbr, int32_t* pair_num, int32_t* rep,
+                                    void* ws, size_t ws_bytes, vc_stream_t stream_) {
+    VC_CHECK_ARG(n == 0 || rep, "null pointer");
+    return vc::subm_rulebook_dev(indices, n, nullptr, ndim, batch_size, spatial_shape, ksize, dilation, nbr, pair_num, ws, ws_bytes,
+                                 (cudaStream_t)stream_, rep);
 }
 
 extern "C" int vc_conv_out_shape(int ndim, const int32_t* spatial_shape, const int32_t* ksize, const int32_t* stride,

@@ -67,6 +67,7 @@ struct WArgs {
     int n_host;
     int* tile_counter;          // [passes] or NULL
     int K, S, groups_per_pass;
+    int det_chunks;             // > 0: deterministic mode, scratch = [det_chunks][K][in_c][out_c] (see tc3_wgrad)
     int* err;
 };
 
@@ -127,6 +128,11 @@ __global__ void __launch_bounds__(W_THREADS, 2) tc_wgrad_half_kernel(const WArgs
     const bool dead = a.err != nullptr && *reinterpret_cast<volatile int*>(a.err) != 0;
     const int n_tiles = dead ? 0 : (n + TCM - 1) / TCM;
     int* counter = a.tile_counter != nullptr ? a.tile_counter + blockIdx.y : nullptr;
+    // deterministic mode: tiles [c * tpc, (c + 1) * tpc) form chunk c, claimed whole (from the row count alone: the same split
+    // for every grid); each chunk's sum goes to its own partial image
+    const int tpc = a.det_chunks > 0 ? max(1, (n_tiles + a.det_chunks - 1) / a.det_chunks) : 0;
+    const int n_chunks = tpc > 0 ? (n_tiles + tpc - 1) / tpc : 0;
+    const size_t part_floats = (size_t)K * a.in_c * a.out_c;
     int ntb = W_NTB;            // table buffers in use == tiles a CTA holds claimed at once (see conv_tc2.cu)
     if (counter != nullptr) {
         int d = n_tiles / (3 * (int)gridDim.x);
@@ -142,10 +148,29 @@ __global__ void __launch_bounds__(W_THREADS, 2) tc_wgrad_half_kernel(const WArgs
         int tq0 = -1, tq1 = -1, tq2 = -1, tq3 = -1;
         bool stop = false;
         int claimed = 0;
+        int c_next = 0, c_end = 0;          // deterministic mode: the rest of the claimed chunk
         for (int it = 0;; ++it) {
             const int tb = it % ntb;
             int tile = -1;
-            if (!stop) {
+            if (!stop && tpc > 0) {
+                if (c_next >= c_end) {
+                    int chunk;
+                    if (counter != nullptr) {
+                        chunk = lane == 0 ? atomicAdd(counter, 1) : 0;
+                        chunk = __shfl_sync(0xffffffffu, chunk, 0);
+                    } else {
+                        chunk = blockIdx.x + claimed * gridDim.x;
+                    }
+                    ++claimed;
+                    if (chunk >= n_chunks) {
+                        stop = true;
+                    } else {
+                        c_next = chunk * tpc;
+                        c_end = min(n_tiles, c_next + tpc);
+                    }
+                }
+                if (!stop) tile = c_next++;
+            } else if (!stop) {
                 if (counter != nullptr) {
                     tile = lane == 0 ? atomicAdd(counter, 1) : 0;
                     tile = __shfl_sync(0xffffffffu, tile, 0);
@@ -306,10 +331,25 @@ __global__ void __launch_bounds__(W_THREADS, 2) tc_wgrad_half_kernel(const WArgs
         int s = 0;
         uint32_t ph = 0;
         int n_done = 0;
+        int chunk = -1;                          // deterministic mode: chunk the accumulators belong to
         for (int it = 0;; ++it) {
             const int tb = it % ntb, db = it & 1;
             W_WAIT(&tbl_full[tb], (uint32_t)((it / ntb) & 1), 0x221);
-            if (tile_s[tb] < 0) break;
+            const int tile = tile_s[tb];
+            if (tile < 0) break;
+            if (tpc > 0 && tile / tpc != chunk) {
+                if (n_done > 0) {                // the previous chunk is complete: its partial image, then start from zero
+#pragma unroll
+                    for (int gg = 0; gg < W_MAXG; ++gg) wg_fence_acc(acc[gg]);
+                    wgrad_flush<CI, CO, W_MAXG>(acc, wg, t, g_count, k_begin, k_count, a.in_c, a.out_c,
+                                                a.scratch + (size_t)chunk * part_floats);
+#pragma unroll
+                    for (int gg = 0; gg < W_MAXG; ++gg)
+#pragma unroll
+                        for (int j = 0; j < CO / 2; ++j) acc[gg][j] = 0.f;
+                }
+                chunk = tile / tpc;
+            }
             __syncwarp();
             if (lane == 0) mbar_arrive(&tbl_empty[tb]);
             if (!mbar_spin(doutf0 + 8u * db, (uint32_t)((it >> 1) & 1), 4096u) &&
@@ -342,7 +382,9 @@ __global__ void __launch_bounds__(W_THREADS, 2) tc_wgrad_half_kernel(const WArgs
         }
 #pragma unroll
         for (int gg = 0; gg < W_MAXG; ++gg) wg_fence_acc(acc[gg]);
-        if (n_done > 0) wgrad_flush<CI, CO, W_MAXG>(acc, wg, t, g_count, k_begin, k_count, a.in_c, a.out_c, a.scratch);
+        if (n_done > 0)
+            wgrad_flush<CI, CO, W_MAXG>(acc, wg, t, g_count, k_begin, k_count, a.in_c, a.out_c,
+                                        a.scratch + (tpc > 0 ? (size_t)chunk * part_floats : 0));
     }
 done:
     cp_async_wait<0>();
@@ -385,7 +427,8 @@ int launch_wgrad3(const WArgs& a0, int n_cap, int max_ctas, cudaStream_t stream)
 // scratch: [K][cin][cout] fp32, ZERO on entry (the kernel accumulates); tile_counter: `wgrad3_passes(cin, cout, K)` ints, zero;
 // at most max_ctas CTAs per pass
 int tc3_wgrad(int cin, int cout, const void* in_bf16, const void* dout_bf16, const int32_t* nbr, long long pitch, float* scratch,
-              int n_rows, const int* n_dev, int K, int* err, cudaStream_t stream, int* tile_counter, int max_ctas, int in_ld) {
+              int n_rows, const int* n_dev, int K, int* err, cudaStream_t stream, int* tile_counter, int max_ctas, int in_ld,
+              int det_chunks) {
     if (n_rows == 0) return VC_OK;
     if (!tc2_ch_ok(cin) || !tc2_ch_ok(cout) || K < 1 || K > MAXK_TC) {
         set_error("tensor-core wgrad: unsupported shape (%d -> %d channels, K=%d)", cin, cout, K);
@@ -399,7 +442,7 @@ int tc3_wgrad(int cin, int cout, const void* in_bf16, const void* dout_bf16, con
     }
     a.in = (const __nv_bfloat16*)in_bf16; a.in_c = cin; a.in_ld = in_ld; a.dout = (const __nv_bfloat16*)dout_bf16; a.out_c = cout; a.nbr = nbr;
     a.pitch = pitch; a.scratch = scratch; a.n_dev = n_dev; a.n_host = n_rows; a.tile_counter = tile_counter; a.K = K; a.S = 0;
-    a.groups_per_pass = 0; a.err = err;
+    a.groups_per_pass = 0; a.err = err; a.det_chunks = det_chunks;
     const int ci = tc_pad16(cin), co = tc_pad16(cout);
 #define VC_W_CASE(A, B) \
     if (ci == A && co == B) return launch_wgrad3<A, B>(a, n_rows, max_ctas, stream);
@@ -429,7 +472,14 @@ __global__ void __launch_bounds__(256) wgrad_finalize_kernel(WgradFinTable t) {
     const WgradFinEntry& e = t.e[lo];
     const int j = i - e.first;                       // index in the parameter layout: coalesced writes
     const int ci = j % e.cin, k = (j / e.cin) % e.K, co = j / (e.cin * e.K);
-    e.dw[j] = __ldg(e.scratch + ((size_t)k * e.cin + ci) * e.cout + co);
+    const size_t o = ((size_t)k * e.cin + ci) * e.cout + co, img = (size_t)e.K * e.cin * e.cout;
+    if (e.n_part == 1) {
+        e.dw[j] = __ldg(e.scratch + o);
+    } else {                    // deterministic mode: the chunk images in chunk order, in float64, rounded once
+        double v = 0.0;
+        for (int p = 0; p < e.n_part; ++p) v += (double)__ldg(e.scratch + p * img + o);
+        e.dw[j] = (float)v;
+    }
 }
 
 int wgrad_finalize(WgradFinTable& t, cudaStream_t stream) {
@@ -492,5 +542,45 @@ extern "C" int vc_conv_wgrad_tc(const void* in_bf16, const void* dout_bf16, cons
     WgradFinTable T;
     T.n = 1;
     T.e[0].scratch = (const float*)ws; T.e[0].dw = dw; T.e[0].cin = cin; T.e[0].cout = cout; T.e[0].K = K; T.e[0].first = 0;
+    T.e[0].n_part = 1;
+    return wgrad_finalize(T, stream);
+}
+
+extern "C" size_t vc_conv_wgrad_tc_det_ws_bytes(int n_out, int cin, int cout, int K) {
+    (void)n_out;
+    const size_t passes = tc2_ch_ok(cin) && tc2_ch_ok(cout) && K >= 1 ? (size_t)wgrad3_passes(cin, cout, K) : 0;
+    const size_t bytes = (size_t)WGRAD_DET_CHUNKS * K * cin * cout * sizeof(float) + passes * sizeof(int);
+    return (bytes + 255) & ~(size_t)255;
+}
+
+extern "C" int vc_conv_wgrad_tc_det(const void* in_bf16, const void* dout_bf16, const int32_t* nbr, float* dw, int n_out,
+                                    int cin, int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag,
+                                    vc_stream_t stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    VC_CHECK_ARG(n_out >= 0 && K >= 1 && K <= MAXK_TC && dw, "bad arguments");
+    if (!tc2_ch_ok(cin) || !tc2_ch_ok(cout)) {
+        set_error("tensor-core wgrad: unsupported channels cin=%d cout=%d", cin, cout);
+        return VC_ERR_UNSUPPORTED;
+    }
+    if (n_out == 0) {
+        VC_CUDA(cudaMemsetAsync(dw, 0, (size_t)K * cin * cout * 4, stream));
+        return VC_OK;
+    }
+    VC_CHECK_ARG(in_bf16 && dout_bf16 && nbr && ws, "null pointer");
+    const size_t need = vc_conv_wgrad_tc_det_ws_bytes(n_out, cin, cout, K);
+    if (ws_bytes < need) {
+        set_error("deterministic tensor-core wgrad workspace %zu < %zu", ws_bytes, need);
+        return VC_ERR_WORKSPACE;
+    }
+    const size_t pbytes = (size_t)WGRAD_DET_CHUNKS * K * cin * cout * sizeof(float);
+    VC_CUDA(cudaMemsetAsync(ws, 0, need, stream));
+    int rc = tc3_wgrad(cin, cout, in_bf16, dout_bf16, nbr, n_out, (float*)ws, n_out, nullptr, K, err_flag, stream,
+                       reinterpret_cast<int*>((char*)ws + pbytes), g_wgrad3_ctas > 0 ? g_wgrad3_ctas : num_sms(), 0,
+                       WGRAD_DET_CHUNKS);
+    if (rc) return rc;
+    WgradFinTable T;
+    T.n = 1;
+    T.e[0].scratch = (const float*)ws; T.e[0].dw = dw; T.e[0].cin = cin; T.e[0].cout = cout; T.e[0].K = K; T.e[0].first = 0;
+    T.e[0].n_part = WGRAD_DET_CHUNKS;
     return wgrad_finalize(T, stream);
 }

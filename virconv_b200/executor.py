@@ -43,7 +43,8 @@ VC_ERR_WORKSPACE = -3
 OPI, OPF, PCOLS = 24, 8, 9
 # the timing records' kinds: enum ConvKind of csrc/executor.cu
 KIND_NAMES = {0: 'conv_fwd', 1: 'conv_fwd_tc', 2: 'conv_dgrad', 3: 'conv_dgrad_tc', 4: 'conv_dgrad_scatter',
-              5: 'conv_wgrad', 6: 'conv_wgrad_tc', 7: 'conv_dgrad_scatter_tc'}
+              5: 'conv_wgrad', 6: 'conv_wgrad_tc', 7: 'conv_dgrad_scatter_tc', 8: 'conv_dgrad_gather2d',
+              9: 'conv_dgrad_gather2d_tc'}
 
 
 def _t3(v, nd, fill):
@@ -259,6 +260,20 @@ def _throttle(plan, dev):
     return q
 
 
+def empty_scratch(n, dtype, dev):
+    """torch.empty for library-owned scratch (arenas, the flat gradient buffer) whose every read element the library writes
+    first.  Under torch.use_deterministic_algorithms torch would fill the block with NaN on the CURRENT stream; an arena
+    belongs to a side stream while the main stream writes it too, so that fill would race with the main stream's first
+    writes (and cost a pass over gigabytes per step)."""
+    import torch.utils.deterministic as tud
+    fill = tud.fill_uninitialized_memory
+    tud.fill_uninitialized_memory = False
+    try:
+        return torch.empty(n, dtype=dtype, device=dev)
+    finally:
+        tud.fill_uninitialized_memory = fill
+
+
 def _alloc_arena(plan, nbytes, dev, stream):
     """One arena for this step.  The host may run several steps ahead of the GPU (no per-step synchronisation), so that
     many arenas are alive at once; a fresh multi-GB block costs a cudaMalloc of tens of milliseconds when it lands in
@@ -271,10 +286,10 @@ def _alloc_arena(plan, nbytes, dev, stream):
         ctx.__enter__()
     try:
         if plan.reserved.get(key) != nbytes:
-            hold = [torch.empty(nbytes, dtype=torch.uint8, device=dev) for _ in range(ARENAS_IN_FLIGHT)]
+            hold = [empty_scratch(nbytes, torch.uint8, dev) for _ in range(ARENAS_IN_FLIGHT)]
             del hold
             plan.reserved[key] = nbytes
-        return torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        return empty_scratch(nbytes, torch.uint8, dev)
     finally:
         if ctx is not None:
             ctx.__exit__(None, None, None)
@@ -295,7 +310,7 @@ def reserve_blocks(tag, nbytes, dev, stream=None, count=16):
     if ctx is not None:
         ctx.__enter__()
     try:
-        hold = [torch.empty(nbytes, dtype=torch.uint8, device=dev) for _ in range(count)]
+        hold = [empty_scratch(nbytes, torch.uint8, dev) for _ in range(count)]
         del hold
     finally:
         if ctx is not None:
@@ -345,6 +360,11 @@ class _Run:
     def indices(self, iset):
         p, n, ndim, s0, s1, s2 = self.query(2, iset)[:6]
         return _view(self.arena, p, (n, 1 + ndim), torch.int32), [s0, s1, s2][:ndim]
+
+    def deterministic_bytes(self):
+        """(deterministic mode or not, arena bytes its partials, tables and operands take in this run so far)."""
+        used, det_bytes, det = self.query(0, 0)[:3]
+        return bool(det), det_bytes
 
     def count(self, iset):
         """Static mode: the device int32[1] row count of an index set (a view into the arena)."""
@@ -491,7 +511,8 @@ def _index_streams(dev, inputs_ready=False):
 def _exec_forward(plan, feats, coords, spatial_shape, batch_size, proj, training, precision, static, arena, side, side2,
                   side_waits_main, seed=None):
     """One vc_exec_forward_seeded call (only one phase where static.phase says so) -> (return code, state blob).  seed:
-    device int64[1] of the plan's layer discards."""
+    device int64[1] of the plan's layer discards.  torch.are_deterministic_algorithms_enabled() selects the deterministic
+    mode (flags bit 2), which the state records for the backward; a captured graph keeps the mode of its capture."""
     oi, of, lf, _, _ = plan.finalize()
     tab, lib, dev = _layer_ptrs(plan), _lib.load(), feats.device
     state = np.zeros(lib.vc_exec_state_bytes(), dtype=np.uint8)
@@ -499,7 +520,8 @@ def _exec_forward(plan, feats, coords, spatial_shape, batch_size, proj, training
         oi.ctypes.data, of.ctypes.data, oi.shape[0], tab.ctypes.data, lf.ctypes.data, len(plan.layers), feats.data_ptr(),
         feats.shape[1], coords.data_ptr(), feats.shape[0], _lib.host_i32(spatial_shape), int(batch_size),
         proj.data_ptr() if proj is not None else None, int(training), int(precision == 'bf16'),
-        1 | ((static.phase if static is not None else 0) << 8), arena.data_ptr(), arena.numel(), _pinned(dev).data_ptr(),
+        1 | (4 if torch.are_deterministic_algorithms_enabled() else 0) | ((static.phase if static is not None else 0) << 8),
+        arena.data_ptr(), arena.numel(), _pinned(dev).data_ptr(),
         ops.tc_error_flag(dev).data_ptr(), state.ctypes.data, state.size, ops._stream(),
         side.cuda_stream if side is not None else None, int(side_waits_main),
         static.caps_array().ctypes.data if static is not None else None, static.n_dev.data_ptr() if static is not None else None,
@@ -531,7 +553,7 @@ class PlanFn(torch.autograd.Function):
                 # (inside a capture: the graph's own pool.  No record_stream: the side / wgrad streams are forked from and
                 #  joined back into the calling stream inside vc_exec_forward / vc_exec_backward, so every later use of the
                 #  block in the calling stream's order comes after all of this step's uses)
-                arena = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+                arena = empty_scratch(nbytes, torch.uint8, dev)
             elif side_obj is not None:
                 # The arena belongs to the SIDE stream (its index kernels are the first writers, possibly while main still
                 # runs the previous step); main's uses are registered with record_stream, so the caching allocator recycles
@@ -572,7 +594,7 @@ class PlanFn(torch.autograd.Function):
         dev = run.arena.device
         if run.static is None:
             reserve_blocks(('flat_grad', id(plan)), 4 * int(offs[-1]), dev)
-        flat = torch.empty(int(offs[-1]), dtype=torch.float32, device=dev)
+        flat = empty_scratch(int(offs[-1]), torch.float32, dev)     # (every element is written by vc_exec_backward)
         tab = _layer_ptrs(plan, flat.data_ptr())
         gs = [None if g is None else g.contiguous() for g in grads]
         slots = np.array([slot for _, slot, _ in plan.published], dtype=np.int32)

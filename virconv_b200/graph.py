@@ -316,7 +316,7 @@ class _PipeInstance(GraphedStep):
         torch.cuda.current_stream(self.dev).wait_stream(s)
         torch.cuda.synchronize(self.dev)
         plan = self.model._plan()
-        self.arena = torch.empty(executor._arena_bytes(plan, self.cap0, self.dev, True), dtype=torch.uint8, device=self.dev)
+        self.arena = executor.empty_scratch(executor._arena_bytes(plan, self.cap0, self.dev, True), torch.uint8, self.dev)
         for p in self.params:
             p.grad = None
         self.overflow.zero_()
