@@ -407,7 +407,14 @@ class VirConv8x(nn.Module):
     """VirConv-T / VirConv-S backbone (spconv_backbone.py:232-535): a LiDAR stream whose submanifold convs share one
     rulebook per stage (indice_keys 'subm1'..'subm4') plus, when `MM`, the virtual-point stream of NRConv blocks.
     Eval mode batches the ROT_NUM transformed copies along x into one [D, H, 4W] tensor (:360,:418-432) and splits the
-    published tensors afterwards."""
+    published tensors afterwards.
+
+    Static mode (CUDA-graph capturable training forward, graph.GraphedStep): each stream takes its own executor.StaticSpec —
+    batch_dict['virconv_static'] for the LiDAR stream, batch_dict['virconv_static_mm'] for the virtual-point stream, whose
+    inputs are then capacity sized — and the MM stream reads the shared projection block batch_dict['virconv_proj'] ([B,28]
+    on the device).  The nine published tensors follow VirConvL8x's static contract (capacity-sized features with a zero
+    tail, indices with a -1 tail, device int32 `.num_rows`), as do the device-drawn StVD lists in 'stvd_kept_rows'.  The eval
+    forward has no static form and raises ValueError when given a StaticSpec."""
 
     def __init__(self, model_cfg, input_channels, grid_size, discard_mode='spconv2_compat', precision='fp32',
                  discard_rng='numpy', **kwargs):
@@ -499,20 +506,59 @@ class VirConv8x(nn.Module):
         mode = plan.layers[0][1].training
         return all(bn.training == mode for _, bn in plan.layers)
 
-    def _run(self, plan, feats, coords, shape, batch_size, proj, names, seed=None):
-        """-> (run record, published tensors)"""
+    @property
+    def static_streams(self):
+        """Batch-key suffixes of the input streams of a static-mode training forward: '' = the LiDAR stream
+        ('voxel_features', 'voxel_coords', 'virconv_static'), '_mm' = the virtual-point stream ('voxel_features_mm',
+        'voxel_coords_mm', 'virconv_static_mm')."""
+        return ('', '_mm') if self.mm else ('',)
+
+    def _check_static(self, batch_dict, rot_num):
+        """Static mode (one executor.StaticSpec per stream) covers what runs through the plan executor in a training forward;
+        anything else would silently compute over capacity-sized buffers as if every row were valid."""
+        given = [s for s in ('', '_mm') if batch_dict.get('virconv_static' + s) is not None]
+        if not given:
+            return False
+        if not self.training:
+            raise ValueError('VirConv8x: static mode covers the training forward only — the eval forward batches the ROT_NUM '
+                             'copies along x and splits the published tensors with data-dependent row counts (decompose_tensor)')
+        if rot_num != 1:
+            raise ValueError('VirConv8x: static mode takes one copy per stream (no transform_param)')
+        if set(given) != set(self.static_streams):
+            raise ValueError('VirConv8x: static mode needs a StaticSpec for each stream: %s'
+                             % ', '.join("batch_dict['virconv_static%s']" % s for s in self.static_streams))
+        if any(batch_dict['virconv_static' + s].phase != 0 for s in given):
+            raise ValueError('VirConv8x: phased static execution (graph.PipelinedStep) covers VirConvL8x only')
+        if self.mm:
+            if batch_dict.get('virconv_proj') is None:
+                raise ValueError("VirConv8x: static mode needs batch_dict['virconv_proj'] (ops.projection_params on the device)")
+            if self._discarding() and (self.discard_rng != 'device' or batch_dict.get('stvd_keep_rows') is not None):
+                raise ValueError("VirConv8x: static mode runs the StVD layer discard in the plan (discard_rng='device'); "
+                                 'host-drawn or caller-given kept rows have no static form')
+        return True
+
+    def _discarding(self):
+        return self.training and self.discard_mode == 'paper' and self.layer_discard_rate != 0
+
+    def _run(self, plan, feats, coords, shape, batch_size, proj, names, seed=None, static=None, stream=''):
+        """-> (run record, published tensors).  static: the stream's StaticSpec (capacity-sized feats / coords)."""
         ci = spconv._as_i32(coords)
         run, res = executor.run_plan(plan, feats, ci, shape, batch_size, proj, plan.layers[0][1].training,
-                                     plan.layers[0][0].precision, seed=seed)
+                                     plan.layers[0][0].precision, static=static, seed=seed)
+        executor.note_last_run(self, run, stream)     # (graph.GraphedStep sizes each stream's capacities from an exact run)
         return run, _published_tensors(run, res, names, ci, shape, batch_size)
 
-    def _lidar_stream(self, feats, coords, shape, batch_size):
+    def _lidar_stream(self, feats, coords, shape, batch_size, static=None):
         plan = self._plan_lidar()
         if not plan.is_current():          # a sub-module was replaced after the plan was built
             self._plan_lidar_cache = None
             plan = self._plan_lidar()
         if self._plan_usable(plan, feats):
-            return self._run(plan, feats, coords, shape, batch_size, None, ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4', 'out'))[1]
+            return self._run(plan, feats, coords, shape, batch_size, None, ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4', 'out'),
+                             static=static)[1]
+        if static is not None:
+            raise ValueError('VirConv8x static mode: the LiDAR stream cannot run through the plan executor (%s)'
+                             % _module_path_reason(feats, plan))
         _module_path_under_determinism(_module_path_reason(feats, plan))
         x = spconv.SparseConvTensor(feats, coords.int(), shape, batch_size)
         x1 = self.conv1(self.conv_input(x))
@@ -533,11 +579,12 @@ class VirConv8x(nn.Module):
         batch_size = batch_dict['batch_size']
         sfx = [''] + [str(i) for i in range(1, rot_num)]
         strides = {'x_conv1': 1, 'x_conv2': 2, 'x_conv3': 4, 'x_conv4': 8}
+        static = self._check_static(batch_dict, rot_num)
         ops.stats_arena(batch_dict['voxel_features'].device).reset()
         if self.training:
             for s in sfx:
                 x1, x2, x3, x4, out = self._lidar_stream(batch_dict['voxel_features' + s], batch_dict['voxel_coords' + s],
-                                                         self.sparse_shape, batch_size)
+                                                         self.sparse_shape, batch_size, batch_dict.get('virconv_static'))
                 batch_dict.update({
                     'encoded_spconv_tensor' + s: out, 'encoded_spconv_tensor_stride' + s: 8,
                     'multi_scale_3d_features' + s: {'x_conv1': x1, 'x_conv2': x2, 'x_conv3': x3, 'x_conv4': x4},
@@ -560,23 +607,27 @@ class VirConv8x(nn.Module):
                                                     'x_conv4': decompose_tensor(x4, i, batch_size)},
                     'multi_scale_3d_strides' + s: dict(strides)})
         if self.mm:
-            calib = batch_dict['calib']
+            calib = batch_dict.get('calib')
             for i, s in enumerate(sfx):
                 feats, coords = batch_dict['voxel_features_mm' + s], batch_dict['voxel_coords_mm' + s]
                 trans = batch_dict['aug_param'] if 'aug_param' in batch_dict else None
                 if 'transform_param' in batch_dict:
                     trans = batch_dict['transform_param'][:, i, :]
-                discarding = self.training and self.discard_mode == 'paper' and self.layer_discard_rate != 0
+                discarding = self._discarding()
                 # device-drawn discards run in the plan; host-drawn or caller-given kept rows on the module path
                 stvd = discarding and self.discard_rng == 'device' and batch_dict.get('stvd_keep_rows') is None
                 if not self._plan_mm(stvd).is_current():
                     self._plan_mm_cache = self._plan_mm_stvd_cache = None
                 if (stvd or not discarding) and self._plan_usable(self._plan_mm(stvd), feats):
-                    side = ops.side(feats.device).stream if executor.TWO_STREAMS else None
-                    proj = ops.projection_params(calib, trans, batch_size, feats.device, side)
+                    # static mode: the shared projection block is already on the device ('virconv_proj', [B,28])
+                    proj = batch_dict['virconv_proj'] if static else None
+                    if proj is None:
+                        side = ops.side(feats.device).stream if executor.TWO_STREAMS else None
+                        proj = ops.projection_params(calib, trans, batch_size, feats.device, side)
                     seed = stvd_seed(batch_dict, feats.device) if stvd else None
                     run, (x1, x2, x3, x4) = self._run(self._plan_mm(stvd), feats, coords, self.sparse_shape, batch_size, proj,
-                                                      ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4'), seed)
+                                                      ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4'), seed,
+                                                      batch_dict.get('virconv_static_mm'), '_mm')
                     if stvd:
                         batch_dict['stvd_kept_rows' + s] = run.kept_rows()
                     batch_dict.update({
@@ -584,6 +635,9 @@ class VirConv8x(nn.Module):
                         'multi_scale_3d_features_mm' + s: {'x_conv1': x1, 'x_conv2': x2, 'x_conv3': x3, 'x_conv4': x4},
                         'multi_scale_3d_strides' + s: dict(strides)})
                     continue
+                if static:
+                    raise ValueError('VirConv8x static mode: the virtual-point stream cannot run through the plan executor (%s)'
+                                     % _module_path_reason(feats, self._plan_mm(stvd)))
                 _module_path_under_determinism(_module_path_reason(feats, self._plan_mm(stvd), discarding and not stvd))
                 proj = ops.projection_params(calib, trans, batch_size, feats.device)
                 x = spconv.SparseConvTensor(feats, coords.int(), self.sparse_shape, batch_size)

@@ -8,6 +8,7 @@ and returns ordinary tensors (features with autograd history, indices) that live
 """
 from __future__ import annotations
 
+import copy
 import ctypes
 import os
 import weakref
@@ -666,26 +667,38 @@ def run_plan(plan, feats, coords_i32, spatial_shape, batch_size, proj, training,
 
 class RunCounts:
     """What outlives a run record (whose arena goes back to the allocator with the step's tensors): the row count of every
-    strided conv's output set, for sizing a StaticSpec."""
+    strided conv's output set, for sizing a StaticSpec.  Read from the run's host-side state blob on first use: every
+    exact-mode forward keeps one, and only capacity sizing ever asks."""
 
     def __init__(self, run):
-        self.rows = {}
-        if run.static is None:               # (a static run's counts live on the device)
+        self._rows, self._src = ({}, None) if run.static is not None else (None, copy.copy(run))
+        if self._src is not None:
+            self._src.arena = None           # (the counts are host values: the step's arena need not stay alive for them)
+
+    @property
+    def rows(self):
+        if self._rows is None:
+            run, self._src, self._rows = self._src, None, {}
             for rb, (keys, ndim, i_in, i_out) in run.plan.rb_keys.items():
                 if i_out != i_in and i_out != 0:
-                    self.rows[i_out] = int(run.query(2, i_out)[1])
+                    self._rows[i_out] = int(run.query(2, i_out)[1])
+        return self._rows
 
 
-_LAST_RUNS = weakref.WeakKeyDictionary()     # model -> RunCounts of its most recent exact-mode run
+_LAST_RUNS = weakref.WeakKeyDictionary()     # model -> {stream: RunCounts of the most recent exact-mode run of that stream}
 
 
-def note_last_run(model, run):
+def note_last_run(model, run, stream=''):
+    """Keep the row counts of an exact-mode run of one of `model`'s plans.  stream: the batch-key suffix of the input stream
+    the plan ran on — '' for VirConvL8x and VirConv8x's LiDAR stream, '_mm' for VirConv8x's virtual-point stream — so that
+    one exact step sizes the StaticSpec of every stream."""
     if run.static is None:
-        _LAST_RUNS[model] = RunCounts(run)
+        _LAST_RUNS.setdefault(model, {})[stream] = RunCounts(run)
 
 
-def last_run(model):
-    return _LAST_RUNS.get(model)
+def last_run(model, stream=''):
+    """RunCounts of the most recent exact-mode run of `model`'s plan on `stream` (see note_last_run), or None."""
+    return _LAST_RUNS.get(model, {}).get(stream)
 
 
 def measured_caps(run, margin=1.3, grain=1024):

@@ -6,7 +6,7 @@ The plan executor's static mode (`executor.StaticSpec`, `vc_exec_forward(..., ca
 data-dependent row count in device memory and sizes every buffer from host-side capacities, so nothing in a step reads a
 device value on the host; `GraphedStep` captures such a step once and replays it:
 
-    step = GraphedStep(model, loss_fn, params)          # model: VirConvL8x in train / eval mode
+    step = GraphedStep(model, loss_fn, params)          # model: VirConvL8x in train / eval mode, or VirConv8x in train mode
     for batch in loader:
         loss = step(batch)                              # copies the batch into the graph's input buffers, replays
         optimizer.step()                                # parameter .grad tensors are rewritten in place by every replay
@@ -15,6 +15,10 @@ Published tensors inside the graph are capacity sized: `t.features` [cap, C] wit
 -1 tail, `t.num_rows` a device int32[1]; `loss_fn(batch_dict)` must use `num_rows` where the reference uses `shape[0]`.
 A batch whose row counts exceed the captured capacities is detected through the executor's overflow flag (read back
 asynchronously, one step late) and handled by re-capturing with larger capacities and re-running that batch.
+
+A model with several input streams (`model.static_streams`: VirConv8x with MM has the LiDAR stream '' and the virtual-point
+stream '_mm') gets input buffers, an input capacity, a device row count and an overflow flag per stream; the batch keys of a
+stream carry its suffix ('voxel_features_mm', 'points_mm', 'virconv_static_mm').
 """
 from __future__ import annotations
 
@@ -58,11 +62,25 @@ def masked_mean(t):
     return _MaskedMean.apply(t.features, getattr(t, 'num_rows', None))
 
 
+class _Stream:
+    """The graph's input side of one stream of the model (batch-key suffix `sfx`, position `i` in the step's device row-count
+    and overflow vectors): its capacity-sized input buffers and the StaticSpec capacities of its plan."""
+
+    def __init__(self, sfx, i):
+        self.sfx, self.i = sfx, i
+        self.caps = {}
+        self.cap0 = 0             # input rows the buffers hold (voxels)
+        self.cap_pts = 0          # with the in-graph voxeliser: input points the point buffer holds
+        self.prev_n = 0
+
+
 class GraphedStep:
     def __init__(self, model, loss_fn, params=None, margin=1.3, grain=1024, warmup=2, check_overflow=True, voxelizer=None):
         """voxelizer: None — batches carry `voxel_features` / `voxel_coords` (what the reference's dataloader + MeanVFE
         deliver); or a dict(point_cloud_range, voxel_size, max_points_per_voxel, max_voxels, vfe_model) — batches carry the
-        collated raw `points` [N, 1+C] and the hash-grid voxelisation + VFE (vc_voxelize_mean) run INSIDE the graph."""
+        collated raw `points` [N, 1+C] and the hash-grid voxelisation + VFE (vc_voxelize_mean) run INSIDE the graph.  With a
+        two-stream model the batch also carries `points_mm`, voxelised by a second call with the entries `max_voxels_mm`
+        (default: `max_voxels`) and `vfe_model_mm` (default: None, the plain mean)."""
         self.model, self.loss_fn = model, loss_fn
         self.vox = dict(voxelizer) if voxelizer is not None else None
         self.params = list(model.parameters()) if params is None else list(params)
@@ -70,95 +88,113 @@ class GraphedStep:
         self.margin, self.grain, self.warmup = margin, grain, warmup
         self.check_overflow = check_overflow
         self.graph = None
-        self.cap0 = 0
-        self.caps = {}
+        self.streams = [_Stream(s, i) for i, s in enumerate(getattr(model, 'static_streams', ('',)))]
         self.recaptures = 0
         self.launches_per_replay = 0
-        self._pending = []        # (event, pinned slot) of the replays whose overflow flag has not been looked at yet
+        self._pending = []        # (event, pinned slot) of the replays whose overflow flags have not been looked at yet
         self._slot = 0
+
+    @property
+    def cap0(self):
+        """Input row capacity of the first (for VirConvL8x: the only) stream."""
+        return self.streams[0].cap0
 
     # ------------------------------------------------------------------------------------------------
     def _round(self, n):
         return (int(n * self.margin) + self.grain - 1) // self.grain * self.grain
 
+    def _vox_arg(self, st, key):
+        """A voxeliser setting for stream `st`: `key + st.sfx` where the dict has it, else `key` — except the virtual-point
+        stream's VFE, which defaults to the plain mean: the reference's MeanVFE applies its MODEL to the LiDAR stream only
+        (mean_vfe.py:51-58)."""
+        if key + st.sfx in self.vox:
+            return self.vox[key + st.sfx]
+        if key == 'vfe_model' and st.sfx == '_mm':
+            return None
+        return self.vox[key]
+
+    def _voxelize(self, st, points, batch_size, static=False):
+        v = self.vox
+        return ops.voxelize_mean(points, batch_size, v['point_cloud_range'], v['voxel_size'], v['max_points_per_voxel'],
+                                 self._vox_arg(st, 'max_voxels'), self._vox_arg(st, 'vfe_model'), static=static)
+
     def _exact_step(self, batch):
-        """One ordinary (exact-shape, host-synchronised) step; also measures the row counts of this batch."""
+        """One ordinary (exact-shape, host-synchronised) step; also measures the row counts of this batch, per stream."""
         for p in self.params:
             p.grad = None
         bd = dict(batch)
         if self.vox is not None:
-            v = self.vox
-            f, c, _ = ops.voxelize_mean(batch['points'], int(batch['batch_size']), v['point_cloud_range'], v['voxel_size'],
-                                        v['max_points_per_voxel'], v['max_voxels'], v['vfe_model'])
-            bd.update(voxel_features=f, voxel_coords=c)
+            for st in self.streams:
+                f, c, _ = self._voxelize(st, batch['points' + st.sfx], int(batch['batch_size']))
+                bd.update({'voxel_features' + st.sfx: f, 'voxel_coords' + st.sfx: c})
         out = self.model(bd)
         loss = self.loss_fn(out)
         loss.backward()
-        return loss.detach(), executor.last_run(self.model)
+        return loss.detach(), [executor.last_run(self.model, st.sfx) for st in self.streams]
 
-    def _make_buffers(self, batch, run):
-        for k, v in executor.measured_caps(run, self.margin, self.grain).items():
-            self.caps[k] = max(self.caps.get(k, 0), v)
+    def _make_buffers(self, batch, runs):
         B = int(batch['batch_size'])
-        if self.vox is not None:
-            pts = batch['points']
-            dev = self.params[0].device
-            self.cap_pts = max(getattr(self, 'cap_pts', 0), self._round(pts.shape[0]))
-            # unused tail rows: last sample's batch index, coordinates far outside the range (dropped by the voxeliser)
-            row = torch.zeros(pts.shape[1], dtype=torch.float32)
-            row[0] = B - 1
-            row[1:4] = -1.0e6
-            self.sentinel = row.to(dev)
-            self.pts = self.sentinel.repeat(self.cap_pts, 1).contiguous()
-            self._prev_n = 0
-            self.cap0 = B * int(self.vox['max_voxels'])
-        else:
-            dev = batch['voxel_features'].device
-            vf, vc = batch['voxel_features'], batch['voxel_coords']
-            self.cap0 = max(self.cap0, self._round(vf.shape[0]))
-            self.vf = torch.zeros((self.cap0, vf.shape[1]), dtype=torch.float32, device=dev)
-            self.vc = torch.full((self.cap0, vc.shape[1]), -1, dtype=vc.dtype, device=dev)
+        dev = self.params[0].device if self.vox is not None else batch['voxel_features'].device
+        for st, run in zip(self.streams, runs):
+            for k, v in executor.measured_caps(run, self.margin, self.grain).items():
+                st.caps[k] = max(st.caps.get(k, 0), v)
+            if self.vox is not None:
+                pts = batch['points' + st.sfx]
+                st.cap_pts = max(st.cap_pts, self._round(pts.shape[0]))
+                # unused tail rows: last sample's batch index, coordinates far outside the range (dropped by the voxeliser)
+                row = torch.zeros(pts.shape[1], dtype=torch.float32)
+                row[0] = B - 1
+                row[1:4] = -1.0e6
+                st.sentinel = row.to(dev)
+                st.pts = st.sentinel.repeat(st.cap_pts, 1).contiguous()
+                st.prev_n = 0
+                st.cap0 = B * int(self._vox_arg(st, 'max_voxels'))
+            else:
+                vf, vc = batch['voxel_features' + st.sfx], batch['voxel_coords' + st.sfx]
+                st.cap0 = max(st.cap0, self._round(vf.shape[0]))
+                st.vf = torch.zeros((st.cap0, vf.shape[1]), dtype=torch.float32, device=dev)
+                st.vc = torch.full((st.cap0, vc.shape[1]), -1, dtype=vc.dtype, device=dev)
+        ns = len(self.streams)
         self.dev, self.B = dev, B
-        self.n_dev = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.overflow = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.n_dev = torch.zeros(ns, dtype=torch.int32, device=dev)        # input rows of each stream
+        self.overflow = torch.zeros(ns, dtype=torch.int32, device=dev)     # each stream's StaticSpec overflow flag
         self.proj = torch.zeros((B, 28), dtype=torch.float32, device=dev)
         # pinned staging for the small per-step host values: a ring of slots, each guarded by an event recorded after its
         # upload — the host runs several replays ahead of the GPU, and rewriting ONE pinned buffer before the previous
-        # step's asynchronous copy has executed would hand that step the next step's row count / projection
+        # step's asynchronous copy has executed would hand that step the next step's row counts / projection
         self.STAGE_SLOTS = 8
         self.proj_host = torch.zeros((self.STAGE_SLOTS, B, 28), dtype=torch.float32).pin_memory()
-        self.n_host = torch.zeros((self.STAGE_SLOTS, 1), dtype=torch.int32).pin_memory()
+        self.n_host = torch.zeros((self.STAGE_SLOTS, ns), dtype=torch.int32).pin_memory()
         self._stage_ev = [None] * self.STAGE_SLOTS
         self._stage = 0
-        self.ovf_host = torch.zeros(8, dtype=torch.int32).pin_memory()
+        self.ovf_host = torch.zeros((8, ns), dtype=torch.int32).pin_memory()
         self.err_host = torch.zeros(8, dtype=torch.int32).pin_memory()
         self._pending, self._slot = [], 0
-        self.spec = executor.StaticSpec(self.n_dev, self.caps, self.overflow, alias_params=True)
+        for st in self.streams:
+            st.spec = executor.StaticSpec(self.n_dev[st.i:st.i + 1], st.caps, self.overflow[st.i:st.i + 1], alias_params=True)
 
     def _load(self, batch):
-        """Copy one batch into the graph's input buffers (asynchronous, current stream)."""
+        """Copy one batch into the graph's input buffers (asynchronous, current stream).  False (nothing copied) when a
+        stream's input does not fit."""
+        key = 'points' if self.vox is not None else 'voxel_features'
+        ns = [batch[key + st.sfx].shape[0] for st in self.streams]
+        if any(n > (st.cap_pts if self.vox is not None else st.cap0) for st, n in zip(self.streams, ns)):
+            return False
         if self.vox is not None:
-            pts = batch['points']
-            n = pts.shape[0]
-            if n > self.cap_pts:
-                return False
-            self.pts[:n].copy_(pts, non_blocking=True)
-            if self._prev_n > n:                       # rows of the previous (larger) batch still sit behind this one
-                self.pts[n:self._prev_n] = self.sentinel
-            self._prev_n = n
-        else:
-            vf, vc = batch['voxel_features'], batch['voxel_coords']
-            n = vf.shape[0]
-            if n > self.cap0:
-                return False
+            for st, n in zip(self.streams, ns):
+                st.pts[:n].copy_(batch['points' + st.sfx], non_blocking=True)
+                if st.prev_n > n:                      # rows of the previous (larger) batch still sit behind this one
+                    st.pts[n:st.prev_n] = st.sentinel
+                st.prev_n = n
         slot = self._stage
         self._stage = (slot + 1) % self.STAGE_SLOTS
         if self._stage_ev[slot] is not None:
             self._stage_ev[slot].synchronize()         # (8 steps back: has long completed unless the GPU is far behind)
         if self.vox is None:
-            self.vf[:n].copy_(vf, non_blocking=True)
-            self.vc[:n].copy_(vc, non_blocking=True)
-            self.n_host[slot, 0] = n
+            for st, n in zip(self.streams, ns):
+                st.vf[:n].copy_(batch['voxel_features' + st.sfx], non_blocking=True)
+                st.vc[:n].copy_(batch['voxel_coords' + st.sfx], non_blocking=True)
+                self.n_host[slot, st.i] = n
             self.n_dev.copy_(self.n_host[slot], non_blocking=True)
         trans = batch.get('aug_param')
         self.proj_host[slot].copy_(torch.from_numpy(ops.projection_params_host(batch['calib'], trans, self.B)))
@@ -169,17 +205,21 @@ class GraphedStep:
         return True
 
     def _static_batch(self, batch):
-        bd = {k: v for k, v in batch.items() if k not in ('voxel_features', 'voxel_coords', 'points')}
-        if self.vox is not None:
-            v = self.vox
-            f, c, num, n_dev = ops.voxelize_mean(self.pts, self.B, v['point_cloud_range'], v['voxel_size'], v['max_points_per_voxel'],
-                                                 v['max_voxels'], v['vfe_model'], static=True)
-            spec = executor.StaticSpec(n_dev, self.caps, self.overflow, alias_params=True)
-            bd.update(voxel_features=f, voxel_coords=c, voxel_num_points=num, virconv_static=spec, virconv_proj=self.proj)
-        else:
-            spec = self.spec
-            bd.update(voxel_features=self.vf, voxel_coords=self.vc, virconv_static=spec, virconv_proj=self.proj)
-        self._cur_spec = spec
+        drop = {k + st.sfx for st in self.streams for k in ('voxel_features', 'voxel_coords', 'points')}
+        bd = {k: v for k, v in batch.items() if k not in drop}
+        specs = []
+        for st in self.streams:
+            if self.vox is not None:
+                f, c, num, n_dev = self._voxelize(st, st.pts, self.B, static=True)
+                spec = executor.StaticSpec(n_dev, st.caps, self.overflow[st.i:st.i + 1], alias_params=True)
+                bd.update({'voxel_features' + st.sfx: f, 'voxel_coords' + st.sfx: c, 'voxel_num_points' + st.sfx: num})
+            else:
+                spec = st.spec
+                bd.update({'voxel_features' + st.sfx: st.vf, 'voxel_coords' + st.sfx: st.vc})
+            bd['virconv_static' + st.sfx] = spec
+            specs.append(spec)
+        bd['virconv_proj'] = self.proj
+        self._cur_specs = specs
         return bd
 
     def _static_step(self, batch):
@@ -187,7 +227,9 @@ class GraphedStep:
         loss = self.loss_fn(out)
         # torch.autograd.grad w.r.t. the per-call leaf aliases the executor made of the parameters (executor.run_plan): no
         # long-lived AccumulateGrad node (which remembers the stream it was created on) takes part in a captured backward
-        alias = self._cur_spec.param_aliases
+        alias = {}
+        for spec in self._cur_specs:
+            alias.update(spec.param_aliases)
         grads = torch.autograd.grad(loss, [alias.get(id(p), p) for p in self.params], allow_unused=True)
         for p, g in zip(self.params, grads):
             p.grad = g
@@ -195,9 +237,9 @@ class GraphedStep:
 
     def _capture(self, batch):
         torch.cuda.synchronize(self.dev)
-        loss_e, run = self._exact_step(batch)
-        assert run is not None, 'GraphedStep needs a backbone running through the plan executor'
-        self._make_buffers(batch, run)
+        loss_e, runs = self._exact_step(batch)
+        assert all(r is not None for r in runs), 'GraphedStep needs a backbone running each stream through the plan executor'
+        self._make_buffers(batch, runs)
         assert self._load(batch)
         # warm-up of the static path on a side stream (allocator pools, lazy kernel attributes), as torch.cuda.graphs asks for
         s = torch.cuda.Stream(device=self.dev)
@@ -223,12 +265,12 @@ class GraphedStep:
 
     # ------------------------------------------------------------------------------------------------
     def _overflowed(self):
-        """Largest overflow reported by the replays that have COMPLETED so far (never blocks: the flag of a step is read
-        back asynchronously and looked at when its event has fired, typically one or two calls later)."""
+        """Largest overflow reported by the replays that have COMPLETED so far, over all streams (never blocks: the flags of
+        a step are read back asynchronously and looked at when its event has fired, typically one or two calls later)."""
         worst = 0
         while self._pending and self._pending[0][0].query():
             ev, slot = self._pending.pop(0)
-            worst = max(worst, int(self.ovf_host[slot]))
+            worst = max(worst, int(self.ovf_host[slot].max()))
             if int(self.err_host[slot]) != 0:
                 raise _lib.VirConvLibraryError('a tensor-core kernel\'s pipeline wait timed out inside a replayed step '
                                                '(error flag set): the results of that step are invalid')
@@ -249,15 +291,15 @@ class GraphedStep:
             assert self._load(batch)
         self.graph.replay()
         if self.check_overflow:
-            if len(self._pending) >= self.ovf_host.numel():     # (host far ahead of the GPU: wait for the oldest read-back)
+            if len(self._pending) >= self.ovf_host.shape[0]:    # (host far ahead of the GPU: wait for the oldest read-back)
                 self._pending[0][0].synchronize()
                 if self._overflowed():
                     self.margin *= 1.25
                     self._capture(batch)
                     return self(batch)
             slot = self._slot
-            self._slot = (slot + 1) % self.ovf_host.numel()
-            self.ovf_host[slot:slot + 1].copy_(self.overflow, non_blocking=True)
+            self._slot = (slot + 1) % self.ovf_host.shape[0]
+            self.ovf_host[slot].copy_(self.overflow, non_blocking=True)
             self.err_host[slot:slot + 1].copy_(ops.tc_error_flag(self.dev), non_blocking=True)
             self.overflow.zero_()
             ev = torch.cuda.Event()
@@ -302,9 +344,9 @@ class _PipeInstance(GraphedStep):
 
     def _capture(self, batch):
         torch.cuda.synchronize(self.dev)
-        loss_e, run = self._exact_step(batch)
-        assert run is not None, 'PipelinedStep needs a backbone running through the plan executor'
-        self._make_buffers(batch, run)
+        loss_e, runs = self._exact_step(batch)
+        assert all(r is not None for r in runs), 'PipelinedStep needs a backbone running through the plan executor'
+        self._make_buffers(batch, runs)
         assert self._load(batch)
         s = torch.cuda.Stream(device=self.dev)
         s.wait_stream(torch.cuda.current_stream(self.dev))
@@ -346,6 +388,10 @@ class PipelinedStep:
     to the buffer set of the step that just ran."""
 
     def __init__(self, model, loss_fn, params=None, **kwargs):
+        streams = tuple(getattr(model, 'static_streams', ('',)))
+        if streams != ('',):
+            raise ValueError('PipelinedStep phases a one-stream backbone (VirConvL8x); %s has the input streams %s, which have '
+                             'no phased form: use GraphedStep' % (type(model).__name__, streams))
         self.inst = [_PipeInstance(model, loss_fn, params, **kwargs) for _ in range(2)]
         self.params = self.inst[0].params
         self.dev = self.inst[0].dev
@@ -389,11 +435,11 @@ class PipelinedStep:
         for p, g in zip(self.params, inst.grads):
             p.grad = g
         if inst.check_overflow:
-            if len(inst._pending) >= inst.ovf_host.numel():
+            if len(inst._pending) >= inst.ovf_host.shape[0]:
                 inst._pending[0][0].synchronize()
             slot = inst._slot
-            inst._slot = (slot + 1) % inst.ovf_host.numel()
-            inst.ovf_host[slot:slot + 1].copy_(inst.overflow, non_blocking=True)
+            inst._slot = (slot + 1) % inst.ovf_host.shape[0]
+            inst.ovf_host[slot].copy_(inst.overflow, non_blocking=True)
             inst.err_host[slot:slot + 1].copy_(ops.tc_error_flag(self.dev), non_blocking=True)
             inst.overflow.zero_()
             e2 = torch.cuda.Event()
