@@ -53,6 +53,9 @@ long long vc_launch_count(void);
 int vc_set_pdl(int enable);
 /* BatchNorm backward as ONE cooperative launch (reduction, grid-wide barrier, apply; default on) or as two launches (0). */
 int vc_set_bn_fused(int enable);
+/* BatchNorm + ReLU of the tensor-core conv forward inside the conv's own launch (1, the default; cooperative: conv, grid-wide
+ * barrier, apply) or as a separate apply kernel (0).  Read when a forward is enqueued (a captured graph keeps its choice). */
+int vc_set_conv_bn_fused(int enable);
 /* Tensor-core conv kernel selector: accepts 1 (the persistent kernel, csrc/conv_tc2.cu, the only one); else VC_ERR_INVALID. */
 int vc_set_tc_variant(int variant);
 /* A/B aid for the persistent tensor-core conv kernel (conv_tc2.cu): CTAs per SM, 0 = automatic (two when each still gets a
@@ -176,6 +179,19 @@ int vc_conv_wgrad_tc(const void* in_bf16, const void* dout_bf16, const int32_t* 
 size_t vc_conv_fwd_det_ws_bytes(int n_out, int cin, int cout, int K);
 int vc_conv_fwd_det(int precision, const void* in, const float* w, const int32_t* nbr, float* out, int n_out, int cin, int cout,
                     int K, double* bn_sums, void* ws, size_t ws_bytes, int32_t* err_flag, vc_stream_t stream);
+/* Conv forward on tensor cores followed by BatchNorm + ReLU (vc_bn_apply_relu_f32's arithmetic), as the plan executor runs
+ * it: with vc_set_conv_bn_fused(1) in ONE cooperative launch (a grid-wide barrier between the conv and the apply), else the
+ * conv, then the apply kernel; both give the same bits.  x [n_out, cout]: the conv's fp32 output (kept for backward);
+ * y / y_bf16 (either may be NULL) at row pitches y_ld / yb_ld (multiples of 4, >= cout: a column slice of a wider matrix).
+ * n_dev (optional, device int): the row count, n_out is then the capacity and the output rows [count, n_out) are zeroed.
+ * deterministic: the BN sums from per-128-row-tile partials added in tile order (vc_conv_fwd_det).  cin, cout in
+ * {8,16,32,64}.  ws >= vc_conv_bn_relu_tc_ws_bytes(n_out, cin, cout, K). */
+size_t vc_conv_bn_relu_tc_ws_bytes(int n_out, int cin, int cout, int K);
+int vc_conv_bn_relu_tc(const void* in_bf16, const float* w, const int32_t* nbr, float* x, int n_out, const int32_t* n_dev, int cin,
+                       int cout, int K, int deterministic, const float* gamma, const float* beta, float* running_mean,
+                       float* running_var, long long* num_batches_tracked, float momentum, float eps, int training, float* y,
+                       int y_ld, void* y_bf16, int yb_ld, float* stats_out, void* ws, size_t ws_bytes, int32_t* err_flag,
+                       vc_stream_t stream);
 /* vc_conv_wgrad_tc with the rows split into 32 runs of consecutive 128-row tiles (from n_out alone); a CTA claims whole
  * runs, each run's sum goes to its own fp32 image, and the images are added in run order.  The CTA cap of
  * vc_conv_wgrad_tc3_config applies (0: one CTA per SM).  ws >= vc_conv_wgrad_tc_det_ws_bytes(...) (32 images). */

@@ -28,6 +28,7 @@ SIGNATURES = {
     'vc_launch_count': (ctypes.c_longlong, []),
     'vc_set_pdl': (_I, [_I]),
     'vc_set_bn_fused': (_I, [_I]),
+    'vc_set_conv_bn_fused': (_I, [_I]),
     'vc_set_tc_variant': (_I, [_I]),
     'vc_conv_tc2_config': (_I, [_I]),
     'vc_conv_wgrad_tc3_config': (_I, [_I, _I]),
@@ -53,6 +54,9 @@ SIGNATURES = {
     'vc_conv_wgrad_tc': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _Z, _P, _P]),
     'vc_conv_fwd_det_ws_bytes': (_Z, [_I, _I, _I, _I]),
     'vc_conv_fwd_det': (_I, [_I, _P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _P, _P]),
+    'vc_conv_bn_relu_tc_ws_bytes': (_Z, [_I, _I, _I, _I]),
+    'vc_conv_bn_relu_tc': (_I, [_P, _P, _P, _P, _I, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _F, _F, _I, _P, _I, _P, _I, _P, _P, _Z,
+                                _P, _P]),
     'vc_conv_wgrad_tc_det_ws_bytes': (_Z, [_I, _I, _I, _I]),
     'vc_conv_wgrad_tc_det': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _Z, _P, _P]),
     'vc_bn_bwd_det_ws_bytes': (_Z, [_I, _I]),
@@ -142,6 +146,8 @@ def load():
     # programmatic dependent launch of the conv / BN chain: implemented and parity-tested, but not measured faster
     # -> off unless asked for
     lib.vc_set_pdl(1 if os.environ.get('VIRCONV_PDL', '0') == '1' else 0)
+    # BatchNorm + ReLU inside the tensor-core conv forward (one cooperative launch per layer); 0 for A/B runs
+    lib.vc_set_conv_bn_fused(0 if os.environ.get('VIRCONV_CONV_BN_FUSED', '1') == '0' else 1)
     _lib = lib
     return lib
 

@@ -10,19 +10,10 @@
 // coefficients from those sums.  The float64 accumulators make the fp32-rounded results independent of the
 // atomic arrival order for all practical purposes (each addend is an fp32 tile partial, < 2^12 of them).
 #include <cooperative_groups.h>
-#include <cuda_bf16.h>
 
-#include "common.cuh"
+#include "bn_common.cuh"
 
 namespace vc {
-
-__device__ __forceinline__ uint2 pack_bf16x4(float4 v) {
-    __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
-    uint2 o;
-    o.x = *reinterpret_cast<uint32_t*>(&a);
-    o.y = *reinterpret_cast<uint32_t*>(&b);
-    return o;
-}
 
 // y = relu(x*scale + shift); train: statistics from `sums`, eval: from the running buffers.
 // stats_out [4, c] = scale, shift, mean, invstd (block 0).  grid-stride over float4 with stride % (c/4) == 0.
@@ -45,38 +36,9 @@ __global__ void __launch_bounds__(256) bn_apply_relu_kernel(
     const size_t stride = (size_t)gridDim.x * blockDim.x;
     const int cg = (int)(i0 % c4);
     __shared__ float sc_s[128], sh_s[128];
-    if (threadIdx.x < c) {   // one thread per channel derives scale / shift (float64 once per block, not per thread)
-        const int ch = threadIdx.x;
-        float mean, invstd;
-        double var = 0.0;
-        if (training) {
-            const double n = (double)(n_rows > 0 ? n_rows : 1);
-            const double m = sums[ch] / n;
-            var = sums[c + ch] / n - m * m;
-            if (var < 0.0) var = 0.0;
-            mean = (float)m;
-            invstd = (float)(1.0 / sqrt(var + (double)eps));
-        } else {
-            mean = running_mean[ch];
-            invstd = 1.f / sqrtf(running_var[ch] + eps);
-        }
-        const float scv = gamma[ch] * invstd;
-        const float shv = beta[ch] - mean * scv;
-        sc_s[ch] = scv;
-        sh_s[ch] = shv;
-        if (blockIdx.x == 0) {
-            stats_out[ch] = scv;
-            stats_out[c + ch] = shv;
-            stats_out[2 * c + ch] = mean;
-            stats_out[3 * c + ch] = invstd;
-            if (training) {
-                const double n = (double)n_rows;
-                const double unbiased = n_rows > 1 ? var * n / (n - 1.0) : var;
-                running_mean[ch] = (1.f - momentum) * running_mean[ch] + momentum * mean;
-                running_var[ch] = (1.f - momentum) * running_var[ch] + momentum * (float)unbiased;
-            }
-        }
-    }
+    if (threadIdx.x < c)   // one thread per channel derives scale / shift (float64 once per block, not per thread)
+        bn_channel(training ? sums[threadIdx.x] : 0.0, training ? sums[c + threadIdx.x] : 0.0, threadIdx.x, c, n_rows, gamma, beta,
+                   running_mean, running_var, momentum, eps, training, sc_s, sh_s, blockIdx.x == 0, stats_out);
     if (training && blockIdx.x == 0 && threadIdx.x == 0 && num_batches_tracked != nullptr) *num_batches_tracked += 1;
     __syncthreads();
     float sc[4], sh[4];
@@ -87,12 +49,7 @@ __global__ void __launch_bounds__(256) bn_apply_relu_kernel(
     }
     const bool dense = y_ld4 == c4 && yb_ld4 == c4;
     for (size_t i = i0; i < n4; i += stride) {
-        float4 v = x[i];
-        v.x = fmaf(v.x, sc[0], sh[0]); v.y = fmaf(v.y, sc[1], sh[1]);
-        v.z = fmaf(v.z, sc[2], sh[2]); v.w = fmaf(v.w, sc[3], sh[3]);
-        if (relu) {
-            v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
-        }
+        const float4 v = bn_relu4(x[i], sc, sh, relu);
         const size_t r = i / c4;
         const size_t oy = dense ? i : r * y_ld4 + cg, ob = dense ? i : r * yb_ld4 + cg;
         if (y != nullptr) y[oy] = v;
@@ -121,16 +78,8 @@ __global__ void __launch_bounds__(256) bn_sums_reduce_kernel(const double* __res
     pdl_launch_dependents();
     const int rows = n_dev != nullptr ? min(cap_rows, __ldg(n_dev)) : cap_rows;
     const int n_parts = (rows + rows_per_part - 1) / rows_per_part;
-    const int j = blockIdx.x;
-    double v = 0.0;
-    for (int p = threadIdx.x; p < n_parts; p += 256) v += part[(size_t)p * 2 * c + j];
-    red[threadIdx.x] = v;
-    __syncthreads();
-    for (int s = 128; s > 0; s >>= 1) {
-        if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) sums[j] = red[0];
+    const double v = bn_sums_column(part, n_parts, c, blockIdx.x, red);
+    if (threadIdx.x == 0) sums[blockIdx.x] = v;
 }
 
 // BN backward, deterministic: chunk ch = rows [ch * BN_DET_ROWS, ...) -> part[ch][2][c] = (sum g, sum g*xhat) in float64.

@@ -208,13 +208,32 @@ int add_rows_ld_dev(float* dst, int ld, const float* src, int cap, const int* n_
 
 // ---- conv_tc2.cu (persistent tensor-core conv: forward and gather dgrad) ----
 int num_sms();   // of the current device
+// BatchNorm + ReLU run by a forward conv launch itself, after a grid-wide barrier (the arguments of bn_apply_relu_dev; relu on)
+struct BnTail {
+    const float *gamma, *beta;
+    float *running_mean, *running_var;
+    long long* nbt;          // num_batches_tracked (may be NULL)
+    float momentum, eps;
+    int training;
+    double* sums;            // [2, c] channel sums: zeroed by the caller (deterministic mode: written from the tile partials)
+    float* y;                // fp32 output (may be NULL), row pitch y_ld
+    int y_ld;
+    void* yb;                // bf16 shadow (may be NULL), row pitch yb_ld
+    int yb_ld;
+    float* stats;            // [4, c] scale, shift, mean, invstd
+    int tail_zero;           // zero the output rows [count, capacity)
+    int* bar;                // grid-barrier counter, zeroed by the caller
+};
+extern int g_conv_bn_fused;  // vc_set_conv_bn_fused; cleared for good when the device refuses the cooperative launch
 size_t tc_image_bytes(int cin, int cout, int K, int layout);
 bool tc2_ch_ok(int c);
 int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_t* nbr, long long pitch, float* out, int n_rows,
              const int* n_dev, int K, double* bn_sums, int* err, cudaStream_t stream, const float* addend,
              int* tile_counter = nullptr, int flags = 0,   // flags: bit 0 sparse offsets (strided dgrad), bit 1 early tables
              int in_ld = 0,                                // row pitch of in_bf16 (0: kc)
-             double* bn_part = nullptr);                   // deterministic BN sums: [tiles, 2, nr] per 128-row tile (bn_sums NULL)
+             double* bn_part = nullptr,                    // deterministic BN sums: [tiles, 2, nr] per 128-row tile (bn_sums NULL)
+             const BnTail* bn = nullptr,                   // forward only: BN + ReLU in the same launch when g_conv_bn_fused
+             bool* bn_done = nullptr);                     // set when it ran (else the caller launches the apply)
 // fp32 gather conv forward (vc_conv_fwd_f32) whose BN channel sums go to bn_part [tiles, 2, cout] per 128-row tile instead
 int conv_fwd_f32_part(const float* in, const float* w, const int32_t* nbr, float* out, int n_out, int cin, int cout, int K,
                       double* bn_part, void* ws, size_t ws_bytes, cudaStream_t stream);

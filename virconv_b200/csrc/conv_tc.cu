@@ -235,6 +235,47 @@ extern "C" int vc_conv_fwd_det(int precision, const void* in, const float* w, co
     return bn_sums_reduce_dev(part, n_out, nullptr, TCM, cout, bn_sums, stream);
 }
 
+extern "C" size_t vc_conv_bn_relu_tc_ws_bytes(int n_out, int cin, int cout, int K) {
+    if (n_out < 0 || cin <= 0 || cout <= 0 || K < 1) return 0;
+    return det_w_bytes(cin, cout, K) + ((size_t)cdiv(n_out > 0 ? n_out : 1, TCM) + 1) * 2 * cout * sizeof(double) + 256;
+}
+
+extern "C" int vc_conv_bn_relu_tc(const void* in_bf16, const float* w, const int32_t* nbr, float* x, int n_out, const int32_t* n_dev,
+                                  int cin, int cout, int K, int deterministic, const float* gamma, const float* beta,
+                                  float* running_mean, float* running_var, long long* num_batches_tracked, float momentum, float eps,
+                                  int training, float* y, int y_ld, void* y_bf16, int yb_ld, float* stats_out, void* ws,
+                                  size_t ws_bytes, int32_t* err_flag, vc_stream_t stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    VC_CHECK_ARG(n_out >= 0 && K >= 1 && K <= MAXK_TC, "bad n=%d or K=%d", n_out, K);
+    if (!tc2_ch_ok(cin) || !tc2_ch_ok(cout)) {
+        set_error("unsupported channels cin=%d cout=%d (need 8/16/32/64)", cin, cout);
+        return VC_ERR_UNSUPPORTED;
+    }
+    if (n_out == 0) return VC_OK;
+    VC_CHECK_ARG(in_bf16 && w && nbr && x && ws && (y || y_bf16), "null pointer");
+    VC_CHECK_ARG(y_ld % 4 == 0 && yb_ld % 4 == 0 && y_ld >= cout && yb_ld >= cout, "bad output pitch");
+    if (ws_bytes < vc_conv_bn_relu_tc_ws_bytes(n_out, cin, cout, K)) {
+        set_error("conv + BN workspace %zu < %zu", ws_bytes, vc_conv_bn_relu_tc_ws_bytes(n_out, cin, cout, K));
+        return VC_ERR_WORKSPACE;
+    }
+    const size_t wb = det_w_bytes(cin, cout, K);
+    double* sums = reinterpret_cast<double*>((char*)ws + wb);
+    int* bar = reinterpret_cast<int*>(sums + 2 * cout);
+    double* part = deterministic && training ? reinterpret_cast<double*>((char*)bar + 256) : nullptr;
+    VC_CUDA(cudaMemsetAsync(sums, 0, 2 * cout * sizeof(double) + 256, stream));
+    int rc = tc_one_image(w, ws, cin, cout, K, 0, 0, 1, stream);
+    if (rc) return rc;
+    const BnTail bt{gamma, beta, running_mean, running_var, num_batches_tracked, momentum, eps, training, sums, y, y_ld, y_bf16, yb_ld,
+                    stats_out, n_dev != nullptr, bar};
+    bool done = false;
+    rc = tc2_conv(cin, cout, in_bf16, ws, nbr, n_out, x, n_out, n_dev, K, training ? sums : nullptr, err_flag, stream, nullptr, nullptr,
+                  0, 0, part, &bt, &done);
+    if (rc || done) return rc;
+    if (part && (rc = bn_sums_reduce_dev(part, n_out, n_dev, TCM, cout, sums, stream)) != VC_OK) return rc;
+    return bn_apply_relu_dev(x, sums, n_out, n_dev, cout, gamma, beta, running_mean, running_var, num_batches_tracked, momentum, eps,
+                             training, y, y_ld, y_bf16, yb_ld, stats_out, 1, n_dev != nullptr, stream);
+}
+
 /* din[nbr[k,o], :] += dout[o, :] @ w[:, k, :] on tensor cores (many-to-one tables; din zeroed by the caller) */
 extern "C" int vc_conv_dgrad_scatter_tc(const void* dout_bf16, const float* w, const int32_t* nbr, float* din, int n_out,
                                         int cin, int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag,

@@ -26,9 +26,12 @@
 // Every mbarrier wait is time-bounded (2 s): a wedged pipeline stores a code in the error flag and the roles leave their loops.
 // Replaces spconv `ops.indice_conv` / `indice_conv_backward` (input gradient) behind spconv_backbone.py:89,92-93,113,563-564.
 // Algorithmic bytes per launch: N_in*C_in*2 + N_out*C_out*4 + P*8 + K*C_in*C_out*2;  FLOPs 2*P*C_in*C_out.
+#include "bn_common.cuh"
 #include "tc_common.cuh"
 
 namespace vc {
+
+int g_conv_bn_fused = 1;     // 1: BatchNorm + ReLU inside the forward conv (cooperative launch); 0: separate apply kernel
 
 int num_sms() {
     static int sms = 0;
@@ -89,6 +92,7 @@ struct PArgs {
     int scan_k;                // the loader lists the kernel offsets that touch each tile (strided-conv dgrad: most do not)
     int ntb_alloc;             // neighbour-table buffers in shared memory (2 when two CTAs share an SM, else P_NTB)
     int* err;
+    BnTail bn;                 // bn.bar != NULL: BatchNorm + ReLU after a grid-wide barrier (forward, cooperative launch)
 };
 
 #ifdef VC_TC_TRACE
@@ -122,6 +126,39 @@ __device__ __forceinline__ void pclock(long long* g_trace2, int role, int& idx) 
     do {                                                              \
         if (!mbar_wait_t((bar), (parity), a.err, (code))) goto done;  \
     } while (0)
+
+// Grid-wide barrier of a cooperative launch: the k-th barrier waits until the counter `bar` (zeroed before the launch) reaches
+// target = k * gridDim.x.  Time-bounded like the pipeline waits: after 2 s it stores 0x160 in the error flag and the block
+// gets false.
+__device__ __forceinline__ bool grid_barrier(int* bar, int target, int* err, int* ok_s) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        atomicAdd(bar, 1);
+        int ok = 1;
+        unsigned long long t0 = 0;
+        for (unsigned spin = 0;; ++spin) {
+            int v;
+            asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(bar) : "memory");
+            if (v >= target) break;
+            if ((spin & 63u) == 63u) {
+                unsigned long long t;
+                asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+                if (t0 == 0) {
+                    t0 = t;
+                } else if (t - t0 > 2000000000ULL) {
+                    if (err) atomicCAS(err, 0, 0x160);
+                    ok = 0;
+                    break;
+                }
+            }
+        }
+        __threadfence();
+        *ok_s = ok;
+    }
+    __syncthreads();
+    return *ok_s != 0;
+}
 
 __device__ __forceinline__ void sts_zero16(uint32_t saddr) {
     asm volatile("st.shared.v4.b32 [%0], {%1, %1, %1, %1};" ::"r"(saddr), "r"(0u) : "memory");
@@ -567,6 +604,61 @@ done:
         mbar_wait_t(&wres_bar, 0u, a.err, 0x150);
     }
     __syncthreads();
+    if (a.bn.bar == nullptr) return;
+
+    // ---------------------------------------------------------------- fused BatchNorm + ReLU (bn_apply_relu_kernel's work)
+    // Once every CTA has stored its tiles and added its channel sums, the whole output is read back and normalised,
+    // grid-stride over float4 like the apply kernel: the layer's fp32 output (<= 20 MB) is still in L2 whichever SM wrote it.
+    __shared__ int ok_s;
+    const BnTail& b = a.bn;
+    const int oc = a.out_c;
+    bool ok = grid_barrier(b.bar, gridDim.x, a.err, &ok_s);
+    if (ok && b.training && a.bn_part != nullptr) {
+        // deterministic mode: the tile partials in tile order (bn_sums_reduce_kernel's arithmetic), one column per CTA
+        const int n_parts = (n + TCM - 1) / TCM;
+        for (int j = blockIdx.x; j < 2 * oc; j += gridDim.x) {
+            const double v = bn_sums_column(a.bn_part, n_parts, oc, j, red_s[0]);
+            if (tid == 0) b.sums[j] = v;
+        }
+        ok = grid_barrier(b.bar, 2 * gridDim.x, a.err, &ok_s);
+    }
+    if (!ok) return;
+    float* sc_s = stg;            // (the staging buffer is dead: >= 64 x 17 floats)
+    float* sh_s = stg + oc;
+    if (tid < oc)
+        bn_channel(b.training ? __ldcg(b.sums + tid) : 0.0, b.training ? __ldcg(b.sums + oc + tid) : 0.0, tid, oc, n, b.gamma, b.beta,
+                   b.running_mean, b.running_var, b.momentum, b.eps, b.training, sc_s, sh_s, blockIdx.x == 0, b.stats);
+    if (b.training && blockIdx.x == 0 && tid == 0 && b.nbt != nullptr) *b.nbt += 1;
+    __syncthreads();
+    static_assert(P_THREADS % 16 == 0, "the fused apply keeps each thread on one channel group (c / 4 <= 16)");
+    const int c4 = oc >> 2;
+    const size_t n4 = (size_t)n * c4, stride = (size_t)gridDim.x * P_THREADS;
+    const size_t i0 = (size_t)blockIdx.x * P_THREADS + tid;
+    const int cg = (int)(i0 % c4);
+    float sc[4], sh[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        sc[j] = sc_s[cg * 4 + j];
+        sh[j] = sh_s[cg * 4 + j];
+    }
+    const float4* x4 = reinterpret_cast<const float4*>(a.out);
+    float4* y4 = reinterpret_cast<float4*>(b.y);
+    uint2* yb = reinterpret_cast<uint2*>(b.yb);
+    const int y_ld4 = b.y_ld >> 2, yb_ld4 = b.yb_ld >> 2;
+    for (size_t i = i0; i < n4; i += stride) {
+        const float4 v = bn_relu4(__ldcg(x4 + i), sc, sh, 1);     // (written by other CTAs of this grid: not through L1)
+        const size_t r = i / c4;
+        if (y4 != nullptr) y4[r * y_ld4 + cg] = v;
+        if (yb != nullptr) yb[r * yb_ld4 + cg] = pack_bf16x4(v);
+    }
+    if (b.tail_zero) {
+        const size_t t4 = (size_t)a.n_host * c4;
+        for (size_t i = n4 + i0; i < t4; i += stride) {
+            const size_t r = i / c4;
+            if (y4 != nullptr) y4[r * y_ld4 + cg] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (yb != nullptr) yb[r * yb_ld4 + cg] = make_uint2(0u, 0u);
+        }
+    }
 }
 
 // weight images for the kernel above: per offset k a [NRp rows][KCp] bf16 matrix, K-major, rows = one swizzle span,
@@ -611,7 +703,7 @@ bool plan_smem(int K, size_t budget, int ntb, size_t resident_max, int min_stage
 }
 
 template <int KC, int NR>
-int launch_persist(const PArgs& a0, int n_cap, cudaStream_t stream) {
+int launch_persist(const PArgs& a0, int n_cap, cudaStream_t stream, bool* bn_done) {
     PArgs a = a0;
     // Two CTAs per SM (half the shared memory each, 2 table buffers) when the ring still has VC_P_MIN_STAGES2 stages: two
     // independent pipelines per SM (each a serial chain of barrier wait -> MMA issue -> release per stage) and room for CTAs
@@ -637,6 +729,34 @@ int launch_persist(const PArgs& a0, int n_cap, cudaStream_t stream) {
     const int tiles = cdiv(n_cap, TCM);
     const int slots = ctas * num_sms();
     const int grid = tiles < slots ? (tiles < 1 ? 1 : tiles) : slots;
+    if (a.bn.bar != nullptr) {
+        // The grid-wide barrier needs every CTA resident at once: a cooperative launch, which starts only when ALL its CTAs fit.
+        // At two CTAs per SM that means waiting until the index stream's rulebook kernels have left the SMs (measured: 0.14 ms
+        // per step SLOWER than the separate apply kernel); at one CTA per SM the grid fits beside them and the step gets
+        // 0.15 ms faster (DESIGN.md section 8).  Same shared-memory plan, half the CTAs.
+        const int cgrid = grid < num_sms() ? grid : num_sms();
+        cudaLaunchConfig_t cfg{};
+        cfg.gridDim = dim3(cgrid);
+        cfg.blockDim = dim3(P_THREADS);
+        cfg.dynamicSmemBytes = p.smem;
+        cfg.stream = stream;
+        cudaLaunchAttribute at[2]{};
+        at[0].id = cudaLaunchAttributeCooperative;
+        at[0].val.cooperative = 1;
+        at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        at[1].val.programmaticStreamSerializationAllowed = 1;
+        cfg.attrs = at;
+        cfg.numAttrs = g_pdl ? 2 : 1;
+        if (cudaLaunchKernelEx(&cfg, kern, a) == cudaSuccess) {
+            count_launch();
+            *bn_done = true;
+            return VC_OK;
+        }
+        // (a device / driver configuration that refuses it: the conv alone, the caller applies BN, for good)
+        cudaGetLastError();
+        g_conv_bn_fused = 0;
+        a.bn = BnTail{};
+    }
     VC_LAUNCH_CHAIN(kern, dim3(grid), dim3(P_THREADS), p.smem, stream, a);
     return VC_OK;
 }
@@ -700,7 +820,8 @@ bool tc2_ch_ok(int c) { return c == 8 || c == 16 || c == 32 || c == 64; }
 // (layout 1).  n_dev (optional) overrides n_rows on the device; n_rows is then the capacity the grid is sized for.
 int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_t* nbr, long long pitch, float* out,
              int n_rows, const int* n_dev, int K, double* bn_sums, int* err, cudaStream_t stream, const float* addend,
-             int* tile_counter, int flags, int in_ld, double* bn_part) {
+             int* tile_counter, int flags, int in_ld, double* bn_part, const BnTail* bn, bool* bn_done) {
+    if (bn_done != nullptr) *bn_done = false;
     if (n_rows == 0) return VC_OK;
     if (!tc2_ch_ok(kc) || !tc2_ch_ok(nr) || K < 1 || K > MAXK_TC) {
         set_error("tensor-core conv: unsupported shape (%d -> %d channels, K=%d)", kc, nr, K);
@@ -716,9 +837,20 @@ int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_
     a.out = out; a.out_c = nr; a.addend = addend; a.bn_sums = bn_part ? nullptr : bn_sums; a.bn_part = bn_part; a.n_dev = n_dev; a.n_host = n_rows; a.tile_counter = tile_counter;
     a.K = K; a.S = 0; a.w_resident = 0; a.ntb_alloc = P_NTB; a.scan_k = flags & 1; a.early_tables = (flags >> 1) & 1;
     a.err = err;
+    a.bn = BnTail{};
+    bool done_dummy = false;
+    if (bn != nullptr && g_conv_bn_fused) {
+        if (!bn->bar || !bn->stats || !bn->gamma || !bn->beta || !bn->running_mean || !bn->running_var || (!bn->y && !bn->yb) ||
+            (bn->training && !bn->sums) || bn->y_ld % 4 || bn->yb_ld % 4 || bn->y_ld < nr || bn->yb_ld < nr || addend) {
+            set_error("tensor-core conv: bad fused BatchNorm arguments");
+            return VC_ERR_INVALID;
+        }
+        a.bn = *bn;
+    }
+    if (bn_done == nullptr) bn_done = &done_dummy;
     const int kcp = tc_pad16(kc), nrp = tc_pad16(nr);
 #define VC_P_CASE(A, B) \
-    if (kcp == A && nrp == B) return launch_persist<A, B>(a, n_rows, stream);
+    if (kcp == A && nrp == B) return launch_persist<A, B>(a, n_rows, stream, bn_done);
     VC_P_CASE(16, 16) VC_P_CASE(16, 32) VC_P_CASE(16, 64)
     VC_P_CASE(32, 16) VC_P_CASE(32, 32) VC_P_CASE(32, 64)
     VC_P_CASE(64, 16) VC_P_CASE(64, 32) VC_P_CASE(64, 64)
@@ -737,6 +869,11 @@ extern "C" int vc_debug_set_trace2(long long* buf) {
 extern "C" int vc_conv_tc2_config(int ctas_per_sm) {
     VC_CHECK_ARG(ctas_per_sm >= 0 && ctas_per_sm <= 2, "CTAs per SM must be 0 (automatic), 1 or 2");
     vc::g_p_ctas = ctas_per_sm;
+    return VC_OK;
+}
+
+extern "C" int vc_set_conv_bn_fused(int enable) {
+    vc::g_conv_bn_fused = enable ? 1 : 0;
     return VC_OK;
 }
 

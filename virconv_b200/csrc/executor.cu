@@ -57,7 +57,10 @@ struct RBk {
     int K, n_in, n_out, subm, unique, ev, prod;
     G2Prep g2;             // deterministic mode, many-to-one table: the gather-form dgrad's groups and table (gather2d.cu)
 };
-constexpr int CTR_PER_LAYER = 16;  // forward, dgrad, up to 14 wgrad passes (C_in = C_out = 64, K = 27: 14 groups, one per pass in wgrad_tc3)
+constexpr int CTR_PER_LAYER = 20;  // forward, dgrad, up to 14 wgrad passes (C_in = C_out = 64, K = 27: 14 groups, one per pass in wgrad_tc3),
+                                   // the forward's grid barrier (BN inside the conv); a multiple of 4: the wgrad accumulators
+                                   // that follow the counters are accessed as float4
+constexpr int CTR_BN_BAR = 16;
 
 // conv launches of a layer; the values are the timing records' kinds (vc_exec_timing_read, executor.KIND_NAMES)
 enum ConvKind : int { K_NONE = -1 /* no input gradient */, K_FWD_F32 = 0, K_FWD_TC = 1, K_DGRAD_F32 = 2, K_DGRAD_TC = 3,
@@ -625,6 +628,7 @@ int fwd_cbr(FwdCtx& C, int i, const int* o, int s) {
         part = p_;
         S->det_bytes += pb;
     }
+    bool bn_done = false;
     if (L.fwd == K_FWD_TC && R.n_out > 0) {
         if (!X.bf16) {   // no producer wrote a shadow (network input): cast once
             VC_CHECK_ARG(X.ld == X.c, "op %d: no bf16 copy of a strided input", i);
@@ -633,11 +637,15 @@ int fwd_cbr(FwdCtx& C, int i, const int* o, int s) {
             X.bf16 = xb;
         }
         Timed t(K_FWD_TC, li, st);
+        // BatchNorm + ReLU in the same launch (conv_tc2.cu): one kernel and one pass over x fewer per layer
+        const BnTail bt{C.P<const float>(li, P_GAMMA), C.P<const float>(li, P_BETA), C.P<float>(li, P_RM), C.P<float>(li, P_RV),
+                        C.P<long long>(li, P_NBT), C.lf[2 * li + 1], C.lf[2 * li], S->training, L.sums, y, y_ld, yb, y_ld, stats,
+                        C.S->is_static, L.tile_ctr + CTR_BN_BAR};
         // (flag bit 1: the rulebook was built on another stream and joined by an event, or by an earlier call, so the kernel
         //  may load its first table slices before its griddepcontrol.wait — conv_tc2.cu)
         if (C.do_feat)
             VC_TRY(tc2_conv(L.cin, L.cout, X.bf16, L.wimg_fwd, R.nbr, R.n_out, x, R.n_out, R.n_out_dev, R.K, sums, C.err, st, nullptr,
-                            L.tile_ctr, (!C.do_idx || C.st[R.prod] != C.st[s]) ? 2 : 0, X.ld, part));
+                            L.tile_ctr, (!C.do_idx || C.st[R.prod] != C.st[s]) ? 2 : 0, X.ld, part, &bt, &bn_done));
     } else {   // (also a tensor-core layer without output rows)
         const size_t wsb = vc_conv_ws_bytes(L.cin, L.cout, R.K);
         VC_ALLOC(ws, void*, wsb);
@@ -648,8 +656,9 @@ int fwd_cbr(FwdCtx& C, int i, const int* o, int s) {
         else if (C.do_feat)
             VC_TRY(vc_conv_fwd_f32(X.f32, C.P<const float>(li, P_W), R.nbr, x, R.n_out, L.cin, L.cout, R.K, sums, ws, wsb, st));
     }
-    if (C.do_feat && part && R.n_out > 0) VC_TRY(bn_sums_reduce_dev(part, R.n_out, R.n_out_dev, VC_TILE_ROWS, L.cout, L.sums, st));
-    if (C.do_feat)
+    if (C.do_feat && !bn_done && part && R.n_out > 0)
+        VC_TRY(bn_sums_reduce_dev(part, R.n_out, R.n_out_dev, VC_TILE_ROWS, L.cout, L.sums, st));
+    if (C.do_feat && !bn_done)
         VC_TRY(bn_apply_relu_dev(x, L.sums, R.n_out, R.n_out_dev, L.cout, C.P<const float>(li, P_GAMMA), C.P<const float>(li, P_BETA),
                                  C.P<float>(li, P_RM), C.P<float>(li, P_RV), C.P<long long>(li, P_NBT), C.lf[2 * li + 1], C.lf[2 * li],
                                  S->training, y, y_ld, yb, y_ld, stats, 1, C.S->is_static, st));
