@@ -317,6 +317,37 @@ int vc_dense_f32(const float* features, const int32_t* indices, int n, int c, in
 int vc_dense_bwd_f32(const float* dout, const int32_t* indices, int n, int c, int ndim, int batch_size,
                      const int32_t* spatial_shape, float* dfeatures, vc_stream_t stream);
 
+/* Row-counted forms of the three calls above for a static-mode (capacity-sized) tensor: `cap` rows of indices / features,
+ * n_dev (device int32[1]) the valid ones.  Rows at or past *n_dev are skipped (their -1 index tail is never used as an
+ * address); the dense() gradient of those rows is zero.  Otherwise the same results as vc_voxel2pinds / vc_dense_f32 /
+ * vc_dense_bwd_f32 on the valid rows. */
+int vc_voxel2pinds_rows(const int32_t* indices, int cap, const int32_t* n_dev, int ndim, int batch_size,
+                        const int32_t* spatial_shape, int32_t* out, vc_stream_t stream);
+int vc_dense_rows_f32(const float* features, const int32_t* indices, int cap, const int32_t* n_dev, int c, int ndim,
+                      int batch_size, const int32_t* spatial_shape, float* out, vc_stream_t stream);
+int vc_dense_rows_bwd_f32(const float* dout, const int32_t* indices, int cap, const int32_t* n_dev, int c, int ndim,
+                          int batch_size, const int32_t* spatial_shape, float* dfeatures, vc_stream_t stream);
+
+/* Test-time x-batching of the ROT_NUM transformed copies (spconv_backbone.py:339-471, csrc/xbatch.cu), no host read:
+ *   vc_xbatch_pack : R copies (host arrays of R device pointers: features [caps[i], c] fp32, coordinates [caps[i], 4] int32
+ *                    (b, z, y, x), row counts n_dev[i] int32[1]) -> out [cap_out >= sum(caps)]: the valid rows of copy 0,
+ *                    copy 1, ... in order (= torch.cat of the exact rows) with x += i * W; zero feature / -1 coordinate
+ *                    tail; *n_out_dev = the total.  One launch.
+ *   vc_xbatch_split: the device form of `decompose_tensor` (:314-337).  A published tensor (features [cap, c] fp32, c in
+ *                    {16, 32, 64} else VC_ERR_UNSUPPORTED; indices [cap, 4] int32; *n_dev valid rows) of a grid of x extent
+ *                    Wt -> R outputs of capacity cap (host arrays of R device pointers).  q = Wt / 4; output i = the rows
+ *                    with i*q < x < (i+1)*q (strict: the x == i*q column is in no copy, :325) in the parent's order, with
+ *                    x -= i*q; zero feature / -1 index tail; *n_out_dev[i] its rows.  ws >= vc_xbatch_split_ws_bytes(cap, R).
+ *                    Three launches (tile counts of every copy, one scan, ballot-ranked emit).
+ * R outside [1, 4] -> VC_ERR_INVALID (the reference's x-batching factor is 4, :360). */
+int vc_xbatch_pack(const float* const* features, const int32_t* const* coords, const int32_t* const* n_dev,
+                   const int32_t* caps /*host [R]*/, int R, int c, int W, int cap_out, float* out_features, int32_t* out_coords,
+                   int32_t* n_out_dev, vc_stream_t stream);
+size_t vc_xbatch_split_ws_bytes(int cap, int R);
+int vc_xbatch_split(const float* features, const int32_t* indices, int cap, const int32_t* n_dev, int c, int Wt, int R,
+                    float* const* out_features, int32_t* const* out_indices, int32_t* const* n_out_dev, void* ws, size_t ws_bytes,
+                    vc_stream_t stream);
+
 /* NRConv channel concat (spconv_backbone.py:227): out[:, :ca] = a, out[:, ca:] = b, plus an optional bf16 shadow. */
 int vc_cat2_f32(const float* a, const float* b, float* out, void* out_bf16 /*may be NULL*/, int n, int ca, int cb,
                 vc_stream_t stream);

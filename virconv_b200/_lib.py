@@ -19,6 +19,7 @@ _Z = c_size_t
 _HOST = ctypes.POINTER(c_int32)
 _HOSTF = ctypes.POINTER(c_float)
 _HOSTD = ctypes.POINTER(c_double)
+_HOSTP = ctypes.POINTER(c_void_p)        # host array of device pointers
 _D = c_double
 
 # name -> (restype, argtypes).  Every symbol include/virconv_b200.h declares.
@@ -73,6 +74,12 @@ SIGNATURES = {
     'vc_voxelize_ws_bytes': (_Z, [_I, _I, _I]),
     'vc_voxelize_mean': (_I, [_P, _I, _I, _I, _HOSTF, _HOSTF, _I, _I, _I, _P, _P, _P, _P, _P, _P, _Z, _P]),
     'vc_voxel2pinds': (_I, [_P, _I, _I, _I, _HOST, _P, _P]),
+    'vc_voxel2pinds_rows': (_I, [_P, _I, _P, _I, _I, _HOST, _P, _P]),
+    'vc_dense_rows_f32': (_I, [_P, _P, _I, _P, _I, _I, _I, _HOST, _P, _P]),
+    'vc_dense_rows_bwd_f32': (_I, [_P, _P, _I, _P, _I, _I, _I, _HOST, _P, _P]),
+    'vc_xbatch_pack': (_I, [_HOSTP, _HOSTP, _HOSTP, _HOST, _I, _I, _I, _I, _P, _P, _P, _P]),
+    'vc_xbatch_split_ws_bytes': (_Z, [_I, _I]),
+    'vc_xbatch_split': (_I, [_P, _P, _I, _P, _I, _I, _I, _HOSTP, _HOSTP, _HOSTP, _P, _Z, _P]),
     'vc_cat2_f32': (_I, [_P, _P, _P, _P, _I, _I, _I, _P]),
     'vc_masked_mean_ws_bytes': (_Z, []),
     'vc_masked_mean_f32': (_I, [_P, ctypes.c_longlong, _I, _P, _P, _P, _Z, _P]),
@@ -164,6 +171,10 @@ def host_i32(vals):
 
 def host_f32(vals):
     return (c_float * len(vals))(*[float(v) for v in vals])
+
+
+def host_ptrs(vals):
+    return (c_void_p * len(vals))(*[int(v) for v in vals])
 
 
 def host_f64(vals):

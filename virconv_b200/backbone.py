@@ -403,6 +403,25 @@ def decompose_tensor(t, i, batch_size):
     return spconv.SparseConvTensor(feats, sub, [t.spatial_shape[0], t.spatial_shape[1], q], batch_size)
 
 
+class EvalStaticSpec:
+    """Static (CUDA-graph capturable) test-time forward of VirConv8x over R = 1..4 transformed copies, given as
+    batch_dict['virconv_eval_static'] (graph.GraphedForward builds one per capture).  The copies' inputs are the capacity-sized
+    'voxel_features{i}' / 'voxel_coords{i}' (LiDAR, int32 coordinates) and 'voxel_features_mm{i}' / 'voxel_coords_mm{i}'
+    (virtual points), i = '', '1', '2', ... as the reference suffixes them.
+      lidar        executor.StaticSpec of the x-batched LiDAR plan over [D, H, 4W]; its n_dev receives the packed row count
+                   (ops.xbatch_pack writes it on the device);
+      lidar_counts R device int32[1]: the valid rows of each LiDAR copy;
+      mm           R executor.StaticSpecs, one per copy of the virtual-point stream (n_dev: that copy's valid rows);
+      proj         [R, B, 28] device projection blocks (ops.projection_params of each copy's transform)."""
+
+    def __init__(self, lidar, lidar_counts, mm=(), proj=None):
+        self.lidar, self.lidar_counts, self.mm, self.proj = lidar, list(lidar_counts), list(mm), proj
+
+    @property
+    def rot_num(self):
+        return len(self.lidar_counts)
+
+
 class VirConv8x(nn.Module):
     """VirConv-T / VirConv-S backbone (spconv_backbone.py:232-535): a LiDAR stream whose submanifold convs share one
     rulebook per stage (indice_keys 'subm1'..'subm4') plus, when `MM`, the virtual-point stream of NRConv blocks.
@@ -414,7 +433,9 @@ class VirConv8x(nn.Module):
     inputs are then capacity sized — and the MM stream reads the shared projection block batch_dict['virconv_proj'] ([B,28]
     on the device).  The nine published tensors follow VirConvL8x's static contract (capacity-sized features with a zero
     tail, indices with a -1 tail, device int32 `.num_rows`), as do the device-drawn StVD lists in 'stvd_kept_rows'.  The eval
-    forward has no static form and raises ValueError when given a StaticSpec."""
+    forward raises ValueError when given those training StaticSpecs; its static form (graph.GraphedForward) takes an
+    EvalStaticSpec in batch_dict['virconv_eval_static']: ops.xbatch_pack -> the LiDAR plan over [D, H, 4W] ->
+    ops.xbatch_split of x_conv3, x_conv4 and out, and one static run of the virtual-point plan per copy."""
 
     def __init__(self, model_cfg, input_channels, grid_size, discard_mode='spconv2_compat', precision='fp32',
                  discard_rng='numpy', **kwargs):
@@ -537,6 +558,74 @@ class VirConv8x(nn.Module):
                                  'host-drawn or caller-given kept rows have no static form')
         return True
 
+    def _check_eval_static(self, batch_dict, rot_num):
+        """-> the EvalStaticSpec of a static test-time forward, or None.  (Runs after _check_static: given the training specs
+        too, an eval forward raises their refusal first.)"""
+        spec = batch_dict.get('virconv_eval_static')
+        if spec is None:
+            return None
+        if self.training:
+            raise ValueError("VirConv8x: batch_dict['virconv_eval_static'] is the test-time forward (model.eval()); a static "
+                             "training forward takes virconv_static / virconv_static_mm (graph.GraphedStep)")
+        if not 1 <= rot_num <= ops.XBATCH_MAX:
+            raise ValueError('VirConv8x: the x-batched eval forward takes 1..%d transformed copies (the factor 4 of the [D, H, 4W] '
+                             'grid is fixed, spconv_backbone.py:360); transform_param has %d' % (ops.XBATCH_MAX, rot_num))
+        if spec.rot_num != rot_num or (self.mm and len(spec.mm) != rot_num):
+            raise ValueError('VirConv8x: the EvalStaticSpec describes %d LiDAR / %d virtual-point copies, transform_param %d'
+                             % (spec.rot_num, len(spec.mm), rot_num))
+        if spec.lidar is None or (self.mm and (spec.proj is None or tuple(spec.proj.shape[:2]) != (rot_num, batch_dict['batch_size']))):
+            raise ValueError('VirConv8x: the EvalStaticSpec needs the packed LiDAR StaticSpec and [R, B, 28] projection blocks')
+        sfx = [''] + [str(i) for i in range(1, rot_num)]
+        keys = [k + s for s in sfx for k in ('voxel_features', 'voxel_coords')]
+        if self.mm:
+            keys += [k + '_mm' + s for s in sfx for k in ('voxel_features', 'voxel_coords')]
+        missing = [k for k in keys if batch_dict.get(k) is None]
+        if missing:
+            raise ValueError('VirConv8x static eval forward: the batch has no %s' % ', '.join(missing))
+        return spec
+
+    def _eval_static_forward(self, batch_dict, spec, sfx, batch_size, strides):
+        """The eval forward below with every row count on the device (see EvalStaticSpec)."""
+        R = len(sfx)
+        feats = [batch_dict['voxel_features' + s] for s in sfx]
+        coords = [spconv._as_i32(batch_dict['voxel_coords' + s]) for s in sfx]
+        pf, pc, _ = ops.xbatch_pack(feats, coords, spec.lidar_counts, self.sparse_shape[2], spec.lidar.n_dev)
+        big = [self.sparse_shape[0], self.sparse_shape[1], self.sparse_shape[2] * 4]      # factor 4 is hard-coded (:360)
+        _, _, x3, x4, out = self._lidar_stream(pf, pc, big, batch_size, static=spec.lidar)
+
+        def split(t):
+            q = t.spatial_shape[2] // 4
+            parts = []
+            for f, idx, n in ops.xbatch_split(t.features, spconv._as_i32(t.indices), t.num_rows, t.spatial_shape[2], R):
+                p = spconv.SparseConvTensor(f, idx, [t.spatial_shape[0], t.spatial_shape[1], q], batch_size)
+                p.num_rows = n
+                parts.append(p)
+            return parts
+
+        x3s, x4s, outs = split(x3), split(x4), split(out)
+        for i, s in enumerate(sfx):
+            batch_dict.update({
+                'encoded_spconv_tensor' + s: outs[i], 'encoded_spconv_tensor_stride' + s: 8,
+                'multi_scale_3d_features' + s: {'x_conv1': None, 'x_conv2': None, 'x_conv3': x3s[i], 'x_conv4': x4s[i]},
+                'multi_scale_3d_strides' + s: dict(strides)})
+        if not self.mm:
+            return batch_dict
+        if not self._plan_mm(False).is_current():
+            self._plan_mm_cache = self._plan_mm_stvd_cache = None
+        plan = self._plan_mm(False)
+        for i, s in enumerate(sfx):
+            f, c = batch_dict['voxel_features_mm' + s], batch_dict['voxel_coords_mm' + s]
+            if not self._plan_usable(plan, f):
+                raise ValueError('VirConv8x static eval forward: the virtual-point stream cannot run through the plan executor (%s)'
+                                 % _module_path_reason(f, plan))
+            _, (x1, x2, x3, x4) = self._run(plan, f, c, self.sparse_shape, batch_size, spec.proj[i],
+                                            ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4'), None, spec.mm[i], '_mm' + s)
+            batch_dict.update({
+                'encoded_spconv_tensor_stride_mm' + s: 8,
+                'multi_scale_3d_features_mm' + s: {'x_conv1': x1, 'x_conv2': x2, 'x_conv3': x3, 'x_conv4': x4},
+                'multi_scale_3d_strides' + s: dict(strides)})
+        return batch_dict
+
     def _discarding(self):
         return self.training and self.discard_mode == 'paper' and self.layer_discard_rate != 0
 
@@ -580,7 +669,10 @@ class VirConv8x(nn.Module):
         sfx = [''] + [str(i) for i in range(1, rot_num)]
         strides = {'x_conv1': 1, 'x_conv2': 2, 'x_conv3': 4, 'x_conv4': 8}
         static = self._check_static(batch_dict, rot_num)
+        eval_static = self._check_eval_static(batch_dict, rot_num)
         ops.stats_arena(batch_dict['voxel_features'].device).reset()
+        if eval_static is not None:
+            return self._eval_static_forward(batch_dict, eval_static, sfx, batch_size, strides)
         if self.training:
             for s in sfx:
                 x1, x2, x3, x4, out = self._lidar_stream(batch_dict['voxel_features' + s], batch_dict['voxel_coords' + s],
@@ -627,7 +719,7 @@ class VirConv8x(nn.Module):
                     seed = stvd_seed(batch_dict, feats.device) if stvd else None
                     run, (x1, x2, x3, x4) = self._run(self._plan_mm(stvd), feats, coords, self.sparse_shape, batch_size, proj,
                                                       ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4'), seed,
-                                                      batch_dict.get('virconv_static_mm'), '_mm')
+                                                      batch_dict.get('virconv_static_mm'), '_mm' + s)
                     if stvd:
                         batch_dict['stvd_kept_rows' + s] = run.kept_rows()
                     batch_dict.update({

@@ -76,12 +76,18 @@ __global__ void __launch_bounds__(256) index2uv_kernel(const int4* __restrict__ 
     o[2] = vi;
 }
 
+// n_dev (may be NULL): device row count of a capacity-sized tensor (n = capacity); rows at or past it are not scattered, and
+// their gradient is zero
 __global__ void dense_kernel(const float* __restrict__ feat, const int32_t* __restrict__ idx, int n, int c, int ndim,
-                             long long spatial, const int* __restrict__ shape_dev_unused, int s0, int s1, int s2,
+                             long long spatial, const int* __restrict__ n_dev, int s0, int s1, int s2,
                              float* __restrict__ out, int backward, float* __restrict__ dfeat) {
     long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (long long)n * c) return;
     int row = (int)(t / c), ch = (int)(t % c);
+    if (n_dev != nullptr && row >= __ldg(n_dev)) {
+        if (backward) dfeat[t] = 0.f;
+        return;
+    }
     const int32_t* p = idx + (size_t)row * (1 + ndim);
     long long cell = p[1];
     if (ndim >= 2) cell = cell * s1 + p[2];
@@ -267,13 +273,14 @@ extern "C" int vc_index2uv(const int32_t* indices, int n, int batch_size, const 
 }
 
 static int dense_common(const float* features, const int32_t* indices, int n, int c, int ndim, int batch_size,
-                        const int32_t* shape, float* dense, float* dfeat, int backward, cudaStream_t stream) {
+                        const int32_t* shape, float* dense, float* dfeat, int backward, cudaStream_t stream,
+                        const int32_t* n_dev = nullptr) {
     VC_CHECK_ARG(n >= 0 && c > 0 && ndim >= 1 && ndim <= VC_MAX_NDIM && batch_size > 0 && shape, "bad dense arguments");
     if (n == 0) return VC_OK;
     long long spatial = 1;
     for (int d = 0; d < ndim; ++d) spatial *= shape[d];
     long long total = (long long)n * c;
-    dense_kernel<<<cdiv(total, 256), 256, 0, stream>>>(features, indices, n, c, ndim, spatial, nullptr, shape[0],
+    dense_kernel<<<cdiv(total, 256), 256, 0, stream>>>(features, indices, n, c, ndim, spatial, n_dev, shape[0],
                                                        ndim > 1 ? shape[1] : 1, ndim > 2 ? shape[2] : 1, dense, backward,
                                                        dfeat);
     VC_LAUNCH_CHECK();
@@ -289,6 +296,19 @@ extern "C" int vc_dense_bwd_f32(const float* dout, const int32_t* indices, int n
                                 const int32_t* spatial_shape, float* dfeatures, vc_stream_t stream_) {
     return dense_common(nullptr, indices, n, c, ndim, batch_size, spatial_shape, const_cast<float*>(dout), dfeatures, 1,
                         (cudaStream_t)stream_);
+}
+
+extern "C" int vc_dense_rows_f32(const float* features, const int32_t* indices, int cap, const int32_t* n_dev, int c, int ndim,
+                                 int batch_size, const int32_t* spatial_shape, float* out, vc_stream_t stream_) {
+    VC_CHECK_ARG(n_dev, "vc_dense_rows_f32: null row count");
+    return dense_common(features, indices, cap, c, ndim, batch_size, spatial_shape, out, nullptr, 0, (cudaStream_t)stream_, n_dev);
+}
+
+extern "C" int vc_dense_rows_bwd_f32(const float* dout, const int32_t* indices, int cap, const int32_t* n_dev, int c, int ndim,
+                                     int batch_size, const int32_t* spatial_shape, float* dfeatures, vc_stream_t stream_) {
+    VC_CHECK_ARG(n_dev, "vc_dense_rows_bwd_f32: null row count");
+    return dense_common(nullptr, indices, cap, c, ndim, batch_size, spatial_shape, const_cast<float*>(dout), dfeatures, 1,
+                        (cudaStream_t)stream_, n_dev);
 }
 
 extern "C" int vc_gather_rows(const void* in, const int32_t* rows, void* out, int n_rows, int row_bytes,

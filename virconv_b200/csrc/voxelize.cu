@@ -236,11 +236,13 @@ __global__ void __launch_bounds__(256) vox_emit_kernel(const float* __restrict__
     oc[0] = b; oc[1] = cc[2]; oc[2] = cc[1]; oc[3] = cc[0];
 }
 
-// dense voxel -> row map of `generate_voxel2pinds` (pcdet/utils/spconv_utils.py:13-21); out pre-filled with -1
-__global__ void voxel2pinds_kernel(const int32_t* __restrict__ idx, int n, int ndim, int s1, int s2, long long spatial,
-                                   int32_t* __restrict__ out) {
+// dense voxel -> row map of `generate_voxel2pinds` (pcdet/utils/spconv_utils.py:13-21); out pre-filled with -1.  n_dev (may
+// be NULL): device row count of a capacity-sized index tensor (n = capacity); rows at or past it are skipped
+__global__ void voxel2pinds_kernel(const int32_t* __restrict__ idx, int n, const int* __restrict__ n_dev, int ndim, int s1, int s2,
+                                   long long spatial, int32_t* __restrict__ out) {
     int row = blockIdx.x * blockDim.x + threadIdx.x;
     if (row >= n) return;
+    if (n_dev != nullptr && row >= __ldg(n_dev)) return;
     const int32_t* p = idx + (size_t)row * (1 + ndim);
     long long cell = p[1];
     if (ndim >= 2) cell = cell * s1 + p[2];
@@ -341,17 +343,27 @@ extern "C" int vc_voxelize_mean(const float* points, int n_points, int c, int ba
     return VC_OK;
 }
 
-extern "C" int vc_voxel2pinds(const int32_t* indices, int n, int ndim, int batch_size, const int32_t* spatial_shape,
-                              int32_t* out, vc_stream_t stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
+static int voxel2pinds_common(const int32_t* indices, int n, const int32_t* n_dev, int ndim, int batch_size,
+                              const int32_t* spatial_shape, int32_t* out, cudaStream_t stream) {
     VC_CHECK_ARG(n >= 0 && ndim >= 1 && ndim <= VC_MAX_NDIM && batch_size > 0 && spatial_shape && out, "bad arguments");
     long long spatial = 1;
     for (int d = 0; d < ndim; ++d) spatial *= spatial_shape[d];
     VC_CUDA(cudaMemsetAsync(out, 0xFF, (size_t)batch_size * spatial * 4, stream));
     if (n == 0) return VC_OK;
     VC_CHECK_ARG(indices, "null pointer");
-    voxel2pinds_kernel<<<cdiv(n, 256), 256, 0, stream>>>(indices, n, ndim, ndim > 1 ? spatial_shape[1] : 1,
+    voxel2pinds_kernel<<<cdiv(n, 256), 256, 0, stream>>>(indices, n, n_dev, ndim, ndim > 1 ? spatial_shape[1] : 1,
                                                          ndim > 2 ? spatial_shape[2] : 1, spatial, out);
     VC_LAUNCH_CHECK();
     return VC_OK;
+}
+
+extern "C" int vc_voxel2pinds(const int32_t* indices, int n, int ndim, int batch_size, const int32_t* spatial_shape,
+                              int32_t* out, vc_stream_t stream_) {
+    return voxel2pinds_common(indices, n, nullptr, ndim, batch_size, spatial_shape, out, (cudaStream_t)stream_);
+}
+
+extern "C" int vc_voxel2pinds_rows(const int32_t* indices, int cap, const int32_t* n_dev, int ndim, int batch_size,
+                                   const int32_t* spatial_shape, int32_t* out, vc_stream_t stream_) {
+    VC_CHECK_ARG(n_dev, "vc_voxel2pinds_rows: null row count");
+    return voxel2pinds_common(indices, cap, n_dev, ndim, batch_size, spatial_shape, out, (cudaStream_t)stream_);
 }

@@ -609,16 +609,25 @@ def index2uv(indices, batch_size, params, stride, pts_range=(0, -40, -3, 70.4, 4
 # dense / gather
 # ------------------------------------------------------------------------------------------------
 class DenseFn(torch.autograd.Function):
+    """`SparseConvTensor.dense()`.  num_rows (device int32[1], may be None): the valid rows of a static-mode tensor whose
+    features / indices are capacity sized (vc_dense_rows_f32: the -1 index tail is never scattered, its gradient is zero)."""
+
     @staticmethod
-    def forward(ctx, feats, indices, batch_size, spatial_shape):
-        _require_cuda(feats, indices)
+    def forward(ctx, feats, indices, batch_size, spatial_shape, num_rows=None):
+        _require_cuda(feats, indices, num_rows)
         lib = _lib.load()
         n, c = feats.shape
         nd = indices.shape[1] - 1
         out = torch.zeros((batch_size, c, *spatial_shape), dtype=torch.float32, device=feats.device)
-        check(lib.vc_dense_f32(_p(feats.contiguous()), _p(indices), n, c, nd, int(batch_size), host_i32(spatial_shape),
-                               _p(out), _stream()), 'vc_dense_f32')
+        if num_rows is None:
+            check(lib.vc_dense_f32(_p(feats.contiguous()), _p(indices), n, c, nd, int(batch_size), host_i32(spatial_shape),
+                                   _p(out), _stream()), 'vc_dense_f32')
+        else:
+            assert num_rows.dtype == torch.int32 and num_rows.numel() == 1 and indices.shape[0] == n
+            check(lib.vc_dense_rows_f32(_p(feats.contiguous()), _p(indices), n, _p(num_rows), c, nd, int(batch_size),
+                                        host_i32(spatial_shape), _p(out), _stream()), 'vc_dense_rows_f32')
         ctx.save_for_backward(indices)
+        ctx.num_rows = num_rows
         ctx.meta = (n, c, nd, int(batch_size), list(spatial_shape))
         return out
 
@@ -628,9 +637,13 @@ class DenseFn(torch.autograd.Function):
         (indices,) = ctx.saved_tensors
         n, c, nd, bs, shape = ctx.meta
         df = torch.empty((n, c), dtype=torch.float32, device=dout.device)
-        check(lib.vc_dense_bwd_f32(_p(dout.contiguous()), _p(indices), n, c, nd, bs, host_i32(shape), _p(df), _stream()),
-              'vc_dense_bwd_f32')
-        return df, None, None, None
+        if ctx.num_rows is None:
+            check(lib.vc_dense_bwd_f32(_p(dout.contiguous()), _p(indices), n, c, nd, bs, host_i32(shape), _p(df), _stream()),
+                  'vc_dense_bwd_f32')
+        else:
+            check(lib.vc_dense_rows_bwd_f32(_p(dout.contiguous()), _p(indices), n, _p(ctx.num_rows), c, nd, bs, host_i32(shape),
+                                            _p(df), _stream()), 'vc_dense_rows_bwd_f32')
+        return df, None, None, None, None
 
 
 def gather_rows(t, rows):
@@ -719,12 +732,74 @@ def voxelize_mean(points, batch_size, pc_range=(0, -40, -3, 70.4, 40, 1), voxel_
     return out + (voxels[:m],) if want_voxels else out
 
 
-def voxel2pinds(indices, batch_size, spatial_shape):
-    """Dense voxel -> row map (`generate_voxel2pinds`, pcdet/utils/spconv_utils.py:13-21)."""
-    _require_cuda(indices)
+def voxel2pinds(indices, batch_size, spatial_shape, num_rows=None):
+    """Dense voxel -> row map (`generate_voxel2pinds`, pcdet/utils/spconv_utils.py:13-21).  num_rows (device int32[1]): the
+    valid rows of a static-mode tensor's capacity-sized indices (`t.num_rows`); the -1 tail is skipped."""
+    _require_cuda(indices, num_rows)
     lib = _lib.load()
     indices = indices.to(torch.int32).contiguous()
     out = torch.empty((int(batch_size), *[int(s) for s in spatial_shape]), dtype=torch.int32, device=indices.device)
-    check(lib.vc_voxel2pinds(_p(indices), indices.shape[0], indices.shape[1] - 1, int(batch_size), host_i32(spatial_shape),
-                             _p(out), _stream()), 'vc_voxel2pinds')
+    if num_rows is None:
+        check(lib.vc_voxel2pinds(_p(indices), indices.shape[0], indices.shape[1] - 1, int(batch_size), host_i32(spatial_shape),
+                                 _p(out), _stream()), 'vc_voxel2pinds')
+        return out
+    assert num_rows.dtype == torch.int32 and num_rows.numel() == 1
+    check(lib.vc_voxel2pinds_rows(_p(indices), indices.shape[0], _p(num_rows), indices.shape[1] - 1, int(batch_size),
+                                  host_i32(spatial_shape), _p(out), _stream()), 'vc_voxel2pinds_rows')
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# test-time x-batching of the ROT_NUM transformed copies (csrc/xbatch.cu)
+# ------------------------------------------------------------------------------------------------
+XBATCH_MAX = 4          # the reference batches at most 4 copies along x (spconv_backbone.py:360)
+
+
+def xbatch_pack(feats, coords, counts, width, n_out=None):
+    """R <= 4 capacity-sized copies (features [cap_i, C] fp32, coordinates [cap_i, 4] int32, device int32[1] row counts) ->
+    (features [sum cap_i, C], coordinates [sum cap_i, 4], n_out): the valid rows of copy 0, copy 1, ... in order with
+    x += i * width (torch.cat of the exact rows), zero / -1 tail; n_out (given or fresh) receives the total row count."""
+    R = len(feats)
+    if not 1 <= R <= XBATCH_MAX or len(coords) != R or len(counts) != R:
+        raise ValueError('xbatch_pack: 1..%d copies, one coordinate tensor and count each (got %d, %d, %d)'
+                         % (XBATCH_MAX, R, len(coords), len(counts)))
+    _require_cuda(*feats, *coords, *counts)
+    lib = _lib.load()
+    feats = [f.contiguous() for f in feats]
+    for f, c, n in zip(feats, coords, counts):
+        assert f.dtype == torch.float32 and f.shape[1] == feats[0].shape[1], (f.dtype, f.shape)
+        assert c.dtype == torch.int32 and c.is_contiguous() and c.shape == (f.shape[0], 4), (c.dtype, c.shape)
+        assert n.dtype == torch.int32 and n.numel() == 1
+    dev, C = feats[0].device, feats[0].shape[1]
+    cap = sum(f.shape[0] for f in feats)
+    out_f = torch.empty((cap, C), dtype=torch.float32, device=dev)
+    out_c = torch.empty((cap, 4), dtype=torch.int32, device=dev)
+    if n_out is None:
+        n_out = torch.empty((1,), dtype=torch.int32, device=dev)
+    assert n_out.dtype == torch.int32 and n_out.numel() == 1 and n_out.device == dev
+    check(lib.vc_xbatch_pack(_lib.host_ptrs([f.data_ptr() for f in feats]), _lib.host_ptrs([c.data_ptr() for c in coords]),
+                             _lib.host_ptrs([n.data_ptr() for n in counts]), host_i32([f.shape[0] for f in feats]), R, C,
+                             int(width), cap, _p(out_f), _p(out_c), _p(n_out), _stream()), 'vc_xbatch_pack')
+    return out_f, out_c, n_out
+
+
+def xbatch_split(feats, indices, num_rows, width, R):
+    """The device form of backbone.decompose_tensor for all R copies at once: a capacity-sized tensor (features [cap, C] fp32,
+    indices [cap, 4] int32, device int32[1] row count) over a grid of x extent `width` -> R (features, indices, num_rows),
+    each of capacity cap: copy i holds the rows with i*q < x < (i+1)*q, q = width // 4, in order, x -= i*q; zero / -1 tail."""
+    if not 1 <= R <= XBATCH_MAX:
+        raise ValueError('xbatch_split: 1..%d copies, got %d' % (XBATCH_MAX, R))
+    _require_cuda(feats, indices, num_rows)
+    lib = _lib.load()
+    feats = feats.contiguous()
+    assert feats.dtype == torch.float32 and indices.dtype == torch.int32 and indices.is_contiguous()
+    assert indices.shape == (feats.shape[0], 4) and num_rows.dtype == torch.int32 and num_rows.numel() == 1
+    cap, C, dev = feats.shape[0], feats.shape[1], feats.device
+    outs = [(torch.empty((cap, C), dtype=torch.float32, device=dev), torch.empty((cap, 4), dtype=torch.int32, device=dev),
+             torch.empty((1,), dtype=torch.int32, device=dev)) for _ in range(R)]
+    ws = _ws(lib.vc_xbatch_split_ws_bytes(cap, R), dev)
+    check(lib.vc_xbatch_split(_p(feats), _p(indices), cap, _p(num_rows), C, int(width), R,
+                              _lib.host_ptrs([o[0].data_ptr() for o in outs]), _lib.host_ptrs([o[1].data_ptr() for o in outs]),
+                              _lib.host_ptrs([o[2].data_ptr() for o in outs]), _p(ws), ws.numel(), _stream()),
+          'vc_xbatch_split')
+    return outs

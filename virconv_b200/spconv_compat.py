@@ -73,7 +73,10 @@ class SparseConvTensor:
         return None if key is None else self.indice_dict.get(key)
 
     def dense(self, channels_first=True):
-        out = ops.DenseFn.apply(self._features, _as_i32(self.indices), self.batch_size, self.spatial_shape)
+        if self.num_rows is None:
+            out = ops.DenseFn.apply(self._features, _as_i32(self.indices), self.batch_size, self.spatial_shape)
+        else:           # static mode: only the valid rows are scattered (the index tail is -1)
+            out = ops.DenseFn.apply(self._features, _as_i32(self.indices), self.batch_size, self.spatial_shape, self.num_rows)
         if channels_first:
             return out
         nd = len(self.spatial_shape)
