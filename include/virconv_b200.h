@@ -664,11 +664,16 @@ int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_ops, const 
                      int n_layers, const int32_t* pub_slots, const uint64_t* ext_grads, int n_pub, void* arena,
                      size_t arena_bytes, int32_t* err_flag, void* state, vc_stream_t stream, vc_stream_t wgrad_stream);
 /* Read a state blob.  what 0: out[0] = arena bytes in use, out[1] = of them, the deterministic mode's partials, tables and
- * operands, out[2] = deterministic mode;  1 (feature slot id): f32 ptr, bf16 ptr, rows, c;
- * 2 (index set): idx ptr, n, ndim, shape[3];  3 (rulebook): nbr, nbr_bwd, pair_num ptrs, K, n_in, n_out, subm, unique;
- * 4 (layer): x ptr, y ptr, stats ptr, forward runs on the tensor cores, rulebook id, in slot, out slot;  5 (op index of a
- * DISCARD): keep ptr, kept rows (exact mode; static mode: the capacity), kept_dev ptr, n_in, site.  out: >= 8 int64
- * (host). */
+ * operands, out[2] = deterministic mode;  1 (feature slot id): f32 ptr, bf16 ptr, rows, c, row pitch of f32 / bf16,
+ * gradient ptr, row pitch of the gradient (after vc_exec_backward: the slot's final input gradient; a published slot no
+ * layer reads keeps the caller's ext_grads pointer);  2 (index set): idx ptr, n, ndim, shape[3];  3 (rulebook): nbr,
+ * nbr_bwd, pair_num ptrs, K, n_in, n_out, subm, unique;  4 (layer): x ptr, y ptr, stats ptr, forward runs on the tensor
+ * cores, rulebook id, in slot, out slot;  5 (op index of a DISCARD): keep ptr, kept rows (exact mode; static mode: the
+ * capacity), kept_dev ptr, n_in, site;  6 (layer, after vc_exec_backward): the upstream gradient ptr vc_exec_backward read
+ * and its row pitch, the BN backward's fp32 dx ptr (0 where no fp32 kernel reads it) and bf16 dx ptr (0 in fp32 mode),
+ * then the forward, weight-gradient and input-gradient kinds (vc_exec_timing_read's kinds, -1: no input gradient); all
+ * pointers 0 where nothing flowed back into the layer.  The arena is never reused inside a step, so every pointer stays
+ * valid until the arena is released.  out: >= 8 int64 (host). */
 int vc_exec_query(const void* state, int what, int id, long long* out);
 /* Optional per-launch timing of the conv kernels (bench.py's roofline pass): vc_exec_timing(1) clears and arms it,
  * vc_exec_timing_read synchronises and returns up to max_records (ms, [kind, layer]) records; kind 0 fwd f32, 1 fwd tc,

@@ -181,6 +181,7 @@ def test_executor_plan_layout_and_host_side_validation(lib_built):
     assert rc == -1 and b'unknown kind' in lib.vc_last_error()
     out = (ctypes.c_longlong * 8)()
     assert lib.vc_exec_query(state.ctypes.data, 0, 0, out) == -1        # not a valid state blob
+    assert lib.vc_exec_query(state.ctypes.data, 6, 0, out) == -1        # (the backward operands of a layer, too)
 
 
 def test_model_with_a_built_plan_can_be_copied_and_pickled():

@@ -75,6 +75,12 @@ struct Layer {
     void *wimg_fwd, *wimg_dgrad;
     int in_slot, out_slot, rb, cin, cout;
     ConvKind fwd, dgrad, wgrad;   // chosen by choose_kernels
+    // what vc_exec_backward used for this layer (vc_exec_query 6): the upstream gradient (row pitch dy_ld) and the BN
+    // backward's outputs, dx (NULL where no fp32 reader exists) and its bf16 shadow dxb (bf16 mode)
+    const float* dy;
+    float* dx;
+    void* dxb;
+    int dy_ld;
 };
 struct Disc {              // a DISCARD op (StVD layer discard): what its selection left behind
     int32_t *keep, *pos;   // keep [n_in]: kept rows ascending, tail -1; pos [n_in]: position in keep or -1
@@ -733,6 +739,7 @@ extern "C" int vc_exec_query(const void* state, int what, int id, long long* out
             VC_CHECK_ARG(id >= 0 && id < MAX_F, "slot id");
             const FSlot& f = S->f[id];
             out[0] = (long long)(uintptr_t)f.f32; out[1] = (long long)(uintptr_t)f.bf16; out[2] = f.rows; out[3] = f.c;
+            out[4] = f.ld; out[5] = (long long)(uintptr_t)f.grad; out[6] = f.gld;
             return VC_OK;
         }
         case 2: {
@@ -762,6 +769,13 @@ extern "C" int vc_exec_query(const void* state, int what, int id, long long* out
             const Disc& d = S->disc[id];
             out[0] = (long long)(uintptr_t)d.keep; out[1] = d.k; out[2] = (long long)(uintptr_t)d.kept_dev; out[3] = d.n_in;
             out[4] = d.site;
+            return VC_OK;
+        }
+        case 6: {
+            VC_CHECK_ARG(id >= 0 && id < MAX_L, "layer id");
+            const Layer& l = S->layer[id];
+            out[0] = (long long)(uintptr_t)l.dy; out[1] = l.dy_ld; out[2] = (long long)(uintptr_t)l.dx;
+            out[3] = (long long)(uintptr_t)l.dxb; out[4] = l.fwd; out[5] = l.wgrad; out[6] = l.dgrad;
             return VC_OK;
         }
     }
@@ -1057,6 +1071,7 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
         float* dgamma = C.P<float>(li, P_DGAMMA);
         float* dbeta = C.P<float>(li, P_DBETA);
         const size_t wn = (size_t)R.K * L.cin * L.cout;
+        L.dy = nullptr; L.dy_ld = 0; L.dx = nullptr; L.dxb = nullptr;
         if (Y.grad_state == G_EMPTY || R.n_out == 0) {   // nothing flowed back into this layer
             VC_CUDA(cudaMemsetAsync(dw, 0, wn * 4, st));
             VC_CUDA(cudaMemsetAsync(dgamma, 0, (size_t)L.cout * 4, st));
@@ -1077,6 +1092,7 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
             VC_ALLOC(t, void*, elems * 2 * (L.dgrad == K_DGRAD_GATHER2D_TC ? 2 : 1));
             dxb = t;
         }
+        L.dy = Y.grad; L.dy_ld = Y.gld; L.dx = dx; L.dxb = dxb;
         double* bpart = nullptr;   // deterministic mode: BN backward partials per BN_DET_ROWS chunk, added in chunk order
         if (S->deterministic) {
             const size_t pb = (size_t)cdiv(R.n_out, BN_DET_ROWS) * 2 * L.cout * 8;

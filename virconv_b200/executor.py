@@ -168,6 +168,18 @@ class Plan:
                 row[22] = 1
         self._final = None
 
+    def slot_isets(self):
+        """{feature slot: the index set whose rows it holds}"""
+        out = {0: 0}
+        for r in self.rows_i:
+            if r[0] == OP_CBR:
+                out[r[3]] = self.rb_keys[r[4]][3]
+            elif r[0] == OP_CAT:
+                out[r[4]] = out[r[2]]
+            elif r[0] == OP_DISCARD:
+                out[r[19]] = r[3]
+        return out
+
     def finalize(self):
         if self._final is None:
             oi = np.ascontiguousarray(np.array(self.rows_i, dtype=np.int32).reshape(-1, OPI))
@@ -319,23 +331,27 @@ def reserve_blocks(tag, nbytes, dev, stream=None, count=16):
     _POOLED[key] = nbytes
 
 
-def _view(arena, ptr, shape, dtype):
+def _view(arena, ptr, shape, dtype, ld=None):
     """A tensor over arena memory at device address `ptr` that is NOT an autograd view of the arena (Tensor.set_ on the
-    shared storage), so it can be returned from an autograd Function and outlive the arena tensor object."""
+    shared storage), so it can be returned from an autograd Function and outlive the arena tensor object.  ld: row pitch
+    of a 2-D [rows, c] view (> c: a column slice of a wider matrix)."""
     esz = torch.empty(0, dtype=dtype).element_size()
     off = ptr - arena.data_ptr()
     assert off >= 0 and off % esz == 0
-    n = 1
-    for s in shape:
-        n *= int(s)
+    shape = tuple(int(s) for s in shape)
+    if ld is None:
+        strides, acc = [], 1
+        for s in reversed(shape):
+            strides.append(acc)
+            acc *= s
+        strides = tuple(reversed(strides))
+    else:
+        assert len(shape) == 2 and ld >= shape[1]
+        strides = (int(ld), 1)
+    n = 1 + sum((s - 1) * st for s, st in zip(shape, strides)) if all(shape) else 0
     assert off + n * esz <= arena.numel()
     t = torch.empty(0, dtype=dtype, device=arena.device)
-    strides, acc = [], 1
-    for s in reversed(shape):
-        strides.append(acc)
-        acc *= int(s)
-    t.set_(arena.untyped_storage(), off // esz + arena.storage_offset() // esz, tuple(int(s) for s in shape),
-           tuple(reversed(strides)))
+    t.set_(arena.untyped_storage(), off // esz + arena.storage_offset() // esz, shape, strides)
     return t
 
 
@@ -368,8 +384,11 @@ class _Run:
         return bool(det), det_bytes
 
     def count(self, iset):
-        """Static mode: the device int32[1] row count of an index set (a view into the arena)."""
+        """Static mode: the device int32[1] row count of an index set (a view into the arena, or the StaticSpec's own n_dev
+        for the input's rows)."""
         p = self.query(2, iset)[6]
+        if p and self.static is not None and p == self.static.n_dev.data_ptr():
+            return self.static.n_dev
         return _view(self.arena, p, (1,), torch.int32) if p else None
 
     def kept_rows(self):
@@ -391,6 +410,61 @@ class _Run:
         nbw = _view(self.arena, pbw, (K, n_in), torch.int32) if pbw else None
         pn = _view(self.arena, ppn, (K,), torch.int32) if ppn else None
         return nbr, nbw, pn, dict(K=K, n_in=n_in, n_out=n_out, subm=bool(subm), unique=bool(unique))
+
+    def _rows_view(self, ptr, rows, c, ld, dtype, iset):
+        """[rows, c] view with row pitch ld, None for a null pointer or memory outside the arena; static mode: `rows` is the
+        capacity and the view carries the device row count of index set `iset` as `.num_rows`."""
+        if not ptr or not (self.arena.data_ptr() <= ptr < self.arena.data_ptr() + self.arena.numel()):
+            return None
+        t = _view(self.arena, ptr, (rows, c), dtype, ld)
+        if self.static is not None:
+            t.num_rows = self.static.n_dev if iset == 0 else self.count(iset)
+        return t
+
+    def slot(self, slot):
+        """Feature slot `slot` as {'f32', 'bf16', 'grad'}: [rows, c] views honouring each buffer's row pitch (a column slice of
+        an in-place concat, or of its gradient, has a pitch above c), None where the run keeps no such buffer.  After the
+        backward, 'grad' is the slot's final input gradient (None for a published slot no layer reads: its gradient is the
+        caller's own tensor).  Static mode: capacity rows, the device row count as `.num_rows`."""
+        f32, bf16, rows, c, ld, grad, gld = self.query(1, slot)[:7]
+        iset = self.plan.slot_isets()[slot]
+        if slot == 0:        # the caller's input features
+            x = self.feats
+            if self.static is not None:
+                x = x.view(x.shape)
+                x.num_rows = self.static.n_dev
+        return {'f32': x if slot == 0 else self._rows_view(f32, rows, c, ld, torch.float32, iset),
+                'bf16': self._rows_view(bf16, rows, c, ld, torch.bfloat16, iset),
+                'grad': self._rows_view(grad, rows, c, gld, torch.float32, iset)}
+
+    def layer_forward(self, layer):
+        """{'x': the conv's fp32 output [n_out, c_out], 'stats': [4, c_out] = BN scale, shift, mean, invstd, 'rb', 'in_slot',
+        'out_slot'} of `layer` (static mode: x with `.num_rows`); its input and output are slot(in_slot) / slot(out_slot)."""
+        x, _, stats, _, rb, in_slot, out_slot = self.query(4, layer)[:7]
+        n_out, cout = self.query(3, rb)[5], self.plan.layers[layer][0].out_channels
+        return {'x': self._rows_view(x, n_out, cout, cout, torch.float32, self.plan.slot_isets()[out_slot]),
+                'stats': _view(self.arena, stats, (4, cout), torch.float32), 'rb': rb, 'in_slot': in_slot, 'out_slot': out_slot}
+
+    def layer_backward(self, layer):
+        """What the backward used for `layer`: {'dy': upstream gradient (None where it is the caller's own gradient tensor of a
+        published slot), 'dx' / 'dxb': the BN backward's fp32 / bf16 output (each None where the run did not write it),
+        [n_out, c_out] views, static mode with `.num_rows`} and the kernel
+        names it ran ('fwd', 'wgrad', 'dgrad'; 'dgrad' None for a layer without an input gradient).  The gather-form dgrad
+        of a many-to-one table reads [dx; S] (fp32) or [dxb; S] (bf16), S the sums of dx over the rows of each pixel at
+        its lowest row: 'sums' is that S, else None."""
+        dy, dy_ld, dx, dxb, fwd, wgrad, dgrad = self.query(6, layer)[:7]
+        rb, out_slot = self.query(4, layer)[4], self.query(4, layer)[6]
+        n_out, cout = self.query(3, rb)[5], self.plan.layers[layer][0].out_channels
+        iset = self.plan.slot_isets()[out_slot]
+        out = {'dy': self._rows_view(dy, n_out, cout, dy_ld, torch.float32, iset),
+               'dx': self._rows_view(dx, n_out, cout, cout, torch.float32, iset),
+               'dxb': self._rows_view(dxb, n_out, cout, cout, torch.bfloat16, iset),
+               'fwd': KIND_NAMES[fwd], 'wgrad': KIND_NAMES[wgrad], 'dgrad': KIND_NAMES.get(dgrad), 'sums': None}
+        if out['dgrad'] in ('conv_dgrad_gather2d', 'conv_dgrad_gather2d_tc'):
+            tc = out['dgrad'] == 'conv_dgrad_gather2d_tc'
+            p, dt = (dxb, torch.bfloat16) if tc else (dx, torch.float32)
+            out['sums'] = self._rows_view(p + n_out * cout * (2 if tc else 4), n_out, cout, cout, dt, iset)
+        return out
 
 
 class LazyIndiceDict(dict):
@@ -576,7 +650,7 @@ class PlanFn(torch.autograd.Function):
             tail.record()
             inflight.append(tail)
         run = _Run(plan, arena, state, precision)
-        run.static, run.n0, run.training, run.with_bwd = static, n0, bool(training), bool(with_bwd)
+        run.static, run.n0, run.training, run.with_bwd, run.feats = static, n0, bool(training), bool(with_bwd), feats
         holder.append(run)
         if not with_bwd:
             _note_arena_use(plan, dev, False, run.query(0, 0)[0], n0)
