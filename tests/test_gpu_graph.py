@@ -179,6 +179,36 @@ def test_graph_recaptures_when_a_batch_does_not_fit(lib_built):
     assert abs(float(loss) - l_big) < 1e-5 * max(1.0, abs(l_big))
 
 
+def test_graph_resets_the_input_tail_of_a_shrinking_batch(lib_built):
+    """A larger batch, then a smaller one through the same captured step (voxelised batches): the published x_conv1, whose
+    indices are the graph's input coordinates, keeps its -1 tail past `num_rows` — no row of the larger batch is left
+    behind — and loss and gradients equal the exact step's."""
+    from virconv_b200.graph import GraphedStep
+    model = _model('bf16')
+    big = _batch([71, 72])
+    small = _batch([73, 74], n_lidar=2048, n_virtual=3000, max_voxels=2500)
+    l_s, g_s, _ = _exact(model, small)
+    held = {}
+
+    def loss_fn(out):
+        held['x_conv1'] = out['multi_scale_3d_features']['x_conv1']
+        return _loss(out)
+
+    step = GraphedStep(model, loss_fn, margin=1.35, grain=256)
+    step(big)
+    loss = step(small)
+    torch.cuda.synchronize()
+    assert _err_flag() == 0 and step.recaptures == 1
+    x1 = held['x_conv1']                                            # (the tensor of the capture: the replays rewrite it)
+    rows = int(x1.num_rows.item())
+    assert rows == small['voxel_features'].shape[0] < big['voxel_features'].shape[0]
+    assert torch.equal(x1.indices[:rows], small['voxel_coords'].int())
+    assert bool((x1.indices[rows:] == -1).all())
+    assert abs(float(loss) - l_s) < 1e-5 * max(1.0, abs(l_s))
+    for name, p in model.named_parameters():
+        assert _grad_close(p.grad, g_s[name]), name
+
+
 def test_graph_with_in_graph_voxeliser(lib_built):
     """bench.py's e2e path: raw collated points are the step's input, hash-grid voxelisation + MeanVFE run inside the
     captured graph (capacity-sized point buffer with an out-of-range tail, device voxel count); result against the exact

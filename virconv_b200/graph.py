@@ -20,11 +20,13 @@ A model with several input streams (`model.static_streams`: VirConv8x with MM ha
 stream '_mm') gets input buffers, an input capacity, a device row count and an overflow flag per stream; the batch keys of a
 stream carry its suffix ('voxel_features_mm', 'points_mm', 'virconv_static_mm').
 
-`GraphedForward` (end of the file) does the same for the test-time backbone forward, ROT_NUM transformed copies included.
+`PipelinedStep` runs the same step as two graphs over two buffer sets, and `GraphedForward` (end of the file) the test-time
+backbone forward, ROT_NUM transformed copies included.  All three share one core (`_Captured`): the input buffers and their
+loader (`_Inputs`), the capture sequence, and the read-back ring of the overflow and error flags (`_Flags`); each keeps its own
+static body and its own reaction to an overflow.
 """
 from __future__ import annotations
 
-import numpy as np
 import torch
 
 from . import _lib, executor, ops
@@ -64,19 +66,271 @@ def masked_mean(t):
     return _MaskedMean.apply(t.features, getattr(t, 'num_rows', None))
 
 
+def _round(n, margin, grain):
+    return (int(n * margin) + grain - 1) // grain * grain
+
+
 class _Stream:
-    """The graph's input side of one stream of the model (batch-key suffix `sfx`, position `i` in the step's device row-count
-    and overflow vectors): its capacity-sized input buffers and the StaticSpec capacities of its plan."""
+    """One input stream of a captured model (batch-key suffix `sfx`, position `i` in the device row-count vector) and its
+    capacity-sized input buffers: fp32 features `vf` [cap0, C] with a zero tail and int32 coordinates `vc` [cap0, 4] with a
+    -1 tail, or, with the in-graph voxeliser, the points `pts` [cap_pts, 1+C] with a `sentinel` tail."""
 
     def __init__(self, sfx, i):
         self.sfx, self.i = sfx, i
-        self.caps = {}
-        self.cap0 = 0             # input rows the buffers hold (voxels)
+        self.cap0 = 0             # input rows the plan sees (voxels)
         self.cap_pts = 0          # with the in-graph voxeliser: input points the point buffer holds
-        self.prev_n = 0
+        self.prev_n = 0           # input rows of the last batch loaded
 
 
-class GraphedStep:
+class _Inputs:
+    """The input side of a captured graph: the buffers of every stream, the device row counts `n_dev` (one per stream, then
+    `extra_counts` more that the graph itself writes), the device projection blocks `proj` [copies, B, 28], and the pinned
+    staging ring the small per-call host values go through.  vox: the voxeliser dict or None; vox_arg(stream, key): its
+    setting for one stream (_Captured._vox_arg)."""
+
+    SLOTS = 8
+
+    def __init__(self, sfxs, vox, vox_arg, copies=1, extra_counts=0):
+        self.streams = [_Stream(s, i) for i, s in enumerate(sfxs)]
+        self.vox, self.vox_arg, self.copies, self.extra_counts = vox, vox_arg, copies, extra_counts
+        self.B = None
+
+    def _voxelize(self, st, points, batch_size, static=False):
+        v = self.vox
+        return ops.voxelize_mean(points, batch_size, v['point_cloud_range'], v['voxel_size'], v['max_points_per_voxel'],
+                                 self.vox_arg(st, 'max_voxels'), self.vox_arg(st, 'vfe_model'), static=static)
+
+    def exact_batch(self, batch):
+        """`batch` as an exact (host-synchronised) run takes it: with the voxeliser, every stream's points voxelised."""
+        bd = dict(batch)
+        if self.vox is not None:
+            for st in self.streams:
+                f, c, _ = self._voxelize(st, batch['points' + st.sfx], int(batch['batch_size']))
+                bd.update({'voxel_features' + st.sfx: f, 'voxel_coords' + st.sfx: c})
+        return bd
+
+    def allocate(self, batch, dev, margin, grain):
+        """(Re)allocate every buffer for `batch`; the input capacities only grow."""
+        B = int(batch['batch_size'])
+        for st in self.streams:
+            if self.vox is not None:
+                pts = batch['points' + st.sfx]
+                st.cap_pts = max(st.cap_pts, _round(pts.shape[0], margin, grain))
+                row = torch.zeros(pts.shape[1], dtype=torch.float32)
+                row[0] = B - 1
+                row[1:4] = -1.0e6             # unused tail rows: last sample, out of range (the voxeliser drops them)
+                st.sentinel = row.to(dev)
+                st.pts = st.sentinel.repeat(st.cap_pts, 1).contiguous()
+                st.cap0 = B * int(self.vox_arg(st, 'max_voxels'))
+            else:
+                vf = batch['voxel_features' + st.sfx]
+                st.cap0 = max(st.cap0, _round(vf.shape[0], margin, grain))
+                st.vf = torch.zeros((st.cap0, vf.shape[1]), dtype=torch.float32, device=dev)
+                st.vc = torch.full((st.cap0, 4), -1, dtype=torch.int32, device=dev)
+            st.prev_n = 0
+        ns = len(self.streams) + self.extra_counts
+        self.B = B
+        self.n_dev = torch.zeros(ns, dtype=torch.int32, device=dev)
+        self.proj = torch.zeros((self.copies, B, 28), dtype=torch.float32, device=dev)
+        # pinned staging for the small per-call host values: a ring of slots, each guarded by an event recorded after its
+        # upload — the host runs several replays ahead of the GPU, and rewriting ONE pinned buffer before the previous
+        # call's asynchronous copy has executed would hand that call the next call's row counts / projection
+        self.proj_host = torch.zeros((self.SLOTS, self.copies, B, 28), dtype=torch.float32).pin_memory()
+        self.n_host = torch.zeros((self.SLOTS, ns), dtype=torch.int32).pin_memory()
+        self._stage_ev, self._stage = [None] * self.SLOTS, 0
+
+    def load(self, batch, transforms):
+        """Copy one batch into the buffers (asynchronous, current stream), with `transforms` (one per copy) for the projection
+        blocks; False (nothing copied) when a stream does not fit.  Rows a larger earlier batch left behind are reset to the
+        tail values, so that the voxeliser drops them and the published input index set (x_conv1's indices, which are the
+        coordinate buffer) keeps its -1 tail."""
+        key = 'points' if self.vox is not None else 'voxel_features'
+        ns = [batch[key + st.sfx].shape[0] for st in self.streams]
+        if any(n > (st.cap_pts if self.vox is not None else st.cap0) for st, n in zip(self.streams, ns)):
+            return False
+        slot = self._stage
+        self._stage = (slot + 1) % self.SLOTS
+        if self._stage_ev[slot] is not None:
+            self._stage_ev[slot].synchronize()         # (8 calls back: has long completed unless the GPU is far behind)
+        for st, n in zip(self.streams, ns):
+            if self.vox is not None:
+                st.pts[:n].copy_(batch['points' + st.sfx], non_blocking=True)
+                if st.prev_n > n:
+                    st.pts[n:st.prev_n] = st.sentinel
+            else:
+                st.vf[:n].copy_(batch['voxel_features' + st.sfx], non_blocking=True)
+                st.vc[:n].copy_(batch['voxel_coords' + st.sfx], non_blocking=True)     # (float32 coordinates -> int32)
+                if st.prev_n > n:
+                    st.vf[n:st.prev_n] = 0
+                    st.vc[n:st.prev_n] = -1
+                self.n_host[slot, st.i] = n
+            st.prev_n = n
+        if self.vox is None:
+            self.n_dev.copy_(self.n_host[slot], non_blocking=True)
+        for i, trans in enumerate(transforms):
+            self.proj_host[slot, i].copy_(torch.from_numpy(ops.projection_params_host(batch['calib'], trans, self.B)))
+        self.proj.copy_(self.proj_host[slot], non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record()
+        self._stage_ev[slot] = ev
+        return True
+
+    def static_batch(self, batch):
+        """-> (`batch` with every stream's inputs replaced by the capacity-sized ones, {stream suffix: device int32[1] row
+        count}); with the voxeliser, vc_voxelize_mean runs here (inside the graph) once per stream."""
+        drop = {k + st.sfx for st in self.streams for k in ('voxel_features', 'voxel_coords', 'points')}
+        bd = {k: v for k, v in batch.items() if k not in drop}
+        counts = {}
+        for st in self.streams:
+            if self.vox is not None:
+                f, c, bd['voxel_num_points' + st.sfx], counts[st.sfx] = self._voxelize(st, st.pts, self.B, static=True)
+            else:
+                f, c, counts[st.sfx] = st.vf, st.vc, self.n_dev[st.i:st.i + 1]
+            bd.update({'voxel_features' + st.sfx: f, 'voxel_coords' + st.sfx: c})
+        return bd, counts
+
+
+class _Flags:
+    """The overflow flags of a captured graph's StaticSpecs (`overflow`, one per plan key) and the library's error flag, read
+    back after every replay through a ring of pinned slots, each guarded by an event: the host looks at a replay's flags
+    once its event has fired, without waiting for the GPU.  Every replay that overflowed is appended to `events` as {plan
+    key: rows that did not fit}."""
+
+    SLOTS = 8
+
+    def __init__(self, keys, dev, events):
+        self.keys, self.dev, self.events = list(keys), dev, events
+        self.overflow = torch.zeros(len(self.keys), dtype=torch.int32, device=dev)
+        self.ovf_host = torch.zeros((self.SLOTS, len(self.keys)), dtype=torch.int32).pin_memory()
+        self.err_host = torch.zeros(self.SLOTS, dtype=torch.int32).pin_memory()
+        self.pending, self.slot = [], 0      # (event, slot) of the replays whose flags have not been looked at yet
+
+    def flag(self, key):
+        """The device int32[1] overflow flag of plan `key` (for its StaticSpec)."""
+        j = self.keys.index(key)
+        return self.overflow[j:j + 1]
+
+    def wait_if_full(self):
+        """With every slot in flight (the host far ahead of the GPU), wait for the oldest replay's flags -> whether it waited."""
+        if len(self.pending) < self.SLOTS:
+            return False
+        self.pending[0][0].synchronize()
+        return True
+
+    def push(self):
+        """After a replay (current stream): copy its flags into the next slot, zero `overflow`, record the slot's event
+        (waiting first when every slot is in flight) -> the event."""
+        self.wait_if_full()
+        slot = self.slot
+        self.slot = (slot + 1) % self.SLOTS
+        self.ovf_host[slot].copy_(self.overflow, non_blocking=True)
+        self.err_host[slot:slot + 1].copy_(ops.tc_error_flag(self.dev), non_blocking=True)
+        self.overflow.zero_()
+        ev = torch.cuda.Event()
+        ev.record()
+        self.pending.append((ev, slot))
+        return ev
+
+    def worst(self):
+        """The largest overflow, over every flag, of the replays whose flags have arrived (never blocks)."""
+        worst = 0
+        while self.pending and self.pending[0][0].query():
+            slot = self.pending.pop(0)[1]
+            if int(self.err_host[slot]) != 0:
+                raise _lib.VirConvLibraryError("a tensor-core kernel's pipeline wait timed out inside a replay (error flag "
+                                               "set): the results of that replay are invalid")
+            vals = [int(v) for v in self.ovf_host[slot]]
+            if max(vals):
+                self.events.append({k: v for k, v in zip(self.keys, vals) if v})
+            worst = max(worst, max(vals))
+        return worst
+
+
+class _Captured:
+    """What GraphedStep, PipelinedStep's buffer sets and GraphedForward share: the input side (`inputs`, an _Inputs), the
+    StaticSpec capacities of every plan (`caps`, {plan key: {index set: rows}}), the flag ring (`flags`) and the capture
+    sequence (_capture).  A subclass sets `inputs` and defines _recapture(batch) and _transforms(batch) (the projection
+    transform of each copy)."""
+
+    def __init__(self, dev, voxelizer, margin, grain, warmup):
+        self.dev = dev
+        self.vox = dict(voxelizer) if voxelizer is not None else None
+        self.margin, self.grain, self.warmup = margin, grain, warmup
+        self.caps = {}
+        self.graphs = []
+        self.flags = None
+        self.recaptures = 0
+        self.launches_per_replay = 0
+        self.overflow_events = []         # {plan key: rows that did not fit} of every replay that overflowed
+
+    @property
+    def streams(self):
+        return self.inputs.streams
+
+    @property
+    def ovf_host(self):
+        """[8, plan] pinned: the overflow flags of the last replays, one slot each."""
+        return self.flags.ovf_host
+
+    def _vox_arg(self, st, key):
+        """Voxeliser setting `key` for input stream `st`.  The virtual-point streams ('_mm', '_mm1', ...) read the '_mm' entry
+        where the dict has it, and their VFE defaults to the plain mean: the reference's MeanVFE applies its MODEL to the
+        LiDAR stream only (mean_vfe.py:51-58).  Every other stream reads the base entry."""
+        if st.sfx.startswith('_mm'):
+            if key + '_mm' in self.vox:
+                return self.vox[key + '_mm']
+            if key == 'vfe_model':
+                return None
+        return self.vox[key]
+
+    def _load(self, batch):
+        return self.inputs.load(batch, self._transforms(batch))
+
+    def _grow(self, batch):
+        self.margin *= 1.25
+        self._recapture(batch)
+
+    def _capture(self, batch, exact, warm, bodies, prepare=None):
+        """Capture `bodies` (callables of the batch) as one CUDA graph each, in order, for `batch` -> their results; the
+        graphs go to `graphs`.  exact(batch) runs the batch exactly and returns {plan key: its executor.last_run}, which
+        sizes the plans' capacities (they only grow) and the flag ring; the buffers are sized from the batch, which is
+        loaded; warm(batch) runs `warmup` times on a side stream (allocator pools, lazy kernel attributes, arena sizes), as
+        torch.cuda.graphs asks for; prepare() runs after it, outside any graph."""
+        torch.cuda.synchronize(self.dev)
+        self.graphs = []
+        runs = exact(batch)
+        for key, run in runs.items():
+            caps = self.caps.setdefault(key, {})
+            for k, v in executor.measured_caps(run, self.margin, self.grain).items():
+                caps[k] = max(caps.get(k, 0), v)
+        self.inputs.allocate(batch, self.dev, self.margin, self.grain)
+        self.flags = _Flags(runs, self.dev, self.overflow_events)
+        assert self._load(batch)
+        s = torch.cuda.Stream(device=self.dev)
+        s.wait_stream(torch.cuda.current_stream(self.dev))
+        with torch.cuda.stream(s):
+            for _ in range(max(self.warmup, 1)):
+                warm(batch)
+        torch.cuda.current_stream(self.dev).wait_stream(s)
+        torch.cuda.synchronize(self.dev)
+        if prepare is not None:
+            prepare()
+        self.flags.overflow.zero_()
+        lib = _lib.load()
+        l0 = lib.vc_launch_count()
+        graphs, outs = [], []
+        for body in bodies:
+            graphs.append(torch.cuda.CUDAGraph())
+            with torch.cuda.graph(graphs[-1]):
+                outs.append(body(batch))
+        self.launches_per_replay = int(lib.vc_launch_count() - l0)     # this library's kernels inside one replay
+        self.graphs = graphs
+        self.recaptures += 1
+        torch.cuda.synchronize(self.dev)
+        return outs
+
+
+class GraphedStep(_Captured):
     def __init__(self, model, loss_fn, params=None, margin=1.3, grain=1024, warmup=2, check_overflow=True, voxelizer=None):
         """voxelizer: None — batches carry `voxel_features` / `voxel_coords` (what the reference's dataloader + MeanVFE
         deliver); or a dict(point_cloud_range, voxel_size, max_points_per_voxel, max_voxels, vfe_model) — batches carry the
@@ -84,229 +338,77 @@ class GraphedStep:
         two-stream model the batch also carries `points_mm`, voxelised by a second call with the entries `max_voxels_mm`
         (default: `max_voxels`) and `vfe_model_mm` (default: None, the plain mean)."""
         self.model, self.loss_fn = model, loss_fn
-        self.vox = dict(voxelizer) if voxelizer is not None else None
         self.params = list(model.parameters()) if params is None else list(params)
-        self.dev = self.params[0].device
-        self.margin, self.grain, self.warmup = margin, grain, warmup
+        super().__init__(self.params[0].device, voxelizer, margin, grain, warmup)
         self.check_overflow = check_overflow
-        self.graph = None
-        self.streams = [_Stream(s, i) for i, s in enumerate(getattr(model, 'static_streams', ('',)))]
-        self.recaptures = 0
-        self.launches_per_replay = 0
-        self._pending = []        # (event, pinned slot) of the replays whose overflow flags have not been looked at yet
-        self._slot = 0
+        self.inputs = _Inputs(getattr(model, 'static_streams', ('',)), self.vox, self._vox_arg)
 
     @property
     def cap0(self):
         """Input row capacity of the first (for VirConvL8x: the only) stream."""
         return self.streams[0].cap0
 
-    # ------------------------------------------------------------------------------------------------
-    def _round(self, n):
-        return (int(n * self.margin) + self.grain - 1) // self.grain * self.grain
+    def _transforms(self, batch):
+        return [batch.get('aug_param')]
 
-    def _vox_arg(self, st, key):
-        """A voxeliser setting for stream `st`: `key + st.sfx` where the dict has it, else `key` — except the virtual-point
-        stream's VFE, which defaults to the plain mean: the reference's MeanVFE applies its MODEL to the LiDAR stream only
-        (mean_vfe.py:51-58)."""
-        if key + st.sfx in self.vox:
-            return self.vox[key + st.sfx]
-        if key == 'vfe_model' and st.sfx == '_mm':
-            return None
-        return self.vox[key]
-
-    def _voxelize(self, st, points, batch_size, static=False):
-        v = self.vox
-        return ops.voxelize_mean(points, batch_size, v['point_cloud_range'], v['voxel_size'], v['max_points_per_voxel'],
-                                 self._vox_arg(st, 'max_voxels'), self._vox_arg(st, 'vfe_model'), static=static)
-
-    def _exact_step(self, batch):
-        """One ordinary (exact-shape, host-synchronised) step; also measures the row counts of this batch, per stream."""
+    def _clear_grads(self):
         for p in self.params:
             p.grad = None
-        bd = dict(batch)
-        if self.vox is not None:
-            for st in self.streams:
-                f, c, _ = self._voxelize(st, batch['points' + st.sfx], int(batch['batch_size']))
-                bd.update({'voxel_features' + st.sfx: f, 'voxel_coords' + st.sfx: c})
-        out = self.model(bd)
-        loss = self.loss_fn(out)
-        loss.backward()
-        return loss.detach(), [executor.last_run(self.model, st.sfx) for st in self.streams]
 
-    def _make_buffers(self, batch, runs):
-        B = int(batch['batch_size'])
-        dev = self.params[0].device if self.vox is not None else batch['voxel_features'].device
-        for st, run in zip(self.streams, runs):
-            for k, v in executor.measured_caps(run, self.margin, self.grain).items():
-                st.caps[k] = max(st.caps.get(k, 0), v)
-            if self.vox is not None:
-                pts = batch['points' + st.sfx]
-                st.cap_pts = max(st.cap_pts, self._round(pts.shape[0]))
-                # unused tail rows: last sample's batch index, coordinates far outside the range (dropped by the voxeliser)
-                row = torch.zeros(pts.shape[1], dtype=torch.float32)
-                row[0] = B - 1
-                row[1:4] = -1.0e6
-                st.sentinel = row.to(dev)
-                st.pts = st.sentinel.repeat(st.cap_pts, 1).contiguous()
-                st.prev_n = 0
-                st.cap0 = B * int(self._vox_arg(st, 'max_voxels'))
-            else:
-                vf, vc = batch['voxel_features' + st.sfx], batch['voxel_coords' + st.sfx]
-                st.cap0 = max(st.cap0, self._round(vf.shape[0]))
-                st.vf = torch.zeros((st.cap0, vf.shape[1]), dtype=torch.float32, device=dev)
-                st.vc = torch.full((st.cap0, vc.shape[1]), -1, dtype=vc.dtype, device=dev)
-        ns = len(self.streams)
-        self.dev, self.B = dev, B
-        self.n_dev = torch.zeros(ns, dtype=torch.int32, device=dev)        # input rows of each stream
-        self.overflow = torch.zeros(ns, dtype=torch.int32, device=dev)     # each stream's StaticSpec overflow flag
-        self.proj = torch.zeros((B, 28), dtype=torch.float32, device=dev)
-        # pinned staging for the small per-step host values: a ring of slots, each guarded by an event recorded after its
-        # upload — the host runs several replays ahead of the GPU, and rewriting ONE pinned buffer before the previous
-        # step's asynchronous copy has executed would hand that step the next step's row counts / projection
-        self.STAGE_SLOTS = 8
-        self.proj_host = torch.zeros((self.STAGE_SLOTS, B, 28), dtype=torch.float32).pin_memory()
-        self.n_host = torch.zeros((self.STAGE_SLOTS, ns), dtype=torch.int32).pin_memory()
-        self._stage_ev = [None] * self.STAGE_SLOTS
-        self._stage = 0
-        self.ovf_host = torch.zeros((8, ns), dtype=torch.int32).pin_memory()
-        self.err_host = torch.zeros(8, dtype=torch.int32).pin_memory()
-        self._pending, self._slot = [], 0
-        for st in self.streams:
-            st.spec = executor.StaticSpec(self.n_dev[st.i:st.i + 1], st.caps, self.overflow[st.i:st.i + 1], alias_params=True)
-
-    def _load(self, batch):
-        """Copy one batch into the graph's input buffers (asynchronous, current stream).  False (nothing copied) when a
-        stream's input does not fit."""
-        key = 'points' if self.vox is not None else 'voxel_features'
-        ns = [batch[key + st.sfx].shape[0] for st in self.streams]
-        if any(n > (st.cap_pts if self.vox is not None else st.cap0) for st, n in zip(self.streams, ns)):
-            return False
-        if self.vox is not None:
-            for st, n in zip(self.streams, ns):
-                st.pts[:n].copy_(batch['points' + st.sfx], non_blocking=True)
-                if st.prev_n > n:                      # rows of the previous (larger) batch still sit behind this one
-                    st.pts[n:st.prev_n] = st.sentinel
-                st.prev_n = n
-        slot = self._stage
-        self._stage = (slot + 1) % self.STAGE_SLOTS
-        if self._stage_ev[slot] is not None:
-            self._stage_ev[slot].synchronize()         # (8 steps back: has long completed unless the GPU is far behind)
-        if self.vox is None:
-            for st, n in zip(self.streams, ns):
-                st.vf[:n].copy_(batch['voxel_features' + st.sfx], non_blocking=True)
-                st.vc[:n].copy_(batch['voxel_coords' + st.sfx], non_blocking=True)
-                self.n_host[slot, st.i] = n
-            self.n_dev.copy_(self.n_host[slot], non_blocking=True)
-        trans = batch.get('aug_param')
-        self.proj_host[slot].copy_(torch.from_numpy(ops.projection_params_host(batch['calib'], trans, self.B)))
-        self.proj.copy_(self.proj_host[slot], non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record()
-        self._stage_ev[slot] = ev
-        return True
+    def _exact(self, batch):
+        """One ordinary (exact-shape, host-synchronised) step -> the row counts of each stream's plan run."""
+        self._clear_grads()
+        self.loss_fn(self.model(self.inputs.exact_batch(batch))).backward()
+        runs = {st.sfx: executor.last_run(self.model, st.sfx) for st in self.streams}
+        assert all(r is not None for r in runs.values()), \
+            'a captured step needs a backbone running each stream through the plan executor'
+        return runs
 
     def _static_batch(self, batch):
-        drop = {k + st.sfx for st in self.streams for k in ('voxel_features', 'voxel_coords', 'points')}
-        bd = {k: v for k, v in batch.items() if k not in drop}
-        specs = []
+        bd, counts = self.inputs.static_batch(batch)
         for st in self.streams:
-            if self.vox is not None:
-                f, c, num, n_dev = self._voxelize(st, st.pts, self.B, static=True)
-                spec = executor.StaticSpec(n_dev, st.caps, self.overflow[st.i:st.i + 1], alias_params=True)
-                bd.update({'voxel_features' + st.sfx: f, 'voxel_coords' + st.sfx: c, 'voxel_num_points' + st.sfx: num})
-            else:
-                spec = st.spec
-                bd.update({'voxel_features' + st.sfx: st.vf, 'voxel_coords' + st.sfx: st.vc})
-            bd['virconv_static' + st.sfx] = spec
-            specs.append(spec)
-        bd['virconv_proj'] = self.proj
-        self._cur_specs = specs
+            bd['virconv_static' + st.sfx] = executor.StaticSpec(counts[st.sfx], self.caps[st.sfx], self.flags.flag(st.sfx),
+                                                                alias_params=True)
+        bd['virconv_proj'] = self.inputs.proj[0]
         return bd
 
     def _static_step(self, batch):
-        out = self.model(self._static_batch(batch))
-        loss = self.loss_fn(out)
+        bd = self._static_batch(batch)
+        loss = self.loss_fn(self.model(bd))
         # torch.autograd.grad w.r.t. the per-call leaf aliases the executor made of the parameters (executor.run_plan): no
         # long-lived AccumulateGrad node (which remembers the stream it was created on) takes part in a captured backward
         alias = {}
-        for spec in self._cur_specs:
-            alias.update(spec.param_aliases)
+        for st in self.streams:
+            alias.update(bd['virconv_static' + st.sfx].param_aliases)
         grads = torch.autograd.grad(loss, [alias.get(id(p), p) for p in self.params], allow_unused=True)
         for p, g in zip(self.params, grads):
             p.grad = g
         return loss.detach()
 
-    def _capture(self, batch):
-        torch.cuda.synchronize(self.dev)
-        loss_e, runs = self._exact_step(batch)
-        assert all(r is not None for r in runs), 'GraphedStep needs a backbone running each stream through the plan executor'
-        self._make_buffers(batch, runs)
-        assert self._load(batch)
-        # warm-up of the static path on a side stream (allocator pools, lazy kernel attributes), as torch.cuda.graphs asks for
-        s = torch.cuda.Stream(device=self.dev)
-        s.wait_stream(torch.cuda.current_stream(self.dev))
-        with torch.cuda.stream(s):
-            for _ in range(max(self.warmup, 1)):
-                for p in self.params:
-                    p.grad = None
-                self._static_step(batch)
-        torch.cuda.current_stream(self.dev).wait_stream(s)
-        torch.cuda.synchronize(self.dev)
-        for p in self.params:
-            p.grad = None
-        self.overflow.zero_()
-        self.graph = torch.cuda.CUDAGraph()
-        lib = _lib.load()
-        l0 = lib.vc_launch_count()
-        with torch.cuda.graph(self.graph):
-            self.loss = self._static_step(batch)
-        self.launches_per_replay = int(lib.vc_launch_count() - l0)     # this library's kernels inside one replay
-        self.recaptures += 1
-        torch.cuda.synchronize(self.dev)
+    def _warm(self, batch):
+        self._clear_grads()
+        self._static_step(batch)
 
-    # ------------------------------------------------------------------------------------------------
-    def _overflowed(self):
-        """Largest overflow reported by the replays that have COMPLETED so far, over all streams (never blocks: the flags of
-        a step are read back asynchronously and looked at when its event has fired, typically one or two calls later)."""
-        worst = 0
-        while self._pending and self._pending[0][0].query():
-            ev, slot = self._pending.pop(0)
-            worst = max(worst, int(self.ovf_host[slot].max()))
-            if int(self.err_host[slot]) != 0:
-                raise _lib.VirConvLibraryError('a tensor-core kernel\'s pipeline wait timed out inside a replayed step '
-                                               '(error flag set): the results of that step are invalid')
-        return worst
+    def _recapture(self, batch):
+        self.loss, = self._capture(batch, self._exact, self._warm, [self._static_step], self._clear_grads)
 
     def __call__(self, batch):
         """-> the step's loss (a device tensor owned by the graph: read or copy it before the next call)."""
-        if self.graph is None:
-            self._capture(batch)
-        if self.check_overflow and self._overflowed():
+        if not self.graphs:
+            self._recapture(batch)
+        if self.check_overflow and self.flags.worst():
             # an EARLIER batch did not fit: its gradients were computed on clamped row sets.  Grow and re-capture; the
             # caller sees the event through `recaptures` (a training loop may want to discard those optimizer steps).
-            self.margin *= 1.25
-            self._capture(batch)
+            self._grow(batch)
         if not self._load(batch):
-            self.margin *= 1.25
-            self._capture(batch)            # more input rows than the input buffers hold
+            self._grow(batch)               # more input rows than the input buffers hold
             assert self._load(batch)
-        self.graph.replay()
+        self.graphs[0].replay()
         if self.check_overflow:
-            if len(self._pending) >= self.ovf_host.shape[0]:    # (host far ahead of the GPU: wait for the oldest read-back)
-                self._pending[0][0].synchronize()
-                if self._overflowed():
-                    self.margin *= 1.25
-                    self._capture(batch)
-                    return self(batch)
-            slot = self._slot
-            self._slot = (slot + 1) % self.ovf_host.shape[0]
-            self.ovf_host[slot].copy_(self.overflow, non_blocking=True)
-            self.err_host[slot:slot + 1].copy_(ops.tc_error_flag(self.dev), non_blocking=True)
-            self.overflow.zero_()
-            ev = torch.cuda.Event()
-            ev.record()
-            self._pending.append((ev, slot))
+            if self.flags.wait_if_full() and self.flags.worst():
+                self._grow(batch)
+                return self(batch)
+            self.flags.push()
         return self.loss
 
 
@@ -317,65 +419,34 @@ class _PipeInstance(GraphedStep):
 
     def __init__(self, *args, **kwargs):
         super().__init__(*args, **kwargs)
-        self.g_idx = self.g_feat = None
         self.feat_done = None
         self.grads = None
-
-    def _static_batch(self, batch):
-        bd = super()._static_batch(batch)
-        spec = bd['virconv_static']
-        spec.phase, spec.arena = 0, None            # (the spec object is shared between calls when there is no voxeliser)
-        return bd
 
     def _index_part(self, batch):
         bd = self._static_batch(batch)              # (in-graph voxeliser, if any)
         spec = bd['virconv_static']
         spec.phase, spec.arena = 1, self.arena
         self.model.index_phase(bd)
-        return bd
+        self._bd = bd                               # (the feature graph continues from it)
 
-    def _feature_part(self, bd):
-        spec = bd['virconv_static']
+    def _feature_part(self, batch):
+        spec = self._bd['virconv_static']
         spec.phase = 2
-        out = self.model(bd)
-        loss = self.loss_fn(out)
+        loss = self.loss_fn(self.model(self._bd))
         alias = spec.param_aliases
         grads = torch.autograd.grad(loss, [alias.get(id(p), p) for p in self.params], allow_unused=True)
         self.grads = list(grads)
         return loss.detach()
 
-    def _capture(self, batch):
-        torch.cuda.synchronize(self.dev)
-        loss_e, runs = self._exact_step(batch)
-        assert all(r is not None for r in runs), 'PipelinedStep needs a backbone running through the plan executor'
-        self._make_buffers(batch, runs)
-        assert self._load(batch)
-        s = torch.cuda.Stream(device=self.dev)
-        s.wait_stream(torch.cuda.current_stream(self.dev))
-        with torch.cuda.stream(s):
-            for _ in range(max(self.warmup, 1)):        # unphased static steps: allocator pools, kernel attributes, arena size
-                for p in self.params:
-                    p.grad = None
-                self._static_step(batch)
-        torch.cuda.current_stream(self.dev).wait_stream(s)
-        torch.cuda.synchronize(self.dev)
+    def _prepare(self):
+        # the arena both graphs share, sized from what the (unphased) warm-up steps used
         plan = self.model._plan()
         self.arena = executor.empty_scratch(executor._arena_bytes(plan, self.cap0, self.dev, True), torch.uint8, self.dev)
-        for p in self.params:
-            p.grad = None
-        self.overflow.zero_()
-        lib = _lib.load()
-        l0 = lib.vc_launch_count()
-        self.g_idx = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.g_idx):
-            self._bd = self._index_part(batch)
-        self.g_feat = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.g_feat):
-            self.loss = self._feature_part(self._bd)
-        self.launches_per_replay = int(lib.vc_launch_count() - l0)
-        self.recaptures += 1
+        self._clear_grads()
+
+    def _recapture(self, batch):
+        _, self.loss = self._capture(batch, self._exact, self._warm, [self._index_part, self._feature_part], self._prepare)
         self.feat_done = None
-        torch.cuda.synchronize(self.dev)
 
 
 class PipelinedStep:
@@ -412,11 +483,10 @@ class PipelinedStep:
         inst = self.inst[self.t & 1]
         self.t += 1
         main = torch.cuda.current_stream(self.dev)
-        if inst.g_feat is None:
-            inst._capture(batch)
-        if inst.check_overflow and inst._overflowed():
-            inst.margin *= 1.25
-            inst._capture(batch)
+        if not inst.graphs:
+            inst._recapture(batch)
+        if inst.check_overflow and inst.flags.worst():
+            inst._grow(batch)
         with torch.cuda.stream(self.s_idx):
             if inst.feat_done is not None:
                 self.s_idx.wait_event(inst.feat_done)          # the buffer set's previous step (two steps back) is through
@@ -424,35 +494,25 @@ class PipelinedStep:
                 self.s_idx.wait_stream(main)
             ok = inst._load(batch)
             if ok:
-                inst.g_idx.replay()
+                inst.graphs[0].replay()
                 ev = torch.cuda.Event()
                 ev.record(self.s_idx)
         if not ok:                                             # more input rows than the buffers hold: grow, re-capture, run again
-            inst.margin *= 1.25
-            inst._capture(batch)
+            inst._grow(batch)
             self.t -= 1
             return self(batch)
         main.wait_event(ev)
-        inst.g_feat.replay()
+        inst.graphs[1].replay()
         for p, g in zip(self.params, inst.grads):
             p.grad = g
         if inst.check_overflow:
-            if len(inst._pending) >= inst.ovf_host.shape[0]:
-                inst._pending[0][0].synchronize()
-            slot = inst._slot
-            inst._slot = (slot + 1) % inst.ovf_host.shape[0]
-            inst.ovf_host[slot].copy_(inst.overflow, non_blocking=True)
-            inst.err_host[slot:slot + 1].copy_(ops.tc_error_flag(self.dev), non_blocking=True)
-            inst.overflow.zero_()
-            e2 = torch.cuda.Event()
-            e2.record()
-            inst._pending.append((e2, slot))
+            inst.flags.push()
         inst.feat_done = torch.cuda.Event()
         inst.feat_done.record(main)
         return inst.loss
 
 
-class GraphedForward:
+class GraphedForward(_Captured):
     """The test-time backbone forward as ONE CUDA graph: VirConvL8x (one copy) or VirConv8x over R = 1..4 transformed copies
     (X_TRANS, ROT_NUM; the batch keys carry the reference's suffixes '', '1', '2', ...), with the model in eval mode.
 
@@ -472,16 +532,15 @@ class GraphedForward:
     'spatial_features_stride{i}' per copy.
 
     Capacities: every plan of every copy gets its own StaticSpec, sized from one exact eval forward of the first batch (times
-    `margin`), and its own overflow flag.  check_overflow='sync' (default): each call reads this replay's overflow and error
-    flags before returning; a batch that did not fit is re-run after a re-capture with larger capacities, so a returned
-    result never comes from clamped row sets.  'async': the flags are read one call late, as GraphedStep does (the result of
-    an overflowing batch is then returned, and `recaptures` grows on the next call).
+    `margin`; a re-capture with the same number of copies only grows them), and its own overflow flag.
+    check_overflow='sync' (default): each call reads this replay's overflow and error flags before returning; a batch that
+    did not fit is re-run after a re-capture with larger capacities, so a returned result never comes from clamped row sets.
+    'async': the flags are read one call late, as GraphedStep does (the result of an overflowing batch is then returned, and
+    `recaptures` grows on the next call).
 
     voxelizer: as GraphedStep's — the batch then carries 'points{i}' (and 'points_mm{i}' for VirConv8x with MM) instead of the
     voxel keys, and vc_voxelize_mean runs inside the graph once per stream and copy; the virtual-point stream's settings are
     the '_mm' entries ('max_voxels_mm', 'vfe_model_mm', default the plain mean)."""
-
-    STAGE_SLOTS = 8
 
     def __init__(self, model, margin=1.3, voxelizer=None, bev=False, check_overflow='sync', grain=1024, warmup=2):
         from .backbone import VirConv8x, VirConvL8x
@@ -492,17 +551,13 @@ class GraphedForward:
                              'is graph.GraphedStep)')
         if check_overflow not in ('sync', 'async'):
             raise ValueError("check_overflow: 'sync' or 'async', got %r" % (check_overflow,))
+        super().__init__(next(model.parameters()).device, voxelizer, margin, grain, warmup)
         self.model = model
         self.x_batched = isinstance(model, VirConv8x)
         self.mm = self.x_batched and model.mm
-        self.vox = dict(voxelizer) if voxelizer is not None else None
-        self.margin, self.grain, self.warmup, self.bev, self.check_overflow = margin, grain, warmup, bool(bev), check_overflow
-        self.dev = next(model.parameters()).device
-        self.graph, self.R = None, None
-        self.recaptures = 0
-        self.launches_per_replay = 0
-        self.overflow_events = []         # {plan key: rows that did not fit} of every replay that overflowed
-        self._pending, self._slot = [], 0
+        self.bev, self.check_overflow = bool(bev), check_overflow
+        self.R = None
+        self.inputs = None
 
     # -- the copies of a batch and their streams ------------------------------------------------------------------
     @staticmethod
@@ -535,23 +590,9 @@ class GraphedForward:
             raise ValueError('GraphedForward: the batch has no %s' % ', '.join(missing))
         return R
 
-    def _vox_arg(self, st, key):
-        """A voxeliser setting for input stream `st` ('_mm...' streams: the '_mm' entry where given; their VFE defaults to the
-        plain mean, as GraphedStep's)."""
-        if st.sfx.startswith('_mm'):
-            if key + '_mm' in self.vox:
-                return self.vox[key + '_mm']
-            if key == 'vfe_model':
-                return None
-        return self.vox[key]
-
-    def _voxelize(self, st, points, batch_size, static=False):
-        v = self.vox
-        return ops.voxelize_mean(points, batch_size, v['point_cloud_range'], v['voxel_size'], v['max_points_per_voxel'],
-                                 self._vox_arg(st, 'max_voxels'), self._vox_arg(st, 'vfe_model'), static=static)
-
-    def _round(self, n):
-        return (int(n * self.margin) + self.grain - 1) // self.grain * self.grain
+    def _transforms(self, batch):
+        tp = batch.get('transform_param')
+        return [tp[:, i, :] if tp is not None else batch.get('aug_param') for i in range(self.R)]
 
     def _bev(self, out):
         """HeightCompression (height_compression.py:15-36) of every copy."""
@@ -565,117 +606,31 @@ class GraphedForward:
 
     # -- capture ---------------------------------------------------------------------------------------------------
     def _exact(self, batch):
-        """One exact eager eval forward (host-synchronised): measures every plan's row counts."""
+        """One exact eager eval forward (host-synchronised) -> the row counts of every plan run."""
         executor._LAST_RUNS.pop(self.model, None)
-        bd = dict(batch)
-        B = int(batch['batch_size'])
+        bd = self.inputs.exact_batch(batch)
         with torch.no_grad():
-            if self.vox is not None:
-                for st in self.streams:
-                    f, c, _ = self._voxelize(st, batch['points' + st.sfx], B)
-                    bd.update({'voxel_features' + st.sfx: f, 'voxel_coords' + st.sfx: c})
             self.model(bd)
-        runs = [executor.last_run(self.model, k) for k in self.plan_keys]
-        if any(r is None for r in runs):
+        runs = {k: executor.last_run(self.model, k) for k in self.plan_streams(self.R)}
+        if any(r is None for r in runs.values()):
             from .backbone import _module_path_reason
-            st = self.streams[0]
             raise ValueError('GraphedForward: the eval forward does not run through the plan executor (%s)'
-                             % _module_path_reason(bd['voxel_features' + st.sfx]))
+                             % _module_path_reason(bd['voxel_features' + self.streams[0].sfx]))
         return runs
 
-    def _make_buffers(self, batch, runs):
-        B = int(batch['batch_size'])
-        self.B = B
-        self.caps = {}
-        for k, run in zip(self.plan_keys, runs):
-            self.caps[k] = executor.measured_caps(run, self.margin, self.grain)
-        for st in self.streams:
-            if self.vox is not None:
-                pts = batch['points' + st.sfx]
-                st.cap_pts = self._round(pts.shape[0])
-                row = torch.zeros(pts.shape[1], dtype=torch.float32)
-                row[0] = B - 1
-                row[1:4] = -1.0e6             # out of range: the voxeliser drops the unused tail rows
-                st.sentinel = row.to(self.dev)
-                st.pts = st.sentinel.repeat(st.cap_pts, 1).contiguous()
-                st.cap0 = B * int(self._vox_arg(st, 'max_voxels'))
-            else:
-                vf = batch['voxel_features' + st.sfx]
-                st.cap0 = self._round(vf.shape[0])
-                st.vf = torch.zeros((st.cap0, vf.shape[1]), dtype=torch.float32, device=self.dev)
-                st.vc = torch.full((st.cap0, 4), -1, dtype=torch.int32, device=self.dev)
-            st.prev_n = 0
-        ns = len(self.streams)
-        self.n_dev = torch.zeros(ns + 1, dtype=torch.int32, device=self.dev)       # input rows per stream; [-1]: packed LiDAR rows
-        self.overflow = torch.zeros(len(self.plan_keys), dtype=torch.int32, device=self.dev)
-        self.proj = torch.zeros((self.R, B, 28), dtype=torch.float32, device=self.dev)
-        S = self.STAGE_SLOTS
-        self.proj_host = torch.zeros((S, self.R, B, 28), dtype=torch.float32).pin_memory()
-        self.n_host = torch.zeros((S, ns + 1), dtype=torch.int32).pin_memory()
-        self._stage_ev, self._stage = [None] * S, 0
-        self.ovf_host = torch.zeros((8, len(self.plan_keys)), dtype=torch.int32).pin_memory()
-        self.err_host = torch.zeros(8, dtype=torch.int32).pin_memory()
-        self._pending, self._slot = [], 0
-
-    def _load(self, batch):
-        """Copy one batch into the input buffers (asynchronous, current stream); False (nothing copied) when a stream does not
-        fit.  Rows a larger earlier batch left behind are reset to the tail values, so published input-set tensors keep
-        their zero / -1 tails."""
-        key = 'points' if self.vox is not None else 'voxel_features'
-        ns = [batch[key + st.sfx].shape[0] for st in self.streams]
-        if any(n > (st.cap_pts if self.vox is not None else st.cap0) for st, n in zip(self.streams, ns)):
-            return False
-        slot = self._stage
-        self._stage = (slot + 1) % self.STAGE_SLOTS
-        if self._stage_ev[slot] is not None:
-            self._stage_ev[slot].synchronize()
-        for st, n in zip(self.streams, ns):
-            if self.vox is not None:
-                st.pts[:n].copy_(batch['points' + st.sfx], non_blocking=True)
-                if st.prev_n > n:
-                    st.pts[n:st.prev_n] = st.sentinel
-            else:
-                st.vf[:n].copy_(batch['voxel_features' + st.sfx], non_blocking=True)
-                st.vc[:n].copy_(batch['voxel_coords' + st.sfx], non_blocking=True)
-                if st.prev_n > n:
-                    st.vf[n:st.prev_n] = 0
-                    st.vc[n:st.prev_n] = -1
-                self.n_host[slot, st.i] = n
-            st.prev_n = n
-        if self.vox is None:
-            self.n_dev.copy_(self.n_host[slot], non_blocking=True)
-        tp = batch.get('transform_param')
-        for i in range(self.R):
-            trans = tp[:, i, :] if tp is not None else batch.get('aug_param')
-            self.proj_host[slot, i].copy_(torch.from_numpy(ops.projection_params_host(batch['calib'], trans, self.B)))
-        self.proj.copy_(self.proj_host[slot], non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record()
-        self._stage_ev[slot] = ev
-        return True
-
+    @torch.no_grad()
     def _static_forward(self, batch):
         from .backbone import EvalStaticSpec
-        drop = {k + st.sfx for st in self.streams for k in ('voxel_features', 'voxel_coords', 'points')}
-        bd = {k: v for k, v in batch.items() if k not in drop}
-        counts = {}
-        for st in self.streams:
-            if self.vox is not None:
-                f, c, num, n = self._voxelize(st, st.pts, self.B, static=True)
-                bd['voxel_num_points' + st.sfx] = num
-            else:
-                f, c, n = st.vf, st.vc, self.n_dev[st.i:st.i + 1]
-            bd.update({'voxel_features' + st.sfx: f, 'voxel_coords' + st.sfx: c})
-            counts[st.sfx] = n
-        ovf = {k: self.overflow[j:j + 1] for j, k in enumerate(self.plan_keys)}
+        bd, counts = self.inputs.static_batch(batch)
+        flag = self.flags.flag
         if self.x_batched:
             sfx = self._sfx(self.R)
-            lidar = executor.StaticSpec(self.n_dev[-1:], self.caps[''], ovf[''])
-            mm = [executor.StaticSpec(counts['_mm' + s], self.caps['_mm' + s], ovf['_mm' + s]) for s in sfx] if self.mm else []
-            bd['virconv_eval_static'] = EvalStaticSpec(lidar, [counts[s] for s in sfx], mm, self.proj)
+            lidar = executor.StaticSpec(self.inputs.n_dev[-1:], self.caps[''], flag(''))
+            mm = [executor.StaticSpec(counts['_mm' + s], self.caps['_mm' + s], flag('_mm' + s)) for s in sfx] if self.mm else []
+            bd['virconv_eval_static'] = EvalStaticSpec(lidar, [counts[s] for s in sfx], mm, self.inputs.proj)
         else:
-            bd['virconv_static'] = executor.StaticSpec(counts[''], self.caps[''], ovf[''])
-            bd['virconv_proj'] = self.proj[0]
+            bd['virconv_static'] = executor.StaticSpec(counts[''], self.caps[''], flag(''))
+            bd['virconv_proj'] = self.inputs.proj[0]
         before = set(bd)
         out = self.model(bd)
         if self.bev:
@@ -683,88 +638,35 @@ class GraphedForward:
         self._published = [k for k in out if k not in before]
         return out
 
-    def _capture(self, batch, R):
-        torch.cuda.synchronize(self.dev)
-        self.R = R
-        self.streams = [_Stream(s, i) for i, s in enumerate(self.input_streams(R))]
-        self.plan_keys = self.plan_streams(R)
-        runs = self._exact(batch)
-        self._make_buffers(batch, runs)
-        assert self._load(batch)
-        s = torch.cuda.Stream(device=self.dev)          # warm-up of the static path (allocator pools, arena sizes)
-        s.wait_stream(torch.cuda.current_stream(self.dev))
-        with torch.cuda.stream(s), torch.no_grad():
-            for _ in range(max(self.warmup, 1)):
-                self._static_forward(batch)
-        torch.cuda.current_stream(self.dev).wait_stream(s)
-        torch.cuda.synchronize(self.dev)
-        self.overflow.zero_()
-        self.graph = None
-        graph = torch.cuda.CUDAGraph()
-        lib = _lib.load()
-        l0 = lib.vc_launch_count()
-        with torch.no_grad(), torch.cuda.graph(graph):
-            self.out = self._static_forward(batch)
-        self.graph = graph
-        self.launches_per_replay = int(lib.vc_launch_count() - l0)
-        self.recaptures += 1
-        torch.cuda.synchronize(self.dev)
+    def _recapture(self, batch):
+        self.out, = self._capture(batch, self._exact, self._static_forward, [self._static_forward])
 
     # -- replay ----------------------------------------------------------------------------------------------------
-    def _flags_to_host(self):
-        slot = self._slot
-        self._slot = (slot + 1) % self.ovf_host.shape[0]
-        self.ovf_host[slot].copy_(self.overflow, non_blocking=True)
-        self.err_host[slot:slot + 1].copy_(ops.tc_error_flag(self.dev), non_blocking=True)
-        self.overflow.zero_()
-        ev = torch.cuda.Event()
-        ev.record()
-        return ev, slot
-
-    def _flag_values(self, slot):
-        """-> the largest row count of one replay that did not fit (0: none); a non-zero one is also recorded in
-        `overflow_events` as {plan key: rows}."""
-        if int(self.err_host[slot]) != 0:
-            raise _lib.VirConvLibraryError("a tensor-core kernel's pipeline wait timed out inside a replayed forward (error flag "
-                                           "set): the results of that forward are invalid")
-        vals = [int(v) for v in self.ovf_host[slot]]
-        if max(vals):
-            self.overflow_events.append({k: v for k, v in zip(self.plan_keys, vals) if v})
-        return max(vals)
-
-    def _overflowed(self):
-        """'async': the largest overflow of the replays that have completed so far (never blocks)."""
-        worst = 0
-        while self._pending and self._pending[0][0].query():
-            worst = max(worst, self._flag_values(self._pending.pop(0)[1]))
-        return worst
-
-    def _grow(self, batch, R):
-        self.margin *= 1.25
-        self._capture(batch, R)
-
     def __call__(self, batch):
         """-> the batch dict plus the published tensors of this forward (owned by the graph: valid until the next call)."""
         R = self.copies(batch)
-        if self.graph is None or R != self.R or int(batch['batch_size']) != self.B:
-            self._capture(batch, R)
-        if self.check_overflow == 'async' and self._overflowed():
-            self._grow(batch, R)           # an EARLIER batch did not fit: its result came from clamped row sets
+        if R != self.R:
+            # other copies, other streams and plans: buffers and capacities start afresh
+            self.R, self.caps = R, {}
+            # (n_dev[-1]: the packed LiDAR rows, written in the graph)
+            self.inputs = _Inputs(self.input_streams(R), self.vox, self._vox_arg, copies=R, extra_counts=1)
+            self.graphs = []
+        if not self.graphs or int(batch['batch_size']) != self.inputs.B:
+            self._recapture(batch)
+        if self.check_overflow == 'async' and self.flags.worst():
+            self._grow(batch)              # an EARLIER batch did not fit: its result came from clamped row sets
         while True:
             if not self._load(batch):
-                self._grow(batch, R)       # more input rows than the buffers hold
+                self._grow(batch)          # more input rows than the buffers hold
                 continue
-            self.graph.replay()
+            self.graphs[0].replay()
             if self.check_overflow == 'sync':
-                ev, slot = self._flags_to_host()
-                ev.synchronize()
-                if self._flag_values(slot):
-                    self._grow(batch, R)   # this batch did not fit: re-capture and run it again
+                self.flags.push().synchronize()
+                if self.flags.worst():
+                    self._grow(batch)      # this batch did not fit: re-capture and run it again
                     continue
             else:
-                if len(self._pending) >= self.ovf_host.shape[0]:
-                    self._pending[0][0].synchronize()
-                self._pending.append(self._flags_to_host())
+                self.flags.push()
             break
         res = dict(batch)
         res.update({k: self.out[k] for k in self._published})
