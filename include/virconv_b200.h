@@ -59,7 +59,8 @@ int vc_set_conv_bn_fused(int enable);
 /* Tensor-core conv kernel selector: accepts 1 (the persistent kernel, csrc/conv_tc2.cu, the only one); else VC_ERR_INVALID. */
 int vc_set_tc_variant(int variant);
 /* A/B aid for the persistent tensor-core conv kernel (conv_tc2.cu): CTAs per SM, 0 = automatic (two when each still gets a
- * ring of >= 2 stages in half the shared memory), 1 or 2 = forced. */
+ * ring of >= 2 stages in half the shared memory), 1 or 2 = forced.  The cooperative conv + BN grid keeps one CTA per SM
+ * unless 2 is forced. */
 int vc_conv_tc2_config(int ctas_per_sm);
 /* The plan executor's weight-gradient launches (csrc/wgrad_tc3.cu): variant must be 1 (the only kernel); max_ctas caps
  * their CTAs (0, the default: half the SMs, so that each shares its SM with a dgrad CTA of the main stream). */

@@ -2,13 +2,16 @@
 kernel's duration, the gap from its end to the BN apply's start, the BN apply's duration and the gap to the next conv, from
 torch.profiler over ~20 replays of the captured VirConv-L training step (GraphedStep with the in-graph voxeliser, bench's
 batch and loss).  With the BN apply fused into the conv (VIRCONV_CONV_BN_FUSED=1) the apply columns read 0 and the conv
-column includes it.  Run on the GPU:
+column includes it.  Per replay it also prints the index phase: the span from the first index kernel (hash insert, probes,
+strided-conv count / emit / tables, projections) to the last, the time from the voxeliser's last kernel to the first conv,
+and the span of the forward's conv chain.  Run on the GPU:
 
     python profiles/forward_bn_gap.py [--replays 20]
 
 Prints the card name and power limit with the numbers: a kernel time is only meaningful with what it was measured on."""
 import argparse
 import os
+import re
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -22,6 +25,47 @@ from virconv_b200.backbone import VirConvL8x  # noqa: E402
 from virconv_b200.graph import GraphedStep, masked_mean  # noqa: E402
 
 CONV, APPLY, REDUCE = 'tc_conv_persist', 'bn_apply_relu', 'bn_sums_reduce'
+INDEX = re.compile(r'\b(hash_insert|subm_probe|conv_mark|scan_local|scan_blocks|conv_emit_indices|conv_tables|index2uv|g2_[a-z_]+|'
+                   r'stvd_gather_idx)_kernel')
+VOX = re.compile(r'\b(vox_[a-z]+|vscan_local)_kernel')
+
+
+def forward_windows(events):
+    """events: (start_ns, end_ns, name, stream) of every kernel, all replays -> one list of (sorted) kernel events per
+    replay, from its voxeliser's first kernel to its first backward kernel."""
+    replays, fwd = [], False
+    for ev in sorted(events):
+        name = ev[2]
+        if 'vox_insert' in name and not fwd:      # (the in-graph voxeliser's first kernel)
+            fwd = True
+            replays.append([ev])
+        elif 'masked_mean_bwd' in name or 'bn_bwd' in name:
+            fwd = False
+        elif fwd:
+            replays[-1].append(ev)
+    return replays
+
+
+def index_phase(events):
+    """-> per replay {'idx_span', 'vox_to_conv', 'conv_chain', 'kernels'}: first index kernel start -> last index kernel
+    end, voxeliser's last kernel end -> first conv start, first conv start -> last conv end (ns), and per index kernel name
+    [launches, summed duration in ns]."""
+    out = []
+    for evs in forward_windows(events):
+        idx = [ev for ev in evs if INDEX.search(ev[2])]
+        vox = [ev for ev in evs if VOX.search(ev[2])]
+        conv = [ev for ev in evs if CONV in ev[2]]
+        if not (idx and vox and conv):
+            continue
+        kernels = {}
+        for ev in idx:
+            k = kernels.setdefault(INDEX.search(ev[2]).group(1), [0, 0])
+            k[0] += 1
+            k[1] += ev[1] - ev[0]
+        out.append({'idx_span': max(e[1] for e in idx) - min(e[0] for e in idx),
+                    'vox_to_conv': conv[0][0] - max(e[1] for e in vox),
+                    'conv_chain': max(e[1] for e in conv) - conv[0][0], 'kernels': kernels})
+    return out
 
 
 def forward_layers(events):
@@ -29,20 +73,8 @@ def forward_layers(events):
     its first backward kernel (the loss of an early output may run before the forward ends: a graph orders by dependency).
     The forward's layers are a strict chain of conv -> BN kernels; a graph replay may put them on any of its streams, so
     they are ordered by time alone.  Returns one list of layer rows per replay."""
-    events = sorted(events)
-    replays, cur, fwd = [], None, False
-    for ev in events:
-        name = ev[2]
-        if 'vox_insert' in name and not fwd:      # (the in-graph voxeliser's first kernel)
-            fwd = True
-            cur = []
-            replays.append(cur)
-        elif 'masked_mean_bwd' in name or 'bn_bwd' in name:
-            fwd = False
-        elif fwd:
-            cur.append(ev)
     out = []
-    for evs in replays:
+    for evs in forward_windows(events):
         chain = [ev for ev in evs if CONV in ev[2] or APPLY in ev[2] or REDUCE in ev[2]]
         layers = []
         for j, ev in enumerate(chain):
@@ -119,6 +151,18 @@ def main():
     print(f'  sum {tot["conv"]:8.1f} {tot["gap_apply"]:8.1f} {tot["apply"]:9.1f} {tot["gap_next"]:10.1f}')
     print(f'BN apply + both gaps: {(tot["gap_apply"] + tot["apply"] + tot["gap_next"]) / 1e3:.3f} ms/step; '
           f'conv + apply + gaps: {sum(tot.values()) / 1e3:.3f} ms/step')
+    ph = index_phase(events)
+    print(f'index phase ({len(ph)} replays, us: mean [min, max]):')
+    for k, label in (('idx_span', 'first -> last index kernel'), ('vox_to_conv', 'voxeliser end -> first conv'),
+                     ('conv_chain', 'first conv start -> last conv end')):
+        v = [r[k] / 1e3 for r in ph]
+        print(f'  {label:34s} {sum(v) / len(v):8.1f} [{min(v):.1f}, {max(v):.1f}]')
+    names = sorted({n for r in ph for n in r['kernels']}, key=lambda n: -sum(r['kernels'].get(n, [0, 0])[1] for r in ph))
+    print('  index kernels (per replay: launches, summed duration us; the two index streams overlap):')
+    for n in names:
+        c = sum(r['kernels'].get(n, [0, 0])[0] for r in ph) / len(ph)
+        t = sum(r['kernels'].get(n, [0, 0])[1] for r in ph) / len(ph) / 1e3
+        print(f'    {n:20s} {c:6.1f} {t:8.1f}')
 
 
 if __name__ == '__main__':

@@ -133,7 +133,8 @@ static inline cudaError_t launch_chain(void (*kern)(KP...), dim3 grid, dim3 bloc
 // `n_dev` (optional): the row count lives in device memory and `n` / `n_out` are capacities (static mode, graph capturable)
 int subm_rulebook_dev(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size, const int32_t* spatial_shape,
                       const int32_t* ksize, const int32_t* dilation, int32_t* nbr, int32_t* pair_num, void* ws, size_t ws_bytes,
-                      cudaStream_t stream, int32_t* rep = nullptr);   // rep (optional): [n] lowest row at each row's coordinate
+                      cudaStream_t stream, int32_t* rep = nullptr,   // rep (optional): [n] lowest row at each row's coordinate
+                      bool unique = false);   // every coordinate held by one row: half the probes (the table is its own transpose)
 int conv_rulebook_count_dev(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size,
                             const int32_t* spatial_shape, const int32_t* ksize, const int32_t* stride, const int32_t* padding,
                             const int32_t* dilation, int32_t* n_out_dev, int cap_out, int* overflow, void* ws, size_t ws_bytes,

@@ -733,8 +733,10 @@ int launch_persist(const PArgs& a0, int n_cap, cudaStream_t stream, bool* bn_don
         // The grid-wide barrier needs every CTA resident at once: a cooperative launch, which starts only when ALL its CTAs fit.
         // At two CTAs per SM that means waiting until the index stream's rulebook kernels have left the SMs (measured: 0.14 ms
         // per step SLOWER than the separate apply kernel); at one CTA per SM the grid fits beside them and the step gets
-        // 0.15 ms faster (DESIGN.md section 8).  Same shared-memory plan, half the CTAs.
-        const int cgrid = grid < num_sms() ? grid : num_sms();
+        // 0.15 ms faster (DESIGN.md section 8).  Same shared-memory plan, half the CTAs.  Running the whole index phase
+        // before the forward instead, so that the grid could take both CTAs of each SM, was slower still (DESIGN.md
+        // section 8, item 3).  vc_conv_tc2_config(2) forces the two-CTA grid (tests, A/B runs).
+        const int cgrid = (g_p_ctas == 2 || grid < num_sms()) ? grid : num_sms();
         cudaLaunchConfig_t cfg{};
         cfg.gridDim = dim3(cgrid);
         cfg.blockDim = dim3(P_THREADS);

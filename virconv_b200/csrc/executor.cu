@@ -400,7 +400,7 @@ int fwd_subm_rb(FwdCtx& C, int i, const int* o, int s) {
     }
     if (C.do_idx) {
         VC_TRY(subm_rulebook_dev(I.idx, I.n, I.n_dev, I.ndim, C.S->batch_size, I.shape, o + F_KS, o + F_DL, R.nbr, R.pair_num, ws, wsb,
-                                 C.st[s], rep));
+                                 C.st[s], rep, R.unique != 0));
         if (rep) VC_TRY(gather2d_prep_dev(R.nbr, rep, R.K, I.n, I.n_dev, R.g2, C.st[s]));
     }
     C.produced(R, s);

@@ -90,11 +90,15 @@ __device__ __forceinline__ int hash_lookup(const unsigned long long* __restrict_
 // One thread per (output row, kernel offset): grid (ceil(n/256), K).  Every probe chain is independent, so the
 // hash look-ups of all K offsets are in flight together (the per-row loop this replaced was latency bound);
 // nbr[k, row] writes stay fully coalesced.  Pair counts: warp ballot -> shared counter -> one atomic per block.
+// sym (every coordinate held by one row, odd kernel sizes): the table is its own transpose — nbr[k, i] = j exactly when
+// nbr[K-1-k, j] = i, the relation the mirrored dgrad already relies on — so the grid covers the offsets k <= centre only
+// and each neighbour found also writes its mirrored entry (the caller fills the rows k > centre with -1 first): half the
+// hash look-ups, the same table.
 __global__ void __launch_bounds__(256) subm_probe_kernel(const int32_t* __restrict__ idx, int n,
                                                          const int* __restrict__ n_dev, Geom g,
                                                          const unsigned long long* __restrict__ table,
                                                          uint32_t mask, int32_t* __restrict__ nbr,
-                                                         int32_t* __restrict__ pair_num, int32_t* __restrict__ rep) {
+                                                         int32_t* __restrict__ pair_num, int32_t* __restrict__ rep, int sym) {
     __shared__ int cnt;
     const int pitch = n;                  // table rows are [K][capacity]
     if (n_dev != nullptr) n = min(n, __ldg(n_dev));
@@ -132,6 +136,7 @@ __global__ void __launch_bounds__(256) subm_probe_kernel(const int32_t* __restri
                 key = key * (unsigned long long)g.shape[d] + (unsigned long long)v;
             }
             if (ok) res = hash_lookup(table, mask, key);
+            if (sym && res >= 0) nbr[(size_t)(g.K - 1 - k) * pitch + res] = row;
         }
         nbr[(size_t)k * pitch + row] = res;
     } else if (row < pitch) {
@@ -141,7 +146,10 @@ __global__ void __launch_bounds__(256) subm_probe_kernel(const int32_t* __restri
     unsigned m = __ballot_sync(0xffffffffu, res >= 0);
     if ((threadIdx.x & 31) == 0 && m) atomicAdd(&cnt, __popc(m));
     __syncthreads();
-    if (pair_num != nullptr && threadIdx.x == 0 && cnt) atomicAdd(&pair_num[k], cnt);
+    if (pair_num != nullptr && threadIdx.x == 0 && cnt) {
+        atomicAdd(&pair_num[k], cnt);
+        if (sym && k != g.K - 1 - k) atomicAdd(&pair_num[g.K - 1 - k], cnt);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -393,7 +401,7 @@ extern "C" size_t vc_subm_rulebook_ws_bytes(int n) { return (size_t)table_slots(
 
 int vc::subm_rulebook_dev(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size,
                           const int32_t* spatial_shape, const int32_t* ksize, const int32_t* dilation, int32_t* nbr,
-                          int32_t* pair_num, void* ws, size_t ws_bytes, cudaStream_t stream, int32_t* rep) {
+                          int32_t* pair_num, void* ws, size_t ws_bytes, cudaStream_t stream, int32_t* rep, bool unique) {
     Geom g;
     int rc = make_geom(g, ndim, batch_size, spatial_shape, ksize, nullptr, nullptr, dilation);
     if (rc) return rc;
@@ -413,7 +421,12 @@ int vc::subm_rulebook_dev(const int32_t* indices, int n, const int* n_dev, int n
     VC_CUDA(cudaMemsetAsync(table, 0xFF, (size_t)slots * 8, stream));
     hash_insert_kernel<<<cdiv(n, 256), 256, 0, stream>>>(indices, n, n_dev, g, table, slots - 1);
     VC_LAUNCH_CHECK();
-    subm_probe_kernel<<<dim3(cdiv(n, 256), g.K), 256, 0, stream>>>(indices, n, n_dev, g, table, slots - 1, nbr, pair_num, rep);
+    bool sym = unique && rep == nullptr;
+    for (int d = 0; d < ndim; ++d) sym &= (g.ksize[d] & 1) == 1;
+    const int centre = g.K / 2;   // (odd kernel sizes: the centre offset is the middle one)
+    if (sym) VC_CUDA(cudaMemsetAsync(nbr + (size_t)(centre + 1) * n, 0xFF, sizeof(int32_t) * (size_t)(g.K - 1 - centre) * n, stream));
+    subm_probe_kernel<<<dim3(cdiv(n, 256), sym ? centre + 1 : g.K), 256, 0, stream>>>(indices, n, n_dev, g, table, slots - 1, nbr,
+                                                                                      pair_num, rep, sym ? 1 : 0);
     VC_LAUNCH_CHECK();
     return VC_OK;
 }
