@@ -587,6 +587,26 @@ int vc_rcnn_loss(const vc_rcnn_branch* branches /*host[K]*/, int K, double beta,
                  size_t ws_bytes, vc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Part-score RoI pooling of TEDMHead's PART branch (VirConv-T / -S), whose rules csrc/part_pool.cu states.  No host
+ * read; graph-capturable; the backward is bit-identical run to run (fixed-order sums, no float atomics).
+ *   vc_part_pool_fwd <- TEDMHead.obtain_conf_preds (ted_head.py:425-448) with gen_sample_grid and
+ *                       bilinear_interpolate_torch_gridsample (:110-156), all scenes in one call: parts [B, S*S, H, W]
+ *                       and rois [B, N, ld] (ld >= 7) fp32 contiguous, grid size S, GRID_OFFSETS (ox, oy), spatial scale
+ *                       1 / FEATMAP_STRIDE -> out [B * N] fp32 (torch.cat(confi), scene-major).  One launch.
+ *   vc_part_pool_bwd <- its gradient with respect to the part map: g [B * N] (d loss / d out) -> dparts [B, S*S, H, W],
+ *                       every element written.  ws >= vc_part_pool_bwd_ws_bytes(B, N, S) (0 today: the tap records stay
+ *                       in shared memory).  One launch.
+ *   N > VC_PART_POOL_MAX_ROIS or S outside [2, VC_PART_POOL_MAX_GRID] -> VC_ERR_UNSUPPORTED.
+ * ---------------------------------------------------------------------------------------------- */
+#define VC_PART_POOL_MAX_ROIS 1024
+#define VC_PART_POOL_MAX_GRID 16
+int vc_part_pool_fwd(const float* parts, const float* rois, int B, int N, int ld, int S, int H, int W, float ox, float oy,
+                     float scale, float* out, vc_stream_t stream);
+size_t vc_part_pool_bwd_ws_bytes(int B, int N, int S);
+int vc_part_pool_bwd(const float* rois, const float* g, int B, int N, int ld, int S, int H, int W, float ox, float oy,
+                     float scale, float* dparts, void* ws, size_t ws_bytes, vc_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Plan executor: a whole backbone forward / backward in ONE call.  Replaces the Python layer loop of
  * `VirConvL8x.forward` (spconv_backbone.py:609-699), `NRConvBlock.forward` (:207-229) and the two streams of
  * `VirConv8x.forward` (:339-535) together with autograd's reverse walk over them: the host side of ~100 operator

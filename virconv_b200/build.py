@@ -27,10 +27,13 @@ FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-line
 # labels round as torch's elementwise kernels do
 # head_losses.cu: no contraction, so that each float64 operation of the losses and their gradients rounds once, as the
 # float64 restatement in oracle/head_losses.py does
+# part_pool.cu: no contraction, so that the sample positions and bilinear weights round every operation once, as torch's
+# elementwise kernels and grid_sample do
 FILE_FLAGS = {'iou3d_nms.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
               'anchor_targets.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
               'roi_targets.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
-              'head_losses.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off']}
+              'head_losses.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
+              'part_pool.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off']}
 
 
 def flags_for(src):

@@ -33,6 +33,9 @@ the name at module level, and in its own module) and `RoIHeadTemplate.assign_tar
 With `use_fused_losses` `AnchorHeadTemplate.get_loss` and `RoIHeadTemplate.get_loss` are this package's drop-in methods
 (virconv_b200.head_losses): the RPN and RCNN training losses and their gradients in one kernel call each, without a host
 read apart from the one copy of the tb values.
+With `use_fused_part_pool` `TEDMHead.obtain_conf_preds` is this package's drop-in method (virconv_b200.part_pool): the
+PART branch's position-sensitive RoI pooling of VirConv-T / -S in one call per stage, without a host read, with a
+bit-reproducible part-map gradient.
 """
 from __future__ import annotations
 
@@ -223,7 +226,7 @@ def _points_in_boxes_cpu(boxes, points, point_indices):
 
 
 def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=False, use_fused_rpn_targets=False,
-            use_fused_roi_targets=False, use_fused_losses=False):
+            use_fused_roi_targets=False, use_fused_losses=False, use_fused_part_pool=False):
     """Register everything listed in the module docstring.  `reference_root`: put that checkout first on sys.path."""
     if reference_root is not None and reference_root not in sys.path:
         sys.path.insert(0, reference_root)
@@ -314,4 +317,10 @@ def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=F
         aht.get_loss = head_losses.anchor_head_get_loss
         rht = importlib.import_module('pcdet.models.roi_heads.roi_head_template').RoIHeadTemplate
         rht.get_loss = head_losses.roi_head_get_loss
+    if use_fused_part_pool:
+        from . import part_pool
+        ted = importlib.import_module('pcdet.models.roi_heads.ted_head').TEDMHead
+        if ted.obtain_conf_preds is not part_pool.obtain_conf_preds:
+            part_pool._reference_obtain_conf_preds = ted.obtain_conf_preds
+        ted.obtain_conf_preds = part_pool.obtain_conf_preds
     return True
