@@ -607,6 +607,53 @@ int vc_part_pool_bwd(const float* rois, const float* g, int B, int N, int ld, in
                      float scale, float* dparts, void* ws, size_t ws_bytes, vc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Parameter update of the adam_onecycle / adam_cosin step (csrc/optim.cu): what the reference's loop does after
+ * loss.backward() (tools/train_utils/train_utils.py:50-52: clip_grad_norm_, OptimWrapper.step of fastai_optim.py:132-149
+ * over torch.optim.Adam) for EVERY parameter tensor in two launches.  No host read, no allocation; graph-capturable;
+ * bit-identical run to run and for every max_ctas (fixed-order float64 norm, no float atomics).
+ *   segs    device [n_segs]: one entry per parameter tensor, fp32 throughout.  g == NULL: a trainable parameter that got no
+ *           gradient; it takes no part in the norm and is decayed only.
+ *   chunks  device [n_chunks]: the tensors cut into pieces of at most VC_OPTIM_CHUNK elements (off a multiple of 4), made
+ *           by the caller once from the element counts.
+ *   hyper   device float64[5]: lr, beta1 (the CURRENT momentum), beta2, eps, wd.
+ *   counters device int64[2]: t = steps applied so far, and steps skipped.  The call advances one of them.
+ *   guards  HOST array of n_guards (<= VC_OPTIM_MAX_GUARDS) device int32 words, read by the norm pass.
+ *   status  device, written by the norm pass: total_norm = sqrt(sum g^2); clip_coef = min(1, max_norm / (total_norm + 1e-6))
+ *           (1 when max_norm < 0: no clipping); apply = total_norm is finite and every guard word is zero; then the step's
+ *           scalars, formed in float64 and rounded to fp32 once.
+ * With apply == 0 nothing is written to p, m, v or t and `skipped` grows by one.  Otherwise, per element, with
+ * gh = clip_coef * g and t counting this step:
+ *   p <- p * (1 - wd * lr);  m <- m + (1 - beta1) * (gh - m);  v <- beta2 * v + (1 - beta2) * gh^2;
+ *   p <- p - lr / (1 - beta1^t) * m / (sqrt(v) / sqrt(1 - beta2^t) + eps).
+ * The gradients are never written.  ws >= vc_optim_ws_bytes(n_chunks), ZEROED by the caller before the first call and
+ * left alone afterwards (the norm pass's ticket resets itself).  max_ctas > 0 caps both grids (0: one CTA per chunk).
+ * ---------------------------------------------------------------------------------------------- */
+#define VC_OPTIM_CHUNK 4096
+#define VC_OPTIM_MAX_GUARDS 8
+typedef struct {
+    float* p;
+    const float* g; /* may be NULL */
+    float* m;       /* exp_avg */
+    float* v;       /* exp_avg_sq */
+    long long n;
+} vc_optim_seg;
+typedef struct {
+    int32_t seg;
+    int32_t len;
+    long long off;
+} vc_optim_chunk;
+typedef struct {
+    double total_norm, clip_coef;
+    int32_t apply;
+    float clip, decay, step_size, bc2_sqrt, eps, w1, beta2, w2;
+    int32_t pad[3];
+} vc_optim_status; /* 64 bytes */
+size_t vc_optim_ws_bytes(int n_chunks);
+int vc_optim_step(const vc_optim_seg* segs, int n_segs, const vc_optim_chunk* chunks, int n_chunks, double max_norm,
+                  const int32_t* const* guards /*host[n_guards]*/, int n_guards, const double* hyper, long long* counters,
+                  vc_optim_status* status, int max_ctas, void* ws, size_t ws_bytes, vc_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Plan executor: a whole backbone forward / backward in ONE call.  Replaces the Python layer loop of
  * `VirConvL8x.forward` (spconv_backbone.py:609-699), `NRConvBlock.forward` (:207-229) and the two streams of
  * `VirConv8x.forward` (:339-535) together with autograd's reverse walk over them: the host side of ~100 operator

@@ -11,6 +11,13 @@ device value on the host; `GraphedStep` captures such a step once and replays it
         loss = step(batch)                              # copies the batch into the graph's input buffers, replays
         optimizer.step()                                # parameter .grad tensors are rewritten in place by every replay
 
+or, with the update inside the graph (optim.FusedAdamOneCycle; clipping, weight decay and Adam in two more launches):
+
+    step = GraphedStep(model, loss_fn, optimizer=opt, max_grad_norm=10.0)
+    for it, batch in enumerate(loader):
+        scheduler.step(it)                              # sets opt.lr / opt.mom; staged to the device by the next call
+        loss = step(batch)
+
 Published tensors inside the graph are capacity sized: `t.features` [cap, C] with a zero tail, `t.indices` [cap, 4] with a
 -1 tail, `t.num_rows` a device int32[1]; `loss_fn(batch_dict)` must use `num_rows` where the reference uses `shape[0]`.
 A batch whose row counts exceed the captured capacities is detected through the executor's overflow flag (read back
@@ -331,15 +338,33 @@ class _Captured:
 
 
 class GraphedStep(_Captured):
-    def __init__(self, model, loss_fn, params=None, margin=1.3, grain=1024, warmup=2, check_overflow=True, voxelizer=None):
+    def __init__(self, model, loss_fn, params=None, margin=1.3, grain=1024, warmup=2, check_overflow=True, voxelizer=None,
+                 optimizer=None, max_grad_norm=None):
         """voxelizer: None — batches carry `voxel_features` / `voxel_coords` (what the reference's dataloader + MeanVFE
         deliver); or a dict(point_cloud_range, voxel_size, max_points_per_voxel, max_voxels, vfe_model) — batches carry the
         collated raw `points` [N, 1+C] and the hash-grid voxelisation + VFE (vc_voxelize_mean) run INSIDE the graph.  With a
         two-stream model the batch also carries `points_mm`, voxelised by a second call with the entries `max_voxels_mm`
-        (default: `max_voxels`) and `vfe_model_mm` (default: None, the plain mean)."""
+        (default: `max_voxels`) and `vfe_model_mm` (default: None, the plain mean).
+
+        optimizer: None — the caller updates the parameters after each call; or an optim.FusedAdamOneCycle — the captured
+        body ends with its two update launches (clipping to `max_grad_norm`, None: no clipping), reading the gradients of
+        that replay, with every plan's overflow flag and the tensor-core error flag as guard words: a replay that raised one
+        skips its own update (optimizer.skipped_steps()) instead of applying gradients of clamped row sets.  Each call
+        stages the optimizer's current lr / mom before the replay, so a scheduler sets them as it does for an eager step.
+        The exact and warm-up runs of a capture update nothing, and a re-capture keeps the optimizer's state.  Parameters are
+        updated in place at fixed addresses: the executor re-casts its bf16 operands from them in every replay, so the next
+        replay computes with the new weights with no further action.  A world size above one is refused: the gradient
+        all-reduce has to sit between backward and update (use parallel.allreduce_gradients and the eager step())."""
         self.model, self.loss_fn = model, loss_fn
         self.params = list(model.parameters()) if params is None else list(params)
         super().__init__(self.params[0].device, voxelizer, margin, grain, warmup)
+        if optimizer is not None and torch.distributed.is_available() and torch.distributed.is_initialized() \
+                and torch.distributed.get_world_size() > 1:
+            raise ValueError('GraphedStep(optimizer=...) updates inside the graph, before any gradient all-reduce could run: with '
+                             'a world size of %d call parallel.allreduce_gradients and the optimizer\'s eager step()'
+                             % torch.distributed.get_world_size())
+        self.optimizer, self.max_grad_norm = optimizer, max_grad_norm
+        self._binding = None          # the optimizer's segment table of the current capture (set by _bind_optimizer)
         self.check_overflow = check_overflow
         self.inputs = _Inputs(getattr(model, 'static_streams', ('',)), self.vox, self._vox_arg)
 
@@ -383,19 +408,36 @@ class GraphedStep(_Captured):
         grads = torch.autograd.grad(loss, [alias.get(id(p), p) for p in self.params], allow_unused=True)
         for p, g in zip(self.params, grads):
             p.grad = g
+        if self._binding is not None:
+            self._binding.set_grads([p.grad for p in self.optimizer.all_params])
+            self._binding.launch(self.max_grad_norm)
         return loss.detach()
 
     def _warm(self, batch):
         self._clear_grads()
         self._static_step(batch)
 
+    def _bind_optimizer(self):
+        # after the warm-up runs (which update nothing: no binding yet), outside the graph: the table's buffers and the
+        # guard words of this capture's flags
+        self._clear_grads()
+        if self.optimizer is not None:
+            self._binding = self.optimizer.bind([self.flags.overflow, ops.tc_error_flag(self.dev)])
+
     def _recapture(self, batch):
-        self.loss, = self._capture(batch, self._exact, self._warm, [self._static_step], self._clear_grads)
+        self._binding = None
+        self.loss, = self._capture(batch, self._exact, self._warm, [self._static_step], self._bind_optimizer)
 
     def __call__(self, batch):
         """-> the step's loss (a device tensor owned by the graph: read or copy it before the next call)."""
         if not self.graphs:
             self._recapture(batch)
+        if self.optimizer is not None:
+            self.optimizer.stage_hyper()
+            if self.check_overflow:
+                # look at the oldest replay's flags BEFORE this replay, not after it: a batch whose update ran inside the graph
+                # must not run a second time
+                self.flags.wait_if_full()
         if self.check_overflow and self.flags.worst():
             # an EARLIER batch did not fit: its gradients were computed on clamped row sets.  Grow and re-capture; the
             # caller sees the event through `recaptures` (a training loop may want to discard those optimizer steps).
@@ -462,6 +504,9 @@ class PipelinedStep:
 
     def __init__(self, model, loss_fn, params=None, **kwargs):
         streams = tuple(getattr(model, 'static_streams', ('',)))
+        if kwargs.get('optimizer') is not None:
+            raise ValueError('PipelinedStep overlaps the index work of step t+1 with the feature work of step t and has no '
+                             'in-graph update: pass optimizer= to GraphedStep, or call the optimizer\'s step() after each call')
         if streams != ('',):
             raise ValueError('PipelinedStep phases a one-stream backbone (VirConvL8x); %s has the input streams %s, which have '
                              'no phased form: use GraphedStep' % (type(model).__name__, streams))

@@ -36,6 +36,12 @@ read apart from the one copy of the tb values.
 With `use_fused_part_pool` `TEDMHead.obtain_conf_preds` is this package's drop-in method (virconv_b200.part_pool): the
 PART branch's position-sensitive RoI pooling of VirConv-T / -S in one call per stage, without a host read, with a
 bit-reproducible part-map gradient.
+With `use_fused_optimizer` `train_utils.optimization.build_optimizer` (tools/train_utils/optimization/__init__.py:11-36, the
+name tools/train.py imports with tools/ on sys.path) returns this package's optim.FusedAdamOneCycle for OPTIMIZER
+adam_onecycle / adam_cosin and calls the reference's function for every other value, and the `clip_grad_norm_` name
+`train_utils.train_utils` imported at module level records its max_norm for the next step() of the fused optimizer that
+owns those parameters, leaving the gradients alone (parameters no fused optimizer owns go to torch's function): the
+reference's train_one_epoch (train_utils.py:13-71) then runs unchanged, with clipping, decay and Adam in two launches.
 """
 from __future__ import annotations
 
@@ -225,8 +231,34 @@ def _points_in_boxes_cpu(boxes, points, point_indices):
     return 1
 
 
+def _fused_build_optimizer(reference_build):
+    def build_optimizer(model, optim_cfg):
+        """build_optimizer (optimization/__init__.py:11-36) with the adam_onecycle / adam_cosin branch on vc_optim_step."""
+        if optim_cfg.OPTIMIZER not in ('adam_onecycle', 'adam_cosin'):
+            return reference_build(model, optim_cfg)
+        from .optim import FusedAdamOneCycle
+        return FusedAdamOneCycle.from_model(model, wd=optim_cfg.WEIGHT_DECAY, lr=3e-3, betas=(0.9, 0.99))
+    build_optimizer._reference = reference_build
+    return build_optimizer
+
+
+def _fused_clip_grad_norm_(parameters, max_norm, *args, **kwargs):
+    """clip_grad_norm_ as train_utils.py:50 calls it: the fused optimizers owning `parameters` clip inside their next step();
+    what is left goes to torch's function.  -> None or torch's result for the rest (train_one_epoch ignores it)."""
+    from . import optim
+    params = [parameters] if isinstance(parameters, torch.Tensor) else list(parameters)
+    ids = {id(p) for p in params}
+    for opt in optim.live_optimizers():
+        own = opt.owns(ids)
+        if own:
+            opt.clip_grad_norm(max_norm)
+            ids -= own
+    rest = [p for p in params if id(p) in ids and p.grad is not None]
+    return torch.nn.utils.clip_grad_norm_(rest, max_norm, *args, **kwargs) if rest else None
+
+
 def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=False, use_fused_rpn_targets=False,
-            use_fused_roi_targets=False, use_fused_losses=False, use_fused_part_pool=False):
+            use_fused_roi_targets=False, use_fused_losses=False, use_fused_part_pool=False, use_fused_optimizer=False):
     """Register everything listed in the module docstring.  `reference_root`: put that checkout first on sys.path."""
     if reference_root is not None and reference_root not in sys.path:
         sys.path.insert(0, reference_root)
@@ -323,4 +355,13 @@ def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=F
         if ted.obtain_conf_preds is not part_pool.obtain_conf_preds:
             part_pool._reference_obtain_conf_preds = ted.obtain_conf_preds
         ted.obtain_conf_preds = part_pool.obtain_conf_preds
+    if use_fused_optimizer:
+        import os
+        tools = os.path.join(reference_root, 'tools') if reference_root is not None else None
+        if tools is not None and tools not in sys.path:
+            sys.path.append(tools)              # (tools/train.py runs from tools/: `from train_utils.optimization import ...`)
+        om = importlib.import_module('train_utils.optimization')
+        if not hasattr(om.build_optimizer, '_reference'):
+            om.build_optimizer = _fused_build_optimizer(om.build_optimizer)
+        importlib.import_module('train_utils.train_utils').clip_grad_norm_ = _fused_clip_grad_norm_
     return True
