@@ -154,6 +154,10 @@ int vc_cast_f32_bf16(const float* in, void* out_bf16, long long n_elements /* mu
 size_t vc_conv_tc_ws_bytes(int cin, int cout, int K);
 int vc_conv_fwd_tc(const void* in_bf16, const float* w, const int32_t* nbr, float* out, int n_out, int cin, int cout,
                    int K, double* bn_sums, void* ws, size_t ws_bytes, int32_t* err_flag, vc_stream_t stream);
+/* vc_conv_fwd_tc over input rows of pitch in_ld bf16 elements (>= cin, multiple of 8): `in` may be a column slice of a
+ * wider matrix, as the plan executor reads an in-place concat; the other columns are never read. */
+int vc_conv_fwd_tc_ld(const void* in_bf16, int in_ld, const float* w, const int32_t* nbr, float* out, int n_out, int cin,
+                      int cout, int K, double* bn_sums, void* ws, size_t ws_bytes, int32_t* err_flag, vc_stream_t stream);
 /* din[nbr[k,o], :] += dout[o, :] @ w[:, k, :] on tensor cores, for many-to-one tables (image branch); din zeroed by the
  * caller; the dout tile is contiguous, the result is scattered with 8-byte vector reductions. */
 int vc_conv_dgrad_scatter_tc(const void* dout_bf16, const float* w, const int32_t* nbr, float* din, int n_out, int cin,
@@ -199,6 +203,9 @@ int vc_conv_bn_relu_tc(const void* in_bf16, const float* w, const int32_t* nbr, 
 size_t vc_conv_wgrad_tc_det_ws_bytes(int n_out, int cin, int cout, int K);
 int vc_conv_wgrad_tc_det(const void* in_bf16, const void* dout_bf16, const int32_t* nbr, float* dw, int n_out, int cin,
                          int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag, vc_stream_t stream);
+/* vc_conv_wgrad_tc_det over input rows of pitch in_ld bf16 elements (>= cin, multiple of 8), as vc_conv_fwd_tc_ld. */
+int vc_conv_wgrad_tc_det_ld(const void* in_bf16, int in_ld, const void* dout_bf16, const int32_t* nbr, float* dw, int n_out,
+                            int cin, int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag, vc_stream_t stream);
 /* vc_bn_relu_bwd_f32 with (sum g, sum g*xhat) reduced per 512-row chunk into float64 partials (ws) and added in chunk order
  * (vc_set_bn_fused selects one cooperative launch or two, with the same result).  ws >= vc_bn_bwd_det_ws_bytes(n, c). */
 size_t vc_bn_bwd_det_ws_bytes(int n, int c);
@@ -233,12 +240,12 @@ int vc_conv_dgrad_gather2d_tc(const void* dout_bf16, const float* w, const int32
  * place with the unbiased variance and *num_batches_tracked (int64, may be NULL) incremented — torch.nn.BatchNorm1d
  * semantics.  training == 0: statistics from the running buffers.  stats_out [4,c] = scale, shift, mean, invstd is
  * kept for backward.  y_bf16 (may be NULL): bf16 shadow of y = the next conv's tensor-core operand.  In place
- * (y == x) allowed. */
+ * (y == x) allowed.  The ReLU is torch.relu's: a NaN stays NaN. */
 int vc_bn_apply_relu_f32(const float* x, const double* sums, int n_rows, int c, const float* gamma, const float* beta,
                          float* running_mean, float* running_var, long long* num_batches_tracked, float momentum,
                          float eps, int training, float* y, void* y_bf16, float* stats_out, int relu, vc_stream_t stream);
 /* Backward of y = relu(gamma*(x-mean)*invstd + beta), stats = the forward's stats_out:
- *   g = dy * (y > 0); dbeta = sum g; dgamma = sum g*xhat;
+ *   g = dy * !(y <= 0) (a NaN y passes dy, as torch's threshold_backward); dbeta = sum g; dgamma = sum g*xhat;
  *   train: dx = gamma*invstd*(g - dbeta/n - xhat*dgamma/n);   eval: dx = gamma*invstd*g.
  * bsums: [2,c] float64 scratch accumulator, zeroed by the caller.  dx_bf16 (may be NULL): bf16 shadow of dx. */
 int vc_bn_relu_bwd_f32(const float* dy, const float* x, const float* y, const float* gamma, const float* stats,

@@ -49,6 +49,7 @@ SIGNATURES = {
     'vc_cast_f32_bf16': (_I, [_P, _P, ctypes.c_longlong, _P]),
     'vc_conv_tc_ws_bytes': (_Z, [_I, _I, _I]),
     'vc_conv_fwd_tc': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _P, _P]),
+    'vc_conv_fwd_tc_ld': (_I, [_P, _I, _P, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _P, _P]),
     'vc_conv_dgrad_tc': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _Z, _P, _P]),
     'vc_conv_dgrad_scatter_tc': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _Z, _P, _P]),
     'vc_conv_wgrad_tc_ws_bytes': (_Z, [_I, _I, _I, _I]),
@@ -60,6 +61,7 @@ SIGNATURES = {
                                 _P, _P]),
     'vc_conv_wgrad_tc_det_ws_bytes': (_Z, [_I, _I, _I, _I]),
     'vc_conv_wgrad_tc_det': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _Z, _P, _P]),
+    'vc_conv_wgrad_tc_det_ld': (_I, [_P, _I, _P, _P, _P, _I, _I, _I, _I, _P, _Z, _P, _P]),
     'vc_bn_bwd_det_ws_bytes': (_Z, [_I, _I]),
     'vc_bn_relu_bwd_det_f32': (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _Z, _P]),
     'vc_subm_rulebook_rep': (_I, [_P, _I, _I, _I, _HOST, _HOST, _HOST, _P, _P, _P, _P, _Z, _P]),

@@ -100,8 +100,8 @@ __device__ __forceinline__ void bn_bwd_chunk_partials(const float4* __restrict__
         for (int row = chk * BN_DET_ROWS + rl; row < end; row += rowlanes) {
             const size_t i = (size_t)row * c4 + cg;
             float4 g = dy[(size_t)row * dy_ld4 + cg], xx = x[i];
-            g.x = fmaf(xx.x, sc.x, sh.x) > 0.f ? g.x : 0.f; g.y = fmaf(xx.y, sc.y, sh.y) > 0.f ? g.y : 0.f;
-            g.z = fmaf(xx.z, sc.z, sh.z) > 0.f ? g.z : 0.f; g.w = fmaf(xx.w, sc.w, sh.w) > 0.f ? g.w : 0.f;
+            g.x = relu_grad(fmaf(xx.x, sc.x, sh.x), g.x); g.y = relu_grad(fmaf(xx.y, sc.y, sh.y), g.y);
+            g.z = relu_grad(fmaf(xx.z, sc.z, sh.z), g.z); g.w = relu_grad(fmaf(xx.w, sc.w, sh.w), g.w);
             s[0] += g.x; s[1] += g.y; s[2] += g.z; s[3] += g.w;
             q[0] = fmaf(g.x, (xx.x - m.x) * is.x, q[0]); q[1] = fmaf(g.y, (xx.y - m.y) * is.y, q[1]);
             q[2] = fmaf(g.z, (xx.z - m.z) * is.z, q[2]); q[3] = fmaf(g.w, (xx.w - m.w) * is.w, q[3]);
@@ -147,8 +147,9 @@ __device__ __forceinline__ void bn_bwd_sum_partials(const double* __restrict__ p
     __syncthreads();
 }
 
-// backward pass 1: sum g and sum g*xhat over rows, g = dy*(y>0); block partial -> float64 atomics on bsums [2, c]
-// (the ReLU mask is recomputed from x with the forward's own scale / shift and fmaf: bit-identical to testing y > 0,
+// backward pass 1: sum g and sum g*xhat over rows, g = dy*!(y<=0) (relu_grad: a NaN activation passes the gradient, as
+// torch's threshold_backward does); block partial -> float64 atomics on bsums [2, c]
+// (the ReLU mask is recomputed from x with the forward's own scale / shift and fmaf: bit-identical to testing y,
 //  so the activation itself is not read again; dy may be a column slice of a wider matrix: row pitch dy_ld4 float4)
 __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const float4* __restrict__ dy, int dy_ld4, const float4* __restrict__ x,
                                                             const float* __restrict__ stats, int n, const int* __restrict__ n_dev,
@@ -171,8 +172,8 @@ __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const float4* __rest
     for (int row = blockIdx.x * rowlanes + rl; row < n; row += gridDim.x * rowlanes) {
         size_t i = (size_t)row * c4 + cg;
         float4 g = dy[(size_t)row * dy_ld4 + cg], xx = x[i];
-        g.x = fmaf(xx.x, sc.x, sh.x) > 0.f ? g.x : 0.f; g.y = fmaf(xx.y, sc.y, sh.y) > 0.f ? g.y : 0.f;
-        g.z = fmaf(xx.z, sc.z, sh.z) > 0.f ? g.z : 0.f; g.w = fmaf(xx.w, sc.w, sh.w) > 0.f ? g.w : 0.f;
+        g.x = relu_grad(fmaf(xx.x, sc.x, sh.x), g.x); g.y = relu_grad(fmaf(xx.y, sc.y, sh.y), g.y);
+        g.z = relu_grad(fmaf(xx.z, sc.z, sh.z), g.z); g.w = relu_grad(fmaf(xx.w, sc.w, sh.w), g.w);
         s[0] += g.x; s[1] += g.y; s[2] += g.z; s[3] += g.w;
         q[0] = fmaf(g.x, (xx.x - m.x) * is.x, q[0]); q[1] = fmaf(g.y, (xx.y - m.y) * is.y, q[1]);
         q[2] = fmaf(g.z, (xx.z - m.z) * is.z, q[2]); q[3] = fmaf(g.w, (xx.w - m.w) * is.w, q[3]);
@@ -249,10 +250,12 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const float4* __restr
     const float4 sh = reinterpret_cast<const float4*>(stats + c)[cg];
     for (size_t i = i0; i < n4; i += stride) {
         float4 g = dy[dy_ld4 == c4 ? i : (i / c4) * dy_ld4 + cg], xx = x[i], r;
-        g.x = fmaf(xx.x, sc.x, sh.x) > 0.f ? g.x : 0.f; g.y = fmaf(xx.y, sc.y, sh.y) > 0.f ? g.y : 0.f;
-        g.z = fmaf(xx.z, sc.z, sh.z) > 0.f ? g.z : 0.f; g.w = fmaf(xx.w, sc.w, sh.w) > 0.f ? g.w : 0.f;
-        r.x = fmaf(a[0], g.x, fmaf(b[0], xx.x, d[0])); r.y = fmaf(a[1], g.y, fmaf(b[1], xx.y, d[1]));
-        r.z = fmaf(a[2], g.z, fmaf(b[2], xx.z, d[2])); r.w = fmaf(a[3], g.w, fmaf(b[3], xx.w, d[3]));
+        g.x = relu_grad(fmaf(xx.x, sc.x, sh.x), g.x); g.y = relu_grad(fmaf(xx.y, sc.y, sh.y), g.y);
+        g.z = relu_grad(fmaf(xx.z, sc.z, sh.z), g.z); g.w = relu_grad(fmaf(xx.w, sc.w, sh.w), g.w);
+        // (eval: b = d = 0 and x does not enter dx, so a NaN x gives gi * g as torch does, not 0 * NaN; 0 is the value
+        // fmaf(0, x, 0) has for every finite x)
+        r.x = fmaf(a[0], g.x, training ? fmaf(b[0], xx.x, d[0]) : 0.f); r.y = fmaf(a[1], g.y, training ? fmaf(b[1], xx.y, d[1]) : 0.f);
+        r.z = fmaf(a[2], g.z, training ? fmaf(b[2], xx.z, d[2]) : 0.f); r.w = fmaf(a[3], g.w, training ? fmaf(b[3], xx.w, d[3]) : 0.f);
         if (dx != nullptr) dx[i] = r;
         if (dx_bf16 != nullptr) dx_bf16[i] = pack_bf16x4(r);
     }
@@ -291,8 +294,8 @@ __global__ void __launch_bounds__(256) bn_bwd_fused_kernel(const float4* __restr
         for (int row = blockIdx.x * rowlanes + rl; row < n_rows; row += gridDim.x * rowlanes) {
             size_t i = (size_t)row * c4 + cg;
             float4 g = dy[(size_t)row * dy_ld4 + cg], xx = x[i];
-            g.x = fmaf(xx.x, sc.x, sh.x) > 0.f ? g.x : 0.f; g.y = fmaf(xx.y, sc.y, sh.y) > 0.f ? g.y : 0.f;
-            g.z = fmaf(xx.z, sc.z, sh.z) > 0.f ? g.z : 0.f; g.w = fmaf(xx.w, sc.w, sh.w) > 0.f ? g.w : 0.f;
+            g.x = relu_grad(fmaf(xx.x, sc.x, sh.x), g.x); g.y = relu_grad(fmaf(xx.y, sc.y, sh.y), g.y);
+            g.z = relu_grad(fmaf(xx.z, sc.z, sh.z), g.z); g.w = relu_grad(fmaf(xx.w, sc.w, sh.w), g.w);
             s[0] += g.x; s[1] += g.y; s[2] += g.z; s[3] += g.w;
             q[0] = fmaf(g.x, (xx.x - m.x) * is.x, q[0]); q[1] = fmaf(g.y, (xx.y - m.y) * is.y, q[1]);
             q[2] = fmaf(g.z, (xx.z - m.z) * is.z, q[2]); q[3] = fmaf(g.w, (xx.w - m.w) * is.w, q[3]);
@@ -358,10 +361,12 @@ __global__ void __launch_bounds__(256) bn_bwd_fused_kernel(const float4* __restr
     const float4 sh = reinterpret_cast<const float4*>(stats + c)[cg];
     for (size_t i = i0; i < n4; i += stride) {
         float4 g = dy[dy_ld4 == c4 ? i : (i / c4) * dy_ld4 + cg], xx = x[i], r;
-        g.x = fmaf(xx.x, sc.x, sh.x) > 0.f ? g.x : 0.f; g.y = fmaf(xx.y, sc.y, sh.y) > 0.f ? g.y : 0.f;
-        g.z = fmaf(xx.z, sc.z, sh.z) > 0.f ? g.z : 0.f; g.w = fmaf(xx.w, sc.w, sh.w) > 0.f ? g.w : 0.f;
-        r.x = fmaf(a[0], g.x, fmaf(b[0], xx.x, d[0])); r.y = fmaf(a[1], g.y, fmaf(b[1], xx.y, d[1]));
-        r.z = fmaf(a[2], g.z, fmaf(b[2], xx.z, d[2])); r.w = fmaf(a[3], g.w, fmaf(b[3], xx.w, d[3]));
+        g.x = relu_grad(fmaf(xx.x, sc.x, sh.x), g.x); g.y = relu_grad(fmaf(xx.y, sc.y, sh.y), g.y);
+        g.z = relu_grad(fmaf(xx.z, sc.z, sh.z), g.z); g.w = relu_grad(fmaf(xx.w, sc.w, sh.w), g.w);
+        // (eval: b = d = 0 and x does not enter dx, so a NaN x gives gi * g as torch does, not 0 * NaN; 0 is the value
+        // fmaf(0, x, 0) has for every finite x)
+        r.x = fmaf(a[0], g.x, training ? fmaf(b[0], xx.x, d[0]) : 0.f); r.y = fmaf(a[1], g.y, training ? fmaf(b[1], xx.y, d[1]) : 0.f);
+        r.z = fmaf(a[2], g.z, training ? fmaf(b[2], xx.z, d[2]) : 0.f); r.w = fmaf(a[3], g.w, training ? fmaf(b[3], xx.w, d[3]) : 0.f);
         if (dx != nullptr) dx[i] = r;
         if (dx_bf16 != nullptr) dx_bf16[i] = pack_bf16x4(r);
     }

@@ -56,7 +56,7 @@ __device__ __forceinline__ float4 bn_relu4(float4 v, const float (&sc)[4], const
     v.x = fmaf(v.x, sc[0], sh[0]); v.y = fmaf(v.y, sc[1], sh[1]);
     v.z = fmaf(v.z, sc[2], sh[2]); v.w = fmaf(v.w, sc[3], sh[3]);
     if (relu) {
-        v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
+        v.x = relu_nan(v.x); v.y = relu_nan(v.y); v.z = relu_nan(v.z); v.w = relu_nan(v.w);
     }
     return v;
 }

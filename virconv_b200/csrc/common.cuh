@@ -273,4 +273,10 @@ struct WgradFinTable {
 };
 int wgrad_finalize(WgradFinTable& t, cudaStream_t stream);
 
+// ReLU with torch's rules, shared by every kernel that applies one (bn_common.cuh, voxel_pool.cu):
+// forward, torch.relu: NaN stays NaN (fmaxf alone would return 0), -0.0 becomes +0
+__device__ __forceinline__ float relu_nan(float v) { return v != v ? v : fmaxf(v, 0.f); }
+// backward, torch's threshold_backward: the gradient passes unless the activation is <= 0, so it passes at NaN
+__device__ __forceinline__ float relu_grad(float pre, float g) { return pre <= 0.f ? 0.f : g; }
+
 }  // namespace vc

@@ -170,7 +170,8 @@ static int tc_one_image(const float* w, void* img, int cin, int cout, int K, int
 }
 
 static int tc_common(const void* feats_bf16, const float* w, const int32_t* nbr, float* out, int n_rows, int cin, int cout,
-                     int K, int mode, int mirror, double* bn_sums, void* ws, size_t ws_bytes, int32_t* err, cudaStream_t stream) {
+                     int K, int mode, int mirror, double* bn_sums, void* ws, size_t ws_bytes, int32_t* err, cudaStream_t stream,
+                     int in_ld = 0) {
     VC_CHECK_ARG(n_rows >= 0 && K >= 1 && K <= MAXK_TC, "bad n=%d or K=%d", n_rows, K);
     if (!tc2_ch_ok(cin) || !tc2_ch_ok(cout)) {
         set_error("tensor-core conv: unsupported channels cin=%d cout=%d", cin, cout);
@@ -186,13 +187,20 @@ static int tc_common(const void* feats_bf16, const float* w, const int32_t* nbr,
     if (rc) return rc;
     int kc = mode == 0 ? cin : cout, nr = mode == 0 ? cout : cin;
     return tc2_conv(kc, nr, feats_bf16, ws, nbr, n_rows, out, n_rows, nullptr, K, bn_sums, err, stream, nullptr, nullptr,
-                    (mode == 1 && !mirror) ? 1 : 0);
+                    (mode == 1 && !mirror) ? 1 : 0, in_ld);
 }
 
 extern "C" int vc_conv_fwd_tc(const void* in_bf16, const float* w, const int32_t* nbr, float* out, int n_out, int cin,
                               int cout, int K, double* bn_sums, void* ws, size_t ws_bytes, int32_t* err_flag,
                               vc_stream_t stream_) {
     return tc_common(in_bf16, w, nbr, out, n_out, cin, cout, K, 0, 0, bn_sums, ws, ws_bytes, err_flag, (cudaStream_t)stream_);
+}
+
+extern "C" int vc_conv_fwd_tc_ld(const void* in_bf16, int in_ld, const float* w, const int32_t* nbr, float* out, int n_out, int cin,
+                                 int cout, int K, double* bn_sums, void* ws, size_t ws_bytes, int32_t* err_flag,
+                                 vc_stream_t stream_) {
+    return tc_common(in_bf16, w, nbr, out, n_out, cin, cout, K, 0, 0, bn_sums, ws, ws_bytes, err_flag, (cudaStream_t)stream_,
+                     in_ld);
 }
 
 static size_t det_w_bytes(int cin, int cout, int K) {

@@ -18,9 +18,10 @@
 //      mean = W E[r], var = diag(W Cov(r) W^T) (biased).  The query pass accumulates the nine moments
 //      (sum r, sum r r^T) in float64; pool_bn_fold_kernel turns them into the statistics, updates the running ones and
 //      folds BN into p = scale * (W r) + shift.  Eval mode folds the running statistics.
-//   5. v = ReLU(f + p); pooled[m, c] = max_s v, argmax = the FIRST slot attaining it (max_pool2d's rule).
-//   6. Backward: dy = g * [pooled > 0] at the argmax slot.  The feature gradient goes to features_in[row(m, argmax)] for
-//      non-empty balls only (the reference zeroes the grouped features of empty balls in place, :99).  The position branch
+//   5. v = ReLU(f + p) (relu_nan: NaN stays NaN); pooled[m, c] = max_s v, argmax = the FIRST slot attaining it, or the
+//      LAST NaN slot if any (max_pool2d's rule: a slot replaces the maximum when it is larger or NaN).
+//   6. Backward: dy = g * [!(pooled <= 0)] at the argmax slot (relu_grad: a NaN maximum passes g).  The feature gradient
+//      goes to features_in[row(m, argmax)] for non-empty balls only (the reference zeroes the grouped features of empty balls in place, :99).  The position branch
 //      needs only the per-channel sums  sum dy  and  sum dy * r  over the argmax slots (dy is zero everywhere else); with the
 //      forward moments they give dW_pos, dgamma, dbeta including the train-mode BN coupling term (pool_bn_grad_kernel).
 //      No gradient flows to xyz / new_xyz.
@@ -33,7 +34,7 @@
 //      a chunk's points are added by a fixed shared-memory tree into the chunk's own partial; the partials are added in
 //      chunk order in float64.  pool_bn_fold_kernel's arithmetic is unchanged.
 //   D2 feature gradient.  grad_features_in[r, c] = the fp32 sum, in ascending m and from 0.0, of
-//      dy[m, c] = grad_pooled[m, c] * [pooled[m, c] > 0] over the non-empty m with idx[m, argmax[m, c]] == r; plain adds
+//      dy[m, c] = grad_pooled[m, c] * [!(pooled[m, c] <= 0)] over the non-empty m with idx[m, argmax[m, c]] == r; plain adds
 //      (a sequential float32 sum on the CPU gives the same bits).  Every row of [0, N) is written, zero where no slot points.
 //   D3 channel sums.  The [C, 4] float64 sums of dy and dy * r are partials per chunk of DET_CHUNK query points (a fixed
 //      per-thread assignment, a fixed butterfly and a fixed order over the warps), added in chunk order.
@@ -145,8 +146,8 @@ __global__ void __launch_bounds__(PB_THREADS) pool_fwd_kernel(int M, int nsample
 #pragma unroll
         for (int j = 0; j < L::CPL; j++) {
             const float x = w0[j] * rx + w1[j] * ry + w2[j] * rz;
-            const float v = fmaxf(f[j] + (sc[j] * x + sh[j]), 0.f);
-            if (v > best[j]) { best[j] = v; arg[j] = s; }
+            const float v = relu_nan(f[j] + (sc[j] * x + sh[j]));
+            if (v > best[j] || v != v) { best[j] = v; arg[j] = s; }
         }
     }
 #pragma unroll
@@ -178,7 +179,7 @@ __global__ void __launch_bounds__(PB_THREADS) pool_bwd_kernel(int M, int nsample
 #pragma unroll
         for (int j = 0; j < L::CPL; j++) {
             const size_t o = (size_t)pt * C + sub + j * L::LPP;
-            const float dy = pooled[o] > 0.f ? grad_pooled[o] : 0.f;
+            const float dy = relu_grad(pooled[o], grad_pooled[o]);
             if (dy == 0.f) continue;
             acc[j][0] += dy;
             if (emp) continue;
@@ -379,7 +380,7 @@ __global__ void __launch_bounds__(PB_THREADS) pool_grad_rows_det_kernel(int N, i
 #pragma unroll
         for (int j = 0; j < L::CPL; j++) {
             const size_t o = (size_t)m * C + sub + j * L::LPP;
-            if (__ldg(argmax + o) == s) acc[j] = __fadd_rn(acc[j], __ldg(pooled + o) > 0.f ? __ldg(grad_pooled + o) : 0.f);
+            if (__ldg(argmax + o) == s) acc[j] = __fadd_rn(acc[j], relu_grad(__ldg(pooled + o), __ldg(grad_pooled + o)));
         }
     }
 #pragma unroll
@@ -410,7 +411,7 @@ __global__ void __launch_bounds__(PB_THREADS) pool_sums_det_kernel(int M, int ns
 #pragma unroll
             for (int j = 0; j < L::CPL; j++) {
                 const size_t o = (size_t)pt * C + sub + j * L::LPP;
-                const float dy = pooled[o] > 0.f ? grad_pooled[o] : 0.f;
+                const float dy = relu_grad(pooled[o], grad_pooled[o]);
                 if (dy == 0.f) continue;
                 acc[j][0] += dy;
                 if (emp) continue;

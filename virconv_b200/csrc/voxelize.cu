@@ -33,9 +33,11 @@ __device__ __forceinline__ bool point_voxel(const float* __restrict__ p, const V
     bool ok = b >= 0 && b < g.batch;
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
-        // floor((p - lo) / vs) in fp32, the arithmetic of the reference voxeliser
-        int v = (int)floorf(__fdiv_rn(__fsub_rn(p[1 + d], g.lo[d]), g.vs[d]));
-        ok &= (v >= 0) & (v < g.grid[d]);
+        // floor((p - lo) / vs) in fp32, the arithmetic of the reference voxeliser.  A NaN would convert to cell 0 and a point
+        // with a NaN coordinate be kept: the reference's range tests are false for NaN, so it is dropped here too
+        const float q = floorf(__fdiv_rn(__fsub_rn(p[1 + d], g.lo[d]), g.vs[d]));
+        const int v = (int)q;
+        ok &= isfinite(q) & (v >= 0) & (v < g.grid[d]);
         c[d] = v;
     }
     return ok;
@@ -191,6 +193,9 @@ __global__ void __launch_bounds__(1024) vox_offsets_kernel(uint32_t* block_sum, 
     }
 }
 
+// the reference's max over a voxel's slots (torch / numpy max): NaN if either is NaN, where fmaxf would drop it
+__device__ __forceinline__ float max_nan(float a, float b) { return (a != a || b != b) ? a + b : fmaxf(a, b); }
+
 // one thread per point: heads that survive the per-sample cap emit their voxel (coords, count, mean / max features)
 __global__ void __launch_bounds__(256) vox_emit_kernel(const float* __restrict__ pts, int n, int stride, int c, VoxGeom g,
                                                        const int32_t* __restrict__ head_of, const uint32_t* __restrict__ bits,
@@ -223,11 +228,11 @@ __global__ void __launch_bounds__(256) vox_emit_kernel(const float* __restrict__
             sum[ch] = __fadd_rn(sum[ch], v);
             if (out_voxels != nullptr) out_voxels[((size_t)row * max_points + r) * c + ch] = v;
         }
-        mx = first ? q[c - 1] : fmaxf(mx, q[c - 1]);
+        mx = first ? q[c - 1] : max_nan(mx, q[c - 1]);
         first = false;
         ++cnt;
     }
-    if (cnt < max_points) mx = fmaxf(mx, 0.f);
+    if (cnt < max_points) mx = max_nan(mx, 0.f);
     float denom = (float)max(cnt, 1);
     for (int ch = 0; ch < c; ++ch) out_feat[(size_t)row * c + ch] = __fdiv_rn(sum[ch], denom);
     if (vfe_max_last) out_feat[(size_t)row * c + c - 1] = mx;

@@ -553,10 +553,8 @@ extern "C" size_t vc_conv_wgrad_tc_det_ws_bytes(int n_out, int cin, int cout, in
     return (bytes + 255) & ~(size_t)255;
 }
 
-extern "C" int vc_conv_wgrad_tc_det(const void* in_bf16, const void* dout_bf16, const int32_t* nbr, float* dw, int n_out,
-                                    int cin, int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag,
-                                    vc_stream_t stream_) {
-    cudaStream_t stream = (cudaStream_t)stream_;
+static int wgrad_tc_det(const void* in_bf16, int in_ld, const void* dout_bf16, const int32_t* nbr, float* dw, int n_out, int cin,
+                        int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag, cudaStream_t stream) {
     VC_CHECK_ARG(n_out >= 0 && K >= 1 && K <= MAXK_TC && dw, "bad arguments");
     if (!tc2_ch_ok(cin) || !tc2_ch_ok(cout)) {
         set_error("tensor-core wgrad: unsupported channels cin=%d cout=%d", cin, cout);
@@ -575,7 +573,7 @@ extern "C" int vc_conv_wgrad_tc_det(const void* in_bf16, const void* dout_bf16, 
     const size_t pbytes = (size_t)WGRAD_DET_CHUNKS * K * cin * cout * sizeof(float);
     VC_CUDA(cudaMemsetAsync(ws, 0, need, stream));
     int rc = tc3_wgrad(cin, cout, in_bf16, dout_bf16, nbr, n_out, (float*)ws, n_out, nullptr, K, err_flag, stream,
-                       reinterpret_cast<int*>((char*)ws + pbytes), g_wgrad3_ctas > 0 ? g_wgrad3_ctas : num_sms(), 0,
+                       reinterpret_cast<int*>((char*)ws + pbytes), g_wgrad3_ctas > 0 ? g_wgrad3_ctas : num_sms(), in_ld,
                        WGRAD_DET_CHUNKS);
     if (rc) return rc;
     WgradFinTable T;
@@ -583,4 +581,16 @@ extern "C" int vc_conv_wgrad_tc_det(const void* in_bf16, const void* dout_bf16, 
     T.e[0].scratch = (const float*)ws; T.e[0].dw = dw; T.e[0].cin = cin; T.e[0].cout = cout; T.e[0].K = K; T.e[0].first = 0;
     T.e[0].n_part = WGRAD_DET_CHUNKS;
     return wgrad_finalize(T, stream);
+}
+
+extern "C" int vc_conv_wgrad_tc_det(const void* in_bf16, const void* dout_bf16, const int32_t* nbr, float* dw, int n_out,
+                                    int cin, int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag,
+                                    vc_stream_t stream_) {
+    return wgrad_tc_det(in_bf16, 0, dout_bf16, nbr, dw, n_out, cin, cout, K, ws, ws_bytes, err_flag, (cudaStream_t)stream_);
+}
+
+extern "C" int vc_conv_wgrad_tc_det_ld(const void* in_bf16, int in_ld, const void* dout_bf16, const int32_t* nbr, float* dw,
+                                       int n_out, int cin, int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag,
+                                       vc_stream_t stream_) {
+    return wgrad_tc_det(in_bf16, in_ld, dout_bf16, nbr, dw, n_out, cin, cout, K, ws, ws_bytes, err_flag, (cudaStream_t)stream_);
 }
