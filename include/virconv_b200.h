@@ -614,6 +614,20 @@ int vc_part_pool_bwd(const float* rois, const float* g, int B, int N, int ld, in
                      float scale, float* dparts, void* ws, size_t ws_bytes, vc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * RoI grid points of TEDMHead.roi_grid_pool / roi_grid_pool_mm, whose rules csrc/roi_grid.cu states.  No host read;
+ * graph-capturable; every operation rounds once in fp32, as torch's elementwise kernels do.
+ *   vc_roi_grid_points <- get_global_grid_points_of_roi (ted_head.py:652-673) and the voxel coordinates of the grid
+ *                         points (:481-485, :528-532) for all scenes and S feature sources in one launch: rois [B, N, ld]
+ *                         (ld >= 7) fp32 contiguous, grid size G (1..64), range3 = point_cloud_range[0:3] and voxel3 =
+ *                         voxel_size as float32 (host), strides [S] (host, >= 1) -> new_xyz [B*N*G^3, 3] fp32 and
+ *                         new_coords [S, B*N*G^3, 4] int32 as (b, x, y, z).
+ *   S > VC_ROI_GRID_MAX_SOURCES -> VC_ERR_UNSUPPORTED.
+ * ---------------------------------------------------------------------------------------------- */
+#define VC_ROI_GRID_MAX_SOURCES 4
+int vc_roi_grid_points(const float* rois, int B, int N, int ld, int G, const float* range3, const float* voxel3,
+                       const int32_t* strides, int S, float* new_xyz, int* new_coords, vc_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Parameter update of the adam_onecycle / adam_cosin step (csrc/optim.cu): what the reference's loop does after
  * loss.backward() (tools/train_utils/train_utils.py:50-52: clip_grad_norm_, OptimWrapper.step of fastai_optim.py:132-149
  * over torch.optim.Adam) for EVERY parameter tensor in two launches.  No host read, no allocation; graph-capturable;

@@ -30,7 +30,9 @@ FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-line
 # part_pool.cu: no contraction, so that the sample positions and bilinear weights round every operation once, as torch's
 # elementwise kernels and grid_sample do
 # optim.cu: no contraction, so that every fp32 operation of the update rounds once, as torch's elementwise kernels do
-FILE_FLAGS = {'iou3d_nms.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
+# roi_grid.cu: no contraction, so that the grid points and their floor divisions round every operation once, as torch's
+# elementwise kernels do
+FILE_FLAGS = {'roi_grid.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],'iou3d_nms.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
               'optim.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
               'anchor_targets.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
               'roi_targets.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],

@@ -36,6 +36,9 @@ read apart from the one copy of the tb values.
 With `use_fused_part_pool` `TEDMHead.obtain_conf_preds` is this package's drop-in method (virconv_b200.part_pool): the
 PART branch's position-sensitive RoI pooling of VirConv-T / -S in one call per stage, without a host read, with a
 bit-reproducible part-map gradient.
+With `use_fused_roi_grid` `TEDMHead.roi_grid_pool` and `roi_grid_pool_mm` are this package's drop-in methods
+(virconv_b200.roi_grid): the grid points and their voxel coordinates in one launch per call, and the voxel -> row map and
+voxel centres of each published tensor built once per forward, without a host read.
 With `use_fused_optimizer` `train_utils.optimization.build_optimizer` (tools/train_utils/optimization/__init__.py:11-36, the
 name tools/train.py imports with tools/ on sys.path) returns this package's optim.FusedAdamOneCycle for OPTIMIZER
 adam_onecycle / adam_cosin and calls the reference's function for every other value, and the `clip_grad_norm_` name
@@ -258,7 +261,7 @@ def _fused_clip_grad_norm_(parameters, max_norm, *args, **kwargs):
 
 
 def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=False, use_fused_rpn_targets=False,
-            use_fused_roi_targets=False, use_fused_losses=False, use_fused_part_pool=False, use_fused_optimizer=False):
+            use_fused_roi_targets=False, use_fused_losses=False, use_fused_part_pool=False, use_fused_optimizer=False, use_fused_roi_grid=False):
     """Register everything listed in the module docstring.  `reference_root`: put that checkout first on sys.path."""
     if reference_root is not None and reference_root not in sys.path:
         sys.path.insert(0, reference_root)
@@ -355,6 +358,15 @@ def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=F
         if ted.obtain_conf_preds is not part_pool.obtain_conf_preds:
             part_pool._reference_obtain_conf_preds = ted.obtain_conf_preds
         ted.obtain_conf_preds = part_pool.obtain_conf_preds
+    if use_fused_roi_grid:
+        from . import roi_grid
+        ted = importlib.import_module('pcdet.models.roi_heads.ted_head').TEDMHead
+        if ted.roi_grid_pool is not roi_grid.roi_grid_pool:
+            roi_grid._reference_roi_grid_pool = ted.roi_grid_pool
+        if ted.roi_grid_pool_mm is not roi_grid.roi_grid_pool_mm:
+            roi_grid._reference_roi_grid_pool_mm = ted.roi_grid_pool_mm
+        ted.roi_grid_pool = roi_grid.roi_grid_pool
+        ted.roi_grid_pool_mm = roi_grid.roi_grid_pool_mm
     if use_fused_optimizer:
         import os
         tools = os.path.join(reference_root, 'tools') if reference_root is not None else None
