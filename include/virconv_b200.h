@@ -62,6 +62,14 @@ int vc_set_tc_variant(int variant);
  * ring of >= 2 stages in half the shared memory), 1 or 2 = forced.  The cooperative conv + BN grid keeps one CTA per SM
  * unless 2 is forced. */
 int vc_conv_tc2_config(int ctas_per_sm);
+/* How the plan executor's forward builds the output sets of chained strided convs (each one's input set is the previous
+ * one's output set, no layer discard between them; csrc/rulebook.cu header): 1 (default) = all of them from the first
+ * input set in one composed pass, exact mode reading all their row counts with one synchronise; 0 = each from the previous
+ * one's emitted indices, one read-back per conv in exact mode (the path every other plan takes).  Same index sets, counts
+ * and tables in both (except after a capacity overflow: see the header of csrc/rulebook.cu); VC_ERR_INVALID for another
+ * value.  Environment VIRCONV_INDEX_ORDER at load time.  Read when a
+ * forward is enqueued (a captured graph keeps its choice). */
+int vc_set_index_order(int mode);
 /* The plan executor's weight-gradient launches (csrc/wgrad_tc3.cu): variant must be 1 (the only kernel); max_ctas caps
  * their CTAs (0, the default: half the SMs, so that each shares its SM with a dgrad CTA of the main stream). */
 int vc_conv_wgrad_tc3_config(int variant, int max_ctas);

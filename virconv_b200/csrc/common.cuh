@@ -143,6 +143,32 @@ int conv_rulebook_fill_phases(const int32_t* indices, int n, const int* n_dev, i
                               const int32_t* spatial_shape, const int32_t* ksize, const int32_t* stride, const int32_t* padding,
                               const int32_t* dilation, int n_out, int32_t* out_indices, int32_t* nbr_fwd, int32_t* nbr_bwd,
                               int32_t* pair_num, void* ws, size_t ws_bytes, cudaStream_t stream, int phases);
+// where a strided conv's output bitmap and its ranks lie: in the workspace of vc_conv_rulebook_count (conv_rank_of) or in
+// that of a chain of strided convs (conv_chain_rank)
+struct ConvRank {
+    const uint32_t *bitmap, *word_rank, *block_sum;
+};
+ConvRank conv_rank_of(int ndim, int batch_size, const int32_t* out_shape, const void* ws);
+// nbr_fwd (-1 filled here) / nbr_bwd / pair counts of one strided conv from its ranked output bitmap
+int conv_rulebook_tables_dev(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size, const int32_t* spatial_shape,
+                             const int32_t* ksize, const int32_t* stride, const int32_t* padding, const int32_t* dilation, int n_out,
+                             ConvRank rank, int32_t* nbr_fwd, int32_t* nbr_bwd, int32_t* pair_num, cudaStream_t stream);
+// L chained strided convs (rulebook.cu header: each level's input set is the previous level's output set): every level's
+// output set from the first input set, in one mark + scan pass and one emit
+constexpr int CONV_CHAIN_MAX = 4;
+struct ConvChain {
+    int L, ndim, batch;
+    const int32_t* shape0;   // input spatial shape of level 0; level l + 1's is level l's output shape
+    const int32_t *ksize[CONV_CHAIN_MAX], *stride[CONV_CHAIN_MAX], *pad[CONV_CHAIN_MAX], *dil[CONV_CHAIN_MAX];
+};
+bool conv_chain_composable(const ConvChain& ch);   // dilation 1 everywhere (the rule needs it), 2 <= L <= CONV_CHAIN_MAX
+size_t conv_chain_ws_bytes(const ConvChain& ch);
+ConvRank conv_chain_rank(const ConvChain& ch, const void* ws, int level);
+// n_out_dev [L]: each level's row count; caps (NULL: no clamp) [L]: capacities, a larger count is clamped and reported
+int conv_chain_count_dev(const ConvChain& ch, const int32_t* indices, int n, const int* n_dev, int32_t* n_out_dev, const int* caps,
+                         int* overflow, void* ws, size_t ws_bytes, cudaStream_t stream);
+// out_idx [L]: output index buffers of caps[l] rows
+int conv_chain_emit_dev(const ConvChain& ch, int32_t* const* out_idx, const int* caps, void* ws, size_t ws_bytes, cudaStream_t stream);
 
 // ---- bn.cu / misc.cu internals used by the plan executor (device row counts, strided outputs) ----
 int bn_apply_relu_dev(const float* x, const double* sums, int n_rows, const int* n_dev, int c, const float* gamma,

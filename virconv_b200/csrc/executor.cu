@@ -123,6 +123,11 @@ constexpr int EV_POOL = 512;   // > the events of one forward / backward call: t
 cudaEvent_t g_ev[EV_POOL];
 int g_ev_dev = -1, g_ev_next = 0;
 
+// How the forward builds the output sets of chained strided convs (vc_set_index_order, VIRCONV_INDEX_ORDER): 1 (default)
+// composed in one pass (fwd_conv_chain); 0 each from the previous one's (count -> read-back -> emit per conv), the path
+// every other plan takes and the reference the tests compare the composed pass with.
+int g_index_order = 1;
+
 int ev_init() {
     int dev = 0;
     VC_CUDA(cudaGetDevice(&dev));
@@ -317,8 +322,8 @@ struct FwdCtx : Ctx {
     int32_t *overflow, *pinned;
     int n_syncs, last_ev[3] = {-1, -1, -1};   // last_ev: latest event of each side stream (joined into main at the end)
     bool do_idx, do_feat, two;   // do_idx / do_feat: enqueue the index / feature operators (both unless phased)
-    // per strided conv op: the workspace its count, indices and tables phases share; done: count and indices are enqueued
-    struct { void* ws; size_t wsb; bool done; } chain[MAX_OPS];
+    // per strided conv op: where its ranked output bitmap lies (for the tables); done: count and indices are enqueued
+    struct { ConvRank rank; bool done; } chain[MAX_OPS];
     template <class T>
     void produced(T& r, int s) {   // r was written on stream s: consumers on the other streams wait for r.ev
         r.prod = s;
@@ -456,7 +461,7 @@ int fwd_conv_count(FwdCtx& C, int j) {
         VC_TRY(conv_rulebook_fill_phases(I.idx, I.n, I.n_dev, I.ndim, C.S->batch_size, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL,
                                          n_out, O.idx, nullptr, nullptr, nullptr, ws, wsb, st, 1));
     C.produced(O, s);
-    C.chain[j] = {ws, wsb, true};
+    C.chain[j] = {conv_rank_of(I.ndim, C.S->batch_size, oshape, ws), true};
     return VC_OK;
 }
 
@@ -532,11 +537,85 @@ int fwd_discard(FwdCtx& C, int i, const int* o) {
     return VC_OK;
 }
 
+// The strided convs chained from op i (each one's input set is the previous one's output set, no layer discard in the plan
+// between them): every level's count and output indices in one composed pass (rulebook.cu), one host read in exact mode.
+// Leaves C.chain[i].done unset where the rule does not apply (a single conv, a dilation); the caller then takes the
+// per-level path.
+int fwd_conv_chain(FwdCtx& C, int i) {
+    const int* o0 = C.op(i);
+    ISet& I = C.S->iset[o0[F_A]];
+    int ops[CONV_CHAIN_MAX];
+    ConvChain ch{};
+    for (int j = i, cur = o0[F_A]; j < C.n_ops && ch.L < CONV_CHAIN_MAX; ++j) {
+        const int* o = C.op(j);
+        if (o[F_KIND] == OP_DISCARD) break;
+        if (o[F_KIND] != OP_CONV_RB) continue;
+        if (o[F_A] != cur || o[F_NDIM] != o0[F_NDIM] || C.chain[j].done) break;
+        ops[ch.L] = j;
+        ch.ksize[ch.L] = o + F_KS; ch.stride[ch.L] = o + F_ST; ch.pad[ch.L] = o + F_PD; ch.dil[ch.L] = o + F_DL;
+        ++ch.L;
+        cur = o[F_B];
+    }
+    ch.ndim = I.ndim; ch.batch = C.S->batch_size; ch.shape0 = I.shape;
+    if (!I.idx || I.ndim != o0[F_NDIM] || !conv_chain_composable(ch)) return VC_OK;
+    const int s = C.two ? o0[F_STREAM] : 0;
+    cudaStream_t st = C.st[s];
+    VC_TRY(wait_for(C, I.ev, I.prod, s));
+    const size_t wsb = conv_chain_ws_bytes(ch);
+    VC_CHECK_ARG(wsb > 0, "op %d: bad chain of strided convs", i);
+    VC_ALLOC(ws, void*, wsb);
+    VC_ALLOC(n_dev, int32_t*, 4 * CONV_CHAIN_MAX);
+    int n_out[CONV_CHAIN_MAX];
+    int32_t* oidx[CONV_CHAIN_MAX];
+    if (C.S->is_static) {
+        for (int l = 0; l < ch.L; ++l) {
+            n_out[l] = C.caps[C.op(ops[l])[F_B]];
+            VC_CHECK_ARG(n_out[l] > 0, "op %d: static mode needs a capacity for index set %d", ops[l], C.op(ops[l])[F_B]);
+        }
+        if (C.do_idx) VC_TRY(conv_chain_count_dev(ch, I.idx, I.n, I.n_dev, n_dev, n_out, C.overflow, ws, wsb, st));
+    } else {
+        VC_TRY(conv_chain_count_dev(ch, I.idx, I.n, nullptr, n_dev, nullptr, nullptr, ws, wsb, st));
+        VC_CUDA(cudaMemcpyAsync(C.pinned + 8, n_dev, 4 * ch.L, cudaMemcpyDeviceToHost, st));
+        // (the pipeline-timeout flag rides along with the first read-back of a step, as in fwd_conv_count)
+        if (C.n_syncs == 0 && C.err != nullptr) VC_CUDA(cudaMemcpyAsync(C.pinned + 15, C.err, 4, cudaMemcpyDeviceToHost, st));
+        VC_CUDA(cudaStreamSynchronize(st));        // the data-dependent sizes of all the chain's convs at once
+        for (int l = 0; l < ch.L; ++l) n_out[l] = C.pinned[8 + l];
+        if (C.n_syncs == 0 && C.err != nullptr && C.pinned[15] != 0) {
+            set_error("a tensor-core kernel's pipeline wait timed out in an earlier step (error flag %d): its results are invalid",
+                      C.pinned[15]);
+            return VC_ERR_PIPELINE;
+        }
+        ++C.n_syncs;
+    }
+    for (int l = 0; l < ch.L; ++l) {
+        const int* o = C.op(ops[l]);
+        ISet& In = C.S->iset[o[F_A]];
+        ISet& O = C.S->iset[o[F_B]];
+        RBk& R = C.S->rb[o[F_C]];
+        int32_t oshape[3] = {0, 0, 0};
+        VC_TRY(vc_conv_out_shape(In.ndim, In.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL, oshape));
+        R.n_in = In.n; R.n_out = n_out[l];
+        R.n_in_dev = In.n_dev; R.n_out_dev = C.S->is_static ? n_dev + l : nullptr;
+        O.n = n_out[l]; O.ndim = In.ndim; O.n_dev = R.n_out_dev;
+        for (int d = 0; d < 3; ++d) O.shape[d] = oshape[d];
+        VC_ALLOC(oi, int32_t*, (size_t)(n_out[l] > 0 ? n_out[l] : 1) * (1 + In.ndim) * 4);
+        O.idx = oidx[l] = oi;
+        if (C.S->is_static && C.do_idx) VC_CUDA(cudaMemsetAsync(oi, 0xFF, (size_t)n_out[l] * (1 + In.ndim) * 4, st));
+        C.chain[ops[l]] = {conv_chain_rank(ch, ws, l), true};
+    }
+    if (C.do_idx) VC_TRY(conv_chain_emit_dev(ch, oidx, n_out, ws, wsb, st));
+    for (int l = 0; l < ch.L; ++l) C.produced(C.S->iset[C.op(ops[l])[F_B]], s);
+    return VC_OK;
+}
+
 int fwd_conv_rb(FwdCtx& C, int i, const int* o, int s) {
-    // First strided conv reached: run the count -> (host reads the row count) -> emit-indices chain of EVERY strided conv of
-    // the plan now, back to back.  Each link only needs the previous link's output indices, and it is the only part of the
-    // forward the host has to wait for; the neighbour tables, submanifold rulebooks and projections queue up behind it
-    // without further synchronisation.
+    // First strided conv reached: the strided convs chained from it get their counts and output indices from one composed
+    // pass (fwd_conv_chain).  Where that rule does not apply (a layer discard between two strided convs, a dilation, a
+    // single conv) or vc_set_index_order(0) asks for it, the loop below is the fallback: the count -> (host reads the row
+    // count) -> emit-indices chain of EVERY strided conv of the plan, back to back.  Each link only needs the previous
+    // link's output indices, and it is the only part of the forward the host has to wait for; the neighbour tables,
+    // submanifold rulebooks and projections queue up behind it without further synchronisation.
+    if (!C.chain[i].done && g_index_order == 1) VC_TRY(fwd_conv_chain(C, i));
     if (!C.chain[i].done) {
         if (C.S->is_static) {
             // no host read to wait for: keep the natural order (count -> indices -> tables per stage), so the tables of an
@@ -562,8 +641,8 @@ int fwd_conv_rb(FwdCtx& C, int i, const int* o, int s) {
     VC_ALLOC(pn, int32_t*, (size_t)R.K * 4);
     R.nbr = nbr; R.nbr_bwd = nbr_bwd; R.pair_num = pn;
     if (C.do_idx)
-        VC_TRY(conv_rulebook_fill_phases(I.idx, I.n, I.n_dev, I.ndim, C.S->batch_size, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL,
-                                         R.n_out, O.idx, R.nbr, R.nbr_bwd, R.pair_num, C.chain[i].ws, C.chain[i].wsb, C.st[s], 2));
+        VC_TRY(conv_rulebook_tables_dev(I.idx, I.n, I.n_dev, I.ndim, C.S->batch_size, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL,
+                                        R.n_out, C.chain[i].rank, R.nbr, R.nbr_bwd, R.pair_num, C.st[s]));
     C.produced(R, s);
     return VC_OK;
 }
@@ -913,6 +992,12 @@ extern "C" int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, 
         if (C.two && C.last_ev[s] >= 0) VC_CUDA(cudaStreamWaitEvent(C.st[0], g_ev[C.last_ev[s]], 0));   // join
     S->used = C.A.used;
     S->magic = STATE_MAGIC;
+    return VC_OK;
+}
+
+extern "C" int vc_set_index_order(int mode) {
+    VC_CHECK_ARG(mode == 0 || mode == 1, "index order must be 0 or 1");
+    g_index_order = mode;
     return VC_OK;
 }
 

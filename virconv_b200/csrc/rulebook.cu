@@ -11,6 +11,21 @@
 //             (ws of vc_conv_rulebook_*) — gives the sorted, duplicate-free output set with no sort.
 // Roofline: all kernels here are HBM/L2-latency bound integer work (no FLOPs); algorithmic bytes per
 // input voxel are stated in DESIGN.md §kernels.
+//
+// Chained strided convs (conv_chain_*): L <= 4 regular convs where each one's input set is the previous one's output set
+// (no layer discard between them).  Their output sets are built from the FIRST input set in one pass instead of L
+// dependent count -> scan -> emit rounds.  Composition rule: with dilation 1, input coordinate c reaches output coordinate o
+// of a level exactly when o * stride lies in [c + pad - (ksize - 1), c + pad] and 0 <= o < oshape, and the grid test and
+// the window factor per dimension (the batch index passes through).  So the level-1 cells reached from one input voxel are
+// a product of per-dimension integer intervals; the cells reached from an interval [lo, hi] are again one interval
+// (c + pad - off covers [lo + pad - ksize + 1, hi + pad] without a hole, so every multiple of the stride in it is hit), and
+// the union over a product of intervals is the product of the per-dimension unions.  Level l's output set is therefore the
+// union over input voxels of one product of intervals, computed level by level from the voxel's own coordinates: exactly
+// the set the per-level chain builds from the previous level's emitted indices, marked into the same bitmap and ranked in
+// the same order (so every index set, count and table is bit-identical).  One exception, only when a capacity is too small:
+// the per-level chain derives level l + 1 from the first `cap` rows of an overflowing level l, the composed pass from all of
+// its cells, so the counts of the levels AFTER the first overflowing one may be larger (the overflow is reported either way
+// and such a step is recomputed with larger capacities).
 #include "common.cuh"
 
 namespace vc {
@@ -223,10 +238,10 @@ __global__ void __launch_bounds__(256) scan_local_kernel(const uint32_t* __restr
 
 // single block: exclusive scan of block sums in place; total -> n_out
 // (cap > 0: the output buffers hold `cap` rows; a larger total is clamped and reported through *overflow)
-__global__ void __launch_bounds__(1024) scan_blocks_kernel(uint32_t* block_sum, int n_blocks, int32_t* n_out, int cap,
-                                                           int* overflow) {
+__device__ __forceinline__ void scan_segment(uint32_t* block_sum, int n_blocks, int32_t* n_out, int cap, int* overflow) {
     __shared__ uint32_t warp_tot[32];
     __shared__ uint32_t carry_s;
+    __syncthreads();   // (a previous segment's thread 0 has read carry_s)
     if (threadIdx.x == 0) carry_s = 0;
     __syncthreads();
     for (int base = 0; base < n_blocks; base += 1024) {
@@ -258,6 +273,11 @@ __global__ void __launch_bounds__(1024) scan_blocks_kernel(uint32_t* block_sum, 
     }
 }
 
+__global__ void __launch_bounds__(1024) scan_blocks_kernel(uint32_t* block_sum, int n_blocks, int32_t* n_out, int cap,
+                                                           int* overflow) {
+    scan_segment(block_sum, n_blocks, n_out, cap, overflow);
+}
+
 __device__ __forceinline__ int cell_rank(const uint32_t* __restrict__ bitmap, const uint32_t* __restrict__ word_rank,
                                          const uint32_t* __restrict__ block_sum, long long lin) {
     long long w = lin >> 5;
@@ -284,6 +304,96 @@ __global__ void conv_emit_indices_kernel(const uint32_t* __restrict__ bitmap, co
             lin /= g.oshape[d];
         }
         int32_t* o = out_idx + (size_t)row * (1 + g.ndim);
+        o[0] = (int32_t)lin;
+        for (int d = 0; d < g.ndim; ++d) o[1 + d] = c[d];
+        ++row;
+    }
+}
+
+// chained strided convs (file header): per level the geometry, where its bitmap / ranks start in the concatenated
+// workspace (w0 words, b0 scan blocks: every level starts on a SCAN_WORDS boundary, so a scan block never spans two
+// levels), and for the emit its output buffer and capacity.  Passed by value.
+struct ChainDesc {
+    int L;
+    Geom g[CONV_CHAIN_MAX];
+    long long w0[CONV_CHAIN_MAX + 1];
+    int b0[CONV_CHAIN_MAX + 1];
+    int32_t* out_idx[CONV_CHAIN_MAX];
+    int cap[CONV_CHAIN_MAX];
+};
+
+// The chain's kernels overload the per-level ones they stand for (conv_mark / scan_blocks / conv_emit_indices), so that a
+// profile names them alike.
+// grid (rows, L): the cells of level blockIdx.y reached from one input row, the product of its per-dimension intervals
+__global__ void conv_mark_kernel(const int32_t* __restrict__ idx, int n, const int* __restrict__ n_dev, ChainDesc cd,
+                                  uint32_t* bitmap) {
+    if (n_dev != nullptr) n = min(n, __ldg(n_dev));
+    const int row = blockIdx.x * blockDim.x + threadIdx.x;
+    if (row >= n) return;
+    const int level = blockIdx.y;
+    int b, lo[VC_MAX_NDIM], hi[VC_MAX_NDIM];
+    load_index(idx, row, cd.g[0].ndim, b, lo);
+    if (!index_ok(cd.g[0], b, lo)) return;
+    for (int d = 0; d < cd.g[0].ndim; ++d) hi[d] = lo[d];
+    for (int l = 0; l <= level; ++l) {
+        const Geom& g = cd.g[l];
+        for (int d = 0; d < g.ndim; ++d) {
+            const int first = lo[d] + g.pad[d] - (g.ksize[d] - 1), last = hi[d] + g.pad[d];   // o * stride in [first, last]
+            const int olo = first <= 0 ? 0 : (first + g.stride[d] - 1) / g.stride[d];
+            const int ohi = last < 0 ? -1 : min(last / g.stride[d], g.oshape[d] - 1);
+            if (olo > ohi) return;   // no cell at this level, hence none further down
+            lo[d] = olo;
+            hi[d] = ohi;
+        }
+    }
+    const Geom& g = cd.g[level];
+    uint32_t* bm = bitmap + cd.w0[level];
+    int c[VC_MAX_NDIM];
+    for (int d = 0; d < g.ndim; ++d) c[d] = lo[d];
+    while (true) {
+        long long lin = b;
+        for (int d = 0; d < g.ndim; ++d) lin = lin * g.oshape[d] + c[d];
+        const uint32_t bit = 1u << (lin & 31);
+        uint32_t* w = bm + (lin >> 5);
+        if (!(*w & bit)) atomicOr(w, bit);
+        int d = g.ndim - 1;   // next cell of the product, last dimension fastest
+        while (d >= 0 && c[d] == hi[d]) { c[d] = lo[d]; --d; }
+        if (d < 0) break;
+        ++c[d];
+    }
+}
+
+// one block: the scan of each level's block sums as its own segment, each level's count clamped to its capacity
+__global__ void __launch_bounds__(1024) scan_blocks_kernel(uint32_t* block_sum, ChainDesc cd, int32_t* n_out,
+                                                                 int* overflow) {
+    for (int l = 0; l < cd.L; ++l)
+        scan_segment(block_sum + cd.b0[l], cd.b0[l + 1] - cd.b0[l], n_out + l, cd.cap[l], overflow);
+}
+
+// one thread per word of all levels (conv_emit_indices_kernel over the level the word belongs to)
+__global__ void conv_emit_indices_kernel(const uint32_t* __restrict__ bitmap, const uint32_t* __restrict__ word_rank,
+                                  const uint32_t* __restrict__ block_sum, ChainDesc cd) {
+    const long long w = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (w >= cd.w0[cd.L]) return;
+    uint32_t word = bitmap[w];
+    if (!word) return;
+    int l = 0;
+    while (w >= cd.w0[l + 1]) ++l;
+    const Geom& g = cd.g[l];
+    const long long wl = w - cd.w0[l];
+    int row = (int)(block_sum[cd.b0[l] + wl / SCAN_WORDS] + word_rank[w]);
+    const int cap = cd.cap[l];
+    while (word) {
+        int bit = __ffs(word) - 1;
+        word &= word - 1;
+        if (row >= cap) return;
+        long long lin = (wl << 5) + bit;
+        int c[VC_MAX_NDIM];
+        for (int d = g.ndim - 1; d >= 0; --d) {
+            c[d] = (int)(lin % g.oshape[d]);
+            lin /= g.oshape[d];
+        }
+        int32_t* o = cd.out_idx[l] + (size_t)row * (1 + g.ndim);
         o[0] = (int32_t)lin;
         for (int d = 0; d < g.ndim; ++d) o[1 + d] = c[d];
         ++row;
@@ -550,6 +660,22 @@ int vc::conv_rulebook_fill_phases(const int32_t* indices, int n, const int* n_de
         VC_LAUNCH_CHECK();
     }
     if (!(phases & 2)) return VC_OK;
+    return conv_rulebook_tables_dev(indices, n, n_dev, ndim, batch_size, spatial_shape, ksize, stride, padding, dilation, n_out,
+                                    ConvRank{w.bitmap, w.word_rank, w.block_sum}, nbr_fwd, nbr_bwd, pair_num, stream);
+}
+
+ConvRank vc::conv_rank_of(int ndim, int batch_size, const int32_t* out_shape, const void* ws) {
+    ConvWs w = conv_ws_layout(ndim, batch_size, out_shape, const_cast<void*>(ws));
+    return ConvRank{w.bitmap, w.word_rank, w.block_sum};
+}
+
+int vc::conv_rulebook_tables_dev(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size,
+                                 const int32_t* spatial_shape, const int32_t* ksize, const int32_t* stride, const int32_t* padding,
+                                 const int32_t* dilation, int n_out, ConvRank rank, int32_t* nbr_fwd, int32_t* nbr_bwd,
+                                 int32_t* pair_num, cudaStream_t stream) {
+    Geom g;
+    int rc = make_geom(g, ndim, batch_size, spatial_shape, ksize, stride, padding, dilation);
+    if (rc) return rc;
     if (pair_num) VC_CUDA(cudaMemsetAsync(pair_num, 0, sizeof(int32_t) * g.K, stream));
     if (n_out > 0) {
         VC_CHECK_ARG(nbr_fwd, "null output pointer");
@@ -557,10 +683,106 @@ int vc::conv_rulebook_fill_phases(const int32_t* indices, int n, const int* n_de
     }
     if (n > 0) {
         VC_CHECK_ARG(nbr_bwd, "null nbr_bwd");
-        conv_tables_kernel<<<dim3(cdiv(n, 256), g.K), 256, 0, stream>>>(indices, n, n_dev, n_out, g, w.bitmap, w.word_rank, w.block_sum,
-                                                             nbr_fwd, nbr_bwd, pair_num);
+        conv_tables_kernel<<<dim3(cdiv(n, 256), g.K), 256, 0, stream>>>(indices, n, n_dev, n_out, g, rank.bitmap, rank.word_rank,
+                                                                         rank.block_sum, nbr_fwd, nbr_bwd, pair_num);
         VC_LAUNCH_CHECK();
     }
+    return VC_OK;
+}
+
+namespace {
+// the chain's geometry and workspace layout: bitmap [W words], word ranks [W], block sums [B], W = cd.w0[L], B = cd.b0[L]
+struct ChainWs {
+    uint32_t *bitmap, *word_rank, *block_sum;
+    size_t bytes;
+};
+int chain_layout(const ConvChain& ch, ChainDesc& cd, ChainWs& w, const void* ws) {
+    VC_CHECK_ARG(ch.L >= 1 && ch.L <= CONV_CHAIN_MAX, "chain of %d strided convs", ch.L);
+    memset(&cd, 0, sizeof(cd));
+    cd.L = ch.L;
+    const int32_t* shape = ch.shape0;
+    for (int l = 0; l < ch.L; ++l) {
+        int rc = make_geom(cd.g[l], ch.ndim, ch.batch, shape, ch.ksize[l], ch.stride[l], ch.pad[l], ch.dil[l]);
+        if (rc) return rc;
+        for (int d = 0; d < ch.ndim; ++d) VC_CHECK_ARG(cd.g[l].dil[d] == 1, "chained strided convs need dilation 1");
+        shape = cd.g[l].oshape;
+        long long cells = ch.batch;
+        for (int d = 0; d < ch.ndim; ++d) cells *= cd.g[l].oshape[d];
+        const long long words = (cells + 31) / 32;
+        const int blocks = (int)((words + SCAN_WORDS - 1) / SCAN_WORDS);
+        cd.b0[l + 1] = cd.b0[l] + blocks;
+        cd.w0[l + 1] = cd.w0[l] + (long long)blocks * SCAN_WORDS;
+    }
+    VC_CHECK_ARG(cd.w0[ch.L] < (1LL << 31), "output grids too large");
+    const size_t a = ((size_t)cd.w0[ch.L] * 4 + 255) / 256 * 256, b = ((size_t)cd.b0[ch.L] * 4 + 255) / 256 * 256;
+    char* p = (char*)const_cast<void*>(ws);
+    w.bitmap = (uint32_t*)p;
+    w.word_rank = (uint32_t*)(p + a);
+    w.block_sum = (uint32_t*)(p + 2 * a);
+    w.bytes = 2 * a + b;
+    return VC_OK;
+}
+}  // namespace
+
+bool vc::conv_chain_composable(const ConvChain& ch) {
+    if (ch.L < 2 || ch.L > CONV_CHAIN_MAX) return false;
+    for (int l = 0; l < ch.L; ++l)
+        for (int d = 0; d < ch.ndim; ++d)
+            if (ch.dil[l][d] != 1) return false;
+    return true;
+}
+
+size_t vc::conv_chain_ws_bytes(const ConvChain& ch) {
+    ChainDesc cd;
+    ChainWs w;
+    return chain_layout(ch, cd, w, nullptr) == VC_OK ? w.bytes : 0;
+}
+
+ConvRank vc::conv_chain_rank(const ConvChain& ch, const void* ws, int level) {
+    ChainDesc cd;
+    ChainWs w;
+    if (chain_layout(ch, cd, w, ws) != VC_OK) return ConvRank{nullptr, nullptr, nullptr};
+    return ConvRank{w.bitmap + cd.w0[level], w.word_rank + cd.w0[level], w.block_sum + cd.b0[level]};
+}
+
+int vc::conv_chain_count_dev(const ConvChain& ch, const int32_t* indices, int n, const int* n_dev, int32_t* n_out_dev, const int* caps,
+                             int* overflow, void* ws, size_t ws_bytes, cudaStream_t stream) {
+    ChainDesc cd;
+    ChainWs w;
+    int rc = chain_layout(ch, cd, w, ws);
+    if (rc) return rc;
+    VC_CHECK_ARG(n >= 0 && n_out_dev && ws, "bad arguments");
+    if (ws_bytes < w.bytes) {
+        set_error("conv chain workspace %zu < %zu", ws_bytes, w.bytes);
+        return VC_ERR_WORKSPACE;
+    }
+    for (int l = 0; l < ch.L; ++l) cd.cap[l] = caps ? caps[l] : 0;
+    VC_CUDA(cudaMemsetAsync(w.bitmap, 0, (size_t)cd.w0[ch.L] * 4, stream));
+    if (n > 0) {
+        conv_mark_kernel<<<dim3(cdiv(n, 256), ch.L), 256, 0, stream>>>(indices, n, n_dev, cd, w.bitmap);
+        VC_LAUNCH_CHECK();
+    }
+    scan_local_kernel<<<cd.b0[ch.L], 256, 0, stream>>>(w.bitmap, cd.w0[ch.L], w.word_rank, w.block_sum);
+    VC_LAUNCH_CHECK();
+    scan_blocks_kernel<<<1, 1024, 0, stream>>>(w.block_sum, cd, n_out_dev, overflow);
+    VC_LAUNCH_CHECK();
+    return VC_OK;
+}
+
+int vc::conv_chain_emit_dev(const ConvChain& ch, int32_t* const* out_idx, const int* caps, void* ws, size_t ws_bytes,
+                            cudaStream_t stream) {
+    ChainDesc cd;
+    ChainWs w;
+    int rc = chain_layout(ch, cd, w, ws);
+    if (rc) return rc;
+    VC_CHECK_ARG(ws && ws_bytes >= w.bytes, "conv chain workspace too small");
+    for (int l = 0; l < ch.L; ++l) {
+        VC_CHECK_ARG(caps[l] <= 0 || out_idx[l], "null output pointer");
+        cd.out_idx[l] = out_idx[l];
+        cd.cap[l] = caps[l];
+    }
+    conv_emit_indices_kernel<<<cdiv(cd.w0[ch.L], 256), 256, 0, stream>>>(w.bitmap, w.word_rank, w.block_sum, cd);
+    VC_LAUNCH_CHECK();
     return VC_OK;
 }
 
