@@ -636,6 +636,34 @@ int vc_roi_grid_points(const float* rois, int B, int N, int ld, int G, const flo
                        const int32_t* strides, int S, float* new_xyz, int* new_coords, vc_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Box decoding of the heads and TEDMHead's cascade stage transforms, whose rules csrc/box_decode.cu states.  One launch
+ * per call, all scenes in one grid; no host read; graph-capturable; every fp32 operation rounds once, as torch's
+ * elementwise kernels do.  All tensors fp32, contiguous, on the device.
+ *   vc_anchor_decode     <- AnchorHeadTemplate.generate_predicted_boxes (anchor_head_template.py:335-382), ResidualCoder
+ *                           with 7 codes: box_preds [B, A, 7], dir_cls [B, A, NB] (NULL: no direction classifier),
+ *                           anchors [A, 7] shared by the scenes, DIR_OFFSET, DIR_LIMIT_OFFSET and period = 2 pi /
+ *                           NUM_DIR_BINS as float32 -> out [B, A, 7].
+ *   vc_anchor_decode_bwd <- its gradient with respect to box_preds: grad [B, A, 7] -> dbox [B, A, 7].
+ *   vc_roi_decode        <- RoIHeadTemplate.generate_predicted_boxes (roi_head_template.py:294-324): box_preds [B*N, 7],
+ *                           rois [B, N, ld] (ld >= 7) -> out [B, N, 7].
+ *   vc_roi_decode_bwd    <- its gradient with respect to box_preds: grad [B, N, 7] -> dbox [B*N, 7].
+ *   vc_box_xtrans        <- TEDMHead.roi_x_trans / roi_score_trans / pred_x_trans (ted_head.py:675-746) over
+ *                           X_TRANS.backward_with_param / forward_with_param (X_transform.py:49-154): boxes [B, N, ld]
+ *                           (ld >= 7), transform_param [B, R, 3] (rotation, flip, scale) -> out [B, N, ld]: the backward
+ *                           transform of stage from_stage, then the forward transform of stage to_stage; a stage < 0 is
+ *                           skipped.  Columns beyond 7 are copied.
+ * ---------------------------------------------------------------------------------------------- */
+int vc_anchor_decode(const float* box_preds, const float* dir_cls, const float* anchors, int B, int A, int NB,
+                     float dir_offset, float dir_limit_offset, float period, float* out, vc_stream_t stream);
+int vc_anchor_decode_bwd(const float* grad, const float* box_preds, const float* anchors, int B, int A, int with_dir,
+                         float* dbox, vc_stream_t stream);
+int vc_roi_decode(const float* box_preds, const float* rois, int B, int N, int ld, float* out, vc_stream_t stream);
+int vc_roi_decode_bwd(const float* grad, const float* box_preds, const float* rois, int B, int N, int ld, float* dbox,
+                      vc_stream_t stream);
+int vc_box_xtrans(const float* boxes, const float* transform_param, int B, int N, int ld, int R, int from_stage,
+                  int to_stage, float* out, vc_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Parameter update of the adam_onecycle / adam_cosin step (csrc/optim.cu): what the reference's loop does after
  * loss.backward() (tools/train_utils/train_utils.py:50-52: clip_grad_norm_, OptimWrapper.step of fastai_optim.py:132-149
  * over torch.optim.Adam) for EVERY parameter tensor in two launches.  No host read, no allocation; graph-capturable;

@@ -130,6 +130,11 @@ SIGNATURES = {
     'vc_part_pool_bwd_ws_bytes': (_Z, [_I, _I, _I]),
     'vc_part_pool_bwd': (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _F, _F, _F, _P, _P, _Z, _P]),
     'vc_roi_grid_points': (_I, [_P, _I, _I, _I, _I, _HOSTF, _HOSTF, _HOST, _I, _P, _P, _P]),
+    'vc_anchor_decode': (_I, [_P, _P, _P, _I, _I, _I, _F, _F, _F, _P, _P]),
+    'vc_anchor_decode_bwd': (_I, [_P, _P, _P, _I, _I, _I, _P, _P]),
+    'vc_roi_decode': (_I, [_P, _P, _I, _I, _I, _P, _P]),
+    'vc_roi_decode_bwd': (_I, [_P, _P, _P, _I, _I, _I, _P, _P]),
+    'vc_box_xtrans': (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P, _P]),
     'vc_optim_ws_bytes': (_Z, [_I]),
     'vc_optim_step': (_I, [_P, _I, _P, _I, _D, _HOSTP, _I, _P, _P, _P, _I, _P, _Z, _P]),
     'vc_exec_state_bytes': (_Z, []),

@@ -32,7 +32,10 @@ FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-line
 # optim.cu: no contraction, so that every fp32 operation of the update rounds once, as torch's elementwise kernels do
 # roi_grid.cu: no contraction, so that the grid points and their floor divisions round every operation once, as torch's
 # elementwise kernels do
+# box_decode.cu: no contraction, so that the decoded boxes, their rotations and the stage transforms round every
+# operation once, as torch's elementwise kernels do
 FILE_FLAGS = {'roi_grid.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],'iou3d_nms.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
+              'box_decode.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
               'optim.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
               'anchor_targets.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
               'roi_targets.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],

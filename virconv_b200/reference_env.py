@@ -39,6 +39,9 @@ bit-reproducible part-map gradient.
 With `use_fused_roi_grid` `TEDMHead.roi_grid_pool` and `roi_grid_pool_mm` are this package's drop-in methods
 (virconv_b200.roi_grid): the grid points and their voxel coordinates in one launch per call, and the voxel -> row map and
 voxel centres of each published tensor built once per forward, without a host read.
+With `use_fused_box_decode` `AnchorHeadTemplate.generate_predicted_boxes`, `RoIHeadTemplate.generate_predicted_boxes` and
+`TEDMHead.roi_x_trans / roi_score_trans / pred_x_trans` are this package's drop-in methods (virconv_b200.box_decode): the
+heads' box decoding and the cascade stage transforms in one launch per call, with transform_param read on the device.
 With `use_fused_optimizer` `train_utils.optimization.build_optimizer` (tools/train_utils/optimization/__init__.py:11-36, the
 name tools/train.py imports with tools/ on sys.path) returns this package's optim.FusedAdamOneCycle for OPTIMIZER
 adam_onecycle / adam_cosin and calls the reference's function for every other value, and the `clip_grad_norm_` name
@@ -261,7 +264,8 @@ def _fused_clip_grad_norm_(parameters, max_norm, *args, **kwargs):
 
 
 def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=False, use_fused_rpn_targets=False,
-            use_fused_roi_targets=False, use_fused_losses=False, use_fused_part_pool=False, use_fused_optimizer=False, use_fused_roi_grid=False):
+            use_fused_roi_targets=False, use_fused_losses=False, use_fused_part_pool=False, use_fused_optimizer=False, use_fused_roi_grid=False,
+            use_fused_box_decode=False):
     """Register everything listed in the module docstring.  `reference_root`: put that checkout first on sys.path."""
     if reference_root is not None and reference_root not in sys.path:
         sys.path.insert(0, reference_root)
@@ -367,6 +371,22 @@ def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=F
             roi_grid._reference_roi_grid_pool_mm = ted.roi_grid_pool_mm
         ted.roi_grid_pool = roi_grid.roi_grid_pool
         ted.roi_grid_pool_mm = roi_grid.roi_grid_pool_mm
+    if use_fused_box_decode:
+        from . import box_decode
+        aht = importlib.import_module('pcdet.models.dense_heads.anchor_head_template').AnchorHeadTemplate
+        rht = importlib.import_module('pcdet.models.roi_heads.roi_head_template').RoIHeadTemplate
+        ted = importlib.import_module('pcdet.models.roi_heads.ted_head').TEDMHead
+        for cls, name, fused, record in (
+                (aht, 'generate_predicted_boxes', box_decode.anchor_generate_predicted_boxes,
+                 '_reference_anchor_generate_predicted_boxes'),
+                (rht, 'generate_predicted_boxes', box_decode.roi_generate_predicted_boxes,
+                 '_reference_roi_generate_predicted_boxes'),
+                (ted, 'roi_x_trans', box_decode.roi_x_trans, '_reference_roi_x_trans'),
+                (ted, 'roi_score_trans', box_decode.roi_score_trans, '_reference_roi_score_trans'),
+                (ted, 'pred_x_trans', box_decode.pred_x_trans, '_reference_pred_x_trans')):
+            if getattr(cls, name) is not fused:
+                setattr(box_decode, record, getattr(cls, name))
+            setattr(cls, name, fused)
     if use_fused_optimizer:
         import os
         tools = os.path.join(reference_root, 'tools') if reference_root is not None else None
