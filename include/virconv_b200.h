@@ -818,6 +818,37 @@ int vc_allreduce_peer_flag_words(int world);
 int vc_allreduce_peer_f32(const uint64_t* peer_bufs, const uint64_t* peer_flags, int rank, int world, float* grads, long long n,
                           long long n_pad, unsigned epoch, float scale, int32_t* err_flag, vc_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * KITTI evaluation (csrc/kitti_eval.cu, geometry in csrc/kitti_eval_geom.cuh): what kitti_object_eval_python/eval.py's
+ * eval_class computes for the three metrics of get_official_eval_result, over a whole evaluation set in nine launches.
+ * Packed input (double, VC_KE_ROW per object, one upload):
+ *   GT row  : bbox x0 y0 x1 y1, alpha, location x y z, dimensions l h w, rotation_y, truncated, occluded,
+ *             class id (car 0, pedestrian 1, cyclist 2, van 3, person_sitting 4, truck 5, other -1), DontCare (1 / 0)
+ *   DT row  : bbox x0 y0 x1 y1, alpha, location x y z, dimensions l h w, rotation_y, score, class id, 0, 0
+ *   offs    : int64 [3][F + 1]: the frames' first GT row, first detection row and first overlap pair
+ *             (pair_off[f + 1] - pair_off[f] = n_gt[f] * n_dt[f])
+ *   lane_mo : double [L] min overlap per lane, L = 3 * C * 3 * K, lane = ((metric * C + class) * 3 + difficulty) * K + k
+ *   vc_kitti_overlaps   <- one metric's per-frame [n_dt, n_gt] blocks (0 image, 1 BEV, 2 3-D) into ov [n_pair]
+ *   vc_kitti_rotate_iou <- rotate_iou_gpu_eval (rotate_iou.py:295): boxes [N, 5], qboxes [K, 5] float32 -> out [N, K]
+ *   vc_kitti_eval       <- eval_class for metrics 0, 1, 2: ov [3][n_pair] and, per lane, out[lane * VC_KE_LANE_W ..]:
+ *                          [0] the number of thresholds T, [1, 42) the thresholds, [42, 206) tp, fp, fn, similarity per
+ *                          threshold, [206, 247) precision, [247, 288) recall, [288, 329) orientation (eval_class's
+ *                          arrays, running max applied).  classes: host array of C class ids.
+ * ---------------------------------------------------------------------------------------------- */
+#define VC_KE_ROW 16
+#define VC_KE_SAMPLES 41
+#define VC_KE_LANE_W 329
+#define VC_KE_MAX_CLASSES 6
+#define VC_KE_MAX_OVERLAPS 10
+int vc_kitti_overlaps(const double* gt, const double* dt, const long long* offs, int F, long long n_pair, int metric,
+                      double* ov, vc_stream_t stream);
+int vc_kitti_rotate_iou(const float* boxes, const float* qboxes, int N, int K, int criterion, float* out,
+                        vc_stream_t stream);
+size_t vc_kitti_eval_ws_bytes(int F, int NG, int ND, int C, int K);
+int vc_kitti_eval(const double* gt, const double* dt, const long long* offs, const double* lane_mo, int F, int NG, int ND,
+                  long long n_pair, int C, const int* classes, int K, int compute_aos, double* ov, double* out, void* ws,
+                  size_t ws_bytes, vc_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

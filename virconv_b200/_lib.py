@@ -146,6 +146,10 @@ SIGNATURES = {
     'vc_exec_query': (_I, [_P, _I, _I, _P]),
     'vc_exec_timing': (_I, [_I]),
     'vc_exec_timing_read': (_I, [_P, _P, _I]),
+    'vc_kitti_overlaps': (_I, [_P, _P, _P, _I, ctypes.c_longlong, _I, _P, _P]),
+    'vc_kitti_rotate_iou': (_I, [_P, _P, _I, _I, _I, _P, _P]),
+    'vc_kitti_eval_ws_bytes': (_Z, [_I, _I, _I, _I, _I]),
+    'vc_kitti_eval': (_I, [_P, _P, _P, _P, _I, _I, _I, ctypes.c_longlong, _I, _HOST, _I, _I, _P, _P, _P, _Z, _P]),
     'vc_allreduce_peer_flag_words': (_I, [_I]),
     'vc_allreduce_peer_f32': (_I, [_P, _P, _I, _I, _P, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_uint, _F, _P, _P]),
 }

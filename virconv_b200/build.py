@@ -34,13 +34,16 @@ FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-line
 # elementwise kernels do
 # box_decode.cu: no contraction, so that the decoded boxes, their rotations and the stage transforms round every
 # operation once, as torch's elementwise kernels do
+# kitti_eval.cu: no contraction, so that the overlaps round every operation once in the types numba gives the
+# reference's kernels (kitti_eval_geom.cuh)
 FILE_FLAGS = {'roi_grid.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],'iou3d_nms.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
               'box_decode.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
               'optim.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
               'anchor_targets.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
               'roi_targets.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
               'head_losses.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
-              'part_pool.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off']}
+              'part_pool.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off'],
+              'kitti_eval.cu': ['-fmad=false', '-Xcompiler', '-ffp-contract=off']}
 
 
 def flags_for(src):

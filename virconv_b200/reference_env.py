@@ -42,6 +42,9 @@ voxel centres of each published tensor built once per forward, without a host re
 With `use_fused_box_decode` `AnchorHeadTemplate.generate_predicted_boxes`, `RoIHeadTemplate.generate_predicted_boxes` and
 `TEDMHead.roi_x_trans / roi_score_trans / pred_x_trans` are this package's drop-in methods (virconv_b200.box_decode): the
 heads' box decoding and the cascade stage transforms in one launch per call, with transform_param read on the device.
+With `use_fused_kitti_eval` `get_official_eval_result`, `get_coco_eval_result` and the imported name `rotate_iou_gpu_eval`
+of kitti_object_eval_python.eval are this package's (virconv_b200.kitti_eval): KittiDatasetMM.evaluation, which imports
+the module inside the method, then runs the KITTI evaluation in nine launches with one upload and one read-back.
 With `use_fused_optimizer` `train_utils.optimization.build_optimizer` (tools/train_utils/optimization/__init__.py:11-36, the
 name tools/train.py imports with tools/ on sys.path) returns this package's optim.FusedAdamOneCycle for OPTIMIZER
 adam_onecycle / adam_cosin and calls the reference's function for every other value, and the `clip_grad_norm_` name
@@ -265,7 +268,7 @@ def _fused_clip_grad_norm_(parameters, max_norm, *args, **kwargs):
 
 def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=False, use_fused_rpn_targets=False,
             use_fused_roi_targets=False, use_fused_losses=False, use_fused_part_pool=False, use_fused_optimizer=False, use_fused_roi_grid=False,
-            use_fused_box_decode=False):
+            use_fused_box_decode=False, use_fused_kitti_eval=False):
     """Register everything listed in the module docstring.  `reference_root`: put that checkout first on sys.path."""
     if reference_root is not None and reference_root not in sys.path:
         sys.path.insert(0, reference_root)
@@ -387,6 +390,12 @@ def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=F
             if getattr(cls, name) is not fused:
                 setattr(box_decode, record, getattr(cls, name))
             setattr(cls, name, fused)
+    if use_fused_kitti_eval:
+        from . import kitti_eval
+        ev = importlib.import_module('pcdet.datasets.kitti.kitti_object_eval_python.eval')
+        ev.get_official_eval_result = kitti_eval.get_official_eval_result
+        ev.get_coco_eval_result = kitti_eval.get_coco_eval_result
+        ev.rotate_iou_gpu_eval = kitti_eval.rotate_iou_eval
     if use_fused_optimizer:
         import os
         tools = os.path.join(reference_root, 'tools') if reference_root is not None else None
