@@ -6,7 +6,11 @@ column includes it.  Per replay it also prints the index phase: the span from th
 strided-conv count / emit / tables, projections) to the last, the time from the voxeliser's last kernel to the first conv,
 and the span of the forward's conv chain.  Run on the GPU:
 
-    python profiles/forward_bn_gap.py [--replays 20]
+    python profiles/forward_bn_gap.py [--replays 20] [--modes 1,2]
+
+--modes: the executor's index orders to compare (vc_set_index_order: 0 per level, 1 composed, 2 composed with the stages'
+index work batched and, in this static-mode step, the index phase first).  Each mode captures its own step; the modes are
+profiled in alternation, two rounds of replays / 2 each, in one process.
 
 Prints the card name and power limit with the numbers: a kernel time is only meaningful with what it was measured on."""
 import argparse
@@ -100,44 +104,21 @@ def forward_layers(events):
     return out
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument('--replays', type=int, default=20)
-    args = ap.parse_args()
-    dev = torch.device('cuda:0')
-    torch.manual_seed(666)
-    model = VirConvL8x(bench.CFG, 8, [1408, 1600, 80], precision='bf16').to(dev).train()
-    params = list(model.parameters())
-    batches = []
-    for i in range(bench.POOL):
-        pb = scenes.make_points_batch([2 * i, 2 * i + 1], bench.N_LIDAR, bench.N_VIRTUAL, training=True)
-        batches.append({'points': torch.from_numpy(pb.points).to(dev), 'batch_size': pb.batch_size, 'calib': pb.calib,
-                        'aug_param': pb.aug_param})
-    vox = dict(point_cloud_range=(0, -40, -3, 70.4, 40, 1), voxel_size=(0.05, 0.05, 0.05), max_points_per_voxel=5,
-               max_voxels=bench.MAX_VOXELS, vfe_model='max')
-
-    def loss_of(out):
-        loss = masked_mean(out['encoded_spconv_tensor'])
-        for t in out['multi_scale_3d_features'].values():
-            loss = loss + masked_mean(t)
-        return loss
-
-    step = GraphedStep(model, loss_of, params, margin=float(os.environ.get('VIRCONV_GRAPH_MARGIN', '1.15')), voxelizer=vox)
-    for i in range(3 * bench.POOL):
-        step(batches[i % bench.POOL])
-    torch.cuda.synchronize()
+def profile_events(step, batches, replays):
     from torch.profiler import ProfilerActivity, profile
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        for i in range(args.replays):
+        for i in range(replays):
             step(batches[i % bench.POOL])
         torch.cuda.synchronize()
-    events = [(e.start_ns(), e.end_ns(), e.name(), e.device_resource_id()) for e in prof.profiler.kineto_results.events()
-              if e.device_type() == torch.autograd.DeviceType.CUDA and e.duration_ns() > 0]
+    return [(e.start_ns(), e.end_ns(), e.name(), e.device_resource_id()) for e in prof.profiler.kineto_results.events()
+            if e.device_type() == torch.autograd.DeviceType.CUDA and e.duration_ns() > 0]
+
+
+def report(events):
     reps = forward_layers(events)
     n_layers = max(len(r) for r in reps)
     reps = [r for r in reps if len(r) == n_layers]
     R = len(reps)
-    print(f'card: {card()}')
     print(f'VIRCONV_CONV_BN_FUSED={os.environ.get("VIRCONV_CONV_BN_FUSED", "1")}: {R} replays, {n_layers} forward layers '
           f'(us, mean over replays)')
     print(f'{"layer":>5} {"conv":>8} {"gap->bn":>8} {"bn apply":>9} {"gap->next":>10}')
@@ -163,6 +144,50 @@ def main():
         c = sum(r['kernels'].get(n, [0, 0])[0] for r in ph) / len(ph)
         t = sum(r['kernels'].get(n, [0, 0])[1] for r in ph) / len(ph) / 1e3
         print(f'    {n:20s} {c:6.1f} {t:8.1f}')
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--replays', type=int, default=20)
+    ap.add_argument('--modes', default='1,2', help='index orders to compare (vc_set_index_order), comma separated')
+    args = ap.parse_args()
+    modes = [int(m) for m in args.modes.split(',')]
+    from virconv_b200 import _lib
+    lib = _lib.load()
+    dev = torch.device('cuda:0')
+    batches = []
+    for i in range(bench.POOL):
+        pb = scenes.make_points_batch([2 * i, 2 * i + 1], bench.N_LIDAR, bench.N_VIRTUAL, training=True)
+        batches.append({'points': torch.from_numpy(pb.points).to(dev), 'batch_size': pb.batch_size, 'calib': pb.calib,
+                        'aug_param': pb.aug_param})
+    vox = dict(point_cloud_range=(0, -40, -3, 70.4, 40, 1), voxel_size=(0.05, 0.05, 0.05), max_points_per_voxel=5,
+               max_voxels=bench.MAX_VOXELS, vfe_model='max')
+
+    def loss_of(out):
+        loss = masked_mean(out['encoded_spconv_tensor'])
+        for t in out['multi_scale_3d_features'].values():
+            loss = loss + masked_mean(t)
+        return loss
+
+    steps = {}
+    for mode in modes:
+        _lib.check(lib.vc_set_index_order(mode), 'vc_set_index_order')   # read when the step is captured
+        torch.manual_seed(666)
+        model = VirConvL8x(bench.CFG, 8, [1408, 1600, 80], precision='bf16').to(dev).train()
+        steps[mode] = GraphedStep(model, loss_of, list(model.parameters()),
+                                  margin=float(os.environ.get('VIRCONV_GRAPH_MARGIN', '1.15')), voxelizer=vox)
+        for i in range(3 * bench.POOL):
+            steps[mode](batches[i % bench.POOL])
+        torch.cuda.synchronize()
+    events = {mode: [] for mode in modes}
+    for _ in range(2):
+        for mode in modes:
+            _lib.check(lib.vc_set_index_order(mode), 'vc_set_index_order')   # (in case the step captures again)
+            events[mode] += profile_events(steps[mode], batches, max(1, args.replays // 2))
+    print(f'card: {card()}')
+    for mode in modes:
+        print(f'--- index order {mode}')
+        report(events[mode])
 
 
 if __name__ == '__main__':

@@ -180,9 +180,10 @@ def load():
     lib.vc_set_pdl(1 if os.environ.get('VIRCONV_PDL', '0') == '1' else 0)
     # BatchNorm + ReLU inside the tensor-core conv forward (one cooperative launch per layer); 0 for A/B runs
     lib.vc_set_conv_bn_fused(0 if os.environ.get('VIRCONV_CONV_BN_FUSED', '1') == '0' else 1)
-    # output sets of chained strided convs: 1 = one composed pass; 0 = one strided conv after the other (A/B runs)
-    if lib.vc_set_index_order(int(os.environ.get('VIRCONV_INDEX_ORDER', '1'))) != 0:
-        raise ValueError('VIRCONV_INDEX_ORDER must be 0 or 1')
+    # index work of chained strided convs: 2 = composed, batched per kind, index phase first in static mode; 1 = composed,
+    # one launch per stage; 0 = one strided conv after the other (A/B runs)
+    if lib.vc_set_index_order(int(os.environ.get('VIRCONV_INDEX_ORDER', '2'))) != 0:
+        raise ValueError('VIRCONV_INDEX_ORDER must be 0, 1 or 2')
     _lib = lib
     return lib
 

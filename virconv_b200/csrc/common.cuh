@@ -170,6 +170,44 @@ int conv_chain_count_dev(const ConvChain& ch, const int32_t* indices, int n, con
 // out_idx [L]: output index buffers of caps[l] rows
 int conv_chain_emit_dev(const ConvChain& ch, int32_t* const* out_idx, const int* caps, void* ws, size_t ws_bytes, cudaStream_t stream);
 
+// The per-stage index work of up to IDX_BATCH_MAX stages, one launch per kind (rulebook.cu, misc.cu): the same kernels, and
+// the same results, as one call per stage.  The caller owns the buffers and clears them first (so that the regions of
+// all stages can be cleared together): hash tables to 0xFF, a mirrored table's rows k > centre to -1, pair counts to 0,
+// nbr_fwd to -1.
+constexpr int IDX_BATCH_MAX = 4;
+bool subm_sym(int ndim, const int32_t* ksize, bool unique);   // the mirrored probe (half the offsets, rows k > centre pre-filled)
+struct SubmStage {   // one submanifold rulebook (subm_rulebook_dev without rep); table: vc_subm_rulebook_ws_bytes(n) bytes
+    const int32_t* idx;
+    int n;
+    const int* n_dev;
+    int ndim;
+    const int32_t *shape, *ksize, *dil;
+    int32_t *nbr, *pair_num;
+    void* table;
+    size_t table_bytes;
+};
+int subm_rulebook_batch_dev(const SubmStage* st, int n_st, int batch_size, bool unique, cudaStream_t stream);
+struct TablesStage {  // one strided conv's tables (conv_rulebook_tables_dev)
+    const int32_t* idx;
+    int n;
+    const int* n_dev;
+    int ndim;
+    const int32_t *shape, *ksize, *stride, *pad, *dil;
+    int n_out;
+    ConvRank rank;
+    int32_t *nbr_fwd, *nbr_bwd, *pair_num;
+};
+int conv_tables_batch_dev(const TablesStage* st, int n_st, int batch_size, cudaStream_t stream);
+struct UVStage {     // one projection (index2uv_dev)
+    const int32_t* idx;
+    int n;
+    const int* n_dev;
+    const float* grid;
+    int stride, u_max, v_max;
+    int32_t* uv;
+};
+int index2uv_batch_dev(const UVStage* st, int n_st, int batch_size, const float* params, cudaStream_t stream);
+
 // ---- bn.cu / misc.cu internals used by the plan executor (device row counts, strided outputs) ----
 int bn_apply_relu_dev(const float* x, const double* sums, int n_rows, const int* n_dev, int c, const float* gamma,
                       const float* beta, float* running_mean, float* running_var, long long* num_batches_tracked, float momentum,
@@ -266,7 +304,8 @@ size_t tc_image_bytes(int cin, int cout, int K, int layout);
 bool tc2_ch_ok(int c);
 int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_t* nbr, long long pitch, float* out, int n_rows,
              const int* n_dev, int K, double* bn_sums, int* err, cudaStream_t stream, const float* addend,
-             int* tile_counter = nullptr, int flags = 0,   // flags: bit 0 sparse offsets (strided dgrad), bit 1 early tables
+             int* tile_counter = nullptr, int flags = 0,   // flags: bit 0 sparse offsets (strided dgrad), bit 1 early tables,
+                                                           // bit 2 no index kernel beside it (the conv + BN grid takes 2 CTAs/SM)
              int in_ld = 0,                                // row pitch of in_bf16 (0: kc)
              double* bn_part = nullptr,                    // deterministic BN sums: [tiles, 2, nr] per 128-row tile (bn_sums NULL)
              const BnTail* bn = nullptr,                   // forward only: BN + ReLU in the same launch when g_conv_bn_fused

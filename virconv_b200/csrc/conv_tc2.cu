@@ -703,7 +703,7 @@ bool plan_smem(int K, size_t budget, int ntb, size_t resident_max, int min_stage
 }
 
 template <int KC, int NR>
-int launch_persist(const PArgs& a0, int n_cap, cudaStream_t stream, bool* bn_done) {
+int launch_persist(const PArgs& a0, int n_cap, cudaStream_t stream, bool* bn_done, bool coop2) {
     PArgs a = a0;
     // Two CTAs per SM (half the shared memory each, 2 table buffers) when the ring still has VC_P_MIN_STAGES2 stages: two
     // independent pipelines per SM (each a serial chain of barrier wait -> MMA issue -> release per stage) and room for CTAs
@@ -735,8 +735,9 @@ int launch_persist(const PArgs& a0, int n_cap, cudaStream_t stream, bool* bn_don
         // per step SLOWER than the separate apply kernel); at one CTA per SM the grid fits beside them and the step gets
         // 0.15 ms faster (DESIGN.md section 8).  Same shared-memory plan, half the CTAs.  Running the whole index phase
         // before the forward instead, so that the grid could take both CTAs of each SM, was slower still (DESIGN.md
-        // section 8, item 3).  vc_conv_tc2_config(2) forces the two-CTA grid (tests, A/B runs).
-        const int cgrid = (g_p_ctas == 2 || grid < num_sms()) ? grid : num_sms();
+        // section 8, item 3) until the index work was batched: with no index kernel beside it (coop2, the executor's index
+        // order 2 in static mode) the grid takes both.  vc_conv_tc2_config(2) forces the two-CTA grid (tests, A/B runs).
+        const int cgrid = (g_p_ctas == 2 || coop2 || grid < num_sms()) ? grid : num_sms();
         cudaLaunchConfig_t cfg{};
         cfg.gridDim = dim3(cgrid);
         cfg.blockDim = dim3(P_THREADS);
@@ -852,7 +853,7 @@ int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_
     if (bn_done == nullptr) bn_done = &done_dummy;
     const int kcp = tc_pad16(kc), nrp = tc_pad16(nr);
 #define VC_P_CASE(A, B) \
-    if (kcp == A && nrp == B) return launch_persist<A, B>(a, n_rows, stream, bn_done);
+    if (kcp == A && nrp == B) return launch_persist<A, B>(a, n_rows, stream, bn_done, (flags >> 2) & 1);
     VC_P_CASE(16, 16) VC_P_CASE(16, 32) VC_P_CASE(16, 64)
     VC_P_CASE(32, 16) VC_P_CASE(32, 32) VC_P_CASE(32, 64)
     VC_P_CASE(64, 16) VC_P_CASE(64, 32) VC_P_CASE(64, 64)

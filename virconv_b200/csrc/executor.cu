@@ -123,10 +123,13 @@ constexpr int EV_POOL = 512;   // > the events of one forward / backward call: t
 cudaEvent_t g_ev[EV_POOL];
 int g_ev_dev = -1, g_ev_next = 0;
 
-// How the forward builds the output sets of chained strided convs (vc_set_index_order, VIRCONV_INDEX_ORDER): 1 (default)
-// composed in one pass (fwd_conv_chain); 0 each from the previous one's (count -> read-back -> emit per conv), the path
-// every other plan takes and the reference the tests compare the composed pass with.
-int g_index_order = 1;
+// How the forward builds the output sets of chained strided convs and their stages' index work (vc_set_index_order,
+// VIRCONV_INDEX_ORDER): 2 (default) composed in one pass (fwd_conv_chain), the index work of the chain's stages batched
+// into one launch per kind (fwd_chain_tables, fwd_chain_stages), and in static mode the whole index phase enqueued before
+// the first feature kernel; 1 composed, the stages' work one launch per stage in the plan's interleaved order; 0 each
+// output set from the previous one's (count -> read-back -> emit per conv), the path every other plan takes.  0 and 1 are
+// the references the tests compare with.
+int g_index_order = 2;
 
 int ev_init() {
     int dev = 0;
@@ -322,6 +325,8 @@ struct FwdCtx : Ctx {
     int32_t *overflow, *pinned;
     int n_syncs, last_ev[3] = {-1, -1, -1};   // last_ev: latest event of each side stream (joined into main at the end)
     bool do_idx, do_feat, two;   // do_idx / do_feat: enqueue the index / feature operators (both unless phased)
+    bool idx_first;              // the whole index phase is enqueued before this walk: no index kernel runs beside a conv
+    bool batched[MAX_OPS];       // op enqueued by a batched call of its chain (fwd_chain_tables, fwd_chain_stages)
     // per strided conv op: where its ranked output bitmap lies (for the tables); done: count and indices are enqueued
     struct { ConvRank rank; bool done; } chain[MAX_OPS];
     template <class T>
@@ -537,6 +542,178 @@ int fwd_discard(FwdCtx& C, int i, const int* o) {
     return VC_OK;
 }
 
+// Index order 2: the tables of all the chain's strided convs in one launch (conv_tables_batch_dev) on the chain's stream.
+// Their nbr_fwd tables lie back to back and their pair counts too: one -1 fill and one zeroing.
+int fwd_chain_tables(FwdCtx& C, const int* ops, int L, int s) {
+    size_t fwd_ints = 0, pn_ints = 0;
+    for (int l = 0; l < L; ++l) {
+        const RBk& R = C.S->rb[C.op(ops[l])[F_C]];
+        fwd_ints += (size_t)R.K * (R.n_out > 0 ? R.n_out : 1);
+        pn_ints += R.K;
+    }
+    VC_ALLOC(fwd_all, int32_t*, fwd_ints * 4);
+    VC_ALLOC(pn_all, int32_t*, pn_ints * 4);
+    TablesStage ts[CONV_CHAIN_MAX];
+    for (int l = 0, fo = 0, po = 0; l < L; ++l) {
+        const int* o = C.op(ops[l]);
+        const ISet& I = C.S->iset[o[F_A]];
+        RBk& R = C.S->rb[o[F_C]];
+        VC_ALLOC(nbr_bwd, int32_t*, (size_t)R.K * I.n * 4);
+        R.nbr = fwd_all + fo; R.nbr_bwd = nbr_bwd; R.pair_num = pn_all + po;
+        fo += R.K * (R.n_out > 0 ? R.n_out : 1);
+        po += R.K;
+        ts[l] = TablesStage{I.idx, I.n, I.n_dev, I.ndim, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL, R.n_out, C.chain[ops[l]].rank,
+                            R.nbr, R.nbr_bwd, R.pair_num};
+        C.batched[ops[l]] = true;
+    }
+    if (C.do_idx) {
+        VC_CUDA(cudaMemsetAsync(pn_all, 0, pn_ints * 4, C.st[s]));
+        VC_CUDA(cudaMemsetAsync(fwd_all, 0xFF, fwd_ints * 4, C.st[s]));
+        VC_TRY(conv_tables_batch_dev(ts, L, C.S->batch_size, C.st[s]));
+    }
+    RBk& R0 = C.S->rb[C.op(ops[0])[F_C]];
+    C.produced(R0, s);   // one event for the batch
+    for (int l = 1; l < L; ++l) {
+        RBk& R = C.S->rb[C.op(ops[l])[F_C]];
+        R.ev = R0.ev; R.prod = R0.prod;
+    }
+    return VC_OK;
+}
+
+// Index order 2: the submanifold rulebooks and projections over the chain's output sets (the stage 2-4 work of the plan's
+// image-branch stream), one launch per kind: hash insert + probe of the 3-D sets, index2uv, hash insert + probe of the
+// projected sets.  Applies when all of them run on one stream and probe alike; else each op keeps its own launches.  The
+// deterministic mode's 2-D rulebooks (the gather-form dgrad's `rep` rows) stay per op.
+int fwd_chain_stages(FwdCtx& C, int i0, const int* ops, int L) {
+    int sub3[IDX_BATCH_MAX], uvop[IDX_BATCH_MAX], sub2[IDX_BATCH_MAX], n3 = 0, nuv = 0, n2 = 0, s = -1;
+    bool ok = true;
+    auto take = [&](int j, int* list, int& n) {
+        const int sj = C.two ? C.op(j)[F_STREAM] : 0;
+        if (n == IDX_BATCH_MAX || (s >= 0 && sj != s)) ok = false;
+        else { list[n++] = j; s = sj; }
+    };
+    for (int j = i0 + 1; j < C.n_ops && ok; ++j) {
+        const int* o = C.op(j);
+        bool from_chain = false;
+        for (int l = 0; l < L; ++l) from_chain |= o[F_A] == C.op(ops[l])[F_B];
+        if (o[F_KIND] == OP_SUBM_RB && from_chain && !(C.S->deterministic && !o[F_X0])) take(j, sub3, n3);
+        else if (o[F_KIND] == OP_INDEX2UV && from_chain) take(j, uvop, nuv);
+    }
+    for (int j = i0 + 1; j < C.n_ops && ok; ++j) {
+        const int* o = C.op(j);
+        bool from_uv = false;
+        for (int u = 0; u < nuv; ++u) from_uv |= o[F_A] == C.op(uvop[u])[F_B];
+        if (o[F_KIND] == OP_SUBM_RB && from_uv && !(C.S->deterministic && !o[F_X0])) take(j, sub2, n2);
+    }
+    for (int a = 1; a < n3; ++a) ok &= C.op(sub3[a])[F_X0] == C.op(sub3[0])[F_X0];
+    for (int a = 1; a < n2; ++a) ok &= C.op(sub2[a])[F_X0] == C.op(sub2[0])[F_X0];
+    if (!ok || s < 0) return VC_OK;
+    for (int a = 0; a < n3; ++a) {
+        const int* o = C.op(sub3[a]);
+        ISet& I = C.S->iset[o[F_A]];
+        VC_CHECK_ARG(I.ndim == o[F_NDIM], "op %d: index set %d has the wrong ndim", sub3[a], o[F_A]);
+        VC_TRY(wait_for(C, I.ev, I.prod, s));
+    }
+    for (int a = 0; a < nuv; ++a) {
+        ISet& I = C.S->iset[C.op(uvop[a])[F_A]];
+        VC_CHECK_ARG(I.ndim == 3 && C.proj, "op %d: index2uv needs a built 3-D index set and projection params", uvop[a]);
+        VC_TRY(wait_for(C, I.ev, I.prod, s));
+    }
+    // pair counts of every rulebook: one region, one zeroing
+    size_t pn_ints = 0;
+    for (int a = 0; a < n3; ++a) pn_ints += C.S->rb[C.op(sub3[a])[F_C]].K;
+    for (int a = 0; a < n2; ++a) pn_ints += C.S->rb[C.op(sub2[a])[F_C]].K;
+    VC_ALLOC(pn_all, int32_t*, pn_ints * 4);
+    if (C.do_idx && pn_ints) VC_CUDA(cudaMemsetAsync(pn_all, 0, pn_ints * 4, C.st[s]));
+    int32_t* pn = pn_all;
+    // 3-D: per stage its table, then its hash table right behind it, so the mirrored rows (k > centre, -1) and the hash table
+    // (EMPTY) are one 0xFF fill
+    SubmStage st3[IDX_BATCH_MAX];
+    for (int a = 0; a < n3; ++a) {
+        const int* o = C.op(sub3[a]);
+        ISet& I = C.S->iset[o[F_A]];
+        RBk& R = C.S->rb[o[F_C]];
+        R.n_in = R.n_out = I.n;
+        R.n_in_dev = R.n_out_dev = I.n_dev;
+        VC_ALLOC(nbr, int32_t*, (size_t)R.K * I.n * 4);
+        const size_t wsb = vc_subm_rulebook_ws_bytes(I.n);
+        VC_ALLOC(ws, void*, wsb);
+        R.nbr = nbr; R.pair_num = pn;
+        pn += R.K;
+        st3[a] = SubmStage{I.idx, I.n, I.n_dev, I.ndim, I.shape, o + F_KS, o + F_DL, R.nbr, R.pair_num, ws, wsb};
+        if (C.do_idx && I.n > 0) {
+            char* from = subm_sym(I.ndim, o + F_KS, R.unique != 0) ? (char*)(nbr + (size_t)(R.K / 2 + 1) * I.n) : (char*)ws;
+            VC_CUDA(cudaMemsetAsync(from, 0xFF, (char*)ws + wsb - from, C.st[s]));
+        }
+        C.batched[sub3[a]] = true;
+    }
+    if (n3) {
+        if (C.do_idx) VC_TRY(subm_rulebook_batch_dev(st3, n3, C.S->batch_size, C.op(sub3[0])[F_X0] != 0, C.st[s]));
+        RBk& R0 = C.S->rb[C.op(sub3[0])[F_C]];
+        C.produced(R0, s);
+        for (int a = 1; a < n3; ++a) {
+            RBk& R = C.S->rb[C.op(sub3[a])[F_C]];
+            R.ev = R0.ev; R.prod = R0.prod;
+        }
+    }
+    UVStage uvs[IDX_BATCH_MAX];
+    for (int a = 0; a < nuv; ++a) {
+        const int* o = C.op(uvop[a]);
+        ISet& I = C.S->iset[o[F_A]];
+        ISet& O = C.S->iset[o[F_B]];
+        VC_ALLOC(uv, int32_t*, (size_t)I.n * 3 * 4);
+        O.idx = uv; O.n = I.n; O.ndim = 2; O.shape[0] = o[F_KS]; O.shape[1] = o[F_KS + 1]; O.shape[2] = 0; O.n_dev = I.n_dev;
+        uvs[a] = UVStage{I.idx, I.n, I.n_dev, C.of + (size_t)uvop[a] * OPF, o[F_X0], o[F_X1], o[F_X2], uv};
+        C.batched[uvop[a]] = true;
+    }
+    if (nuv) {
+        if (C.do_idx) VC_TRY(index2uv_batch_dev(uvs, nuv, C.S->batch_size, C.proj, C.st[s]));
+        ISet& O0 = C.S->iset[C.op(uvop[0])[F_B]];
+        C.produced(O0, s);
+        for (int a = 1; a < nuv; ++a) {
+            ISet& O = C.S->iset[C.op(uvop[a])[F_B]];
+            O.ev = O0.ev; O.prod = O0.prod;
+        }
+    }
+    // 2-D: the hash tables of all stages back to back, one 0xFF fill (the full probe writes every table row)
+    SubmStage st2[IDX_BATCH_MAX];
+    char *t0 = nullptr, *t1 = nullptr;
+    for (int a = 0; a < n2; ++a) {
+        const int* o = C.op(sub2[a]);
+        ISet& I = C.S->iset[o[F_A]];
+        VC_CHECK_ARG(I.idx && I.ndim == o[F_NDIM], "op %d: index set %d not built / wrong ndim", sub2[a], o[F_A]);
+        const size_t wsb = vc_subm_rulebook_ws_bytes(I.n);
+        VC_ALLOC(ws, void*, wsb);
+        if (!t0) t0 = (char*)ws;
+        t1 = (char*)ws + wsb;
+        st2[a] = SubmStage{I.idx, I.n, I.n_dev, I.ndim, I.shape, o + F_KS, o + F_DL, nullptr, nullptr, ws, wsb};
+    }
+    for (int a = 0; a < n2; ++a) {
+        const int* o = C.op(sub2[a]);
+        ISet& I = C.S->iset[o[F_A]];
+        RBk& R = C.S->rb[o[F_C]];
+        R.n_in = R.n_out = I.n;
+        R.n_in_dev = R.n_out_dev = I.n_dev;
+        VC_ALLOC(nbr, int32_t*, (size_t)R.K * I.n * 4);
+        R.nbr = st2[a].nbr = nbr; R.pair_num = st2[a].pair_num = pn;
+        pn += R.K;
+        C.batched[sub2[a]] = true;
+    }
+    if (n2) {
+        if (C.do_idx) {
+            VC_CUDA(cudaMemsetAsync(t0, 0xFF, t1 - t0, C.st[s]));
+            VC_TRY(subm_rulebook_batch_dev(st2, n2, C.S->batch_size, C.op(sub2[0])[F_X0] != 0, C.st[s]));
+        }
+        RBk& R0 = C.S->rb[C.op(sub2[0])[F_C]];
+        C.produced(R0, s);
+        for (int a = 1; a < n2; ++a) {
+            RBk& R = C.S->rb[C.op(sub2[a])[F_C]];
+            R.ev = R0.ev; R.prod = R0.prod;
+        }
+    }
+    return VC_OK;
+}
+
 // The strided convs chained from op i (each one's input set is the previous one's output set, no layer discard in the plan
 // between them): every level's count and output indices in one composed pass (rulebook.cu), one host read in exact mode.
 // Leaves C.chain[i].done unset where the rule does not apply (a single conv, a dilation); the caller then takes the
@@ -605,6 +782,10 @@ int fwd_conv_chain(FwdCtx& C, int i) {
     }
     if (C.do_idx) VC_TRY(conv_chain_emit_dev(ch, oidx, n_out, ws, wsb, st));
     for (int l = 0; l < ch.L; ++l) C.produced(C.S->iset[C.op(ops[l])[F_B]], s);
+    if (g_index_order == 2) {
+        VC_TRY(fwd_chain_tables(C, ops, ch.L, s));
+        VC_TRY(fwd_chain_stages(C, i, ops, ch.L));
+    }
     return VC_OK;
 }
 
@@ -615,7 +796,7 @@ int fwd_conv_rb(FwdCtx& C, int i, const int* o, int s) {
     // count) -> emit-indices chain of EVERY strided conv of the plan, back to back.  Each link only needs the previous
     // link's output indices, and it is the only part of the forward the host has to wait for; the neighbour tables,
     // submanifold rulebooks and projections queue up behind it without further synchronisation.
-    if (!C.chain[i].done && g_index_order == 1) VC_TRY(fwd_conv_chain(C, i));
+    if (!C.chain[i].done && g_index_order >= 1) VC_TRY(fwd_conv_chain(C, i));
     if (!C.chain[i].done) {
         if (C.S->is_static) {
             // no host read to wait for: keep the natural order (count -> indices -> tables per stage), so the tables of an
@@ -631,6 +812,7 @@ int fwd_conv_rb(FwdCtx& C, int i, const int* o, int s) {
         }
     }
     VC_CHECK_ARG(C.chain[i].done, "op %d: index set %d not built", i, o[F_A]);
+    if (C.batched[i]) return VC_OK;
     ISet& I = C.S->iset[o[F_A]];
     ISet& O = C.S->iset[o[F_B]];
     RBk& R = C.S->rb[o[F_C]];
@@ -730,7 +912,8 @@ int fwd_cbr(FwdCtx& C, int i, const int* o, int s) {
         //  may load its first table slices before its griddepcontrol.wait — conv_tc2.cu)
         if (C.do_feat)
             VC_TRY(tc2_conv(L.cin, L.cout, X.bf16, L.wimg_fwd, R.nbr, R.n_out, x, R.n_out, R.n_out_dev, R.K, sums, C.err, st, nullptr,
-                            L.tile_ctr, (!C.do_idx || C.st[R.prod] != C.st[s]) ? 2 : 0, X.ld, part, &bt, &bn_done));
+                            L.tile_ctr, ((!C.do_idx || C.st[R.prod] != C.st[s]) ? 2 : 0) | (C.idx_first ? 4 : 0), X.ld, part, &bt,
+                            &bn_done));
     } else {   // (also a tensor-core layer without output rows)
         const size_t wsb = vc_conv_ws_bytes(L.cin, L.cout, R.K);
         VC_ALLOC(ws, void*, wsb);
@@ -875,13 +1058,14 @@ extern "C" int vc_exec_forward(const int32_t* ops_i, const float* ops_f, int n_o
                                   nullptr);
 }
 
-extern "C" int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, int n_ops, const uint64_t* layer_ptrs,
-                                      const float* layer_f, int n_layers, const float* feats0, int c0, const int32_t* idx0, int n0,
-                                      const int32_t* shape0, int batch_size, const float* proj_params, int training, int precision,
-                                      int flags, void* arena, size_t arena_bytes, int32_t* pinned_host, int32_t* err_flag,
-                                      void* state, size_t state_bytes, vc_stream_t main_stream, vc_stream_t side_stream,
-                                      int side_waits_main, const int32_t* caps, const int32_t* n0_dev, int32_t* overflow_flag,
-                                      vc_stream_t side2_stream, const int64_t* rng_seed_dev) {
+namespace {
+// one walk of the plan (both phases, or the one `flags` selects); idx_first: the index phase was enqueued by a walk before
+int exec_forward(const int32_t* ops_i, const float* ops_f, int n_ops, const uint64_t* layer_ptrs, const float* layer_f,
+                 int n_layers, const float* feats0, int c0, const int32_t* idx0, int n0, const int32_t* shape0, int batch_size,
+                 const float* proj_params, int training, int precision, int flags, void* arena, size_t arena_bytes,
+                 int32_t* pinned_host, int32_t* err_flag, void* state, size_t state_bytes, vc_stream_t main_stream,
+                 vc_stream_t side_stream, int side_waits_main, const int32_t* caps, const int32_t* n0_dev, int32_t* overflow_flag,
+                 vc_stream_t side2_stream, const int64_t* rng_seed_dev, bool idx_first) {
     // static mode and phased execution: include/virconv_b200.h.  Both phases walk the whole plan with the same
     // deterministic bump allocation, so they agree on every address and leave the same state blob.
     const bool is_static = n0_dev != nullptr;
@@ -917,6 +1101,7 @@ extern "C" int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, 
     C.err = err_flag;
     C.proj = proj_params; C.seed = rng_seed_dev; C.caps = caps; C.overflow = overflow_flag; C.pinned = pinned_host;
     C.do_idx = phase != 2; C.do_feat = phase != 1; C.two = C.st[0] != C.st[1];
+    C.idx_first = idx_first;
     plan_step(C, c0, precision, training);
 
     VC_TRY(ev_init());
@@ -979,6 +1164,7 @@ extern "C" int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, 
     for (int i = 0; i < n_ops; ++i) {
         const int* o = C.op(i);
         const int s = C.two ? o[F_STREAM] : 0;
+        if (C.batched[i]) continue;
         switch (o[F_KIND]) {
             case OP_SUBM_RB: VC_TRY(fwd_subm_rb(C, i, o, s)); break;
             case OP_CONV_RB: VC_TRY(fwd_conv_rb(C, i, o, s)); break;
@@ -994,9 +1180,33 @@ extern "C" int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, 
     S->magic = STATE_MAGIC;
     return VC_OK;
 }
+}  // namespace
+
+extern "C" int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, int n_ops, const uint64_t* layer_ptrs,
+                                      const float* layer_f, int n_layers, const float* feats0, int c0, const int32_t* idx0, int n0,
+                                      const int32_t* shape0, int batch_size, const float* proj_params, int training, int precision,
+                                      int flags, void* arena, size_t arena_bytes, int32_t* pinned_host, int32_t* err_flag,
+                                      void* state, size_t state_bytes, vc_stream_t main_stream, vc_stream_t side_stream,
+                                      int side_waits_main, const int32_t* caps, const int32_t* n0_dev, int32_t* overflow_flag,
+                                      vc_stream_t side2_stream, const int64_t* rng_seed_dev) {
+    // Index order 2 in static mode (no host read splits the index phase): the index walk first, then the feature walk, so
+    // that no index kernel is resident while the convs run and the fused conv + BN grids take two CTAs per SM
+    // (conv_tc2.cu launch_persist).
+    const bool idx_first = n0_dev != nullptr && ((flags >> 8) & 3) == 0 && g_index_order == 2 && side_stream != nullptr &&
+                           side_stream != main_stream;
+    const int f = idx_first ? (flags & ~(3 << 8)) : flags;
+    if (idx_first)
+        VC_TRY(exec_forward(ops_i, ops_f, n_ops, layer_ptrs, layer_f, n_layers, feats0, c0, idx0, n0, shape0, batch_size, proj_params,
+                            training, precision, f | (1 << 8), arena, arena_bytes, pinned_host, err_flag, state, state_bytes,
+                            main_stream, side_stream, side_waits_main, caps, n0_dev, overflow_flag, side2_stream, rng_seed_dev, false));
+    return exec_forward(ops_i, ops_f, n_ops, layer_ptrs, layer_f, n_layers, feats0, c0, idx0, n0, shape0, batch_size, proj_params,
+                        training, precision, idx_first ? f | (2 << 8) : flags, arena, arena_bytes, pinned_host, err_flag, state,
+                        state_bytes, main_stream, side_stream, side_waits_main, caps, n0_dev, overflow_flag, side2_stream, rng_seed_dev,
+                        idx_first);
+}
 
 extern "C" int vc_set_index_order(int mode) {
-    VC_CHECK_ARG(mode == 0 || mode == 1, "index order must be 0 or 1");
+    VC_CHECK_ARG(mode >= 0 && mode <= 2, "index order must be 0, 1 or 2");
     g_index_order = mode;
     return VC_OK;
 }

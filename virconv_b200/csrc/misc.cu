@@ -25,11 +25,10 @@ struct UVGrid {
 // Voxel index -> pixel cell.  Every float op is an explicitly rounded fp32 multiply / add / divide in the
 // order oracle/index2uv.py fixes (no FMA contraction), so the integer result is bit-identical to it.
 // Reference arithmetic: spconv_backbone.py:8-24,54-83; X_transform.py:139-154; calibration_kitti.py:120-153.
-__global__ void __launch_bounds__(256) index2uv_kernel(const int4* __restrict__ idx, int n, const int* __restrict__ n_dev,
-                                                       int batch_size, const float* __restrict__ params, UVGrid g, int stride,
-                                                       int u_max, int v_max, int32_t* __restrict__ uv) {
+__device__ __forceinline__ void index2uv_row(const int4* __restrict__ idx, int n, const int* __restrict__ n_dev,
+                                             int batch_size, const float* __restrict__ params, const UVGrid& g, int stride,
+                                             int u_max, int v_max, int32_t* __restrict__ uv, int i) {
     if (n_dev != nullptr) n = min(n, __ldg(n_dev));
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     int4 v = idx[i];  // (b, z, y, x)
     int b = v.x;
@@ -74,6 +73,35 @@ __global__ void __launch_bounds__(256) index2uv_kernel(const int4* __restrict__ 
     o[0] = b;
     o[1] = ui;
     o[2] = vi;
+}
+
+__global__ void __launch_bounds__(256) index2uv_kernel(const int4* __restrict__ idx, int n, const int* __restrict__ n_dev,
+                                                       int batch_size, const float* __restrict__ params, UVGrid g, int stride,
+                                                       int u_max, int v_max, int32_t* __restrict__ uv) {
+    index2uv_row(idx, n, n_dev, batch_size, params, g, stride, u_max, v_max, uv, blockIdx.x * blockDim.x + threadIdx.x);
+}
+
+// up to IDX_BATCH_MAX projections in one launch: stage e owns the blocks blk0[e] .. blk0[e + 1] - 1
+struct UVEntry {
+    const int4* idx;
+    const int* n_dev;
+    int32_t* uv;
+    UVGrid g;
+    int n, stride, u_max, v_max;
+};
+struct UVBatch {
+    int E, batch_size;
+    const float* params;
+    int blk0[IDX_BATCH_MAX + 1];
+    UVEntry e[IDX_BATCH_MAX];
+};
+
+__global__ void __launch_bounds__(256) index2uv_kernel(const __grid_constant__ UVBatch ub) {
+    int i = 0;
+    while (i + 1 < ub.E && (int)blockIdx.x >= ub.blk0[i + 1]) ++i;
+    const UVEntry& e = ub.e[i];
+    index2uv_row(e.idx, e.n, e.n_dev, ub.batch_size, ub.params, e.g, e.stride, e.u_max, e.v_max, e.uv,
+                 (blockIdx.x - ub.blk0[i]) * blockDim.x + threadIdx.x);
 }
 
 // n_dev (may be NULL): device row count of a capacity-sized tensor (n = capacity); rows at or past it are not scattered, and
@@ -263,6 +291,30 @@ int vc::index2uv_dev(const int32_t* indices, int n, const int* n_dev, int batch_
     UVGrid g{grid[0], grid[1], grid[2], grid[3], grid[4], grid[5]};
     index2uv_kernel<<<cdiv(n, 256), 256, 0, stream>>>((const int4*)indices, n, n_dev, batch_size, params, g, stride, u_max, v_max,
                                                       uv_out);
+    VC_LAUNCH_CHECK();
+    return VC_OK;
+}
+
+int vc::index2uv_batch_dev(const UVStage* st, int n_st, int batch_size, const float* params, cudaStream_t stream) {
+    VC_CHECK_ARG(n_st >= 1 && n_st <= IDX_BATCH_MAX && batch_size > 0, "bad index2uv batch");
+    UVBatch ub;
+    memset(&ub, 0, sizeof(ub));
+    ub.batch_size = batch_size;
+    ub.params = params;
+    for (int i = 0; i < n_st; ++i) {
+        const UVStage& s = st[i];
+        VC_CHECK_ARG(s.n >= 0 && s.stride > 0 && s.u_max > 0 && s.v_max > 0 && s.grid, "bad index2uv arguments");
+        if (s.n == 0) continue;
+        VC_CHECK_ARG(s.idx && params && s.uv, "null pointer");
+        UVEntry& e = ub.e[ub.E];
+        e.idx = (const int4*)s.idx; e.n_dev = s.n_dev; e.uv = s.uv; e.n = s.n; e.stride = s.stride; e.u_max = s.u_max;
+        e.v_max = s.v_max;
+        e.g = UVGrid{s.grid[0], s.grid[1], s.grid[2], s.grid[3], s.grid[4], s.grid[5]};
+        ub.blk0[ub.E + 1] = ub.blk0[ub.E] + cdiv(s.n, 256);
+        ++ub.E;
+    }
+    if (ub.E == 0) return VC_OK;
+    index2uv_kernel<<<ub.blk0[ub.E], 256, 0, stream>>>(ub);
     VC_LAUNCH_CHECK();
     return VC_OK;
 }

@@ -65,10 +65,9 @@ __device__ __forceinline__ void load_index(const int32_t* __restrict__ idx, int 
 // ------------------------------------------------------------------------------------------------
 // (every kernel below that takes a row count `n` also takes `n_dev`: when non-NULL the count is read from device memory
 // and `n` is the capacity the grid / buffers were sized for — the plan executor's static mode, CUDA-graph capturable)
-__global__ void hash_insert_kernel(const int32_t* __restrict__ idx, int n, const int* __restrict__ n_dev, Geom g,
-                                   unsigned long long* table, uint32_t mask) {
+__device__ __forceinline__ void hash_insert_row(const int32_t* __restrict__ idx, int n, const int* __restrict__ n_dev,
+                                                const Geom& g, unsigned long long* table, uint32_t mask, int row) {
     if (n_dev != nullptr) n = min(n, __ldg(n_dev));
-    int row = blockIdx.x * blockDim.x + threadIdx.x;
     if (row >= n) return;
     int b, c[VC_MAX_NDIM];
     load_index(idx, row, g.ndim, b, c);
@@ -91,6 +90,11 @@ __global__ void hash_insert_kernel(const int32_t* __restrict__ idx, int n, const
     }
 }
 
+__global__ void hash_insert_kernel(const int32_t* __restrict__ idx, int n, const int* __restrict__ n_dev, Geom g,
+                                   unsigned long long* table, uint32_t mask) {
+    hash_insert_row(idx, n, n_dev, g, table, mask, blockIdx.x * blockDim.x + threadIdx.x);
+}
+
 __device__ __forceinline__ int hash_lookup(const unsigned long long* __restrict__ table, uint32_t mask,
                                            unsigned long long key) {
     uint32_t slot = mix64(key) & mask;
@@ -109,18 +113,17 @@ __device__ __forceinline__ int hash_lookup(const unsigned long long* __restrict_
 // nbr[K-1-k, j] = i, the relation the mirrored dgrad already relies on — so the grid covers the offsets k <= centre only
 // and each neighbour found also writes its mirrored entry (the caller fills the rows k > centre with -1 first): half the
 // hash look-ups, the same table.
-__global__ void __launch_bounds__(256) subm_probe_kernel(const int32_t* __restrict__ idx, int n,
-                                                         const int* __restrict__ n_dev, Geom g,
-                                                         const unsigned long long* __restrict__ table,
-                                                         uint32_t mask, int32_t* __restrict__ nbr,
-                                                         int32_t* __restrict__ pair_num, int32_t* __restrict__ rep, int sym) {
+// (one block: rows bx * 256 ..., offset k; the batched overload below runs it for the block's stage)
+__device__ __forceinline__ void subm_probe_block(const int32_t* __restrict__ idx, int n, const int* __restrict__ n_dev,
+                                                 const Geom& g, const unsigned long long* __restrict__ table, uint32_t mask,
+                                                 int32_t* __restrict__ nbr, int32_t* __restrict__ pair_num,
+                                                 int32_t* __restrict__ rep, int sym, int bx, int k) {
     __shared__ int cnt;
     const int pitch = n;                  // table rows are [K][capacity]
     if (n_dev != nullptr) n = min(n, __ldg(n_dev));
     if (threadIdx.x == 0) cnt = 0;
     __syncthreads();
-    const int row = blockIdx.x * blockDim.x + threadIdx.x;
-    const int k = blockIdx.y;
+    const int row = bx * blockDim.x + threadIdx.x;
     int res = -1;
     if (row < n) {
         int centre = 0;
@@ -156,7 +159,7 @@ __global__ void __launch_bounds__(256) subm_probe_kernel(const int32_t* __restri
         nbr[(size_t)k * pitch + row] = res;
     } else if (row < pitch) {
         nbr[(size_t)k * pitch + row] = -1;    // static mode: rows between the count and the capacity have no neighbours
-        if (rep != nullptr && blockIdx.y == 0) rep[row] = -1;
+        if (rep != nullptr && k == 0) rep[row] = -1;
     }
     unsigned m = __ballot_sync(0xffffffffu, res >= 0);
     if ((threadIdx.x & 31) == 0 && m) atomicAdd(&cnt, __popc(m));
@@ -165,6 +168,52 @@ __global__ void __launch_bounds__(256) subm_probe_kernel(const int32_t* __restri
         atomicAdd(&pair_num[k], cnt);
         if (sym && k != g.K - 1 - k) atomicAdd(&pair_num[g.K - 1 - k], cnt);
     }
+}
+
+__global__ void __launch_bounds__(256) subm_probe_kernel(const int32_t* __restrict__ idx, int n,
+                                                         const int* __restrict__ n_dev, Geom g,
+                                                         const unsigned long long* __restrict__ table,
+                                                         uint32_t mask, int32_t* __restrict__ nbr,
+                                                         int32_t* __restrict__ pair_num, int32_t* __restrict__ rep, int sym) {
+    subm_probe_block(idx, n, n_dev, g, table, mask, nbr, pair_num, rep, sym, blockIdx.x, blockIdx.y);
+}
+
+// Batched per-stage index work (subm_rulebook_batch_dev, conv_tables_batch_dev): up to IDX_BATCH_MAX stages in one launch.
+// The grid's x blocks are the stages' row blocks one after the other (stage e owns blocks blk0[e] .. blk0[e + 1] - 1), so a
+// block belongs to one stage and runs exactly what the per-stage launch runs for that block.  Passed by value.
+struct SubmEntry {
+    const int32_t* idx;
+    const int* n_dev;
+    unsigned long long* table;
+    int32_t *nbr, *pair_num;
+    Geom g;
+    int n, ky;   // ky: offsets probed (centre + 1 with the mirrored probe, else K)
+    uint32_t mask;
+};
+struct SubmBatch {
+    int E, sym;
+    int blk0[IDX_BATCH_MAX + 1];
+    SubmEntry e[IDX_BATCH_MAX];
+};
+
+__device__ __forceinline__ int batch_entry(const int* blk0, int E, int bx) {
+    int e = 0;
+    while (e + 1 < E && bx >= blk0[e + 1]) ++e;
+    return e;
+}
+
+__global__ void hash_insert_kernel(const __grid_constant__ SubmBatch sb) {
+    const int i = batch_entry(sb.blk0, sb.E, blockIdx.x);
+    const SubmEntry& e = sb.e[i];
+    hash_insert_row(e.idx, e.n, e.n_dev, e.g, e.table, e.mask, (blockIdx.x - sb.blk0[i]) * blockDim.x + threadIdx.x);
+}
+
+__global__ void __launch_bounds__(256) subm_probe_kernel(const __grid_constant__ SubmBatch sb) {   // grid (blocks, max ky)
+    const int i = batch_entry(sb.blk0, sb.E, blockIdx.x);
+    const SubmEntry& e = sb.e[i];
+    if ((int)blockIdx.y >= e.ky) return;
+    subm_probe_block(e.idx, e.n, e.n_dev, e.g, e.table, e.mask, e.nbr, e.pair_num, nullptr, sb.sym, blockIdx.x - sb.blk0[i],
+                     blockIdx.y);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -400,20 +449,17 @@ __global__ void conv_emit_indices_kernel(const uint32_t* __restrict__ bitmap, co
     }
 }
 
-__global__ void __launch_bounds__(256) conv_tables_kernel(const int32_t* __restrict__ idx, int n, const int* __restrict__ n_dev,
-                                                          int n_out, Geom g,
-                                                          const uint32_t* __restrict__ bitmap,
-                                                          const uint32_t* __restrict__ word_rank,
-                                                          const uint32_t* __restrict__ block_sum,
-                                                          int32_t* __restrict__ nbr_fwd, int32_t* __restrict__ nbr_bwd,
-                                                          int32_t* __restrict__ pair_num) {   // grid (rows, K)
+__device__ __forceinline__ void conv_tables_block(const int32_t* __restrict__ idx, int n, const int* __restrict__ n_dev,
+                                                  int n_out, const Geom& g, const uint32_t* __restrict__ bitmap,
+                                                  const uint32_t* __restrict__ word_rank,
+                                                  const uint32_t* __restrict__ block_sum, int32_t* __restrict__ nbr_fwd,
+                                                  int32_t* __restrict__ nbr_bwd, int32_t* __restrict__ pair_num, int bx, int k) {
     __shared__ int cnt;
     const int pitch_in = n;               // nbr_bwd rows are [K][input capacity], nbr_fwd rows [K][n_out = output capacity]
     if (n_dev != nullptr) n = min(n, __ldg(n_dev));
     if (threadIdx.x == 0) cnt = 0;
     __syncthreads();
-    const int row = blockIdx.x * blockDim.x + threadIdx.x;
-    const int k = blockIdx.y;
+    const int row = bx * blockDim.x + threadIdx.x;
     int orow = -1;
     if (row < n) {
         int b, c[VC_MAX_NDIM];
@@ -432,6 +478,38 @@ __global__ void __launch_bounds__(256) conv_tables_kernel(const int32_t* __restr
     if ((threadIdx.x & 31) == 0 && m) atomicAdd(&cnt, __popc(m));
     __syncthreads();
     if (pair_num != nullptr && threadIdx.x == 0 && cnt) atomicAdd(&pair_num[k], cnt);
+}
+
+__global__ void __launch_bounds__(256) conv_tables_kernel(const int32_t* __restrict__ idx, int n, const int* __restrict__ n_dev,
+                                                          int n_out, Geom g,
+                                                          const uint32_t* __restrict__ bitmap,
+                                                          const uint32_t* __restrict__ word_rank,
+                                                          const uint32_t* __restrict__ block_sum,
+                                                          int32_t* __restrict__ nbr_fwd, int32_t* __restrict__ nbr_bwd,
+                                                          int32_t* __restrict__ pair_num) {   // grid (rows, K)
+    conv_tables_block(idx, n, n_dev, n_out, g, bitmap, word_rank, block_sum, nbr_fwd, nbr_bwd, pair_num, blockIdx.x, blockIdx.y);
+}
+
+struct TablesEntry {
+    const int32_t* idx;
+    const int* n_dev;
+    ConvRank r;
+    int32_t *nbr_fwd, *nbr_bwd, *pair_num;
+    Geom g;
+    int n, n_out;
+};
+struct TablesBatch {
+    int E;
+    int blk0[IDX_BATCH_MAX + 1];
+    TablesEntry e[IDX_BATCH_MAX];
+};
+
+__global__ void __launch_bounds__(256) conv_tables_kernel(const __grid_constant__ TablesBatch tb) {   // grid (blocks, max K)
+    const int i = batch_entry(tb.blk0, tb.E, blockIdx.x);
+    const TablesEntry& e = tb.e[i];
+    if ((int)blockIdx.y >= e.g.K) return;
+    conv_tables_block(e.idx, e.n, e.n_dev, e.n_out, e.g, e.r.bitmap, e.r.word_rank, e.r.block_sum, e.nbr_fwd, e.nbr_bwd,
+                      e.pair_num, blockIdx.x - tb.blk0[i], blockIdx.y);
 }
 
 // one block per offset: order-preserving compaction of nbr[k, :] into spconv-style pairs
@@ -531,8 +609,7 @@ int vc::subm_rulebook_dev(const int32_t* indices, int n, const int* n_dev, int n
     VC_CUDA(cudaMemsetAsync(table, 0xFF, (size_t)slots * 8, stream));
     hash_insert_kernel<<<cdiv(n, 256), 256, 0, stream>>>(indices, n, n_dev, g, table, slots - 1);
     VC_LAUNCH_CHECK();
-    bool sym = unique && rep == nullptr;
-    for (int d = 0; d < ndim; ++d) sym &= (g.ksize[d] & 1) == 1;
+    const bool sym = rep == nullptr && subm_sym(ndim, ksize, unique);
     const int centre = g.K / 2;   // (odd kernel sizes: the centre offset is the middle one)
     if (sym) VC_CUDA(cudaMemsetAsync(nbr + (size_t)(centre + 1) * n, 0xFF, sizeof(int32_t) * (size_t)(g.K - 1 - centre) * n, stream));
     subm_probe_kernel<<<dim3(cdiv(n, 256), sym ? centre + 1 : g.K), 256, 0, stream>>>(indices, n, n_dev, g, table, slots - 1, nbr,
@@ -687,6 +764,80 @@ int vc::conv_rulebook_tables_dev(const int32_t* indices, int n, const int* n_dev
                                                                          rank.block_sum, nbr_fwd, nbr_bwd, pair_num);
         VC_LAUNCH_CHECK();
     }
+    return VC_OK;
+}
+
+bool vc::subm_sym(int ndim, const int32_t* ksize, bool unique) {
+    bool sym = unique;
+    for (int d = 0; d < ndim; ++d) sym &= (ksize[d] & 1) == 1;
+    return sym;
+}
+
+// The launches of subm_rulebook_dev (rep == NULL) for up to IDX_BATCH_MAX stages: one hash insert and one probe.  The caller
+// has cleared every stage's table (0xFF), its mirrored rows k > centre (-1, when subm_sym) and its pair counts.
+int vc::subm_rulebook_batch_dev(const SubmStage* st, int n_st, int batch_size, bool unique, cudaStream_t stream) {
+    VC_CHECK_ARG(n_st >= 1 && n_st <= IDX_BATCH_MAX, "%d stages in one batch", n_st);
+    SubmBatch sb;
+    memset(&sb, 0, sizeof(sb));
+    sb.sym = -1;
+    int ky = 1;
+    for (int i = 0; i < n_st; ++i) {
+        const SubmStage& s = st[i];
+        SubmEntry& e = sb.e[sb.E];
+        int rc = make_geom(e.g, s.ndim, batch_size, s.shape, s.ksize, nullptr, nullptr, s.dil);
+        if (rc) return rc;
+        VC_CHECK_ARG(s.n >= 0 && s.n < (1 << ROW_BITS), "row count %d out of range", s.n);
+        double cells = (double)batch_size;
+        for (int d = 0; d < s.ndim; ++d) cells *= e.g.shape[d];
+        VC_CHECK_ARG(cells < 1099511627776.0, "grid too large for 40-bit keys");
+        const int sym = subm_sym(s.ndim, s.ksize, unique) ? 1 : 0;
+        VC_CHECK_ARG(sb.sym < 0 || sb.sym == sym, "stages of one batch probe alike");
+        sb.sym = sym;
+        if (s.n == 0) continue;
+        VC_CHECK_ARG(s.idx && s.nbr && s.table, "null pointer");
+        const uint32_t slots = table_slots(s.n);
+        if (s.table_bytes < (size_t)slots * 8) {
+            set_error("subm rulebook workspace %zu < %zu", s.table_bytes, (size_t)slots * 8);
+            return VC_ERR_WORKSPACE;
+        }
+        e.idx = s.idx; e.n = s.n; e.n_dev = s.n_dev; e.table = (unsigned long long*)s.table; e.mask = slots - 1;
+        e.nbr = s.nbr; e.pair_num = s.pair_num;
+        e.ky = sym ? e.g.K / 2 + 1 : e.g.K;
+        ky = e.ky > ky ? e.ky : ky;
+        sb.blk0[sb.E + 1] = sb.blk0[sb.E] + cdiv(s.n, 256);
+        ++sb.E;
+    }
+    if (sb.E == 0) return VC_OK;
+    hash_insert_kernel<<<sb.blk0[sb.E], 256, 0, stream>>>(sb);
+    VC_LAUNCH_CHECK();
+    subm_probe_kernel<<<dim3(sb.blk0[sb.E], ky), 256, 0, stream>>>(sb);
+    VC_LAUNCH_CHECK();
+    return VC_OK;
+}
+
+// conv_rulebook_tables_dev's kernel for up to IDX_BATCH_MAX strided convs in one launch.  The caller has filled every nbr_fwd
+// with -1 and zeroed the pair counts.
+int vc::conv_tables_batch_dev(const TablesStage* st, int n_st, int batch_size, cudaStream_t stream) {
+    VC_CHECK_ARG(n_st >= 1 && n_st <= IDX_BATCH_MAX, "%d stages in one batch", n_st);
+    TablesBatch tb;
+    memset(&tb, 0, sizeof(tb));
+    int K = 1;
+    for (int i = 0; i < n_st; ++i) {
+        const TablesStage& s = st[i];
+        TablesEntry& e = tb.e[tb.E];
+        int rc = make_geom(e.g, s.ndim, batch_size, s.shape, s.ksize, s.stride, s.pad, s.dil);
+        if (rc) return rc;
+        if (s.n == 0) continue;
+        VC_CHECK_ARG(s.idx && s.nbr_bwd && (s.n_out == 0 || s.nbr_fwd), "null pointer");
+        e.idx = s.idx; e.n = s.n; e.n_dev = s.n_dev; e.n_out = s.n_out; e.r = s.rank;
+        e.nbr_fwd = s.nbr_fwd; e.nbr_bwd = s.nbr_bwd; e.pair_num = s.pair_num;
+        K = e.g.K > K ? e.g.K : K;
+        tb.blk0[tb.E + 1] = tb.blk0[tb.E] + cdiv(s.n, 256);
+        ++tb.E;
+    }
+    if (tb.E == 0) return VC_OK;
+    conv_tables_kernel<<<dim3(tb.blk0[tb.E], K), 256, 0, stream>>>(tb);
+    VC_LAUNCH_CHECK();
     return VC_OK;
 }
 
