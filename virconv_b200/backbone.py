@@ -38,6 +38,9 @@ def _cfg_get(cfg, key, default=None):
     return getattr(cfg, key, default) if not hasattr(cfg, 'get') else cfg.get(key, default)
 
 
+norm_fn = partial(nn.BatchNorm1d, eps=1e-3, momentum=0.01)
+
+
 def sparse_block(cin, cout, kernel_size, norm_fn, ndim=3, conv_type='subm', stride=1, padding=0, indice_key=None):
     """conv(bias=False) -> norm -> ReLU, as post_act_block / post_act_block2d (:86-131)."""
     if conv_type == 'subm':
@@ -59,7 +62,6 @@ class NRConvBlock(nn.Module):
         super().__init__()
         self.stride = stride
         self.conv_depth = conv_depth
-        norm_fn = partial(nn.BatchNorm1d, eps=1e-3, momentum=0.01)
         if stride > 1:
             self.down_layer = sparse_block(input_c, output_c, 3, norm_fn, 3, 'spconv', stride, padding,
                                            'sp' + indice_key)
@@ -185,84 +187,190 @@ def discard_rows(t, keep_rows):
     return spconv.SparseConvTensor(feats, idx, t.spatial_shape, t.batch_size)
 
 
-class VirConvL8x(nn.Module):
-    """VirConv-L backbone (fused LiDAR + virtual stream), spconv_backbone.py:538-699."""
+def _copy_transform(batch_dict, i):
+    """The augmentation of transformed copy i: transform_param[:, i] (X_TRANS copies), else aug_param."""
+    if 'transform_param' in batch_dict:
+        return batch_dict['transform_param'][:, i, :]
+    return batch_dict.get('aug_param')
 
-    def __init__(self, model_cfg, input_channels, grid_size, discard_mode='spconv2_compat', precision='fp32',
-                 discard_rng='numpy', **kwargs):
+
+def _publish(batch_dict, sfx, xs, out=None, stream=''):
+    """The keys the detector reads for copy `sfx`: x_conv1..4 (`xs`; None where the eval forward of VirConv8x publishes
+    none) and the encoded tensor `out`.  stream='_mm': VirConv8x's virtual-point stream, which has no encoded tensor and puts
+    '_mm' before the copy suffix — but not in its strides key, as the reference writes it (spconv_backbone.py:527)."""
+    if out is not None:
+        batch_dict['encoded_spconv_tensor' + sfx] = out
+    batch_dict.update({
+        'encoded_spconv_tensor_stride' + stream + sfx: 8,
+        'multi_scale_3d_features' + stream + sfx: dict(zip(('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4'), xs)),
+        'multi_scale_3d_strides' + sfx: {'x_conv1': 1, 'x_conv2': 2, 'x_conv3': 4, 'x_conv4': 8},
+    })
+
+
+class _VirConvBackbone(nn.Module):
+    """What VirConvL8x and VirConv8x share: the config, conv_out, and the virtual-point stream — vir_conv1..4 with the StVD
+    layer discards — run through a cached executor plan or on the per-operator module path."""
+
+    # VirConv8x also discards the stream's input voxels (:489-490): discard site 0, the blocks' sites follow it
+    _input_discard = False
+
+    def __init__(self, model_cfg, grid_size, discard_mode, discard_rng):
         super().__init__()
         self.model_cfg = model_cfg
         self.return_num_features_as_dict = _cfg_get(model_cfg, 'RETURN_NUM_FEATURES_AS_DICT', False)
         self.out_features = _cfg_get(model_cfg, 'OUT_FEATURES', 64)
         self.layer_discard_rate = _cfg_get(model_cfg, 'LAYER_DISCARD_RATE', 0.0)
-        num_filters = list(_cfg_get(model_cfg, 'NUM_FILTERS', [16, 32, 64, 64]))
+        self.num_filters = list(_cfg_get(model_cfg, 'NUM_FILTERS', [16, 32, 64, 64]))
         assert discard_mode in ('spconv2_compat', 'paper')
         assert discard_rng in ('numpy', 'device')
         self.discard_mode, self.discard_rng = discard_mode, discard_rng
-        norm_fn = partial(nn.BatchNorm1d, eps=1e-3, momentum=0.01)
         gs = [int(g) for g in grid_size]
         self.sparse_shape = [gs[2] + 1, gs[1], gs[0]]            # grid_size[::-1] + [1, 0, 0]   (:552)
-
-        self.vir_conv1 = NRConvBlock(input_channels, num_filters[0], stride=1, indice_key='vir1')
-        self.vir_conv2 = NRConvBlock(num_filters[0], num_filters[1], stride=2, indice_key='vir2')
-        self.vir_conv3 = NRConvBlock(num_filters[1], num_filters[2], stride=2, indice_key='vir3')
-        self.vir_conv4 = NRConvBlock(num_filters[2], num_filters[3], stride=2, padding=(0, 1, 1), indice_key='vir4')
-        last_pad = _cfg_get(model_cfg, 'last_pad', 0)
-        self.conv_out = spconv.SparseSequential(
-            spconv.SparseConv3d(num_filters[3], self.out_features, (3, 1, 1), stride=(2, 1, 1), padding=last_pad,
-                                bias=False, indice_key='spconv_down2'),
-            norm_fn(self.out_features), nn.ReLU())
-        spconv.set_precision(self, precision)
         self.num_point_features = self.out_features
         if self.return_num_features_as_dict:
-            self.num_point_features = {'x_conv%d' % (i + 1): num_filters[i] for i in range(4)}
+            self.num_point_features = {'x_conv%d' % (i + 1): self.num_filters[i] for i in range(4)}
 
-    def _maybe_discard(self, t, batch_dict, layer):
-        if not self.training or self.discard_mode != 'paper' or self.layer_discard_rate == 0:
-            return t
-        given = batch_dict.get('stvd_keep_rows')
-        keep = given[layer] if given is not None else stvd_keep_rows(t.features.shape[0], self.layer_discard_rate)
-        return discard_rows(t, keep)
+    def _add_nrconv_blocks(self, input_channels):
+        f = self.num_filters
+        self.vir_conv1 = NRConvBlock(input_channels, f[0], stride=1, indice_key='vir1')
+        self.vir_conv2 = NRConvBlock(f[0], f[1], stride=2, indice_key='vir2')
+        self.vir_conv3 = NRConvBlock(f[1], f[2], stride=2, indice_key='vir3')
+        self.vir_conv4 = NRConvBlock(f[2], f[3], stride=2, padding=(0, 1, 1), indice_key='vir4')
 
+    def _add_conv_out(self):
+        last_pad = _cfg_get(self.model_cfg, 'last_pad', 0)
+        self.conv_out = spconv.SparseSequential(
+            spconv.SparseConv3d(self.num_filters[3], self.out_features, (3, 1, 1), stride=(2, 1, 1), padding=last_pad,
+                                bias=False, indice_key='spconv_down2'),
+            norm_fn(self.out_features), nn.ReLU())
+
+    # -- StVD layer discard ----------------------------------------------------------------------------------
     def _discarding(self):
         return self.training and self.discard_mode == 'paper' and self.layer_discard_rate != 0
 
     def _device_discard(self):
         return self._discarding() and self.discard_rng == 'device'
 
-    # -- native plan (csrc/executor.cu): the whole forward / backward in one C-ABI call each -------------------
-    def _plan(self):
-        """The plan of the current mode: with the three layer discards (sites 0-2, after vir_conv1..3) in a device-drawn
-        paper-mode training forward, without them otherwise; both are cached."""
-        stvd = self._device_discard()
-        attr = '_plan_stvd_cache' if stvd else '_plan_cache'
-        if getattr(self, attr, None) is None:
-            plan = executor.Plan(self.vir_conv1.d3_conv1[0].in_channels)
-            f, iset = 0, 0
-            for i, (blk, s) in enumerate(zip((self.vir_conv1, self.vir_conv2, self.vir_conv3, self.vir_conv4), (1, 2, 4, 8))):
-                f, iset = plan_nrconv(plan, blk, f, iset, s)
-                if stvd and i < 3:
-                    f, iset = plan.discard(f, iset, i, self.layer_discard_rate)
-                plan.publish('x_conv%d' % (i + 1), f, iset)
-            conv = self.conv_out[0]
-            iset, rb = plan.conv_rb(iset, 3, conv.kernel_size, conv.stride, conv.padding, conv.dilation, keys=[conv.indice_key])
-            plan.publish('out', plan.cbr(f, rb, conv, self.conv_out[1], seq=self.conv_out), iset)
+    def _host_discard(self, batch_dict):
+        """Kept rows drawn on the host or given in batch_dict['stvd_keep_rows']: applied on the module path (a device draw
+        runs in the plan)."""
+        return self._discarding() and (self.discard_rng != 'device' or batch_dict.get('stvd_keep_rows') is not None)
+
+    def _maybe_discard(self, t, batch_dict, site):
+        if not self._discarding():
+            return t
+        given = batch_dict.get('stvd_keep_rows')
+        keep = given[site] if given is not None else stvd_keep_rows(t.features.shape[0], self.layer_discard_rate)
+        return discard_rows(t, keep)
+
+    # -- native plans (csrc/executor.cu): the whole forward / backward of a stream in one C-ABI call each ------
+    def _cached_plan(self, attr, build):
+        """The plan cached under `attr`, rebuilt by build() when there is none or it is stale (a sub-module was replaced after
+        it was built, e.g. by SyncBatchNorm conversion).  Copies and pickles of the model drop it (executor.Plan)."""
+        plan = getattr(self, attr, None)
+        if plan is None or not plan.is_current():
+            plan = build()
             setattr(self, attr, plan)
-        return getattr(self, attr)
+        return plan
+
+    def _nrconv_plan(self, stvd):
+        """The virtual-point stream as a plan -> (plan, feature slot, index set) of its last block.  stvd: with the
+        device-drawn layer discards, numbered in stream order — the input voxels (site 0) where the class discards them, then
+        after vir_conv1..3."""
+        plan = executor.Plan(self.vir_conv1.d3_conv1[0].in_channels)
+        f, iset = 0, 0
+        first = int(self._input_discard)
+        if stvd and self._input_discard:
+            f, iset = plan.discard(f, iset, 0, self.layer_discard_rate)
+        for i, (blk, s) in enumerate(zip((self.vir_conv1, self.vir_conv2, self.vir_conv3, self.vir_conv4), (1, 2, 4, 8))):
+            f, iset = plan_nrconv(plan, blk, f, iset, s)
+            if stvd and i < 3:
+                f, iset = plan.discard(f, iset, first + i, self.layer_discard_rate)
+            plan.publish('x_conv%d' % (i + 1), f, iset)
+        return plan, f, iset
+
+    def _plan_conv_out(self, plan, f, iset):
+        """Append conv_out to `plan`, its output published as 'out'."""
+        co = self.conv_out[0]
+        iset, rb = plan.conv_rb(iset, 3, co.kernel_size, co.stride, co.padding, co.dilation, keys=[co.indice_key])
+        plan.publish('out', plan.cbr(f, rb, co, self.conv_out[1], seq=self.conv_out), iset)
+        return plan
+
+    def _run(self, plan, feats, coords, shape, batch_size, proj, stream, seed=None, static=None, inputs_ready=False):
+        """-> (run record, published tensors).  stream: the executor.note_last_run key of the input stream; static: its
+        StaticSpec (capacity-sized feats / coords)."""
+        ci = spconv._as_i32(coords)
+        run, res = executor.run_plan(plan, feats, ci, shape, batch_size, proj, plan.layers[0][1].training,
+                                     plan.layers[0][0].precision, inputs_ready=inputs_ready, static=static, seed=seed)
+        # (graph.GraphedStep sizes each stream's capacities from an exact run.)  The default stream '' is left to
+        # note_last_run's default, so that wrappers of it taking (model, run) keep working for one-stream models
+        if stream:
+            executor.note_last_run(self, run, stream)
+        else:
+            executor.note_last_run(self, run)
+        return run, _published_tensors(run, res, [name for name, _, _ in plan.published], ci, shape, batch_size)
+
+    def _plan_inputs(self, batch_dict, feats, coords, static, stvd, side):
+        """-> (int32 coordinates, StVD seed or None, inputs_ready) of a plan run of the virtual-point stream."""
+        return spconv._as_i32(coords), (stvd_seed(batch_dict, feats.device) if stvd else None), False
+
+    def _nrconv_stream(self, batch_dict, plan, feats, coords, trans, sfx, stream, proj=None, static=None, out=None,
+                       refusal=None):
+        """The virtual-point stream of one copy (batch-key suffix `sfx`, note_last_run key `stream`) -> its published tensors:
+        x_conv1..4, then `out`'s (VirConvL8x's conv_out, which `plan` ends with).  Runs `plan` when _module_path_reason
+        allows it, else the module path with the same discard sites — or raises ValueError(refusal % reason) when given.
+        proj: the [B,28] projection block on the device, else made from batch_dict['calib'] and `trans`; static: the
+        StaticSpec of a static-mode run.  A device-drawn discard records its kept rows in 'stvd_kept_rows' + sfx."""
+        batch_size = batch_dict['batch_size']
+        reason = _module_path_reason(feats, plan, self._host_discard(batch_dict))
+        if reason is None:
+            side = ops.side(feats.device).stream if executor.TWO_STREAMS else None
+            ci, seed, ready = self._plan_inputs(batch_dict, feats, coords, static, bool(plan.discards), side)
+            if proj is None:
+                assert static is None, "static mode needs batch_dict['virconv_proj'] (ops.projection_params on the device)"
+                proj = ops.projection_params(batch_dict.get('calib'), trans, batch_size, feats.device, side)
+            run, xs = self._run(plan, feats, ci, self.sparse_shape, batch_size, proj, stream, seed, static, ready)
+            if seed is not None:
+                batch_dict['stvd_kept_rows' + sfx] = run.kept_rows()
+            return xs
+        if refusal is not None:
+            raise ValueError(refusal % reason)
+        _module_path_under_determinism(reason)
+        proj = ops.projection_params(batch_dict.get('calib'), trans, batch_size, feats.device)
+        x = spconv.SparseConvTensor(feats, coords.int(), self.sparse_shape, batch_size)
+        first = int(self._input_discard)
+        if self._input_discard:
+            x = self._maybe_discard(x, batch_dict, 0)
+        xs = []
+        for i, (blk, s) in enumerate(zip((self.vir_conv1, self.vir_conv2, self.vir_conv3, self.vir_conv4), (1, 2, 4, 8))):
+            x = blk(x, batch_size, proj, s)
+            if i < 3:
+                x = self._maybe_discard(x, batch_dict, first + i)
+            xs.append(x)
+        if out is not None:
+            xs.append(out(x))
+        return tuple(xs)
+
+
+class VirConvL8x(_VirConvBackbone):
+    """VirConv-L backbone (fused LiDAR + virtual stream), spconv_backbone.py:538-699."""
+
+    def __init__(self, model_cfg, input_channels, grid_size, discard_mode='spconv2_compat', precision='fp32',
+                 discard_rng='numpy', **kwargs):
+        super().__init__(model_cfg, grid_size, discard_mode, discard_rng)
+        self._add_nrconv_blocks(input_channels)
+        self._add_conv_out()
+        spconv.set_precision(self, precision)
+
+    def _plan(self):
+        """The plan of the current mode: the virtual-point stream and conv_out, with the three layer discards (sites 0-2,
+        after vir_conv1..3) in a device-drawn paper-mode training forward, without them otherwise; both are cached."""
+        stvd = self._device_discard()
+        return self._cached_plan('_plan_stvd_cache' if stvd else '_plan_cache',
+                                 lambda: self._plan_conv_out(*self._nrconv_plan(stvd)))
 
     def _use_plan(self, feats, batch_dict=None):
-        if not executor.ENABLED or not feats.is_cuda or feats.shape[0] == 0 or feats.requires_grad:
-            return False             # (the plan does not propagate a gradient into the voxel features; the module path does)
-        if self._discarding() and (self.discard_rng != 'device' or (batch_dict or {}).get('stvd_keep_rows') is not None):
-            return False             # host-drawn or caller-given kept rows: the module path
-        plan = self._plan()
-        if not plan.is_current():          # a sub-module was replaced after the plan was built (e.g. SyncBatchNorm conversion)
-            self._plan_cache = self._plan_stvd_cache = None
-            plan = self._plan()
-        if not plan.eligible():            # (checked every forward: dtype / layout / module type may change under .half(), .to())
-            return False
-        mode = plan.layers[0][1].training
-        return all(bn.training == mode for _, bn in plan.layers)
+        return _module_path_reason(feats, self._plan(), self._host_discard(batch_dict or {})) is None
 
     def index_phase(self, batch_dict):
         """Phased static execution (graph.PipelinedStep), phase 1: everything of the forward that depends on the voxel
@@ -272,91 +380,46 @@ class VirConvL8x(nn.Module):
         feats, coords = batch_dict['voxel_features'], batch_dict['voxel_coords']
         static = batch_dict['virconv_static']
         assert static.phase == 1 and self._use_plan(feats, batch_dict)
+        plan = self._plan()
         ci = spconv._as_i32(coords)
         # (the layer discards select their rows in this phase; the feature phase gathers with the same seed)
-        seed = stvd_seed(batch_dict, feats.device) if self._device_discard() else None
-        executor.run_index(self._plan(), feats, ci, self.sparse_shape, batch_dict['batch_size'], batch_dict['virconv_proj'],
-                           self.conv_out[1].training, self.conv_out[0].precision, static, seed)
+        seed = stvd_seed(batch_dict, feats.device) if plan.discards else None
+        executor.run_index(plan, feats, ci, self.sparse_shape, batch_dict['batch_size'], batch_dict['virconv_proj'],
+                           plan.layers[0][1].training, plan.layers[0][0].precision, static, seed)
         batch_dict['virconv_ci'] = ci
         batch_dict['virconv_stvd_seed'] = seed
         return batch_dict
 
+    def _plan_inputs(self, batch_dict, feats, coords, static, stvd, side):
+        if static is not None and static.phase == 2:
+            return batch_dict['virconv_ci'], batch_dict['virconv_stvd_seed'], False     # (index_phase of this very batch)
+        seed = stvd_seed(batch_dict, feats.device) if stvd else None
+        # 'virconv_inputs_ready': the caller's promise that voxel_coords is resident and complete (a prefetched batch) -> the
+        # index pipeline of this step (starting with the .int() of the coordinates, :641) runs on the side stream without
+        # waiting for main, i.e. it may overlap the previous step's backward
+        ready = side is not None and static is None and seed is None and bool(batch_dict.get('virconv_inputs_ready', False))
+        if ready and (coords.dtype != torch.int32 or not coords.is_contiguous()):
+            executor.reserve_blocks('coords_i32', 4 * coords.numel(), feats.device, side)
+            with torch.cuda.stream(side):
+                ci = spconv._as_i32(coords)
+            ci.record_stream(torch.cuda.current_stream(feats.device))   # published as x_conv1's indices
+            return ci, seed, ready
+        return spconv._as_i32(coords), seed, ready
+
     def forward(self, batch_dict):
+        """Static mode ('virconv_static': executor.StaticSpec): capacity-sized inputs + device row count, projection block
+        already on the device ('virconv_proj', [B,28], ops.projection_params) — nothing reads a device value or uploads from
+        pageable memory, so the call can be captured into a CUDA graph."""
         rot_num = batch_dict['transform_param'].shape[1] if 'transform_param' in batch_dict else 1
-        batch_size = batch_dict['batch_size']
-        calib = batch_dict['calib']
         ops.stats_arena(batch_dict['voxel_features'].device).reset()    # one memset for all BN accumulators of this pass
         for i in range(rot_num):
             rid = '' if i == 0 else str(i)
-            feats, coords = batch_dict['voxel_features' + rid], batch_dict['voxel_coords' + rid]
+            feats = batch_dict['voxel_features' + rid]
             feats[:, 4:7] = 0                                    # RGB channels unused (:636), in place like the reference
-            trans = batch_dict['aug_param'] if 'aug_param' in batch_dict else None
-            if 'transform_param' in batch_dict:
-                trans = batch_dict['transform_param'][:, i, :]
-            if self._use_plan(feats, batch_dict):
-                bn_training = self.conv_out[1].training
-                # 'virconv_inputs_ready': the caller's promise that voxel_coords is resident and complete (a prefetched
-                # batch) -> the index pipeline of this step (starting with the .int() of the coordinates, :641) runs on
-                # the side stream without waiting for main, i.e. it may overlap the previous step's backward
-                side = ops.side(feats.device).stream if executor.TWO_STREAMS else None
-                static = batch_dict.get('virconv_static')
-                seed = None
-                if self._device_discard():
-                    seed = batch_dict['virconv_stvd_seed'] if static is not None and static.phase == 2 else \
-                        stvd_seed(batch_dict, feats.device)
-                ready = (side is not None and static is None and seed is None
-                         and bool(batch_dict.get('virconv_inputs_ready', False)))
-                if static is not None and static.phase == 2:
-                    ci = batch_dict['virconv_ci']           # (built by index_phase for this very batch)
-                elif ready and (coords.dtype != torch.int32 or not coords.is_contiguous()):
-                    executor.reserve_blocks('coords_i32', 4 * coords.numel(), feats.device, side)
-                    with torch.cuda.stream(side):
-                        ci = spconv._as_i32(coords)
-                    ci.record_stream(torch.cuda.current_stream(feats.device))   # published as x_conv1's indices
-                else:
-                    ci = spconv._as_i32(coords)
-                # static mode ('virconv_static': executor.StaticSpec): capacity-sized inputs + device row count, projection
-                # block already on the device ('virconv_proj', [B,28], ops.projection_params) — nothing below reads a
-                # device value or uploads from pageable memory, so the call can be captured into a CUDA graph
-                proj = batch_dict.get('virconv_proj')
-                if proj is None:
-                    assert static is None, "static mode needs batch_dict['virconv_proj'] (ops.projection_params on the device)"
-                    proj = ops.projection_params(calib, trans, batch_size, feats.device, side)
-                run, res = executor.run_plan(self._plan(), feats, ci, self.sparse_shape, batch_size, proj, bn_training,
-                                             self.conv_out[0].precision, inputs_ready=ready, static=static, seed=seed)
-                executor.note_last_run(self, run)   # (graph.GraphedStep sizes its capacities from an exact-mode run)
-                x1, x2, x3, x4, out = _published_tensors(run, res, ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4', 'out'), ci,
-                                                         self.sparse_shape, batch_size)
-                if seed is not None:
-                    batch_dict['stvd_kept_rows' + rid] = run.kept_rows()
-                batch_dict.update({
-                    'encoded_spconv_tensor' + rid: out,
-                    'encoded_spconv_tensor_stride' + rid: 8,
-                    'multi_scale_3d_features' + rid: {'x_conv1': x1, 'x_conv2': x2, 'x_conv3': x3, 'x_conv4': x4},
-                    'multi_scale_3d_strides' + rid: {'x_conv1': 1, 'x_conv2': 2, 'x_conv3': 4, 'x_conv4': 8},
-                })
-                continue
-            _module_path_under_determinism(_module_path_reason(
-                feats, self._plan() if executor.ENABLED and feats.is_cuda else None,
-                self._discarding() and (self.discard_rng != 'device' or batch_dict.get('stvd_keep_rows') is not None)))
-            proj = ops.projection_params(calib, trans, batch_size, feats.device)
-            x = spconv.SparseConvTensor(feats, coords.int(), self.sparse_shape, batch_size)
-
-            x1 = self.vir_conv1(x, batch_size, proj, 1)
-            x1 = self._maybe_discard(x1, batch_dict, 0)
-            x2 = self.vir_conv2(x1, batch_size, proj, 2)
-            x2 = self._maybe_discard(x2, batch_dict, 1)
-            x3 = self.vir_conv3(x2, batch_size, proj, 4)
-            x3 = self._maybe_discard(x3, batch_dict, 2)
-            x4 = self.vir_conv4(x3, batch_size, proj, 8)
-            out = self.conv_out(x4)
-
-            batch_dict.update({
-                'encoded_spconv_tensor' + rid: out,
-                'encoded_spconv_tensor_stride' + rid: 8,
-                'multi_scale_3d_features' + rid: {'x_conv1': x1, 'x_conv2': x2, 'x_conv3': x3, 'x_conv4': x4},
-                'multi_scale_3d_strides' + rid: {'x_conv1': 1, 'x_conv2': 2, 'x_conv3': 4, 'x_conv4': 8},
-            })
+            *xs, out = self._nrconv_stream(batch_dict, self._plan(), feats, batch_dict['voxel_coords' + rid],
+                                           _copy_transform(batch_dict, i), rid, '', proj=batch_dict.get('virconv_proj'),
+                                           static=batch_dict.get('virconv_static'), out=self.conv_out)
+            _publish(batch_dict, rid, xs, out)
         return batch_dict
 
 
@@ -375,19 +438,24 @@ def _module_path_under_determinism(reason):
 
 
 def _module_path_reason(feats, plan=None, discard=False):
+    """None when a forward over `feats` may run through the executor `plan`, else why it takes the per-operator module path.
+    discard: it applies host-drawn or caller-given StVD kept rows.  Without a plan (a caller that only knows the plan did
+    not run) the last reason is assumed."""
     if not executor.ENABLED:
         return 'VIRCONV_EXECUTOR=0'
     if not feats.is_cuda:
         return 'features not on a CUDA device'
     if feats.shape[0] == 0:
         return 'no input voxels'
-    if feats.requires_grad:
+    if feats.requires_grad:          # (the plan does not propagate a gradient into the voxel features; the module path does)
         return 'gradient into the voxel features'
     if discard:
         return 'host-drawn or caller-given StVD layer discard'
-    if plan is not None and not plan.eligible():
+    if plan is not None and not plan.eligible():    # (dtype / layout / module type may change under .half(), .to())
         return 'SyncBatchNorm, momentum=None, bias or a non-fp32 module'
-    return 'BatchNorm layers in mixed train / eval modes'
+    if plan is None or any(bn.training != plan.layers[0][1].training for _, bn in plan.layers):
+        return 'BatchNorm layers in mixed train / eval modes'
+    return None
 
 
 def decompose_tensor(t, i, batch_size):
@@ -422,7 +490,7 @@ class EvalStaticSpec:
         return len(self.lidar_counts)
 
 
-class VirConv8x(nn.Module):
+class VirConv8x(_VirConvBackbone):
     """VirConv-T / VirConv-S backbone (spconv_backbone.py:232-535): a LiDAR stream whose submanifold convs share one
     rulebook per stage (indice_keys 'subm1'..'subm4') plus, when `MM`, the virtual-point stream of NRConv blocks.
     Eval mode batches the ROT_NUM transformed copies along x into one [D, H, 4W] tensor (:360,:418-432) and splits the
@@ -437,22 +505,13 @@ class VirConv8x(nn.Module):
     EvalStaticSpec in batch_dict['virconv_eval_static']: ops.xbatch_pack -> the LiDAR plan over [D, H, 4W] ->
     ops.xbatch_split of x_conv3, x_conv4 and out, and one static run of the virtual-point plan per copy."""
 
+    _input_discard = True
+
     def __init__(self, model_cfg, input_channels, grid_size, discard_mode='spconv2_compat', precision='fp32',
                  discard_rng='numpy', **kwargs):
-        super().__init__()
-        self.model_cfg = model_cfg
-        self.return_num_features_as_dict = _cfg_get(model_cfg, 'RETURN_NUM_FEATURES_AS_DICT', False)
-        self.out_features = _cfg_get(model_cfg, 'OUT_FEATURES', 64)
-        self.layer_discard_rate = _cfg_get(model_cfg, 'LAYER_DISCARD_RATE', 0.0)
-        f = list(_cfg_get(model_cfg, 'NUM_FILTERS', [16, 32, 64, 64]))
+        super().__init__(model_cfg, grid_size, discard_mode, discard_rng)
+        f = self.num_filters
         self.mm = bool(_cfg_get(model_cfg, 'MM', False))
-        assert discard_mode in ('spconv2_compat', 'paper')
-        assert discard_rng in ('numpy', 'device')
-        self.discard_mode, self.discard_rng = discard_mode, discard_rng
-        norm_fn = partial(nn.BatchNorm1d, eps=1e-3, momentum=0.01)
-        gs = [int(g) for g in grid_size]
-        self.sparse_shape = [gs[2] + 1, gs[1], gs[0]]
-
         self.conv_input = spconv.SparseSequential(
             spconv.SubMConv3d(input_channels, f[0], 3, padding=1, bias=False, indice_key='subm1'), norm_fn(f[0]), nn.ReLU())
         sub = lambda ci, co, key: sparse_block(ci, co, 3, norm_fn, 3, 'subm', padding=1, indice_key=key)
@@ -462,24 +521,15 @@ class VirConv8x(nn.Module):
         self.conv3 = spconv.SparseSequential(down(f[1], f[2], 'spconv3', 1), sub(f[2], f[2], 'subm3'), sub(f[2], f[2], 'subm3'))
         self.conv4 = spconv.SparseSequential(down(f[2], f[3], 'spconv4', (0, 1, 1)), sub(f[3], f[3], 'subm4'),
                                              sub(f[3], f[3], 'subm4'))
-        last_pad = _cfg_get(model_cfg, 'last_pad', 0)
-        self.conv_out = spconv.SparseSequential(
-            spconv.SparseConv3d(f[3], self.out_features, (3, 1, 1), stride=(2, 1, 1), padding=last_pad, bias=False,
-                                indice_key='spconv_down2'), norm_fn(self.out_features), nn.ReLU())
+        self._add_conv_out()
         if self.mm:
-            self.vir_conv1 = NRConvBlock(input_channels, f[0], stride=1, indice_key='vir1')
-            self.vir_conv2 = NRConvBlock(f[0], f[1], stride=2, indice_key='vir2')
-            self.vir_conv3 = NRConvBlock(f[1], f[2], stride=2, indice_key='vir3')
-            self.vir_conv4 = NRConvBlock(f[2], f[3], stride=2, padding=(0, 1, 1), indice_key='vir4')
+            self._add_nrconv_blocks(input_channels)
         spconv.set_precision(self, precision)
-        self.num_point_features = self.out_features
-        if self.return_num_features_as_dict:
-            self.num_point_features = {'x_conv%d' % (i + 1): f[i] for i in range(4)}
 
     # -- native plans (csrc/executor.cu) -----------------------------------------------------------------------
     def _plan_lidar(self):
         """LiDAR stream (:248-291): the submanifold convs of a stage share one rulebook ('subm1'..'subm4')."""
-        if getattr(self, '_plan_lidar_cache', None) is None:
+        def build():
             plan = executor.Plan(self.conv_input[0].in_channels)
             c0 = self.conv_input[0]
             rb = plan.subm_rb(0, 3, c0.kernel_size, c0.dilation, unique=True, keys=[c0.indice_key])
@@ -489,43 +539,21 @@ class VirConv8x(nn.Module):
             plan.publish('x_conv1', f, iset)
             for name, stage in (('x_conv2', self.conv2), ('x_conv3', self.conv3), ('x_conv4', self.conv4)):
                 down = stage[0][0]
-                iset, rbd = plan.conv_rb(iset, 3, down.kernel_size, down.stride, down.padding, down.dilation, keys=[down.indice_key])
+                iset, rbd = plan.conv_rb(iset, 3, down.kernel_size, down.stride, down.padding, down.dilation,
+                                         keys=[down.indice_key])
                 c1 = stage[1][0]
                 rb = plan.subm_rb(iset, 3, c1.kernel_size, c1.dilation, unique=True, keys=[c1.indice_key])
                 f = plan.cbr(f, rbd, down, stage[0][1], seq=stage[0])
                 f = plan.cbr(f, rb, c1, stage[1][1], seq=stage[1])
                 f = plan.cbr(f, rb, stage[2][0], stage[2][1], seq=stage[2])
                 plan.publish(name, f, iset)
-            co = self.conv_out[0]
-            iset, rbo = plan.conv_rb(iset, 3, co.kernel_size, co.stride, co.padding, co.dilation, keys=[co.indice_key])
-            plan.publish('out', plan.cbr(f, rbo, co, self.conv_out[1], seq=self.conv_out), iset)
-            self._plan_lidar_cache = plan
-        return self._plan_lidar_cache
+            return self._plan_conv_out(plan, f, iset)
+        return self._cached_plan('_plan_lidar_cache', build)
 
     def _plan_mm(self, stvd=False):
         """Virtual-point stream (:468-535).  stvd: with the device-drawn layer discards at sites 0 (the input voxels, :489)
         and 1-3 (after vir_conv1..3); the LiDAR stream has none in the reference."""
-        attr = '_plan_mm_stvd_cache' if stvd else '_plan_mm_cache'
-        if getattr(self, attr, None) is None:
-            plan = executor.Plan(self.vir_conv1.d3_conv1[0].in_channels)
-            f, iset = 0, 0
-            if stvd:
-                f, iset = plan.discard(f, iset, 0, self.layer_discard_rate)
-            for i, (blk, s) in enumerate(zip((self.vir_conv1, self.vir_conv2, self.vir_conv3, self.vir_conv4), (1, 2, 4, 8))):
-                f, iset = plan_nrconv(plan, blk, f, iset, s)
-                if stvd and i < 3:
-                    f, iset = plan.discard(f, iset, i + 1, self.layer_discard_rate)
-                plan.publish('x_conv%d' % (i + 1), f, iset)
-            setattr(self, attr, plan)
-        return getattr(self, attr)
-
-    @staticmethod
-    def _plan_usable(plan, feats):
-        if (not executor.ENABLED or not feats.is_cuda or feats.shape[0] == 0 or feats.requires_grad or not plan.is_current()
-                or not plan.eligible()):
-            return False
-        mode = plan.layers[0][1].training
-        return all(bn.training == mode for _, bn in plan.layers)
+        return self._cached_plan('_plan_mm_stvd_cache' if stvd else '_plan_mm_cache', lambda: self._nrconv_plan(stvd)[0])
 
     @property
     def static_streams(self):
@@ -553,7 +581,7 @@ class VirConv8x(nn.Module):
         if self.mm:
             if batch_dict.get('virconv_proj') is None:
                 raise ValueError("VirConv8x: static mode needs batch_dict['virconv_proj'] (ops.projection_params on the device)")
-            if self._discarding() and (self.discard_rng != 'device' or batch_dict.get('stvd_keep_rows') is not None):
+            if self._host_discard(batch_dict):
                 raise ValueError("VirConv8x: static mode runs the StVD layer discard in the plan (discard_rng='device'); "
                                  'host-drawn or caller-given kept rows have no static form')
         return True
@@ -584,7 +612,7 @@ class VirConv8x(nn.Module):
             raise ValueError('VirConv8x static eval forward: the batch has no %s' % ', '.join(missing))
         return spec
 
-    def _eval_static_forward(self, batch_dict, spec, sfx, batch_size, strides):
+    def _eval_static_forward(self, batch_dict, spec, sfx, batch_size):
         """The eval forward below with every row count on the device (see EvalStaticSpec)."""
         R = len(sfx)
         feats = [batch_dict['voxel_features' + s] for s in sfx]
@@ -604,51 +632,26 @@ class VirConv8x(nn.Module):
 
         x3s, x4s, outs = split(x3), split(x4), split(out)
         for i, s in enumerate(sfx):
-            batch_dict.update({
-                'encoded_spconv_tensor' + s: outs[i], 'encoded_spconv_tensor_stride' + s: 8,
-                'multi_scale_3d_features' + s: {'x_conv1': None, 'x_conv2': None, 'x_conv3': x3s[i], 'x_conv4': x4s[i]},
-                'multi_scale_3d_strides' + s: dict(strides)})
+            _publish(batch_dict, s, (None, None, x3s[i], x4s[i]), outs[i])
         if not self.mm:
             return batch_dict
-        if not self._plan_mm(False).is_current():
-            self._plan_mm_cache = self._plan_mm_stvd_cache = None
-        plan = self._plan_mm(False)
+        plan = self._plan_mm()
         for i, s in enumerate(sfx):
-            f, c = batch_dict['voxel_features_mm' + s], batch_dict['voxel_coords_mm' + s]
-            if not self._plan_usable(plan, f):
-                raise ValueError('VirConv8x static eval forward: the virtual-point stream cannot run through the plan executor (%s)'
-                                 % _module_path_reason(f, plan))
-            _, (x1, x2, x3, x4) = self._run(plan, f, c, self.sparse_shape, batch_size, spec.proj[i],
-                                            ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4'), None, spec.mm[i], '_mm' + s)
-            batch_dict.update({
-                'encoded_spconv_tensor_stride_mm' + s: 8,
-                'multi_scale_3d_features_mm' + s: {'x_conv1': x1, 'x_conv2': x2, 'x_conv3': x3, 'x_conv4': x4},
-                'multi_scale_3d_strides' + s: dict(strides)})
+            xs = self._nrconv_stream(batch_dict, plan, batch_dict['voxel_features_mm' + s], batch_dict['voxel_coords_mm' + s],
+                                     None, s, '_mm' + s, proj=spec.proj[i], static=spec.mm[i],
+                                     refusal='VirConv8x static eval forward: the virtual-point stream cannot run through the '
+                                             'plan executor (%s)')
+            _publish(batch_dict, s, xs, stream='_mm')
         return batch_dict
-
-    def _discarding(self):
-        return self.training and self.discard_mode == 'paper' and self.layer_discard_rate != 0
-
-    def _run(self, plan, feats, coords, shape, batch_size, proj, names, seed=None, static=None, stream=''):
-        """-> (run record, published tensors).  static: the stream's StaticSpec (capacity-sized feats / coords)."""
-        ci = spconv._as_i32(coords)
-        run, res = executor.run_plan(plan, feats, ci, shape, batch_size, proj, plan.layers[0][1].training,
-                                     plan.layers[0][0].precision, static=static, seed=seed)
-        executor.note_last_run(self, run, stream)     # (graph.GraphedStep sizes each stream's capacities from an exact run)
-        return run, _published_tensors(run, res, names, ci, shape, batch_size)
 
     def _lidar_stream(self, feats, coords, shape, batch_size, static=None):
         plan = self._plan_lidar()
-        if not plan.is_current():          # a sub-module was replaced after the plan was built
-            self._plan_lidar_cache = None
-            plan = self._plan_lidar()
-        if self._plan_usable(plan, feats):
-            return self._run(plan, feats, coords, shape, batch_size, None, ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4', 'out'),
-                             static=static)[1]
+        reason = _module_path_reason(feats, plan)
+        if reason is None:
+            return self._run(plan, feats, coords, shape, batch_size, None, '', static=static)[1]
         if static is not None:
-            raise ValueError('VirConv8x static mode: the LiDAR stream cannot run through the plan executor (%s)'
-                             % _module_path_reason(feats, plan))
-        _module_path_under_determinism(_module_path_reason(feats, plan))
+            raise ValueError('VirConv8x static mode: the LiDAR stream cannot run through the plan executor (%s)' % reason)
+        _module_path_under_determinism(reason)
         x = spconv.SparseConvTensor(feats, coords.int(), shape, batch_size)
         x1 = self.conv1(self.conv_input(x))
         x2 = self.conv2(x1)
@@ -656,31 +659,20 @@ class VirConv8x(nn.Module):
         x4 = self.conv4(x3)
         return x1, x2, x3, x4, self.conv_out(x4)
 
-    def _maybe_discard(self, t, batch_dict, layer):
-        if not self.training or self.discard_mode != 'paper' or self.layer_discard_rate == 0:
-            return t
-        given = batch_dict.get('stvd_keep_rows')
-        keep = given[layer] if given is not None else stvd_keep_rows(t.features.shape[0], self.layer_discard_rate)
-        return discard_rows(t, keep)
-
     def forward(self, batch_dict):
         rot_num = batch_dict['transform_param'].shape[1] if 'transform_param' in batch_dict else 1
         batch_size = batch_dict['batch_size']
         sfx = [''] + [str(i) for i in range(1, rot_num)]
-        strides = {'x_conv1': 1, 'x_conv2': 2, 'x_conv3': 4, 'x_conv4': 8}
         static = self._check_static(batch_dict, rot_num)
         eval_static = self._check_eval_static(batch_dict, rot_num)
         ops.stats_arena(batch_dict['voxel_features'].device).reset()
         if eval_static is not None:
-            return self._eval_static_forward(batch_dict, eval_static, sfx, batch_size, strides)
+            return self._eval_static_forward(batch_dict, eval_static, sfx, batch_size)
         if self.training:
             for s in sfx:
-                x1, x2, x3, x4, out = self._lidar_stream(batch_dict['voxel_features' + s], batch_dict['voxel_coords' + s],
-                                                         self.sparse_shape, batch_size, batch_dict.get('virconv_static'))
-                batch_dict.update({
-                    'encoded_spconv_tensor' + s: out, 'encoded_spconv_tensor_stride' + s: 8,
-                    'multi_scale_3d_features' + s: {'x_conv1': x1, 'x_conv2': x2, 'x_conv3': x3, 'x_conv4': x4},
-                    'multi_scale_3d_strides' + s: dict(strides)})
+                *xs, out = self._lidar_stream(batch_dict['voxel_features' + s], batch_dict['voxel_coords' + s],
+                                              self.sparse_shape, batch_size, batch_dict.get('virconv_static'))
+                _publish(batch_dict, s, xs, out)
         else:
             feats, coords = [], []
             for i, s in enumerate(sfx):
@@ -691,55 +683,17 @@ class VirConv8x(nn.Module):
             big = [self.sparse_shape[0], self.sparse_shape[1], self.sparse_shape[2] * 4]      # factor 4 is hard-coded (:360)
             _, _, x3, x4, out = self._lidar_stream(torch.cat(feats, 0), torch.cat(coords), big, batch_size)
             for i, s in enumerate(sfx):
-                batch_dict.update({
-                    'encoded_spconv_tensor' + s: decompose_tensor(out, i, batch_size),
-                    'encoded_spconv_tensor_stride' + s: 8,
-                    'multi_scale_3d_features' + s: {'x_conv1': None, 'x_conv2': None,
-                                                    'x_conv3': decompose_tensor(x3, i, batch_size),
-                                                    'x_conv4': decompose_tensor(x4, i, batch_size)},
-                    'multi_scale_3d_strides' + s: dict(strides)})
+                out_i = decompose_tensor(out, i, batch_size)
+                _publish(batch_dict, s, (None, None, decompose_tensor(x3, i, batch_size), decompose_tensor(x4, i, batch_size)),
+                         out_i)
         if self.mm:
-            calib = batch_dict.get('calib')
             for i, s in enumerate(sfx):
-                feats, coords = batch_dict['voxel_features_mm' + s], batch_dict['voxel_coords_mm' + s]
-                trans = batch_dict['aug_param'] if 'aug_param' in batch_dict else None
-                if 'transform_param' in batch_dict:
-                    trans = batch_dict['transform_param'][:, i, :]
-                discarding = self._discarding()
-                # device-drawn discards run in the plan; host-drawn or caller-given kept rows on the module path
-                stvd = discarding and self.discard_rng == 'device' and batch_dict.get('stvd_keep_rows') is None
-                if not self._plan_mm(stvd).is_current():
-                    self._plan_mm_cache = self._plan_mm_stvd_cache = None
-                if (stvd or not discarding) and self._plan_usable(self._plan_mm(stvd), feats):
-                    # static mode: the shared projection block is already on the device ('virconv_proj', [B,28])
-                    proj = batch_dict['virconv_proj'] if static else None
-                    if proj is None:
-                        side = ops.side(feats.device).stream if executor.TWO_STREAMS else None
-                        proj = ops.projection_params(calib, trans, batch_size, feats.device, side)
-                    seed = stvd_seed(batch_dict, feats.device) if stvd else None
-                    run, (x1, x2, x3, x4) = self._run(self._plan_mm(stvd), feats, coords, self.sparse_shape, batch_size, proj,
-                                                      ('x_conv1', 'x_conv2', 'x_conv3', 'x_conv4'), seed,
-                                                      batch_dict.get('virconv_static_mm'), '_mm' + s)
-                    if stvd:
-                        batch_dict['stvd_kept_rows' + s] = run.kept_rows()
-                    batch_dict.update({
-                        'encoded_spconv_tensor_stride_mm' + s: 8,
-                        'multi_scale_3d_features_mm' + s: {'x_conv1': x1, 'x_conv2': x2, 'x_conv3': x3, 'x_conv4': x4},
-                        'multi_scale_3d_strides' + s: dict(strides)})
-                    continue
-                if static:
-                    raise ValueError('VirConv8x static mode: the virtual-point stream cannot run through the plan executor (%s)'
-                                     % _module_path_reason(feats, self._plan_mm(stvd)))
-                _module_path_under_determinism(_module_path_reason(feats, self._plan_mm(stvd), discarding and not stvd))
-                proj = ops.projection_params(calib, trans, batch_size, feats.device)
-                x = spconv.SparseConvTensor(feats, coords.int(), self.sparse_shape, batch_size)
-                x = self._maybe_discard(x, batch_dict, 0)              # VirConv8x also discards the input voxels (:489-490)
-                x1 = self._maybe_discard(self.vir_conv1(x, batch_size, proj, 1), batch_dict, 1)
-                x2 = self._maybe_discard(self.vir_conv2(x1, batch_size, proj, 2), batch_dict, 2)
-                x3 = self._maybe_discard(self.vir_conv3(x2, batch_size, proj, 4), batch_dict, 3)
-                x4 = self.vir_conv4(x3, batch_size, proj, 8)
-                batch_dict.update({
-                    'encoded_spconv_tensor_stride_mm' + s: 8,
-                    'multi_scale_3d_features_mm' + s: {'x_conv1': x1, 'x_conv2': x2, 'x_conv3': x3, 'x_conv4': x4},
-                    'multi_scale_3d_strides' + s: dict(strides)})
+                # static mode: the shared projection block is already on the device ('virconv_proj', [B,28])
+                xs = self._nrconv_stream(
+                    batch_dict, self._plan_mm(self._device_discard()), batch_dict['voxel_features_mm' + s],
+                    batch_dict['voxel_coords_mm' + s], _copy_transform(batch_dict, i), s, '_mm' + s,
+                    proj=batch_dict['virconv_proj'] if static else None, static=batch_dict.get('virconv_static_mm'),
+                    refusal='VirConv8x static mode: the virtual-point stream cannot run through the plan executor (%s)'
+                    if static else None)
+                _publish(batch_dict, s, xs, stream='_mm')
         return batch_dict
