@@ -48,9 +48,6 @@ int vc_version(void);
 const char* vc_last_error(void);
 /* number of kernels this library has launched so far in this process (bench.py's gpu_launches) */
 long long vc_launch_count(void);
-/* Programmatic dependent launch for the kernels of the conv / BN chain (default on): each starts while its predecessor
- * drains and blocks in `griddepcontrol.wait` before touching dependent data.  0 = plain stream-ordered launches. */
-int vc_set_pdl(int enable);
 /* BatchNorm backward as ONE cooperative launch (reduction, grid-wide barrier, apply; default on) or as two launches (0). */
 int vc_set_bn_fused(int enable);
 /* BatchNorm + ReLU of the tensor-core conv forward inside the conv's own launch (1, the default; cooperative: conv, grid-wide
@@ -60,19 +57,9 @@ int vc_set_conv_bn_fused(int enable);
 int vc_set_tc_variant(int variant);
 /* A/B aid for the persistent tensor-core conv kernel (conv_tc2.cu): CTAs per SM, 0 = automatic (two when each still gets a
  * ring of >= 2 stages in half the shared memory), 1 or 2 = forced.  The cooperative conv + BN grid keeps one CTA per SM
- * unless 2 is forced or no index kernel runs beside it (vc_set_index_order 2 in static mode). */
+ * unless 2 is forced or no index kernel runs beside it (the plan executor's static mode with side streams, which enqueues
+ * the whole index phase before the first feature kernel). */
 int vc_conv_tc2_config(int ctas_per_sm);
-/* How the plan executor's forward builds the output sets of chained strided convs (each one's input set is the previous
- * one's output set, no layer discard between them; csrc/rulebook.cu header): 1 = all of them from the first input set in
- * one composed pass, exact mode reading all their row counts with one synchronise; 0 = each from the previous one's
- * emitted indices, one read-back per conv in exact mode (the path every other plan takes); 2 (default) = composed as 1,
- * and the index work of the chain's stages (the strided convs' tables, the submanifold rulebooks, projections and 2-D
- * rulebooks over their output sets) batched into one launch per kind; in static mode with side streams the whole index
- * phase is then enqueued before the first feature kernel and the fused conv + BatchNorm grids take two CTAs per SM.  Same
- * index sets, counts and tables in all three (except after a capacity overflow: see the header of csrc/rulebook.cu);
- * VC_ERR_INVALID for another value.  Environment VIRCONV_INDEX_ORDER at load time.  Read when a
- * forward is enqueued (a captured graph keeps its choice). */
-int vc_set_index_order(int mode);
 /* The plan executor's weight-gradient launches (csrc/wgrad_tc3.cu): variant must be 1 (the only kernel); max_ctas caps
  * their CTAs (0, the default: half the SMs, so that each shares its SM with a dgrad CTA of the main stream). */
 int vc_conv_wgrad_tc3_config(int variant, int max_ctas);

@@ -6,11 +6,7 @@ column includes it.  Per replay it also prints the index phase: the span from th
 strided-conv count / emit / tables, projections) to the last, the time from the voxeliser's last kernel to the first conv,
 and the span of the forward's conv chain.  Run on the GPU:
 
-    python profiles/forward_bn_gap.py [--replays 20] [--modes 1,2]
-
---modes: the executor's index orders to compare (vc_set_index_order: 0 per level, 1 composed, 2 composed with the stages'
-index work batched and, in this static-mode step, the index phase first).  Each mode captures its own step; the modes are
-profiled in alternation, two rounds of replays / 2 each, in one process.
+    python profiles/forward_bn_gap.py [--replays 20]
 
 Prints the card name and power limit with the numbers: a kernel time is only meaningful with what it was measured on."""
 import argparse
@@ -149,11 +145,7 @@ def report(events):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--replays', type=int, default=20)
-    ap.add_argument('--modes', default='1,2', help='index orders to compare (vc_set_index_order), comma separated')
     args = ap.parse_args()
-    modes = [int(m) for m in args.modes.split(',')]
-    from virconv_b200 import _lib
-    lib = _lib.load()
     dev = torch.device('cuda:0')
     batches = []
     for i in range(bench.POOL):
@@ -169,25 +161,16 @@ def main():
             loss = loss + masked_mean(t)
         return loss
 
-    steps = {}
-    for mode in modes:
-        _lib.check(lib.vc_set_index_order(mode), 'vc_set_index_order')   # read when the step is captured
-        torch.manual_seed(666)
-        model = VirConvL8x(bench.CFG, 8, [1408, 1600, 80], precision='bf16').to(dev).train()
-        steps[mode] = GraphedStep(model, loss_of, list(model.parameters()),
-                                  margin=float(os.environ.get('VIRCONV_GRAPH_MARGIN', '1.15')), voxelizer=vox)
-        for i in range(3 * bench.POOL):
-            steps[mode](batches[i % bench.POOL])
-        torch.cuda.synchronize()
-    events = {mode: [] for mode in modes}
-    for _ in range(2):
-        for mode in modes:
-            _lib.check(lib.vc_set_index_order(mode), 'vc_set_index_order')   # (in case the step captures again)
-            events[mode] += profile_events(steps[mode], batches, max(1, args.replays // 2))
+    torch.manual_seed(666)
+    model = VirConvL8x(bench.CFG, 8, [1408, 1600, 80], precision='bf16').to(dev).train()
+    step = GraphedStep(model, loss_of, list(model.parameters()), margin=float(os.environ.get('VIRCONV_GRAPH_MARGIN', '1.15')),
+                       voxelizer=vox)
+    for i in range(3 * bench.POOL):
+        step(batches[i % bench.POOL])
+    torch.cuda.synchronize()
+    events = profile_events(step, batches, args.replays)
     print(f'card: {card()}')
-    for mode in modes:
-        print(f'--- index order {mode}')
-        report(events[mode])
+    report(events)
 
 
 if __name__ == '__main__':

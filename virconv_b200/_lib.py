@@ -27,10 +27,8 @@ SIGNATURES = {
     'vc_version': (_I, []),
     'vc_last_error': (c_char_p, []),
     'vc_launch_count': (ctypes.c_longlong, []),
-    'vc_set_pdl': (_I, [_I]),
     'vc_set_bn_fused': (_I, [_I]),
     'vc_set_conv_bn_fused': (_I, [_I]),
-    'vc_set_index_order': (_I, [_I]),
     'vc_set_tc_variant': (_I, [_I]),
     'vc_conv_tc2_config': (_I, [_I]),
     'vc_conv_wgrad_tc3_config': (_I, [_I, _I]),
@@ -175,15 +173,8 @@ def load():
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args
-    # programmatic dependent launch of the conv / BN chain: implemented and parity-tested, but not measured faster
-    # -> off unless asked for
-    lib.vc_set_pdl(1 if os.environ.get('VIRCONV_PDL', '0') == '1' else 0)
     # BatchNorm + ReLU inside the tensor-core conv forward (one cooperative launch per layer); 0 for A/B runs
     lib.vc_set_conv_bn_fused(0 if os.environ.get('VIRCONV_CONV_BN_FUSED', '1') == '0' else 1)
-    # index work of chained strided convs: 2 = composed, batched per kind, index phase first in static mode; 1 = composed,
-    # one launch per stage; 0 = one strided conv after the other (A/B runs)
-    if lib.vc_set_index_order(int(os.environ.get('VIRCONV_INDEX_ORDER', '2'))) != 0:
-        raise ValueError('VIRCONV_INDEX_ORDER must be 0, 1 or 2')
     _lib = lib
     return lib
 

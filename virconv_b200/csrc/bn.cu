@@ -26,8 +26,6 @@ __global__ void __launch_bounds__(256) bn_apply_relu_kernel(
     // rows [count, capacity) of the outputs are written as zeros (published tensors keep a defined tail).
     // y_ld4 / yb_ld4: row pitch of the outputs in float4 / uint2 units (>= c/4: the output may be a column slice of a
     // wider matrix — the concat of an NRConv block is written in place, spconv_backbone.py:227).
-    pdl_wait();                 // the conv's output and channel sums
-    pdl_launch_dependents();
     const int cap_rows = n_rows;
     if (n_dev != nullptr) n_rows = min(n_rows, __ldg(n_dev));
     const int c4 = c / 4;
@@ -74,8 +72,6 @@ __global__ void __launch_bounds__(256) bn_apply_relu_kernel(
 __global__ void __launch_bounds__(256) bn_sums_reduce_kernel(const double* __restrict__ part, int cap_rows, const int* __restrict__ n_dev,
                                                              int rows_per_part, int c, double* __restrict__ sums) {
     __shared__ double red[256];
-    pdl_wait();
-    pdl_launch_dependents();
     const int rows = n_dev != nullptr ? min(cap_rows, __ldg(n_dev)) : cap_rows;
     const int n_parts = (rows + rows_per_part - 1) / rows_per_part;
     const double v = bn_sums_column(part, n_parts, c, blockIdx.x, red);
@@ -155,8 +151,6 @@ __global__ void __launch_bounds__(256) bn_bwd_reduce_kernel(const float4* __rest
                                                             const float* __restrict__ stats, int n, const int* __restrict__ n_dev,
                                                             int c, double* __restrict__ bsums, double* __restrict__ part) {
     extern __shared__ float shf[];  // [rowlanes][2][c]
-    pdl_wait();
-    pdl_launch_dependents();
     if (n_dev != nullptr) n = min(n, __ldg(n_dev));
     if (part != nullptr) {          // deterministic: per-chunk partials, summed by the apply kernel
         bn_bwd_chunk_partials(dy, dy_ld4, x, stats, n, c, part, shf);
@@ -201,8 +195,6 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const float4* __restr
                                                            float4* __restrict__ dx, uint2* __restrict__ dx_bf16,
                                                            float* __restrict__ dgamma, float* __restrict__ dbeta, int tail_zero,
                                                            const double* __restrict__ part) {
-    pdl_wait();                 // bsums from the reduce kernel
-    pdl_launch_dependents();
     const int cap_rows = n_rows;
     if (n_dev != nullptr) n_rows = min(n_rows, __ldg(n_dev));
     const int c4 = c / 4;
@@ -404,9 +396,10 @@ int vc::bn_apply_relu_dev(const float* x, const double* sums, int n_rows, const 
     VC_CHECK_ARG(!training || n_rows > 0, "training-mode BN over zero rows");
     VC_CHECK_ARG(n_rows == 0 || (x && (y || y_bf16)), "null pointer");
     VC_CHECK_ARG(y_ld % 4 == 0 && yb_ld % 4 == 0 && y_ld >= c && yb_ld >= c, "bad output pitch");
-    VC_LAUNCH_CHAIN(bn_apply_relu_kernel, dim3(ew_blocks((size_t)n_rows * c / 4)), dim3(256), 0, stream, (const float4*)x, sums,
-                    n_rows, n_dev, c, gamma, beta, running_mean, running_var, num_batches_tracked, momentum, eps, training,
-                    (float4*)y, y_ld / 4, (uint2*)y_bf16, yb_ld / 4, stats_out, relu, tail_zero);
+    bn_apply_relu_kernel<<<dim3(ew_blocks((size_t)n_rows * c / 4)), dim3(256), 0, stream>>>((const float4*)x, sums, n_rows, n_dev,
+        c, gamma, beta, running_mean, running_var, num_batches_tracked, momentum, eps, training, (float4*)y, y_ld / 4,
+        (uint2*)y_bf16, yb_ld / 4, stats_out, relu, tail_zero);
+    VC_LAUNCH_CHECK();
     return VC_OK;
 }
 
@@ -455,12 +448,14 @@ int vc::bn_relu_bwd_dev(const float* dy, int dy_ld, const float* x, const float*
         int blocks = (n + rowlanes - 1) / rowlanes;
         if (blocks > 296) blocks = 296;
         size_t smem = (size_t)rowlanes * 2 * c * sizeof(float);
-        VC_LAUNCH_CHAIN(bn_bwd_reduce_kernel, dim3(blocks), dim3(256), smem, stream, (const float4*)dy, dy_ld / 4, (const float4*)x,
-                        stats, n, n_dev, c, bsums, part);
+        bn_bwd_reduce_kernel<<<dim3(blocks), dim3(256), smem, stream>>>((const float4*)dy, dy_ld / 4, (const float4*)x, stats, n,
+            n_dev, c, bsums, part);
+        VC_LAUNCH_CHECK();
     }
-    VC_LAUNCH_CHAIN(bn_bwd_apply_kernel, dim3(ew_blocks((size_t)n * c / 4)), dim3(256), 0, stream, (const float4*)dy, dy_ld / 4,
-                    (const float4*)x, gamma, stats, bsums, n, n_dev, c, training, (float4*)dx, (uint2*)dx_bf16, dgamma, dbeta,
-                    tail_zero, (const double*)part);
+    bn_bwd_apply_kernel<<<dim3(ew_blocks((size_t)n * c / 4)), dim3(256), 0, stream>>>((const float4*)dy, dy_ld / 4,
+        (const float4*)x, gamma, stats, bsums, n, n_dev, c, training, (float4*)dx, (uint2*)dx_bf16, dgamma, dbeta, tail_zero,
+        (const double*)part);
+    VC_LAUNCH_CHECK();
     return VC_OK;
 }
 
@@ -486,7 +481,8 @@ extern "C" int vc_bn_relu_bwd_f32(const float* dy, const float* x, const float* 
 int vc::bn_sums_reduce_dev(const double* part, int cap_rows, const int* n_dev, int rows_per_part, int c, double* sums,
                            cudaStream_t stream) {
     VC_CHECK_ARG(c_ok(c) && cap_rows >= 0 && rows_per_part > 0 && part && sums, "bad bn sums args");
-    VC_LAUNCH_CHAIN(bn_sums_reduce_kernel, dim3(2 * c), dim3(256), 0, stream, part, cap_rows, n_dev, rows_per_part, c, sums);
+    bn_sums_reduce_kernel<<<dim3(2 * c), dim3(256), 0, stream>>>(part, cap_rows, n_dev, rows_per_part, c, sums);
+    VC_LAUNCH_CHECK();
     return VC_OK;
 }
 

@@ -97,38 +97,6 @@ __device__ __forceinline__ void stage_nbr_tile(const int32_t* __restrict__ nbr, 
     }
 }
 
-// ---- programmatic dependent launch (PDL) for the kernels of the main-stream chain ----
-// Every step is ~160 small dependent kernels on one stream; a plain launch starts only after the previous grid has
-// drained AND been flushed (2-3 us each, 0.4-0.6 ms per step).  Launched with the programmatic-stream-serialisation
-// attribute a kernel may start (block scheduling, prologue) as soon as every CTA of its predecessor has issued
-// `griddepcontrol.launch_dependents`, and blocks in `griddepcontrol.wait` until the predecessor has completed and its
-// writes are visible.  Kernels using this call pdl_wait() before their first global read or write of dependent data;
-// both instructions are no-ops for a normally launched grid.  vc_set_pdl(0) turns the attribute off.
-extern int g_pdl;
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
-template <typename... KP, typename... A>
-static inline cudaError_t launch_chain(void (*kern)(KP...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, A... args) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute at{};
-    at.id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at.val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = &at;
-    cfg.numAttrs = g_pdl ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, kern, static_cast<KP>(args)...);
-}
-
-#define VC_LAUNCH_CHAIN(...)                      \
-    do {                                          \
-        vc::count_launch();                       \
-        VC_CUDA(vc::launch_chain(__VA_ARGS__));   \
-    } while (0)
-
 // ---- shared between rulebook.cu and executor.cu ----
 // `n_dev` (optional): the row count lives in device memory and `n` / `n_out` are capacities (static mode, graph capturable)
 int subm_rulebook_dev(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size, const int32_t* spatial_shape,
@@ -170,13 +138,13 @@ int conv_chain_count_dev(const ConvChain& ch, const int32_t* indices, int n, con
 // out_idx [L]: output index buffers of caps[l] rows
 int conv_chain_emit_dev(const ConvChain& ch, int32_t* const* out_idx, const int* caps, void* ws, size_t ws_bytes, cudaStream_t stream);
 
-// The per-stage index work of up to IDX_BATCH_MAX stages, one launch per kind (rulebook.cu, misc.cu): the same kernels, and
-// the same results, as one call per stage.  The caller owns the buffers and clears them first (so that the regions of
-// all stages can be cleared together): hash tables to 0xFF, a mirrored table's rows k > centre to -1, pair counts to 0,
-// nbr_fwd to -1.
+// The per-stage index work of up to IDX_BATCH_MAX stages, one launch per kind (rulebook.cu, misc.cu): the same results as
+// one call per stage (subm_rulebook_dev and conv_rulebook_tables_dev are batches of one).  The caller owns the buffers and
+// clears them first (so that the regions of all stages can be cleared together): hash tables to 0xFF, a mirrored table's
+// rows k > centre to -1, pair counts to 0, nbr_fwd to -1.
 constexpr int IDX_BATCH_MAX = 4;
 bool subm_sym(int ndim, const int32_t* ksize, bool unique);   // the mirrored probe (half the offsets, rows k > centre pre-filled)
-struct SubmStage {   // one submanifold rulebook (subm_rulebook_dev without rep); table: vc_subm_rulebook_ws_bytes(n) bytes
+struct SubmStage {   // one submanifold rulebook (subm_rulebook_dev); table: vc_subm_rulebook_ws_bytes(n) bytes
     const int32_t* idx;
     int n;
     const int* n_dev;
@@ -185,6 +153,7 @@ struct SubmStage {   // one submanifold rulebook (subm_rulebook_dev without rep)
     int32_t *nbr, *pair_num;
     void* table;
     size_t table_bytes;
+    int32_t* rep;    // optional [n]: lowest row at each row's coordinate (the stage then probes every offset)
 };
 int subm_rulebook_batch_dev(const SubmStage* st, int n_st, int batch_size, bool unique, cudaStream_t stream);
 struct TablesStage {  // one strided conv's tables (conv_rulebook_tables_dev)
@@ -304,8 +273,8 @@ size_t tc_image_bytes(int cin, int cout, int K, int layout);
 bool tc2_ch_ok(int c);
 int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_t* nbr, long long pitch, float* out, int n_rows,
              const int* n_dev, int K, double* bn_sums, int* err, cudaStream_t stream, const float* addend,
-             int* tile_counter = nullptr, int flags = 0,   // flags: bit 0 sparse offsets (strided dgrad), bit 1 early tables,
-                                                           // bit 2 no index kernel beside it (the conv + BN grid takes 2 CTAs/SM)
+             int* tile_counter = nullptr, int flags = 0,   // flags: bit 0 sparse offsets (strided dgrad), bit 1 no index kernel
+                                                           // beside it (the conv + BN grid takes 2 CTAs/SM)
              int in_ld = 0,                                // row pitch of in_bf16 (0: kc)
              double* bn_part = nullptr,                    // deterministic BN sums: [tiles, 2, nr] per 128-row tile (bn_sums NULL)
              const BnTail* bn = nullptr,                   // forward only: BN + ReLU in the same launch when g_conv_bn_fused

@@ -39,8 +39,6 @@ struct Cfg {
 //             mode 1 (dgrad)    wt[k][co][ci] = w[co][kk][ci], kk = mirror ? K-1-k : k
 __global__ void prep_weights_kernel(const float* __restrict__ w, float* __restrict__ wt, int cin, int cout, int K,
                                     int mode, int mirror) {
-    pdl_wait();
-    pdl_launch_dependents();
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     int total = K * cin * cout;
     if (i >= total) return;
@@ -139,8 +137,6 @@ gather_gemm_kernel(const float* __restrict__ in, const float* __restrict__ wt, c
     __shared__ unsigned kmask;
     __shared__ float red[NTHREADS / 32][2][CO];
 
-    pdl_wait();
-    pdl_launch_dependents();
     const int base = blockIdx.x * TM;
     const int nk = stage_nbr(nbr, n_out, K, base, nbr_s, klist, &kmask);
 
@@ -229,8 +225,6 @@ scatter_gemm_kernel(const float* __restrict__ in, const float* __restrict__ wt, 
     __shared__ int klist[MAXK];
     __shared__ unsigned kmask;
 
-    pdl_wait();
-    pdl_launch_dependents();
     const int base = blockIdx.x * TM;
     const int nk = stage_nbr(nbr, n_rows, K, base, nbr_s, klist, &kmask);
     if (nk == 0) return;
@@ -401,7 +395,8 @@ static int launch_gather(const float* in, const float* wt, const int32_t* nbr, f
     size_t smem = Cfg<CI, CO>::smem_gather(K);
     auto kern = gather_gemm_kernel<CI, CO>;
     VC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    VC_LAUNCH_CHAIN(kern, dim3(cdiv(n_out, TM)), dim3(NTHREADS), smem, stream, in, wt, nbr, out, n_out, K, bn_sums, bn_part);
+    kern<<<dim3(cdiv(n_out, TM)), dim3(NTHREADS), smem, stream>>>(in, wt, nbr, out, n_out, K, bn_sums, bn_part);
+    VC_LAUNCH_CHECK();
     return VC_OK;
 }
 template <int CI, int CO>
@@ -410,7 +405,8 @@ static int launch_scatter(const float* in, const float* wt, const int32_t* nbr, 
     size_t smem = Cfg<CI, CO>::smem_scatter(K);
     auto kern = scatter_gemm_kernel<CI, CO>;
     VC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    VC_LAUNCH_CHAIN(kern, dim3(cdiv(n_rows, TM)), dim3(NTHREADS), smem, stream, in, wt, nbr, out, out_ld, n_rows, K);
+    kern<<<dim3(cdiv(n_rows, TM)), dim3(NTHREADS), smem, stream>>>(in, wt, nbr, out, out_ld, n_rows, K);
+    VC_LAUNCH_CHECK();
     return VC_OK;
 }
 template <int CI, int CO>
@@ -462,7 +458,8 @@ extern "C" size_t vc_conv_ws_bytes(int cin, int cout, int K) { return (size_t)K 
 
 static int prep(const float* w, float* wt, int cin, int cout, int K, int mode, int mirror, cudaStream_t stream) {
     int total = K * cin * cout;
-    VC_LAUNCH_CHAIN(prep_weights_kernel, dim3(cdiv(total, 256)), dim3(256), 0, stream, w, wt, cin, cout, K, mode, mirror);
+    prep_weights_kernel<<<dim3(cdiv(total, 256)), dim3(256), 0, stream>>>(w, wt, cin, cout, K, mode, mirror);
+    VC_LAUNCH_CHECK();
     return VC_OK;
 }
 

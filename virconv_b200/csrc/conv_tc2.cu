@@ -88,7 +88,6 @@ struct PArgs {
     int* tile_counter;         // optional (zeroed by the caller): dynamic tile scheduling; NULL: tile = blockIdx.x + i * gridDim.x
     int K, S;
     int w_resident;            // all K weight slices stay in shared memory for the whole launch (else: streamed with the ring)
-    int early_tables;          // the neighbour table (and row count) do not come from the immediately preceding kernel of the stream
     int scan_k;                // the loader lists the kernel offsets that touch each tile (strided-conv dgrad: most do not)
     int ntb_alloc;             // neighbour-table buffers in shared memory (2 when two CTAs share an SM, else P_NTB)
     int* err;
@@ -206,13 +205,6 @@ __global__ void __launch_bounds__(P_THREADS, P_GROUPS == 1 ? 2 : 1) tc_conv_pers
         mbar_init(&wres_bar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    // Programmatic dependent launch: this grid may have started while its predecessor in the stream still runs.  What the
-    // roles read BEFORE their griddepcontrol.wait must not come from that predecessor: the row count, the tile counter and —
-    // when the caller vouches for it (early_tables: the plan executor builds its rulebooks on other streams and joins them with
-    // events) — the neighbour table, so that barrier set-up and the first table loads overlap the
-    // predecessor's tail.  Features, weights, addend and outputs are only touched after the wait.
-    pdl_launch_dependents();
-    if (!a.early_tables) pdl_wait();
     const int n = a.n_dev != nullptr ? min(__ldg(a.n_dev), a.n_host) : a.n_host;
     // a pipeline wait that timed out in an EARLIER launch left the (sticky) error flag set: do nothing, so that whatever went
     // wrong costs one 2-second timeout, not one per launch
@@ -341,7 +333,6 @@ __global__ void __launch_bounds__(P_THREADS, P_GROUPS == 1 ? 2 : 1) tc_conv_pers
     } else if (warp >= P_WARP_PROD0) {
         // ------------------------------------------------------------ gather producers
         const int grp = (warp - P_WARP_PROD0) / P_PROD_WARPS, pw = (warp - P_WARP_PROD0) % P_PROD_WARPS;
-        pdl_wait();                                         // the gathered rows are the predecessor's output
         constexpr int CW = C::CPR < 4 ? C::CPR : 4;         // chunks of one row handled by adjacent lanes (full sectors)
         constexpr int RPI = 32 / CW;                        // rows per warp instruction
         constexpr int NIT = P_ROWS_PER_PROD / RPI;          // row groups per offset and warp
@@ -421,7 +412,6 @@ __global__ void __launch_bounds__(P_THREADS, P_GROUPS == 1 ? 2 : 1) tc_conv_pers
         }
     } else if (warp == P_WARP_W) {
         // ------------------------------------------------------------ weight slices (TMA engine, linear bulk copies)
-        pdl_wait();                                         // (the weight images may come from the kernel just before this one)
         if (wres) {
             if (lane == 0) {
                 const uint32_t total = (uint32_t)(K * C::B_BYTES);
@@ -457,7 +447,6 @@ __global__ void __launch_bounds__(P_THREADS, P_GROUPS == 1 ? 2 : 1) tc_conv_pers
         }
     } else {
         // ------------------------------------------------------------ consumers (warpgroup h: rows [64 h, 64 h + 64) of the tile)
-        pdl_wait();                              // weights / addend / out / bn_sums
         const int wg = warp >> 2, t = tid & 127;
         const int e = tid;                       // 0..255
         const int oc = a.out_c;
@@ -735,21 +724,19 @@ int launch_persist(const PArgs& a0, int n_cap, cudaStream_t stream, bool* bn_don
         // per step SLOWER than the separate apply kernel); at one CTA per SM the grid fits beside them and the step gets
         // 0.15 ms faster (DESIGN.md section 8).  Same shared-memory plan, half the CTAs.  Running the whole index phase
         // before the forward instead, so that the grid could take both CTAs of each SM, was slower still (DESIGN.md
-        // section 8, item 3) until the index work was batched: with no index kernel beside it (coop2, the executor's index
-        // order 2 in static mode) the grid takes both.  vc_conv_tc2_config(2) forces the two-CTA grid (tests, A/B runs).
+        // section 8, item 3) until the index work was batched: with no index kernel beside it (coop2, the executor's static
+        // mode, index phase first) the grid takes both.  vc_conv_tc2_config(2) forces the two-CTA grid (tests, A/B runs).
         const int cgrid = (g_p_ctas == 2 || coop2 || grid < num_sms()) ? grid : num_sms();
         cudaLaunchConfig_t cfg{};
         cfg.gridDim = dim3(cgrid);
         cfg.blockDim = dim3(P_THREADS);
         cfg.dynamicSmemBytes = p.smem;
         cfg.stream = stream;
-        cudaLaunchAttribute at[2]{};
-        at[0].id = cudaLaunchAttributeCooperative;
-        at[0].val.cooperative = 1;
-        at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[1].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = at;
-        cfg.numAttrs = g_pdl ? 2 : 1;
+        cudaLaunchAttribute at{};
+        at.id = cudaLaunchAttributeCooperative;
+        at.val.cooperative = 1;
+        cfg.attrs = &at;
+        cfg.numAttrs = 1;
         if (cudaLaunchKernelEx(&cfg, kern, a) == cudaSuccess) {
             count_launch();
             *bn_done = true;
@@ -760,7 +747,8 @@ int launch_persist(const PArgs& a0, int n_cap, cudaStream_t stream, bool* bn_don
         g_conv_bn_fused = 0;
         a.bn = BnTail{};
     }
-    VC_LAUNCH_CHAIN(kern, dim3(grid), dim3(P_THREADS), p.smem, stream, a);
+    kern<<<dim3(grid), dim3(P_THREADS), p.smem, stream>>>(a);
+    VC_LAUNCH_CHECK();
     return VC_OK;
 }
 
@@ -838,7 +826,7 @@ int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_
     }
     a.in = (const __nv_bfloat16*)in_bf16; a.in_c = kc; a.in_ld = in_ld; a.wimg = (const unsigned char*)wimg; a.nbr = nbr; a.pitch = pitch;
     a.out = out; a.out_c = nr; a.addend = addend; a.bn_sums = bn_part ? nullptr : bn_sums; a.bn_part = bn_part; a.n_dev = n_dev; a.n_host = n_rows; a.tile_counter = tile_counter;
-    a.K = K; a.S = 0; a.w_resident = 0; a.ntb_alloc = P_NTB; a.scan_k = flags & 1; a.early_tables = (flags >> 1) & 1;
+    a.K = K; a.S = 0; a.w_resident = 0; a.ntb_alloc = P_NTB; a.scan_k = flags & 1;
     a.err = err;
     a.bn = BnTail{};
     bool done_dummy = false;
@@ -853,7 +841,7 @@ int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_
     if (bn_done == nullptr) bn_done = &done_dummy;
     const int kcp = tc_pad16(kc), nrp = tc_pad16(nr);
 #define VC_P_CASE(A, B) \
-    if (kcp == A && nrp == B) return launch_persist<A, B>(a, n_rows, stream, bn_done, (flags >> 2) & 1);
+    if (kcp == A && nrp == B) return launch_persist<A, B>(a, n_rows, stream, bn_done, (flags >> 1) & 1);
     VC_P_CASE(16, 16) VC_P_CASE(16, 32) VC_P_CASE(16, 64)
     VC_P_CASE(32, 16) VC_P_CASE(32, 32) VC_P_CASE(32, 64)
     VC_P_CASE(64, 16) VC_P_CASE(64, 32) VC_P_CASE(64, 64)

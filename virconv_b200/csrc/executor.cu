@@ -123,14 +123,6 @@ constexpr int EV_POOL = 512;   // > the events of one forward / backward call: t
 cudaEvent_t g_ev[EV_POOL];
 int g_ev_dev = -1, g_ev_next = 0;
 
-// How the forward builds the output sets of chained strided convs and their stages' index work (vc_set_index_order,
-// VIRCONV_INDEX_ORDER): 2 (default) composed in one pass (fwd_conv_chain), the index work of the chain's stages batched
-// into one launch per kind (fwd_chain_tables, fwd_chain_stages), and in static mode the whole index phase enqueued before
-// the first feature kernel; 1 composed, the stages' work one launch per stage in the plan's interleaved order; 0 each
-// output set from the previous one's (count -> read-back -> emit per conv), the path every other plan takes.  0 and 1 are
-// the references the tests compare with.
-int g_index_order = 2;
-
 int ev_init() {
     int dev = 0;
     VC_CUDA(cudaGetDevice(&dev));
@@ -156,8 +148,8 @@ bool g_timing = false;
 struct Timed {
     int idx;
     cudaStream_t st;
-    Timed(int kind, int layer, cudaStream_t s) : idx(-1), st(s) {
-        if (!g_timing || g_t_n >= T_MAX) return;
+    Timed(int kind, int layer, cudaStream_t s, bool launches = true) : idx(-1), st(s) {   // launches: the kernel is enqueued
+        if (!launches || !g_timing || g_t_n >= T_MAX) return;
         if (g_t_n >= g_t_created) {
             if (cudaEventCreate(&g_t[g_t_n].a) != cudaSuccess || cudaEventCreate(&g_t[g_t_n].b) != cudaSuccess) return;
             g_t_created = g_t_n + 1;
@@ -173,8 +165,6 @@ struct Timed {
 };
 
 __global__ void __launch_bounds__(256) add_kernel(const float4* a, const float4* b, float4* c, size_t n4) {   // c may alias a or b
-    pdl_wait();
-    pdl_launch_dependents();
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const size_t stride = (size_t)gridDim.x * blockDim.x;
     for (; i < n4; i += stride) {
@@ -187,8 +177,6 @@ __global__ void __launch_bounds__(256) add_kernel(const float4* a, const float4*
 // the outputs (in-place accumulation) or be NULL
 __global__ void __launch_bounds__(256) cat2_bwd_kernel(const float4* __restrict__ dcat, int n, int ca4, int cb4,
                                                        float4* da, const float4* a_add, float4* db, const float4* b_add) {
-    pdl_wait();
-    pdl_launch_dependents();
     const int c4 = ca4 + cb4;
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const size_t total = (size_t)n * c4, stride = (size_t)gridDim.x * blockDim.x;
@@ -216,7 +204,8 @@ int ew_grid(size_t n4) {
 
 int launch_add(const float* a, const float* b, float* c, size_t n, cudaStream_t st) {
     if (n == 0) return VC_OK;
-    VC_LAUNCH_CHAIN(add_kernel, dim3(ew_grid(n / 4)), dim3(256), 0, st, (const float4*)a, (const float4*)b, (float4*)c, n / 4);
+    add_kernel<<<dim3(ew_grid(n / 4)), dim3(256), 0, st>>>((const float4*)a, (const float4*)b, (float4*)c, n / 4);
+    VC_LAUNCH_CHECK();
     return VC_OK;
 }
 
@@ -542,7 +531,7 @@ int fwd_discard(FwdCtx& C, int i, const int* o) {
     return VC_OK;
 }
 
-// Index order 2: the tables of all the chain's strided convs in one launch (conv_tables_batch_dev) on the chain's stream.
+// The tables of all the chain's strided convs in one launch (conv_tables_batch_dev) on the chain's stream.
 // Their nbr_fwd tables lie back to back and their pair counts too: one -1 fill and one zeroing.
 int fwd_chain_tables(FwdCtx& C, const int* ops, int L, int s) {
     size_t fwd_ints = 0, pn_ints = 0;
@@ -580,7 +569,7 @@ int fwd_chain_tables(FwdCtx& C, const int* ops, int L, int s) {
     return VC_OK;
 }
 
-// Index order 2: the submanifold rulebooks and projections over the chain's output sets (the stage 2-4 work of the plan's
+// The submanifold rulebooks and projections over the chain's output sets (the stage 2-4 work of the plan's
 // image-branch stream), one launch per kind: hash insert + probe of the 3-D sets, index2uv, hash insert + probe of the
 // projected sets.  Applies when all of them run on one stream and probe alike; else each op keeps its own launches.  The
 // deterministic mode's 2-D rulebooks (the gather-form dgrad's `rep` rows) stay per op.
@@ -782,21 +771,18 @@ int fwd_conv_chain(FwdCtx& C, int i) {
     }
     if (C.do_idx) VC_TRY(conv_chain_emit_dev(ch, oidx, n_out, ws, wsb, st));
     for (int l = 0; l < ch.L; ++l) C.produced(C.S->iset[C.op(ops[l])[F_B]], s);
-    if (g_index_order == 2) {
-        VC_TRY(fwd_chain_tables(C, ops, ch.L, s));
-        VC_TRY(fwd_chain_stages(C, i, ops, ch.L));
-    }
-    return VC_OK;
+    VC_TRY(fwd_chain_tables(C, ops, ch.L, s));
+    return fwd_chain_stages(C, i, ops, ch.L);
 }
 
 int fwd_conv_rb(FwdCtx& C, int i, const int* o, int s) {
     // First strided conv reached: the strided convs chained from it get their counts and output indices from one composed
-    // pass (fwd_conv_chain).  Where that rule does not apply (a layer discard between two strided convs, a dilation, a
-    // single conv) or vc_set_index_order(0) asks for it, the loop below is the fallback: the count -> (host reads the row
-    // count) -> emit-indices chain of EVERY strided conv of the plan, back to back.  Each link only needs the previous
-    // link's output indices, and it is the only part of the forward the host has to wait for; the neighbour tables,
-    // submanifold rulebooks and projections queue up behind it without further synchronisation.
-    if (!C.chain[i].done && g_index_order >= 1) VC_TRY(fwd_conv_chain(C, i));
+    // pass (fwd_conv_chain).  Where the chain rule does not apply (a layer discard between two strided convs, a dilation, a
+    // single conv), the loop below builds them level by level: the count -> (host reads the row count) -> emit-indices
+    // chain of EVERY strided conv of the plan, back to back.  Each link only needs the previous link's output indices, and
+    // it is the only part of the forward the host has to wait for; the neighbour tables, submanifold rulebooks and
+    // projections queue up behind it without further synchronisation.
+    if (!C.chain[i].done) VC_TRY(fwd_conv_chain(C, i));
     if (!C.chain[i].done) {
         if (C.S->is_static) {
             // no host read to wait for: keep the natural order (count -> indices -> tables per stage), so the tables of an
@@ -903,22 +889,19 @@ int fwd_cbr(FwdCtx& C, int i, const int* o, int s) {
             if (C.do_feat) VC_TRY(vc_cast_f32_bf16(X.f32, xb, (long long)X.rows * X.c, st));
             X.bf16 = xb;
         }
-        Timed t(K_FWD_TC, li, st);
+        Timed t(K_FWD_TC, li, st, C.do_feat);
         // BatchNorm + ReLU in the same launch (conv_tc2.cu): one kernel and one pass over x fewer per layer
         const BnTail bt{C.P<const float>(li, P_GAMMA), C.P<const float>(li, P_BETA), C.P<float>(li, P_RM), C.P<float>(li, P_RV),
                         C.P<long long>(li, P_NBT), C.lf[2 * li + 1], C.lf[2 * li], S->training, L.sums, y, y_ld, yb, y_ld, stats,
                         C.S->is_static, L.tile_ctr + CTR_BN_BAR};
-        // (flag bit 1: the rulebook was built on another stream and joined by an event, or by an earlier call, so the kernel
-        //  may load its first table slices before its griddepcontrol.wait — conv_tc2.cu)
         if (C.do_feat)
             VC_TRY(tc2_conv(L.cin, L.cout, X.bf16, L.wimg_fwd, R.nbr, R.n_out, x, R.n_out, R.n_out_dev, R.K, sums, C.err, st, nullptr,
-                            L.tile_ctr, ((!C.do_idx || C.st[R.prod] != C.st[s]) ? 2 : 0) | (C.idx_first ? 4 : 0), X.ld, part, &bt,
-                            &bn_done));
+                            L.tile_ctr, C.idx_first ? 2 : 0, X.ld, part, &bt, &bn_done));
     } else {   // (also a tensor-core layer without output rows)
         const size_t wsb = vc_conv_ws_bytes(L.cin, L.cout, R.K);
         VC_ALLOC(ws, void*, wsb);
         VC_CHECK_ARG(X.f32 && X.ld == X.c, "op %d: the fp32 conv needs a dense fp32 input", i);
-        Timed t(K_FWD_F32, li, st);
+        Timed t(K_FWD_F32, li, st, C.do_feat);
         if (C.do_feat && part)
             VC_TRY(conv_fwd_f32_part(X.f32, C.P<const float>(li, P_W), R.nbr, x, R.n_out, L.cin, L.cout, R.K, part, ws, wsb, st));
         else if (C.do_feat)
@@ -1189,11 +1172,9 @@ extern "C" int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, 
                                       void* state, size_t state_bytes, vc_stream_t main_stream, vc_stream_t side_stream,
                                       int side_waits_main, const int32_t* caps, const int32_t* n0_dev, int32_t* overflow_flag,
                                       vc_stream_t side2_stream, const int64_t* rng_seed_dev) {
-    // Index order 2 in static mode (no host read splits the index phase): the index walk first, then the feature walk, so
-    // that no index kernel is resident while the convs run and the fused conv + BN grids take two CTAs per SM
-    // (conv_tc2.cu launch_persist).
-    const bool idx_first = n0_dev != nullptr && ((flags >> 8) & 3) == 0 && g_index_order == 2 && side_stream != nullptr &&
-                           side_stream != main_stream;
+    // Static mode (no host read splits the index phase): the index walk first, then the feature walk, so that no index
+    // kernel is resident while the convs run and the fused conv + BN grids take two CTAs per SM (conv_tc2.cu launch_persist).
+    const bool idx_first = n0_dev != nullptr && ((flags >> 8) & 3) == 0 && side_stream != nullptr && side_stream != main_stream;
     const int f = idx_first ? (flags & ~(3 << 8)) : flags;
     if (idx_first)
         VC_TRY(exec_forward(ops_i, ops_f, n_ops, layer_ptrs, layer_f, n_layers, feats0, c0, idx0, n0, shape0, batch_size, proj_params,
@@ -1203,12 +1184,6 @@ extern "C" int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, 
                         training, precision, idx_first ? f | (2 << 8) : flags, arena, arena_bytes, pinned_host, err_flag, state,
                         state_bytes, main_stream, side_stream, side_waits_main, caps, n0_dev, overflow_flag, side2_stream, rng_seed_dev,
                         idx_first);
-}
-
-extern "C" int vc_set_index_order(int mode) {
-    VC_CHECK_ARG(mode >= 0 && mode <= 2, "index order must be 0, 1 or 2");
-    g_index_order = mode;
-    return VC_OK;
 }
 
 namespace vc {
@@ -1337,8 +1312,9 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
             if (Bb.grad_state == G_OWN) { db = Bb.grad; b_add = Bb.grad; }
             else { VC_ALLOC(t, float*, (size_t)Bb.rows * Bb.c * 4); db = t; b_add = Bb.grad_state == G_EXT ? Bb.grad : nullptr; }
             if (O.rows > 0) {
-                VC_LAUNCH_CHAIN(cat2_bwd_kernel, dim3(ew_grid((size_t)O.rows * O.c / 4)), dim3(256), 0, st, (const float4*)O.grad,
-                                O.rows, Aa.c / 4, Bb.c / 4, (float4*)da, (const float4*)a_add, (float4*)db, (const float4*)b_add);
+                cat2_bwd_kernel<<<dim3(ew_grid((size_t)O.rows * O.c / 4)), dim3(256), 0, st>>>((const float4*)O.grad, O.rows,
+                    Aa.c / 4, Bb.c / 4, (float4*)da, (const float4*)a_add, (float4*)db, (const float4*)b_add);
+                VC_LAUNCH_CHECK();
             }
             Aa.grad = da; Aa.gld = Aa.c; Aa.grad_state = G_OWN;
             Bb.grad = db; Bb.gld = Bb.c; Bb.grad_state = G_OWN;
@@ -1455,7 +1431,7 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
                                             tc ? dxb : nullptr, st));
                     if (tc)
                         VC_TRY(tc2_conv(L.cout, L.cin, dxb, L.wimg_dgrad, R.g2.nbr_g, R.n_in, tmp, R.n_in, R.n_in_dev, R.K, nullptr, C.err,
-                                        st, nullptr, L.tile_ctr + 1, 2));
+                                        st, nullptr, L.tile_ctr + 1));
                     else
                         VC_TRY(vc_conv_dgrad_f32(dx, C.P<const float>(li, P_W), R.g2.nbr_g, tmp, R.n_in, L.cin, L.cout, R.K, 1, ws, wsb,
                                                  st));
@@ -1466,7 +1442,7 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
                 VC_TRY(contribute_fused(C, X, [&](float* dst, const float* addend) -> int {
                     Timed t(L.dgrad, li, st);
                     return tc2_conv(L.cout, L.cin, dxb, L.wimg_dgrad, table, R.n_in, dst, R.n_in, R.n_in_dev, R.K, nullptr, C.err, st,
-                                    addend, L.tile_ctr + 1, (R.subm ? 0 : 1) | 2);      // (tables from the forward call: early loads allowed)
+                                    addend, L.tile_ctr + 1, R.subm ? 0 : 1);
                 }));
                 break;
             case K_DGRAD_F32:

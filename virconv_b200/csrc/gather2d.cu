@@ -187,8 +187,6 @@ __global__ void __launch_bounds__(G2_BIG_THREADS) g2_sort_big_kernel(const int* 
 __global__ void g2_sum_kernel(const float4* __restrict__ g, const uint2* __restrict__ gb, int c4, const int* __restrict__ cnt,
                               const int* __restrict__ off, const int32_t* __restrict__ rows, int cap, const int* __restrict__ n_dev,
                               float4* u, uint2* ub) {
-    pdl_wait();
-    pdl_launch_dependents();
     const int n = rows_of(cap, n_dev);
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const int r = (int)(t / c4), q = (int)(t % c4);
@@ -219,8 +217,6 @@ __global__ void g2_sum_kernel(const float4* __restrict__ g, const uint2* __restr
 }
 
 __global__ void add_rows_ld_kernel(float4* dst, int ld4, const float4* __restrict__ src, int cap, const int* __restrict__ n_dev, int c4) {
-    pdl_wait();
-    pdl_launch_dependents();
     const size_t total = (size_t)rows_of(cap, n_dev) * c4;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         const size_t r = i / c4, q = i % c4;
@@ -327,8 +323,9 @@ int gather2d_sum_dev(const float* g, const void* g_bf16, int c, const G2Prep& P,
     VC_CHECK_ARG(c > 0 && c % 4 == 0 && (g || g_bf16) && (u || u_bf16), "gather-form 2-D dgrad: bad sum arguments");
     if (cap == 0) return VC_OK;
     const int c4 = c / 4;
-    VC_LAUNCH_CHAIN(g2_sum_kernel, dim3(cdiv((long long)cap * c4, 256)), dim3(256), 0, st, (const float4*)g, (const uint2*)g_bf16, c4,
-                    (const int*)P.cnt, (const int*)P.off, (const int32_t*)P.rows, cap, n_dev, (float4*)u, (uint2*)u_bf16);
+    g2_sum_kernel<<<dim3(cdiv((long long)cap * c4, 256)), dim3(256), 0, st>>>((const float4*)g, (const uint2*)g_bf16, c4,
+        (const int*)P.cnt, (const int*)P.off, (const int32_t*)P.rows, cap, n_dev, (float4*)u, (uint2*)u_bf16);
+    VC_LAUNCH_CHECK();
     return VC_OK;
 }
 
@@ -337,7 +334,8 @@ int add_rows_ld_dev(float* dst, int ld, const float* src, int cap, const int* n_
     if (cap == 0) return VC_OK;
     size_t b = ((size_t)cap * (c / 4) + 255) / 256;
     if (b > 132 * 8) b = 132 * 8;
-    VC_LAUNCH_CHAIN(add_rows_ld_kernel, dim3((int)b), dim3(256), 0, st, (float4*)dst, ld / 4, (const float4*)src, cap, n_dev, c / 4);
+    add_rows_ld_kernel<<<dim3((int)b), dim3(256), 0, st>>>((float4*)dst, ld / 4, (const float4*)src, cap, n_dev, c / 4);
+    VC_LAUNCH_CHECK();
     return VC_OK;
 }
 

@@ -8,7 +8,6 @@ namespace vc {
 
 static thread_local char g_err[512] = "";
 static long long g_launches = 0;
-int g_pdl = 1;
 void count_launch() { ++g_launches; }
 
 void set_error(const char* fmt, ...) {
@@ -146,8 +145,6 @@ __global__ void gather_rows4_kernel(const uint32_t* __restrict__ in, const int32
 // (n_dev: device row count, n = capacity; rows [count, capacity) are written as zeros — the concat is a published tensor)
 __global__ void cat2_kernel(const float4* __restrict__ a, const float4* __restrict__ b, float4* __restrict__ out,
                             uint2* __restrict__ out_bf16, int n, const int* __restrict__ n_dev, int ca4, int cb4) {
-    pdl_wait();
-    pdl_launch_dependents();
     const int cnt = n_dev != nullptr ? min(n, __ldg(n_dev)) : n;
     long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     int w = ca4 + cb4;
@@ -265,8 +262,9 @@ int vc::cat2_dev(const float* a, const float* b, float* out, void* out_bf16, int
     if (n == 0) return VC_OK;
     VC_CHECK_ARG(a && b && out, "null pointer");
     long long total = (long long)n * (ca + cb) / 4;
-    VC_LAUNCH_CHAIN(cat2_kernel, dim3(cdiv(total, 256)), dim3(256), 0, stream, (const float4*)a, (const float4*)b, (float4*)out,
-                    (uint2*)out_bf16, n, n_dev, ca / 4, cb / 4);
+    cat2_kernel<<<dim3(cdiv(total, 256)), dim3(256), 0, stream>>>((const float4*)a, (const float4*)b, (float4*)out,
+        (uint2*)out_bf16, n, n_dev, ca / 4, cb / 4);
+    VC_LAUNCH_CHECK();
     return VC_OK;
 }
 
@@ -278,10 +276,6 @@ extern "C" int vc_cat2_f32(const float* a, const float* b, float* out, void* out
 extern "C" int vc_version(void) { return 100; }
 extern "C" const char* vc_last_error(void) { return g_err; }
 extern "C" long long vc_launch_count(void) { return g_launches; }
-extern "C" int vc_set_pdl(int enable) {
-    vc::g_pdl = enable != 0;
-    return VC_OK;
-}
 
 int vc::index2uv_dev(const int32_t* indices, int n, const int* n_dev, int batch_size, const float* params, const float* grid,
                      int stride, int u_max, int v_max, int32_t* uv_out, cudaStream_t stream) {

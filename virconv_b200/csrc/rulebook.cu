@@ -65,127 +65,17 @@ __device__ __forceinline__ void load_index(const int32_t* __restrict__ idx, int 
 // ------------------------------------------------------------------------------------------------
 // (every kernel below that takes a row count `n` also takes `n_dev`: when non-NULL the count is read from device memory
 // and `n` is the capacity the grid / buffers were sized for — the plan executor's static mode, CUDA-graph capturable)
-__device__ __forceinline__ void hash_insert_row(const int32_t* __restrict__ idx, int n, const int* __restrict__ n_dev,
-                                                const Geom& g, unsigned long long* table, uint32_t mask, int row) {
-    if (n_dev != nullptr) n = min(n, __ldg(n_dev));
-    if (row >= n) return;
-    int b, c[VC_MAX_NDIM];
-    load_index(idx, row, g.ndim, b, c);
-    if (!index_ok(g, b, c)) return;
-    unsigned long long key = (unsigned long long)b;
-    for (int d = 0; d < g.ndim; ++d) key = key * (unsigned long long)g.shape[d] + (unsigned long long)c[d];
-    unsigned long long packed = (key << ROW_BITS) | (unsigned long long)row;
-    uint32_t slot = mix64(key) & mask;
-    while (true) {
-        unsigned long long cur = table[slot];
-        if (cur == HASH_EMPTY) {
-            cur = atomicCAS(&table[slot], HASH_EMPTY, packed);
-            if (cur == HASH_EMPTY) return;
-        }
-        if ((cur >> ROW_BITS) == key) {  // duplicate coordinate: lowest row index wins
-            atomicMin(&table[slot], packed);
-            return;
-        }
-        slot = (slot + 1) & mask;
-    }
-}
 
-__global__ void hash_insert_kernel(const int32_t* __restrict__ idx, int n, const int* __restrict__ n_dev, Geom g,
-                                   unsigned long long* table, uint32_t mask) {
-    hash_insert_row(idx, n, n_dev, g, table, mask, blockIdx.x * blockDim.x + threadIdx.x);
-}
-
-__device__ __forceinline__ int hash_lookup(const unsigned long long* __restrict__ table, uint32_t mask,
-                                           unsigned long long key) {
-    uint32_t slot = mix64(key) & mask;
-    while (true) {
-        unsigned long long cur = __ldg(table + slot);
-        if (cur == HASH_EMPTY) return -1;
-        if ((cur >> ROW_BITS) == key) return (int)(cur & ((1ULL << ROW_BITS) - 1));
-        slot = (slot + 1) & mask;
-    }
-}
-
-// One thread per (output row, kernel offset): grid (ceil(n/256), K).  Every probe chain is independent, so the
-// hash look-ups of all K offsets are in flight together (the per-row loop this replaced was latency bound);
-// nbr[k, row] writes stay fully coalesced.  Pair counts: warp ballot -> shared counter -> one atomic per block.
-// sym (every coordinate held by one row, odd kernel sizes): the table is its own transpose — nbr[k, i] = j exactly when
-// nbr[K-1-k, j] = i, the relation the mirrored dgrad already relies on — so the grid covers the offsets k <= centre only
-// and each neighbour found also writes its mirrored entry (the caller fills the rows k > centre with -1 first): half the
-// hash look-ups, the same table.
-// (one block: rows bx * 256 ..., offset k; the batched overload below runs it for the block's stage)
-__device__ __forceinline__ void subm_probe_block(const int32_t* __restrict__ idx, int n, const int* __restrict__ n_dev,
-                                                 const Geom& g, const unsigned long long* __restrict__ table, uint32_t mask,
-                                                 int32_t* __restrict__ nbr, int32_t* __restrict__ pair_num,
-                                                 int32_t* __restrict__ rep, int sym, int bx, int k) {
-    __shared__ int cnt;
-    const int pitch = n;                  // table rows are [K][capacity]
-    if (n_dev != nullptr) n = min(n, __ldg(n_dev));
-    if (threadIdx.x == 0) cnt = 0;
-    __syncthreads();
-    const int row = bx * blockDim.x + threadIdx.x;
-    int res = -1;
-    if (row < n) {
-        int centre = 0;
-        for (int d = 0; d < g.ndim; ++d) centre = centre * g.ksize[d] + g.ksize[d] / 2;
-        if (k == centre) {
-            res = row;  // identity (spconv Native: out = features @ W[centre])
-            if (rep != nullptr) {   // the lowest row at this row's own coordinate (the row itself when it is outside the grid)
-                int b, c[VC_MAX_NDIM];
-                load_index(idx, row, g.ndim, b, c);
-                int r = row;
-                if (index_ok(g, b, c)) {
-                    unsigned long long key = (unsigned long long)b;
-                    for (int d = 0; d < g.ndim; ++d) key = key * (unsigned long long)g.shape[d] + (unsigned long long)c[d];
-                    r = hash_lookup(table, mask, key);
-                }
-                rep[row] = r;
-            }
-        } else {
-            int b, c[VC_MAX_NDIM];
-            load_index(idx, row, g.ndim, b, c);
-            int off[VC_MAX_NDIM];
-            decode_k(g, k, off);
-            bool ok = index_ok(g, b, c);
-            unsigned long long key = (unsigned long long)b;
-            for (int d = 0; d < g.ndim; ++d) {
-                int v = c[d] + (off[d] - g.ksize[d] / 2) * g.dil[d];
-                ok &= (v >= 0) & (v < g.shape[d]);
-                key = key * (unsigned long long)g.shape[d] + (unsigned long long)v;
-            }
-            if (ok) res = hash_lookup(table, mask, key);
-            if (sym && res >= 0) nbr[(size_t)(g.K - 1 - k) * pitch + res] = row;
-        }
-        nbr[(size_t)k * pitch + row] = res;
-    } else if (row < pitch) {
-        nbr[(size_t)k * pitch + row] = -1;    // static mode: rows between the count and the capacity have no neighbours
-        if (rep != nullptr && k == 0) rep[row] = -1;
-    }
-    unsigned m = __ballot_sync(0xffffffffu, res >= 0);
-    if ((threadIdx.x & 31) == 0 && m) atomicAdd(&cnt, __popc(m));
-    __syncthreads();
-    if (pair_num != nullptr && threadIdx.x == 0 && cnt) {
-        atomicAdd(&pair_num[k], cnt);
-        if (sym && k != g.K - 1 - k) atomicAdd(&pair_num[g.K - 1 - k], cnt);
-    }
-}
-
-__global__ void __launch_bounds__(256) subm_probe_kernel(const int32_t* __restrict__ idx, int n,
-                                                         const int* __restrict__ n_dev, Geom g,
-                                                         const unsigned long long* __restrict__ table,
-                                                         uint32_t mask, int32_t* __restrict__ nbr,
-                                                         int32_t* __restrict__ pair_num, int32_t* __restrict__ rep, int sym) {
-    subm_probe_block(idx, n, n_dev, g, table, mask, nbr, pair_num, rep, sym, blockIdx.x, blockIdx.y);
-}
-
-// Batched per-stage index work (subm_rulebook_batch_dev, conv_tables_batch_dev): up to IDX_BATCH_MAX stages in one launch.
-// The grid's x blocks are the stages' row blocks one after the other (stage e owns blocks blk0[e] .. blk0[e + 1] - 1), so a
-// block belongs to one stage and runs exactly what the per-stage launch runs for that block.  Passed by value.
+// Submanifold rulebooks of up to IDX_BATCH_MAX stages in one launch per kernel (subm_rulebook_batch_dev; a single rulebook is
+// a batch of one).  The grid's x blocks are the stages' row blocks one after the other (stage e owns blocks blk0[e] ..
+// blk0[e + 1] - 1), so a block belongs to one stage.  Passed by value as a __grid_constant__ parameter: the kernels read the
+// geometry in place, with no per-thread copy on the stack.
 struct SubmEntry {
     const int32_t* idx;
     const int* n_dev;
     unsigned long long* table;
     int32_t *nbr, *pair_num;
+    int32_t* rep;   // optional [n]: the lowest row at each row's coordinate (the row itself when it is outside the grid)
     Geom g;
     int n, ky;   // ky: offsets probed (centre + 1 with the mirrored probe, else K)
     uint32_t mask;
@@ -205,15 +95,105 @@ __device__ __forceinline__ int batch_entry(const int* blk0, int E, int bx) {
 __global__ void hash_insert_kernel(const __grid_constant__ SubmBatch sb) {
     const int i = batch_entry(sb.blk0, sb.E, blockIdx.x);
     const SubmEntry& e = sb.e[i];
-    hash_insert_row(e.idx, e.n, e.n_dev, e.g, e.table, e.mask, (blockIdx.x - sb.blk0[i]) * blockDim.x + threadIdx.x);
+    const Geom& g = e.g;
+    const int n = e.n_dev != nullptr ? min(e.n, __ldg(e.n_dev)) : e.n;
+    const int row = (blockIdx.x - sb.blk0[i]) * blockDim.x + threadIdx.x;
+    if (row >= n) return;
+    int b, c[VC_MAX_NDIM];
+    load_index(e.idx, row, g.ndim, b, c);
+    if (!index_ok(g, b, c)) return;
+    unsigned long long key = (unsigned long long)b;
+    for (int d = 0; d < g.ndim; ++d) key = key * (unsigned long long)g.shape[d] + (unsigned long long)c[d];
+    unsigned long long packed = (key << ROW_BITS) | (unsigned long long)row;
+    uint32_t slot = mix64(key) & e.mask;
+    while (true) {
+        unsigned long long cur = e.table[slot];
+        if (cur == HASH_EMPTY) {
+            cur = atomicCAS(&e.table[slot], HASH_EMPTY, packed);
+            if (cur == HASH_EMPTY) return;
+        }
+        if ((cur >> ROW_BITS) == key) {  // duplicate coordinate: lowest row index wins
+            atomicMin(&e.table[slot], packed);
+            return;
+        }
+        slot = (slot + 1) & e.mask;
+    }
 }
 
-__global__ void __launch_bounds__(256) subm_probe_kernel(const __grid_constant__ SubmBatch sb) {   // grid (blocks, max ky)
+__device__ __forceinline__ int hash_lookup(const unsigned long long* __restrict__ table, uint32_t mask,
+                                           unsigned long long key) {
+    uint32_t slot = mix64(key) & mask;
+    while (true) {
+        unsigned long long cur = __ldg(table + slot);
+        if (cur == HASH_EMPTY) return -1;
+        if ((cur >> ROW_BITS) == key) return (int)(cur & ((1ULL << ROW_BITS) - 1));
+        slot = (slot + 1) & mask;
+    }
+}
+
+// One thread per (output row, kernel offset): grid (row blocks, max ky).  Every probe chain is independent, so the
+// hash look-ups of all K offsets are in flight together (the per-row loop this replaced was latency bound);
+// nbr[k, row] writes stay fully coalesced.  Pair counts: warp ballot -> shared counter -> one atomic per block.
+// sym (every coordinate held by one row, odd kernel sizes): the table is its own transpose — nbr[k, i] = j exactly when
+// nbr[K-1-k, j] = i, the relation the mirrored dgrad already relies on — so the grid covers the offsets k <= centre only
+// and each neighbour found also writes its mirrored entry (the caller fills the rows k > centre with -1 first): half the
+// hash look-ups, the same table.
+__global__ void __launch_bounds__(256) subm_probe_kernel(const __grid_constant__ SubmBatch sb) {
     const int i = batch_entry(sb.blk0, sb.E, blockIdx.x);
     const SubmEntry& e = sb.e[i];
-    if ((int)blockIdx.y >= e.ky) return;
-    subm_probe_block(e.idx, e.n, e.n_dev, e.g, e.table, e.mask, e.nbr, e.pair_num, nullptr, sb.sym, blockIdx.x - sb.blk0[i],
-                     blockIdx.y);
+    const Geom& g = e.g;
+    const int k = blockIdx.y, sym = sb.sym;
+    if (k >= e.ky) return;
+    __shared__ int cnt;
+    const int pitch = e.n;                // table rows are [K][capacity]
+    const int n = e.n_dev != nullptr ? min(e.n, __ldg(e.n_dev)) : e.n;
+    if (threadIdx.x == 0) cnt = 0;
+    __syncthreads();
+    const int row = (blockIdx.x - sb.blk0[i]) * blockDim.x + threadIdx.x;
+    int res = -1;
+    if (row < n) {
+        int centre = 0;
+        for (int d = 0; d < g.ndim; ++d) centre = centre * g.ksize[d] + g.ksize[d] / 2;
+        if (k == centre) {
+            res = row;  // identity (spconv Native: out = features @ W[centre])
+            if (e.rep != nullptr) {   // the lowest row at this row's own coordinate (the row itself when it is outside the grid)
+                int b, c[VC_MAX_NDIM];
+                load_index(e.idx, row, g.ndim, b, c);
+                int r = row;
+                if (index_ok(g, b, c)) {
+                    unsigned long long key = (unsigned long long)b;
+                    for (int d = 0; d < g.ndim; ++d) key = key * (unsigned long long)g.shape[d] + (unsigned long long)c[d];
+                    r = hash_lookup(e.table, e.mask, key);
+                }
+                e.rep[row] = r;
+            }
+        } else {
+            int b, c[VC_MAX_NDIM];
+            load_index(e.idx, row, g.ndim, b, c);
+            int off[VC_MAX_NDIM];
+            decode_k(g, k, off);
+            bool ok = index_ok(g, b, c);
+            unsigned long long key = (unsigned long long)b;
+            for (int d = 0; d < g.ndim; ++d) {
+                int v = c[d] + (off[d] - g.ksize[d] / 2) * g.dil[d];
+                ok &= (v >= 0) & (v < g.shape[d]);
+                key = key * (unsigned long long)g.shape[d] + (unsigned long long)v;
+            }
+            if (ok) res = hash_lookup(e.table, e.mask, key);
+            if (sym && res >= 0) e.nbr[(size_t)(g.K - 1 - k) * pitch + res] = row;
+        }
+        e.nbr[(size_t)k * pitch + row] = res;
+    } else if (row < pitch) {
+        e.nbr[(size_t)k * pitch + row] = -1;    // static mode: rows between the count and the capacity have no neighbours
+        if (e.rep != nullptr && k == 0) e.rep[row] = -1;
+    }
+    unsigned m = __ballot_sync(0xffffffffu, res >= 0);
+    if ((threadIdx.x & 31) == 0 && m) atomicAdd(&cnt, __popc(m));
+    __syncthreads();
+    if (e.pair_num != nullptr && threadIdx.x == 0 && cnt) {
+        atomicAdd(&e.pair_num[k], cnt);
+        if (sym && k != g.K - 1 - k) atomicAdd(&e.pair_num[g.K - 1 - k], cnt);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -449,47 +429,8 @@ __global__ void conv_emit_indices_kernel(const uint32_t* __restrict__ bitmap, co
     }
 }
 
-__device__ __forceinline__ void conv_tables_block(const int32_t* __restrict__ idx, int n, const int* __restrict__ n_dev,
-                                                  int n_out, const Geom& g, const uint32_t* __restrict__ bitmap,
-                                                  const uint32_t* __restrict__ word_rank,
-                                                  const uint32_t* __restrict__ block_sum, int32_t* __restrict__ nbr_fwd,
-                                                  int32_t* __restrict__ nbr_bwd, int32_t* __restrict__ pair_num, int bx, int k) {
-    __shared__ int cnt;
-    const int pitch_in = n;               // nbr_bwd rows are [K][input capacity], nbr_fwd rows [K][n_out = output capacity]
-    if (n_dev != nullptr) n = min(n, __ldg(n_dev));
-    if (threadIdx.x == 0) cnt = 0;
-    __syncthreads();
-    const int row = bx * blockDim.x + threadIdx.x;
-    int orow = -1;
-    if (row < n) {
-        int b, c[VC_MAX_NDIM];
-        load_index(idx, row, g.ndim, b, c);
-        long long lin = out_cell(g, b, c, k);
-        if (lin >= 0) {
-            orow = cell_rank(bitmap, word_rank, block_sum, lin);
-            if (orow < n_out) nbr_fwd[(size_t)k * n_out + orow] = row;  // unique writer: (o,k) determines the input cell
-            else orow = -1;                                             // beyond the output capacity (overflow flagged)
-        }
-        nbr_bwd[(size_t)k * pitch_in + row] = orow;
-    } else if (row < pitch_in) {
-        nbr_bwd[(size_t)k * pitch_in + row] = -1;   // static mode: rows between the count and the capacity
-    }
-    unsigned m = __ballot_sync(0xffffffffu, orow >= 0);
-    if ((threadIdx.x & 31) == 0 && m) atomicAdd(&cnt, __popc(m));
-    __syncthreads();
-    if (pair_num != nullptr && threadIdx.x == 0 && cnt) atomicAdd(&pair_num[k], cnt);
-}
-
-__global__ void __launch_bounds__(256) conv_tables_kernel(const int32_t* __restrict__ idx, int n, const int* __restrict__ n_dev,
-                                                          int n_out, Geom g,
-                                                          const uint32_t* __restrict__ bitmap,
-                                                          const uint32_t* __restrict__ word_rank,
-                                                          const uint32_t* __restrict__ block_sum,
-                                                          int32_t* __restrict__ nbr_fwd, int32_t* __restrict__ nbr_bwd,
-                                                          int32_t* __restrict__ pair_num) {   // grid (rows, K)
-    conv_tables_block(idx, n, n_dev, n_out, g, bitmap, word_rank, block_sum, nbr_fwd, nbr_bwd, pair_num, blockIdx.x, blockIdx.y);
-}
-
+// The neighbour tables of up to IDX_BATCH_MAX strided convs in one launch (conv_tables_batch_dev; a single conv is a batch
+// of one), laid out as the submanifold batch above.
 struct TablesEntry {
     const int32_t* idx;
     const int* n_dev;
@@ -504,12 +445,36 @@ struct TablesBatch {
     TablesEntry e[IDX_BATCH_MAX];
 };
 
-__global__ void __launch_bounds__(256) conv_tables_kernel(const __grid_constant__ TablesBatch tb) {   // grid (blocks, max K)
+__global__ void __launch_bounds__(256) conv_tables_kernel(const __grid_constant__ TablesBatch tb) {   // grid (row blocks, max K)
     const int i = batch_entry(tb.blk0, tb.E, blockIdx.x);
     const TablesEntry& e = tb.e[i];
-    if ((int)blockIdx.y >= e.g.K) return;
-    conv_tables_block(e.idx, e.n, e.n_dev, e.n_out, e.g, e.r.bitmap, e.r.word_rank, e.r.block_sum, e.nbr_fwd, e.nbr_bwd,
-                      e.pair_num, blockIdx.x - tb.blk0[i], blockIdx.y);
+    const Geom& g = e.g;
+    const int k = blockIdx.y;
+    if (k >= g.K) return;
+    __shared__ int cnt;
+    const int pitch_in = e.n;             // nbr_bwd rows are [K][input capacity], nbr_fwd rows [K][n_out = output capacity]
+    const int n = e.n_dev != nullptr ? min(e.n, __ldg(e.n_dev)) : e.n;
+    if (threadIdx.x == 0) cnt = 0;
+    __syncthreads();
+    const int row = (blockIdx.x - tb.blk0[i]) * blockDim.x + threadIdx.x;
+    int orow = -1;
+    if (row < n) {
+        int b, c[VC_MAX_NDIM];
+        load_index(e.idx, row, g.ndim, b, c);
+        long long lin = out_cell(g, b, c, k);
+        if (lin >= 0) {
+            orow = cell_rank(e.r.bitmap, e.r.word_rank, e.r.block_sum, lin);
+            if (orow < e.n_out) e.nbr_fwd[(size_t)k * e.n_out + orow] = row;  // unique writer: (o,k) determines the input cell
+            else orow = -1;                                                    // beyond the output capacity (overflow flagged)
+        }
+        e.nbr_bwd[(size_t)k * pitch_in + row] = orow;
+    } else if (row < pitch_in) {
+        e.nbr_bwd[(size_t)k * pitch_in + row] = -1;   // static mode: rows between the count and the capacity
+    }
+    unsigned m = __ballot_sync(0xffffffffu, orow >= 0);
+    if ((threadIdx.x & 31) == 0 && m) atomicAdd(&cnt, __popc(m));
+    __syncthreads();
+    if (e.pair_num != nullptr && threadIdx.x == 0 && cnt) atomicAdd(&e.pair_num[k], cnt);
 }
 
 // one block per offset: order-preserving compaction of nbr[k, :] into spconv-style pairs
@@ -587,35 +552,41 @@ using namespace vc;
 
 extern "C" size_t vc_subm_rulebook_ws_bytes(int n) { return (size_t)table_slots(n) * sizeof(unsigned long long); }
 
+// one submanifold stage's arguments -> its geometry and hash-table slots (0: no row, nothing to launch)
+static int subm_stage_geom(const SubmStage& s, int batch_size, Geom& g, uint32_t& slots) {
+    int rc = make_geom(g, s.ndim, batch_size, s.shape, s.ksize, nullptr, nullptr, s.dil);
+    if (rc) return rc;
+    VC_CHECK_ARG(s.n >= 0 && s.n < (1 << ROW_BITS), "row count %d out of range", s.n);
+    double cells = (double)batch_size;
+    for (int d = 0; d < s.ndim; ++d) cells *= g.shape[d];
+    VC_CHECK_ARG(cells < 1099511627776.0, "grid too large for 40-bit keys");
+    slots = 0;
+    if (s.n == 0) return VC_OK;
+    VC_CHECK_ARG(s.idx && s.nbr && s.table, "null pointer");
+    slots = table_slots(s.n);
+    if (s.table_bytes < (size_t)slots * 8) {
+        set_error("subm rulebook workspace %zu < %zu", s.table_bytes, (size_t)slots * 8);
+        return VC_ERR_WORKSPACE;
+    }
+    return VC_OK;
+}
+
+// one rulebook: its own clears, then a batch of one
 int vc::subm_rulebook_dev(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size,
                           const int32_t* spatial_shape, const int32_t* ksize, const int32_t* dilation, int32_t* nbr,
                           int32_t* pair_num, void* ws, size_t ws_bytes, cudaStream_t stream, int32_t* rep, bool unique) {
+    const SubmStage s{indices, n, n_dev, ndim, spatial_shape, ksize, dilation, nbr, pair_num, ws, ws_bytes, rep};
     Geom g;
-    int rc = make_geom(g, ndim, batch_size, spatial_shape, ksize, nullptr, nullptr, dilation);
+    uint32_t slots;
+    int rc = subm_stage_geom(s, batch_size, g, slots);
     if (rc) return rc;
-    VC_CHECK_ARG(n >= 0 && n < (1 << ROW_BITS), "row count %d out of range", n);
-    double cells = (double)batch_size;
-    for (int d = 0; d < ndim; ++d) cells *= g.shape[d];
-    VC_CHECK_ARG(cells < 1099511627776.0, "grid too large for 40-bit keys");
     if (pair_num) VC_CUDA(cudaMemsetAsync(pair_num, 0, sizeof(int32_t) * g.K, stream));
     if (n == 0) return VC_OK;
-    VC_CHECK_ARG(indices && nbr && ws, "null pointer");
-    uint32_t slots = table_slots(n);
-    if (ws_bytes < (size_t)slots * 8) {
-        set_error("subm rulebook workspace %zu < %zu", ws_bytes, (size_t)slots * 8);
-        return VC_ERR_WORKSPACE;
-    }
-    unsigned long long* table = (unsigned long long*)ws;
-    VC_CUDA(cudaMemsetAsync(table, 0xFF, (size_t)slots * 8, stream));
-    hash_insert_kernel<<<cdiv(n, 256), 256, 0, stream>>>(indices, n, n_dev, g, table, slots - 1);
-    VC_LAUNCH_CHECK();
-    const bool sym = rep == nullptr && subm_sym(ndim, ksize, unique);
+    VC_CUDA(cudaMemsetAsync(ws, 0xFF, (size_t)slots * 8, stream));
     const int centre = g.K / 2;   // (odd kernel sizes: the centre offset is the middle one)
-    if (sym) VC_CUDA(cudaMemsetAsync(nbr + (size_t)(centre + 1) * n, 0xFF, sizeof(int32_t) * (size_t)(g.K - 1 - centre) * n, stream));
-    subm_probe_kernel<<<dim3(cdiv(n, 256), sym ? centre + 1 : g.K), 256, 0, stream>>>(indices, n, n_dev, g, table, slots - 1, nbr,
-                                                                                      pair_num, rep, sym ? 1 : 0);
-    VC_LAUNCH_CHECK();
-    return VC_OK;
+    if (rep == nullptr && subm_sym(ndim, ksize, unique))
+        VC_CUDA(cudaMemsetAsync(nbr + (size_t)(centre + 1) * n, 0xFF, sizeof(int32_t) * (size_t)(g.K - 1 - centre) * n, stream));
+    return subm_rulebook_batch_dev(&s, 1, batch_size, unique, stream);
 }
 
 extern "C" int vc_subm_rulebook(const int32_t* indices, int n, int ndim, int batch_size, const int32_t* spatial_shape,
@@ -746,6 +717,7 @@ ConvRank vc::conv_rank_of(int ndim, int batch_size, const int32_t* out_shape, co
     return ConvRank{w.bitmap, w.word_rank, w.block_sum};
 }
 
+// one strided conv: its own clears, then a batch of one
 int vc::conv_rulebook_tables_dev(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size,
                                  const int32_t* spatial_shape, const int32_t* ksize, const int32_t* stride, const int32_t* padding,
                                  const int32_t* dilation, int n_out, ConvRank rank, int32_t* nbr_fwd, int32_t* nbr_bwd,
@@ -758,13 +730,9 @@ int vc::conv_rulebook_tables_dev(const int32_t* indices, int n, const int* n_dev
         VC_CHECK_ARG(nbr_fwd, "null output pointer");
         VC_CUDA(cudaMemsetAsync(nbr_fwd, 0xFF, (size_t)g.K * n_out * 4, stream));
     }
-    if (n > 0) {
-        VC_CHECK_ARG(nbr_bwd, "null nbr_bwd");
-        conv_tables_kernel<<<dim3(cdiv(n, 256), g.K), 256, 0, stream>>>(indices, n, n_dev, n_out, g, rank.bitmap, rank.word_rank,
-                                                                         rank.block_sum, nbr_fwd, nbr_bwd, pair_num);
-        VC_LAUNCH_CHECK();
-    }
-    return VC_OK;
+    const TablesStage s{indices, n, n_dev, ndim, spatial_shape, ksize, stride, padding, dilation, n_out, rank, nbr_fwd, nbr_bwd,
+                        pair_num};
+    return conv_tables_batch_dev(&s, 1, batch_size, stream);
 }
 
 bool vc::subm_sym(int ndim, const int32_t* ksize, bool unique) {
@@ -773,8 +741,8 @@ bool vc::subm_sym(int ndim, const int32_t* ksize, bool unique) {
     return sym;
 }
 
-// The launches of subm_rulebook_dev (rep == NULL) for up to IDX_BATCH_MAX stages: one hash insert and one probe.  The caller
-// has cleared every stage's table (0xFF), its mirrored rows k > centre (-1, when subm_sym) and its pair counts.
+// The launches of up to IDX_BATCH_MAX submanifold rulebooks: one hash insert and one probe.  The caller has cleared every
+// stage's table (0xFF), its mirrored rows k > centre (-1, when it probes mirrored) and its pair counts.
 int vc::subm_rulebook_batch_dev(const SubmStage* st, int n_st, int batch_size, bool unique, cudaStream_t stream) {
     VC_CHECK_ARG(n_st >= 1 && n_st <= IDX_BATCH_MAX, "%d stages in one batch", n_st);
     SubmBatch sb;
@@ -784,24 +752,15 @@ int vc::subm_rulebook_batch_dev(const SubmStage* st, int n_st, int batch_size, b
     for (int i = 0; i < n_st; ++i) {
         const SubmStage& s = st[i];
         SubmEntry& e = sb.e[sb.E];
-        int rc = make_geom(e.g, s.ndim, batch_size, s.shape, s.ksize, nullptr, nullptr, s.dil);
+        uint32_t slots;
+        int rc = subm_stage_geom(s, batch_size, e.g, slots);
         if (rc) return rc;
-        VC_CHECK_ARG(s.n >= 0 && s.n < (1 << ROW_BITS), "row count %d out of range", s.n);
-        double cells = (double)batch_size;
-        for (int d = 0; d < s.ndim; ++d) cells *= e.g.shape[d];
-        VC_CHECK_ARG(cells < 1099511627776.0, "grid too large for 40-bit keys");
-        const int sym = subm_sym(s.ndim, s.ksize, unique) ? 1 : 0;
+        const int sym = s.rep == nullptr && subm_sym(s.ndim, s.ksize, unique) ? 1 : 0;
         VC_CHECK_ARG(sb.sym < 0 || sb.sym == sym, "stages of one batch probe alike");
         sb.sym = sym;
         if (s.n == 0) continue;
-        VC_CHECK_ARG(s.idx && s.nbr && s.table, "null pointer");
-        const uint32_t slots = table_slots(s.n);
-        if (s.table_bytes < (size_t)slots * 8) {
-            set_error("subm rulebook workspace %zu < %zu", s.table_bytes, (size_t)slots * 8);
-            return VC_ERR_WORKSPACE;
-        }
         e.idx = s.idx; e.n = s.n; e.n_dev = s.n_dev; e.table = (unsigned long long*)s.table; e.mask = slots - 1;
-        e.nbr = s.nbr; e.pair_num = s.pair_num;
+        e.nbr = s.nbr; e.pair_num = s.pair_num; e.rep = s.rep;
         e.ky = sym ? e.g.K / 2 + 1 : e.g.K;
         ky = e.ky > ky ? e.ky : ky;
         sb.blk0[sb.E + 1] = sb.blk0[sb.E] + cdiv(s.n, 256);
@@ -815,8 +774,8 @@ int vc::subm_rulebook_batch_dev(const SubmStage* st, int n_st, int batch_size, b
     return VC_OK;
 }
 
-// conv_rulebook_tables_dev's kernel for up to IDX_BATCH_MAX strided convs in one launch.  The caller has filled every nbr_fwd
-// with -1 and zeroed the pair counts.
+// The tables of up to IDX_BATCH_MAX strided convs in one launch.  The caller has filled every nbr_fwd with -1 and zeroed the
+// pair counts.
 int vc::conv_tables_batch_dev(const TablesStage* st, int n_st, int batch_size, cudaStream_t stream) {
     VC_CHECK_ARG(n_st >= 1 && n_st <= IDX_BATCH_MAX, "%d stages in one batch", n_st);
     TablesBatch tb;

@@ -120,8 +120,6 @@ __global__ void __launch_bounds__(W_THREADS, 2) tc_wgrad_half_kernel(const WArgs
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    pdl_wait();
-    pdl_launch_dependents();
     const int n = a.n_dev != nullptr ? min(__ldg(a.n_dev), a.n_host) : a.n_host;
     // a pipeline wait that timed out in an EARLIER launch left the (sticky) error flag set: do nothing, so that whatever went
     // wrong costs one 2-second timeout, not one per launch
@@ -418,7 +416,8 @@ int launch_wgrad3(const WArgs& a0, int n_cap, int max_ctas, cudaStream_t stream)
     }
     const int tiles = cdiv(n_cap, TCM);
     const int grid = tiles < max_ctas ? (tiles < 1 ? 1 : tiles) : max_ctas;
-    VC_LAUNCH_CHAIN(kern, dim3(grid, passes), dim3(W_THREADS), smem, stream, a);
+    kern<<<dim3(grid, passes), dim3(W_THREADS), smem, stream>>>(a);
+    VC_LAUNCH_CHECK();
     return VC_OK;
 }
 

@@ -59,17 +59,13 @@ def _ws(nbytes, device):
 
 
 # ------------------------------------------------------------------------------------------------
-# side stream: independent work that would otherwise serialise behind latency-bound kernels runs concurrently —
-#   * forward : voxel->pixel projection + the 2-D rulebook of an NRConv block next to its two 3-D convs (on);
-#   * backward: wgrad of layer i next to BN-backward + dgrad of layer i-1 (implemented, off by default, see below).
-# Joined back into the main stream before anything consumes the results; disable with VIRCONV_OVERLAP=0.
+# side stream: the voxel->pixel projection + the 2-D rulebook of an NRConv block run next to its two 3-D convs instead of
+# serialising behind those latency-bound kernels.  Joined back into the main stream before anything consumes the
+# results; disable with VIRCONV_OVERLAP=0.
 # ------------------------------------------------------------------------------------------------
 import os as _os
 
-OVERLAP = _os.environ.get('VIRCONV_OVERLAP', '1') != '0'                      # forward: projection + 2-D rulebook
-# backward wgrad overlap: the persistent wgrad CTAs hold up to 126 KB of shared memory per SM, so the dgrad CTAs behind
-# them cannot co-reside -> off unless asked for
-OVERLAP_WGRAD = _os.environ.get('VIRCONV_OVERLAP_WGRAD', '0') != '0' and OVERLAP
+OVERLAP = _os.environ.get('VIRCONV_OVERLAP', '1') != '0'
 _SIDE = {}
 
 
@@ -78,7 +74,6 @@ class _Side:
         # high priority: the side stream carries the small index kernels the HOST waits on (row counts of the strided
         # convs); they must not queue behind the wide feature kernels of the main stream
         self.stream = torch.cuda.Stream(device=device, priority=-1)
-        self.join_queued = False
 
 
 def side(device) -> _Side:
@@ -486,25 +481,7 @@ class ConvBNReLUFn(torch.autograd.Function):
             bsums = torch.zeros(2 * cout, dtype=torch.float64, device=dy.device)
         check(lib.vc_bn_relu_bwd_f32(_p(dy), _p(x), _p(y), _p(gamma), _p(stats), _p(dx), _p(db), _p(dgamma), _p(dbeta),
                                      rb.n_out, cout, int(ctx.training), _p(bsums), _stream()), 'vc_bn_relu_bwd_f32')
-        dw = None
-        if ctx.needs_input_grad[1] and OVERLAP_WGRAD:
-            # wgrad on the side stream, concurrent with this layer's dgrad and the next layer's BN backward
-            sd = side(dy.device)
-            main = torch.cuda.current_stream()
-            sd.stream.wait_stream(main)                     # dx / db are ready
-            with torch.cuda.stream(sd.stream):
-                dw = conv_wgrad(feats, dx, weight.shape, rb, ctx.precision, ctx.fb, db)
-            _keep_alive_on(sd.stream, feats, dx, ctx.fb, db, rb.nbr)
-            dw.record_stream(main)
-            if not sd.join_queued:                          # join once, when this backward pass ends
-                sd.join_queued = True
-
-                def _join(sd=sd, main=main):
-                    main.wait_stream(sd.stream)
-                    sd.join_queued = False
-                torch.autograd.Variable._execution_engine.queue_callback(_join)
-        elif ctx.needs_input_grad[1]:
-            dw = conv_wgrad(feats, dx, weight.shape, rb, ctx.precision, ctx.fb, db)
+        dw = conv_wgrad(feats, dx, weight.shape, rb, ctx.precision, ctx.fb, db) if ctx.needs_input_grad[1] else None
         din = conv_dgrad(dx, weight, rb, ctx.precision, db) if ctx.needs_input_grad[0] else None
         return din, dw, dgamma, dbeta, None, None, None, None, None, None, None, None, None
 
