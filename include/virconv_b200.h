@@ -60,9 +60,15 @@ int vc_set_tc_variant(int variant);
  * unless 2 is forced or no index kernel runs beside it (the plan executor's static mode with side streams, which enqueues
  * the whole index phase before the first feature kernel). */
 int vc_conv_tc2_config(int ctas_per_sm);
-/* The plan executor's weight-gradient launches (csrc/wgrad_tc3.cu): variant must be 1 (the only kernel); max_ctas caps
- * their CTAs (0, the default: half the SMs, so that each shares its SM with a dgrad CTA of the main stream). */
+/* The plan executor's weight-gradient launches (csrc/wgrad_tc3.cu): variant must be 1 (the only kernel); max_ctas > 0 caps
+ * the CTAs of each launch, over all its passes; 0, the default: half the SMs for each pass, so that each CTA shares its
+ * SM with a dgrad CTA of the main stream. */
 int vc_conv_wgrad_tc3_config(int variant, int max_ctas);
+/* Host-only: the grid of the tensor-core wgrad launch over n_rows output rows of a cin -> cout layer with K offsets under a
+ * CTA cap of max_ctas >= 1.  out[0] = CTAs per pass (0 when n_rows is 0: nothing is launched), out[1] = passes (groups of
+ * kernel offsets whose accumulators fit the registers, blockIdx.y).  out[0] * out[1] <= max_ctas whenever
+ * out[1] <= max_ctas; a launch with more passes than the cap takes one CTA per pass. */
+int vc_wgrad_launch_geometry(int cin, int cout, int K, int n_rows, int max_ctas, int32_t* out);
 
 /* ------------------------------------------------------------------------------------------------
  * Rulebooks.  Replaces spconv `ops.get_indice_pairs`, reached from every conv call site:
@@ -165,7 +171,7 @@ int vc_conv_dgrad_tc(const void* dout_bf16, const float* w, const int32_t* nbr_t
 /* dw[co,k,ci] = sum_o in[nbr[k,o],ci] * dout[o,co] on tensor cores: both operands bf16 (MN-major wgmma), 128/cin
  * kernel offsets stacked along the MMA M dimension, accumulators resident in registers across all tiles of a
  * persistent CTA, which adds them into one fp32 image with vector reductions: the summation order, and so the last
- * bits of dw, vary from run to run.  ws >= vc_conv_wgrad_tc_ws_bytes(...). */
+ * bits of dw, vary from run to run.  One CTA per SM for each pass of offset groups.  ws >= vc_conv_wgrad_tc_ws_bytes(...). */
 size_t vc_conv_wgrad_tc_ws_bytes(int n_out, int cin, int cout, int K);
 int vc_conv_wgrad_tc(const void* in_bf16, const void* dout_bf16, const int32_t* nbr, float* dw, int n_out, int cin,
                      int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag, vc_stream_t stream);
@@ -197,7 +203,7 @@ int vc_conv_bn_relu_tc(const void* in_bf16, const float* w, const int32_t* nbr, 
                        vc_stream_t stream);
 /* vc_conv_wgrad_tc with the rows split into 32 runs of consecutive 128-row tiles (from n_out alone); a CTA claims whole
  * runs, each run's sum goes to its own fp32 image, and the images are added in run order.  The CTA cap of
- * vc_conv_wgrad_tc3_config applies (0: one CTA per SM).  ws >= vc_conv_wgrad_tc_det_ws_bytes(...) (32 images). */
+ * vc_conv_wgrad_tc3_config applies (0: one CTA per SM for each pass, as vc_conv_wgrad_tc).  ws >= vc_conv_wgrad_tc_det_ws_bytes(...) (32 images). */
 size_t vc_conv_wgrad_tc_det_ws_bytes(int n_out, int cin, int cout, int K);
 int vc_conv_wgrad_tc_det(const void* in_bf16, const void* dout_bf16, const int32_t* nbr, float* dw, int n_out, int cin,
                          int cout, int K, void* ws, size_t ws_bytes, int32_t* err_flag, vc_stream_t stream);

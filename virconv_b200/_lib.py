@@ -32,6 +32,7 @@ SIGNATURES = {
     'vc_set_tc_variant': (_I, [_I]),
     'vc_conv_tc2_config': (_I, [_I]),
     'vc_conv_wgrad_tc3_config': (_I, [_I, _I]),
+    'vc_wgrad_launch_geometry': (_I, [_I, _I, _I, _I, _I, _HOST]),
     'vc_subm_rulebook_ws_bytes': (_Z, [_I]),
     'vc_subm_rulebook': (_I, [_P, _I, _I, _I, _HOST, _HOST, _HOST, _P, _P, _P, _Z, _P]),
     'vc_conv_rulebook_ws_bytes': (_Z, [_I, _I, _HOST]),

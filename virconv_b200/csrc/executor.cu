@@ -1275,8 +1275,10 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
     const int training = S->training;
     WgradFinTable fin;          // persistent wgrad kernels accumulate into scratch images; ONE transposing launch at the end
     fin.n = 0;
-    // wgrad CTAs: half the SMs by default, so that a CTA of the dgrad chain fits beside each (DESIGN.md section 4)
-    const int wgrad_ctas = g_wgrad3_ctas > 0 ? g_wgrad3_ctas : (num_sms() + 1) / 2;
+    // CTAs of a wgrad launch: a cap set with vc_conv_wgrad_tc3_config is a budget over all its passes; by default half the
+    // SMs for each pass, so that a CTA of the dgrad chain fits beside each.  (A budget of three quarters of the SMs per
+    // launch ran faster, but fewer CTAs per pass lengthen each CTA's fp32 accumulation: DESIGN.md section 8, item 6)
+    const int half_sms = (num_sms() + 1) / 2;
 
     for (int i = 0; i < MAX_F; ++i) { S->f[i].grad = nullptr; S->f[i].gld = S->f[i].c; S->f[i].grad_state = G_EMPTY; }
     for (int i = 0; i < n_pub; ++i) {
@@ -1373,30 +1375,9 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
         }
         VC_TRY(bn_relu_bwd_dev(Y.grad, Y.gld, L.x, C.P<const float>(li, P_GAMMA), L.stats, dx, dxb, dgamma, dbeta, R.n_out, R.n_out_dev,
                                L.cout, training, L.sums + 2 * L.cout, S->is_static, st, bpart));
-        // wgrad (needs dx / its bf16 shadow: ordered after the BN backward through an event when on its own stream)
-        if (two) {
-            int e = record_on(C, 0);
-            if (e >= 0) VC_CUDA(cudaStreamWaitEvent(wst, g_ev[e], 0));
-        }
-        if (L.wgrad == K_WGRAD_TC) {
-            Timed t(L.wgrad, li, wst);
-            VC_TRY(tc3_wgrad(L.cin, L.cout, X.bf16, dxb, R.nbr, R.n_out, L.wscratch, R.n_out, R.n_out_dev, R.K, C.err, wst,
-                             L.tile_ctr + 2, wgrad_ctas, X.ld, S->deterministic ? WGRAD_DET_CHUNKS : 0));
-            if (fin.n == WGRAD_FIN_MAX) {
-                VC_TRY(wgrad_finalize(fin, wst));
-                fin.n = 0;
-            }
-            WgradFinEntry& fe = fin.e[fin.n++];
-            fe.scratch = L.wscratch; fe.dw = dw; fe.cin = L.cin; fe.cout = L.cout; fe.K = R.K; fe.first = 0;
-            fe.n_part = S->deterministic ? WGRAD_DET_CHUNKS : 1;
-        } else {
-            const size_t wsb = vc_conv_wgrad_ws_bytes(R.n_out, L.cin, L.cout, R.K);
-            VC_ALLOC(ws, void*, wsb);
-            VC_CHECK_ARG(X.f32 && X.ld == X.c, "layer %d: the fp32 wgrad needs a dense fp32 input", li);
-            Timed t(L.wgrad, li, wst);
-            VC_TRY(vc_conv_wgrad_f32(X.f32, dx, R.nbr, dw, R.n_out, L.cin, L.cout, R.K, ws, wsb, wst));
-        }
-        if (two) last_w_ev = record_on(C, 1);
+        // the wgrad needs dx / its bf16 shadow: on its own stream it waits for this event, and it is enqueued after the
+        // dgrad, which is on the critical path (the dgrad's CTAs reach the SMs first)
+        const int bn_ev = two ? record_on(C, 0) : -1;
         // dgrad
         const int32_t* table = R.subm ? R.nbr : R.nbr_bwd;
         const size_t wsb = vc_conv_ws_bytes(L.cin, L.cout, R.K);
@@ -1454,6 +1435,28 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
                 break;
             default: break;   // K_NONE
         }
+        // wgrad
+        if (bn_ev >= 0) VC_CUDA(cudaStreamWaitEvent(wst, g_ev[bn_ev], 0));
+        if (L.wgrad == K_WGRAD_TC) {
+            Timed t(L.wgrad, li, wst);
+            VC_TRY(tc3_wgrad(L.cin, L.cout, X.bf16, dxb, R.nbr, R.n_out, L.wscratch, R.n_out, R.n_out_dev, R.K, C.err, wst,
+                             L.tile_ctr + 2, g_wgrad3_ctas > 0 ? g_wgrad3_ctas : half_sms * wgrad3_passes(L.cin, L.cout, R.K), X.ld,
+                             S->deterministic ? WGRAD_DET_CHUNKS : 0));
+            if (fin.n == WGRAD_FIN_MAX) {
+                VC_TRY(wgrad_finalize(fin, wst));
+                fin.n = 0;
+            }
+            WgradFinEntry& fe = fin.e[fin.n++];
+            fe.scratch = L.wscratch; fe.dw = dw; fe.cin = L.cin; fe.cout = L.cout; fe.K = R.K; fe.first = 0;
+            fe.n_part = S->deterministic ? WGRAD_DET_CHUNKS : 1;
+        } else {
+            const size_t wsb = vc_conv_wgrad_ws_bytes(R.n_out, L.cin, L.cout, R.K);
+            VC_ALLOC(ws, void*, wsb);
+            VC_CHECK_ARG(X.f32 && X.ld == X.c, "layer %d: the fp32 wgrad needs a dense fp32 input", li);
+            Timed t(L.wgrad, li, wst);
+            VC_TRY(vc_conv_wgrad_f32(X.f32, dx, R.nbr, dw, R.n_out, L.cin, L.cout, R.K, ws, wsb, wst));
+        }
+        if (two) last_w_ev = record_on(C, 1);
     }
     if (fin.n > 0) {
         VC_TRY(wgrad_finalize(fin, wst));

@@ -25,7 +25,7 @@
 
 namespace vc {
 
-int g_wgrad3_ctas = 0;      // CTA cap of the plan executor's launches (vc_conv_wgrad_tc3_config); 0 = half the SMs
+int g_wgrad3_ctas = 0;      // CTA cap of the plan executor's launches (vc_conv_wgrad_tc3_config); 0 = half the SMs per pass
 
 namespace {
 
@@ -389,6 +389,15 @@ done:
     __syncthreads();
 }
 
+// CTAs per pass of a launch over n_rows output rows: max_ctas is the budget of the whole launch, split over its passes, so
+// grid.x * passes <= max_ctas whenever passes <= max_ctas.  Every pass keeps at least one CTA, so only a launch with more
+// passes than max_ctas exceeds the cap (by taking one CTA per pass).
+int wgrad3_grid_x(int n_rows, int passes, int max_ctas) {
+    const int tiles = cdiv(n_rows, TCM), per_pass = max_ctas / passes;
+    const int g = tiles < per_pass ? tiles : per_pass;
+    return g < 1 ? 1 : g;
+}
+
 template <int CI, int CO>
 int launch_wgrad3(const WArgs& a0, int n_cap, int max_ctas, cudaStream_t stream) {
     using C = WCfg2<CI, CO>;
@@ -414,9 +423,7 @@ int launch_wgrad3(const WArgs& a0, int n_cap, int max_ctas, cudaStream_t stream)
         VC_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, W_SMEM_BUDGET));
         attr_done = true;
     }
-    const int tiles = cdiv(n_cap, TCM);
-    const int grid = tiles < max_ctas ? (tiles < 1 ? 1 : tiles) : max_ctas;
-    kern<<<dim3(grid, passes), dim3(W_THREADS), smem, stream>>>(a);
+    kern<<<dim3(wgrad3_grid_x(n_cap, passes, max_ctas), passes), dim3(W_THREADS), smem, stream>>>(a);
     VC_LAUNCH_CHECK();
     return VC_OK;
 }
@@ -424,7 +431,7 @@ int launch_wgrad3(const WArgs& a0, int n_cap, int max_ctas, cudaStream_t stream)
 }  // namespace
 
 // scratch: [K][cin][cout] fp32, ZERO on entry (the kernel accumulates); tile_counter: `wgrad3_passes(cin, cout, K)` ints, zero;
-// at most max_ctas CTAs per pass
+// at most max_ctas CTAs over all passes (wgrad3_grid_x)
 int tc3_wgrad(int cin, int cout, const void* in_bf16, const void* dout_bf16, const int32_t* nbr, long long pitch, float* scratch,
               int n_rows, const int* n_dev, int K, int* err, cudaStream_t stream, int* tile_counter, int max_ctas, int in_ld,
               int det_chunks) {
@@ -505,6 +512,14 @@ extern "C" int vc_conv_wgrad_tc3_config(int variant, int max_ctas) {
     return VC_OK;
 }
 
+extern "C" int vc_wgrad_launch_geometry(int cin, int cout, int K, int n_rows, int max_ctas, int32_t* out) {
+    VC_CHECK_ARG(out && n_rows >= 0 && max_ctas >= 1 && K >= 1 && K <= MAXK_TC && tc2_ch_ok(cin) && tc2_ch_ok(cout),
+                 "bad wgrad geometry query (%d -> %d channels, K=%d, %d rows, cap %d)", cin, cout, K, n_rows, max_ctas);
+    out[1] = wgrad3_passes(cin, cout, K);
+    out[0] = n_rows > 0 ? wgrad3_grid_x(n_rows, out[1], max_ctas) : 0;
+    return VC_OK;
+}
+
 extern "C" size_t vc_conv_wgrad_tc_ws_bytes(int n_out, int cin, int cout, int K) {
     // the scratch image all CTAs accumulate into (whatever n_out), then one tile counter per pass
     const size_t passes = tc2_ch_ok(cin) && tc2_ch_ok(cout) && K >= 1 ? (size_t)wgrad3_passes(cin, cout, K) : 0;
@@ -534,9 +549,9 @@ extern "C" int vc_conv_wgrad_tc(const void* in_bf16, const void* dout_bf16, cons
     // accumulate into a zeroed scratch image, then one transposing pass
     const size_t wbytes = (size_t)K * cin * cout * sizeof(float);
     VC_CUDA(cudaMemsetAsync(ws, 0, need, stream));
-    // alone on its stream the kernel measured fastest with one CTA per SM (DESIGN.md section 4)
+    // alone on its stream the kernel measured fastest with one CTA per SM for each pass (DESIGN.md section 4)
     int rc = tc3_wgrad(cin, cout, in_bf16, dout_bf16, nbr, n_out, (float*)ws, n_out, nullptr, K, err_flag, stream,
-                       reinterpret_cast<int*>((char*)ws + wbytes), num_sms());
+                       reinterpret_cast<int*>((char*)ws + wbytes), num_sms() * wgrad3_passes(cin, cout, K));
     if (rc) return rc;
     WgradFinTable T;
     T.n = 1;
@@ -572,7 +587,7 @@ static int wgrad_tc_det(const void* in_bf16, int in_ld, const void* dout_bf16, c
     const size_t pbytes = (size_t)WGRAD_DET_CHUNKS * K * cin * cout * sizeof(float);
     VC_CUDA(cudaMemsetAsync(ws, 0, need, stream));
     int rc = tc3_wgrad(cin, cout, in_bf16, dout_bf16, nbr, n_out, (float*)ws, n_out, nullptr, K, err_flag, stream,
-                       reinterpret_cast<int*>((char*)ws + pbytes), g_wgrad3_ctas > 0 ? g_wgrad3_ctas : num_sms(), in_ld,
+                       reinterpret_cast<int*>((char*)ws + pbytes), g_wgrad3_ctas > 0 ? g_wgrad3_ctas : num_sms() * wgrad3_passes(cin, cout, K), in_ld,
                        WGRAD_DET_CHUNKS);
     if (rc) return rc;
     WgradFinTable T;
