@@ -305,6 +305,28 @@ int vc_stvd_partition(const float* points, int n, int c, int bin_num, double max
 int vc_stvd_gather(const float* points, int n, int c, const int32_t* segs /*host*/, int n_seg, const int32_t* sel_dev,
                    float* out /*[n_out, c]*/, int n_out, void* ws, size_t ws_bytes, vc_stream_t stream);
 
+/* The input front end with the draws on the device, no host read (graph-capturable), csrc/stvd.cu.  points [cap, w] fp32
+ * collated rows (b, x, y, z, ..., indicator), scenes contiguous and ascending, *n_dev (may be NULL: cap) valid rows;
+ * indicator 1 = virtual, 2 = LiDAR, anything else and b outside [0, batch_size) is dropped.  Per scene, the virtual points go
+ * through the StVD input discard (bin_num bins of width max_dis / bin_num, the reference's position / per_bin arithmetic in
+ * float64; a subsampled bin keeps its `per_bin` smallest (u, row), u = word 0 of Philox4x32-10 with counter
+ * (row, 0, 1, draw) and key (seed & 0xffffffff, seed >> 32), seed = *seed_dev, in row order), then
+ *   later_fusion 0: out_points = [LiDAR, kept virtual bins far -> near] per scene, column 4 (intensity) divided by 10;
+ *   later_fusion 1: out_points = LiDAR, out_mm = kept virtual bins far -> near;
+ * rows outside pc_range (host[6], x and y, bounds inclusive) dropped; shuffle != 0: each scene's block of each stream
+ * permuted by a Philox-keyed Feistel bijection (counter domain 2).  src_* (may be NULL) = the input row of every output row.
+ * n_out_dev[2] = rows written per stream; tails: batch column -1, zeros, source -1.  status_dev[B]: bit 0 = the scene has
+ * no virtual point (the reference divides by zero); bit 1 = the scenes of the batch are not contiguous and ascending, and
+ * nothing was kept.  *overflow_dev = max(*overflow_dev, rows that did not fit).
+ * ws >= vc_stvd_input_ws_bytes(cap, batch_size).  A memset and 22 launches. */
+size_t vc_stvd_input_ws_bytes(int cap, int batch_size);
+int vc_stvd_input_front_end(const float* points, int cap, const int32_t* n_dev /*may be NULL*/, int w, int batch_size, int bin_num,
+                            double max_dis, double rate, const float* pc_range /*host[6]*/, int later_fusion, int shuffle,
+                            const int64_t* seed_dev, int draw, float* out_points, int32_t* src_points /*may be NULL*/,
+                            int cap_points, float* out_mm, int32_t* src_mm /*may be NULL*/, int cap_mm,
+                            int32_t* n_out_dev /*[2]*/, int32_t* status_dev /*[B]*/, int32_t* overflow_dev /*[1], may be NULL*/,
+                            void* ws, size_t ws_bytes, vc_stream_t stream);
+
 /* StVD layer discard (`layer_voxel_discard`, spconv_backbone.py:134-147) with the subset drawn on the device, no host read
  * (graph-capturable), csrc/stvd_layer.cu.  Over n rows (n_dev != NULL: *n_dev valid rows of a capacity-n buffer) at discard
  * site `site`: k = int(n_valid * (1 - rate)) evaluated in float64; the kept rows are the k rows with the smallest (u_i, i),

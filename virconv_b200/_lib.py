@@ -90,6 +90,9 @@ SIGNATURES = {
     'vc_stvd_ws_bytes': (_Z, [_I]),
     'vc_stvd_partition': (_I, [_P, _I, _I, _I, ctypes.c_double, _P, _P, _Z, _P]),
     'vc_stvd_gather': (_I, [_P, _I, _I, _HOST, _I, _P, _P, _I, _P, _Z, _P]),
+    'vc_stvd_input_ws_bytes': (_Z, [_I, _I]),
+    'vc_stvd_input_front_end': (_I, [_P, _I, _P, _I, _I, _I, _D, _D, _HOSTF, _I, _I, _P, _I, _P, _P, _I, _P, _P, _I, _P, _P, _P,
+                                     _P, _Z, _P]),
     'vc_stvd_layer_keep_ws_bytes': (_Z, [_I]),
     'vc_stvd_layer_keep': (_I, [_P, _P, _I, _I, _P, _D, _P, _P, _P, _P, _Z, _P]),
     'vc_voxel_query': (_I, [_I, _I, _I, _I, _I, _F, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P]),

@@ -14,6 +14,7 @@
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace vc {
 namespace {
@@ -21,24 +22,6 @@ namespace {
 constexpr int TILE = 256;           // rows per block of the count / emit passes; threads of every selection kernel
 constexpr int SCAN_THREADS = 1024;
 constexpr int PASSES = 4;           // 8-bit digits of a 32-bit key
-
-__device__ __forceinline__ uint32_t philox_word0(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0, uint32_t k1) {
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        if (r) {
-            k0 += 0x9E3779B9u;
-            k1 += 0xBB67AE85u;
-        }
-        const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
-        const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
-        const uint32_t n0 = hi1 ^ c1 ^ k0, n2 = hi0 ^ c3 ^ k1;
-        c0 = n0;
-        c1 = lo1;
-        c2 = n2;
-        c3 = lo0;
-    }
-    return c0;
-}
 
 __device__ __forceinline__ int live_rows(const int* n_dev, int cap) {
     if (!n_dev) return cap;

@@ -36,7 +36,7 @@ from __future__ import annotations
 
 import torch
 
-from . import _lib, executor, ops
+from . import _lib, executor, ops, preprocess
 
 
 class _MaskedMean(torch.autograd.Function):
@@ -101,6 +101,38 @@ class _Inputs:
         self.streams = [_Stream(s, i) for i, s in enumerate(sfxs)]
         self.vox, self.vox_arg, self.copies, self.extra_counts = vox, vox_arg, copies, extra_counts
         self.B = None
+        # the voxeliser dict's `input_discard` entry, dict(rate=0.8, later_fusion=...): the batch carries the collated,
+        # un-split cloud 'points{i}' of each copy, and the StVD input front end (preprocess.input_front_end) turns it into the
+        # streams' points inside the graph, before the voxelisers
+        self.fe = vox.get('input_discard') if vox is not None else None
+        self.training = False         # (set by the owner before a capture: bin_num 2 and the shuffle when training)
+        self.seed = None              # device int64[1]: the front end's draw of the last replay (written inside the graph)
+        if self.fe is not None:
+            mm = any(st.sfx.startswith('_mm') for st in self.streams)
+            if bool(self.fe['later_fusion']) != mm:
+                raise ValueError('input_discard: later_fusion=%s, but the model has the input streams %s (two streams: '
+                                 'later_fusion=True, VirConv-T / -S; one fused stream: later_fusion=False, VirConv-L)'
+                                 % (self.fe['later_fusion'], [st.sfx for st in self.streams]))
+            self.raw = {}             # copy suffix -> [cap, 1+C] input buffer of the un-split cloud
+            self.raw_prev = {}
+
+    def copy_sfx(self):
+        return [''] + [str(i) for i in range(1, self.copies)]
+
+    def _front_end(self, batch_size, static, seed=None, overflow=None, raw=None):
+        """The front end of every copy -> ({stream suffix: its points}, published keys)."""
+        fe, pts, pub = self.fe, {}, {}
+        for i, c in enumerate(self.copy_sfx()):
+            r = preprocess.input_front_end(raw[c], batch_size, self.training, bool(fe['later_fusion']), rate=fe.get('rate', 0.8),
+                                           seed=seed, point_cloud_range=self.vox['point_cloud_range'], draw=i, static=static,
+                                           overflow=overflow)
+            pts[c] = r['points']
+            pub['stvd_input_kept' + c] = r['stvd_input_kept']
+            pub['stvd_input_status' + c] = r['stvd_input_status']
+            if fe['later_fusion']:
+                pts['_mm' + c] = r['points_mm']
+                pub['stvd_input_kept_mm' + c] = r['stvd_input_kept_mm']
+        return pts, pub
 
     def _voxelize(self, st, points, batch_size, static=False):
         v = self.vox
@@ -111,16 +143,32 @@ class _Inputs:
         """`batch` as an exact (host-synchronised) run takes it: with the voxeliser, every stream's points voxelised."""
         bd = dict(batch)
         if self.vox is not None:
+            if self.fe is not None:
+                pts, pub = self._front_end(int(batch['batch_size']), False, raw={c: batch['points' + c] for c in self.copy_sfx()})
+                bd.update(pub)
+                bd.update({'points' + s: p for s, p in pts.items()})
             for st in self.streams:
-                f, c, _ = self._voxelize(st, batch['points' + st.sfx], int(batch['batch_size']))
+                f, c, _ = self._voxelize(st, bd['points' + st.sfx], int(batch['batch_size']))
                 bd.update({'voxel_features' + st.sfx: f, 'voxel_coords' + st.sfx: c})
         return bd
 
     def allocate(self, batch, dev, margin, grain):
         """(Re)allocate every buffer for `batch`; the input capacities only grow."""
         B = int(batch['batch_size'])
+        if self.fe is not None:
+            for c in self.copy_sfx():
+                pts = batch['points' + c]
+                cap = max(self.raw[c].shape[0] if c in self.raw else 0, _round(pts.shape[0], margin, grain))
+                row = torch.zeros(pts.shape[1], dtype=torch.float32)
+                row[0] = B - 1
+                row[1:4] = -1.0e6             # unused tail rows: indicator 0, neither LiDAR nor virtual (the front end drops them)
+                self.raw_sentinel = row.to(dev)
+                self.raw[c] = self.raw_sentinel.repeat(cap, 1).contiguous()
+                self.raw_prev[c] = 0
         for st in self.streams:
-            if self.vox is not None:
+            if self.fe is not None:
+                st.cap0 = B * int(self.vox_arg(st, 'max_voxels'))
+            elif self.vox is not None:
                 pts = batch['points' + st.sfx]
                 st.cap_pts = max(st.cap_pts, _round(pts.shape[0], margin, grain))
                 row = torch.zeros(pts.shape[1], dtype=torch.float32)
@@ -151,14 +199,26 @@ class _Inputs:
         blocks; False (nothing copied) when a stream does not fit.  Rows a larger earlier batch left behind are reset to the
         tail values, so that the voxeliser drops them and the published input index set (x_conv1's indices, which are the
         coordinate buffer) keeps its -1 tail."""
-        key = 'points' if self.vox is not None else 'voxel_features'
-        ns = [batch[key + st.sfx].shape[0] for st in self.streams]
-        if any(n > (st.cap_pts if self.vox is not None else st.cap0) for st, n in zip(self.streams, ns)):
-            return False
+        if self.fe is not None:
+            if any(batch['points' + c].shape[0] > self.raw[c].shape[0] for c in self.copy_sfx()):
+                return False
+        else:
+            key = 'points' if self.vox is not None else 'voxel_features'
+            ns = [batch[key + st.sfx].shape[0] for st in self.streams]
+            if any(n > (st.cap_pts if self.vox is not None else st.cap0) for st, n in zip(self.streams, ns)):
+                return False
         slot = self._stage
         self._stage = (slot + 1) % self.SLOTS
         if self._stage_ev[slot] is not None:
             self._stage_ev[slot].synchronize()         # (8 calls back: has long completed unless the GPU is far behind)
+        if self.fe is not None:
+            for c in self.copy_sfx():
+                n = batch['points' + c].shape[0]
+                self.raw[c][:n].copy_(batch['points' + c], non_blocking=True)
+                if self.raw_prev[c] > n:
+                    self.raw[c][n:self.raw_prev[c]] = self.raw_sentinel
+                self.raw_prev[c] = n
+            ns = []
         for st, n in zip(self.streams, ns):
             if self.vox is not None:
                 st.pts[:n].copy_(batch['points' + st.sfx], non_blocking=True)
@@ -182,15 +242,23 @@ class _Inputs:
         self._stage_ev[slot] = ev
         return True
 
-    def static_batch(self, batch):
+    def static_batch(self, batch, overflow=None):
         """-> (`batch` with every stream's inputs replaced by the capacity-sized ones, {stream suffix: device int32[1] row
-        count}); with the voxeliser, vc_voxelize_mean runs here (inside the graph) once per stream."""
+        count}); with the voxeliser, vc_voxelize_mean runs here (inside the graph) once per stream, after the StVD input front
+        end (one fresh seed per replay from torch's CUDA generator, kept in `seed`; its overflow word `overflow`) when the
+        voxeliser dict asks for it."""
         drop = {k + st.sfx for st in self.streams for k in ('voxel_features', 'voxel_coords', 'points')}
         bd = {k: v for k, v in batch.items() if k not in drop}
         counts = {}
+        pts = {st.sfx: getattr(st, 'pts', None) for st in self.streams}
+        if self.fe is not None:
+            self.seed = torch.randint(preprocess._I64.min, preprocess._I64.max, (1,), dtype=torch.int64, device=self.n_dev.device)
+            pts, pub = self._front_end(self.B, True, seed=self.seed, overflow=overflow, raw=self.raw)
+            bd.update(pub)
+            bd['stvd_input_seed'] = self.seed
         for st in self.streams:
             if self.vox is not None:
-                f, c, bd['voxel_num_points' + st.sfx], counts[st.sfx] = self._voxelize(st, st.pts, self.B, static=True)
+                f, c, bd['voxel_num_points' + st.sfx], counts[st.sfx] = self._voxelize(st, pts[st.sfx], self.B, static=True)
             else:
                 f, c, counts[st.sfx] = st.vf, st.vc, self.n_dev[st.i:st.i + 1]
             bd.update({'voxel_features' + st.sfx: f, 'voxel_coords' + st.sfx: c})
@@ -259,6 +327,8 @@ class _Captured:
     sequence (_capture).  A subclass sets `inputs` and defines _recapture(batch) and _transforms(batch) (the projection
     transform of each copy)."""
 
+    FE_FLAG = 'stvd_input'    # flag-ring key of the StVD input front end's overflow word
+
     def __init__(self, dev, voxelizer, margin, grain, warmup):
         self.dev = dev
         self.vox = dict(voxelizer) if voxelizer is not None else None
@@ -290,6 +360,9 @@ class _Captured:
                 return None
         return self.vox[key]
 
+    def _fe_flag(self):
+        return self.flags.flag(self.FE_FLAG) if self.inputs.fe is not None else None
+
     def _load(self, batch):
         return self.inputs.load(batch, self._transforms(batch))
 
@@ -305,13 +378,14 @@ class _Captured:
         torch.cuda.graphs asks for; prepare() runs after it, outside any graph."""
         torch.cuda.synchronize(self.dev)
         self.graphs = []
+        self.inputs.training = self.model.training
         runs = exact(batch)
         for key, run in runs.items():
             caps = self.caps.setdefault(key, {})
             for k, v in executor.measured_caps(run, self.margin, self.grain).items():
                 caps[k] = max(caps.get(k, 0), v)
         self.inputs.allocate(batch, self.dev, self.margin, self.grain)
-        self.flags = _Flags(runs, self.dev, self.overflow_events)
+        self.flags = _Flags(list(runs) + ([self.FE_FLAG] if self.inputs.fe is not None else []), self.dev, self.overflow_events)
         assert self._load(batch)
         s = torch.cuda.Stream(device=self.dev)
         s.wait_stream(torch.cuda.current_stream(self.dev))
@@ -344,7 +418,12 @@ class GraphedStep(_Captured):
         deliver); or a dict(point_cloud_range, voxel_size, max_points_per_voxel, max_voxels, vfe_model) — batches carry the
         collated raw `points` [N, 1+C] and the hash-grid voxelisation + VFE (vc_voxelize_mean) run INSIDE the graph.  With a
         two-stream model the batch also carries `points_mm`, voxelised by a second call with the entries `max_voxels_mm`
-        (default: `max_voxels`) and `vfe_model_mm` (default: None, the plain mean).
+        (default: `max_voxels`) and `vfe_model_mm` (default: None, the plain mean).  With the entry
+        `input_discard=dict(rate=0.8, later_fusion=...)` the batch carries the collated, un-split cloud `points` (indicator 1
+        virtual, 2 LiDAR) instead, and the StVD input front end (preprocess.input_front_end: split, input discard, VirConv-L
+        re-fusion, range mask, training shuffle) runs inside the graph before the voxelisers, with one fresh seed per replay
+        (published as 'stvd_input_seed', the kept rows as 'stvd_input_kept' / 'stvd_input_kept_mm'); later_fusion=True for a
+        two-stream model, False for VirConv-L.  Its overflow word is one more flag of the ring (key 'stvd_input').
 
         optimizer: None — the caller updates the parameters after each call; or an optim.FusedAdamOneCycle — the captured
         body ends with its two update launches (clipping to `max_grad_norm`, None: no clipping), reading the gradients of
@@ -390,7 +469,7 @@ class GraphedStep(_Captured):
         return runs
 
     def _static_batch(self, batch):
-        bd, counts = self.inputs.static_batch(batch)
+        bd, counts = self.inputs.static_batch(batch, self._fe_flag())
         for st in self.streams:
             bd['virconv_static' + st.sfx] = executor.StaticSpec(counts[st.sfx], self.caps[st.sfx], self.flags.flag(st.sfx),
                                                                 alias_params=True)
@@ -507,6 +586,8 @@ class PipelinedStep:
         if kwargs.get('optimizer') is not None:
             raise ValueError('PipelinedStep overlaps the index work of step t+1 with the feature work of step t and has no '
                              'in-graph update: pass optimizer= to GraphedStep, or call the optimizer\'s step() after each call')
+        if (kwargs.get('voxelizer') or {}).get('input_discard') is not None:
+            raise ValueError('PipelinedStep does not run the StVD input front end (voxelizer input_discard): use GraphedStep')
         if streams != ('',):
             raise ValueError('PipelinedStep phases a one-stream backbone (VirConvL8x); %s has the input streams %s, which have '
                              'no phased form: use GraphedStep' % (type(model).__name__, streams))
@@ -585,7 +666,9 @@ class GraphedForward(_Captured):
 
     voxelizer: as GraphedStep's — the batch then carries 'points{i}' (and 'points_mm{i}' for VirConv8x with MM) instead of the
     voxel keys, and vc_voxelize_mean runs inside the graph once per stream and copy; the virtual-point stream's settings are
-    the '_mm' entries ('max_voxels_mm', 'vfe_model_mm', default the plain mean)."""
+    the '_mm' entries ('max_voxels_mm', 'vfe_model_mm', default the plain mean).  With the voxeliser's `input_discard` entry
+    (GraphedStep) the batch carries the un-split collated cloud 'points{i}' of each copy; each copy goes through the StVD
+    input front end independently (its own draw under the replay's seed, bin_num 10, no shuffle: the test-time settings)."""
 
     def __init__(self, model, margin=1.3, voxelizer=None, bev=False, check_overflow='sync', grain=1024, warmup=2):
         from .backbone import VirConv8x, VirConvL8x
@@ -630,7 +713,10 @@ class GraphedForward(_Captured):
             raise ValueError('GraphedForward: VirConv8x batches 1..%d transformed copies along x (the factor 4 of the '
                              '[D, H, 4W] grid is fixed, spconv_backbone.py:360); transform_param has %d' % (ops.XBATCH_MAX, R))
         keys = (['points'] if self.vox is not None else ['voxel_features', 'voxel_coords'])
-        missing = [k + s for s in self.input_streams(R) for k in keys if batch.get(k + s) is None]
+        if self.vox is not None and self.vox.get('input_discard') is not None:
+            missing = ['points' + s for s in self._sfx(R) if batch.get('points' + s) is None]      # the un-split clouds
+        else:
+            missing = [k + s for s in self.input_streams(R) for k in keys if batch.get(k + s) is None]
         if missing:
             raise ValueError('GraphedForward: the batch has no %s' % ', '.join(missing))
         return R
@@ -666,7 +752,7 @@ class GraphedForward(_Captured):
     @torch.no_grad()
     def _static_forward(self, batch):
         from .backbone import EvalStaticSpec
-        bd, counts = self.inputs.static_batch(batch)
+        bd, counts = self.inputs.static_batch(batch, self._fe_flag())
         flag = self.flags.flag
         if self.x_batched:
             sfx = self._sfx(self.R)
@@ -680,7 +766,7 @@ class GraphedForward(_Captured):
         out = self.model(bd)
         if self.bev:
             self._bev(out)
-        self._published = [k for k in out if k not in before]
+        self._published = [k for k in out if k not in before or k.startswith('stvd_input')]
         return out
 
     def _recapture(self, batch):

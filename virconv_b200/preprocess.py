@@ -102,6 +102,72 @@ def split_and_discard(points, training, input_discard_rate=0.8, later_fusion=Fal
     return {'points': fused}
 
 
+_I64 = torch.iinfo(torch.int64)
+
+
+def input_front_end(points, batch_size, training, later_fusion, rate=0.8, seed=None, n_dev=None,
+                    point_cloud_range=(0, -40, -3, 70.4, 40, 1), bin_num=None, shuffle=None, draw=0, cap=None, static=False,
+                    max_dis=60, overflow=None):
+    """The dataloader's per-frame input flow for a whole collated batch, with every draw on the device and no host read
+    (vc_stvd_input_front_end, csrc/stvd.cu): `points` [N, 1+C] fp32 (b, x, y, z, ..., indicator), scenes contiguous, as
+    `collate_batch` builds it before any split; n_dev (device int32[1]) its valid rows when it is a capacity-sized buffer.
+
+    Per scene: split by the indicator (dataset.py:272,284), the StVD input discard of the virtual points (bin_num 2 when
+    training, 10 at test time; keys from Philox under `seed`, a device int64[1], default one fresh draw of torch's CUDA
+    generator), [LiDAR, kept virtual] with intensity / 10 (later_fusion False, VirConv-L) or the two streams apart
+    (VirConv-T / -S), mask_points_by_range, and when shuffling (default: training) a per-scene pseudo-random permutation of every
+    stream, as the reference's shuffle_points does for 'points' and, with two streams, 'points_mm' (data_processor.py:
+    105-124).  `draw` separates independent draws under one seed (the ROT_NUM copies).
+
+    -> {'points', 'points_mm' (later_fusion), 'stvd_input_kept' (the input row of every 'points' row, and with two streams
+    'stvd_input_kept_mm'), 'stvd_input_status' [B] int32 (1: a scene without virtual points, where the reference raises
+    ZeroDivisionError), 'stvd_input_overflow' int32[1]}.  static=False: exact-size tensors (one host read of the two row
+    counts).  static=True: capacity-sized ones (cap rows, default the input's), tail rows (-1, 0, ...) that the voxeliser
+    drops, each stream tensor carrying its device row count as `.num_rows`; the overflow word (`overflow`, a device int32[1]
+    the call raises to the rows that did not fit, or a fresh zero one) holds the rows that did not fit, and also the rows
+    dropped because the scenes were not contiguous and ascending."""
+    ops._require_cuda(points, n_dev, seed)
+    lib = _lib.load()
+    assert points.dim() == 2 and points.dtype == torch.float32, (points.dtype, points.shape)
+    points = points.contiguous()
+    n, w = points.shape
+    dev = points.device
+    bin_num = int(bin_num if bin_num is not None else (2 if training else 10))
+    shuffle = bool(training if shuffle is None else shuffle)
+    if seed is None:
+        seed = torch.randint(_I64.min, _I64.max, (1,), dtype=torch.int64, device=dev)
+    assert seed.dtype == torch.int64 and seed.numel() == 1 and seed.device == dev
+    if n_dev is not None:
+        assert n_dev.dtype == torch.int32 and n_dev.numel() == 1
+    cap = n if cap is None else int(cap)
+    names = ('points', 'points_mm') if later_fusion else ('points',)
+    outs = [torch.empty((cap, w), dtype=torch.float32, device=dev) for _ in names]
+    srcs = [torch.empty((cap,), dtype=torch.int32, device=dev) for _ in names]
+    counts = torch.empty(2, dtype=torch.int32, device=dev)
+    status = torch.empty(int(batch_size), dtype=torch.int32, device=dev)
+    if overflow is None:
+        overflow = torch.zeros(1, dtype=torch.int32, device=dev)
+    assert overflow.dtype == torch.int32 and overflow.numel() == 1 and overflow.device == dev
+    ws = ops._ws(lib.vc_stvd_input_ws_bytes(n, int(batch_size)), dev)
+    mm = later_fusion
+    check(lib.vc_stvd_input_front_end(points.data_ptr(), n, ops._p(n_dev), w, int(batch_size), bin_num, float(max_dis), float(rate),
+                                      _lib.host_f32(point_cloud_range), int(bool(later_fusion)), int(shuffle), seed.data_ptr(),
+                                      int(draw), outs[0].data_ptr(), srcs[0].data_ptr(), cap,
+                                      outs[1].data_ptr() if mm else None, srcs[1].data_ptr() if mm else None, cap if mm else 0,
+                                      counts.data_ptr(), status.data_ptr(), overflow.data_ptr(), ws.data_ptr(), ws.numel(),
+                                      ops._stream()), 'vc_stvd_input_front_end')
+    res = {'stvd_input_status': status, 'stvd_input_overflow': overflow}
+    rows = counts.tolist() if not static else None
+    for i, (name, o, s) in enumerate(zip(names, outs, srcs)):
+        if static:
+            o.num_rows = s.num_rows = counts[i:i + 1]
+        else:
+            o, s = o[:rows[i]], s[:rows[i]]
+        res[name] = o
+        res['stvd_input_kept' + name[len('points'):]] = s
+    return res
+
+
 class PointsToVoxels(nn.Module):
     """Voxelisation + VFE as a model-side module: reads `batch_dict['points']` ([N, 1+C] fp32 rows (b, x, y, z, ...),
     samples contiguous in batch order — what `collate_batch` builds, dataset.py:349-353) and writes what the dataloader's

@@ -51,10 +51,16 @@ adam_onecycle / adam_cosin and calls the reference's function for every other va
 `train_utils.train_utils` imported at module level records its max_norm for the next step() of the fused optimizer that
 owns those parameters, leaving the gradients alone (parameters no fused optimizer owns go to torch's function): the
 reference's train_one_epoch (train_utils.py:13-71) then runs unchanged, with clipping, decay and Adam in two launches.
+With `use_device_input_discard` `DatasetTemplate.input_point_discard` returns its input, `DataProcessor.shuffle_points` passes
+the frame through and `DataProcessor.mask_points_and_boxes_outside_range` filters the boxes only: `prepare_data` then hands
+over the split but undiscarded, unmasked, unshuffled cloud, and the model side runs the StVD input front end on the device
+(preprocess.input_front_end, or GraphedStep's voxelizer entry `input_discard`).  The points mask has to move with the
+discard: the reference bins the virtual points before the range mask, so masking them first would change every `out_n`.
 """
 from __future__ import annotations
 
 import collections
+import functools
 import collections.abc
 import importlib
 import sys
@@ -266,9 +272,44 @@ def _fused_clip_grad_norm_(parameters, max_norm, *args, **kwargs):
     return torch.nn.utils.clip_grad_norm_(rest, max_norm, *args, **kwargs) if rest else None
 
 
+def _keep_points(self, points, bin_num=2, rate=0.8):
+    """`DatasetTemplate.input_point_discard` under `use_device_input_discard`: the virtual points pass unchanged."""
+    return points
+
+
+def _shuffle_later(self, data_dict=None, config=None):
+    """`DataProcessor.shuffle_points` under `use_device_input_discard`: the order is drawn on the device."""
+    if data_dict is None:
+        return functools.partial(self.shuffle_points, config=config)
+    return data_dict
+
+
+def _mask_boxes_only(self, data_dict=None, config=None):
+    """`DataProcessor.mask_points_and_boxes_outside_range` under `use_device_input_discard`: the boxes of every copy are
+    filtered as before (REMOVE_OUTSIDE_BOXES, min_num_corners), the points are left for the device front end, which masks
+    them after its discard."""
+    if data_dict is None:
+        return functools.partial(self.mask_points_and_boxes_outside_range, config=config)
+    if not config.REMOVE_OUTSIDE_BOXES:
+        return data_dict
+    box_utils = importlib.import_module('pcdet.utils.box_utils')
+    for r in range(self.rot_num):
+        key = 'gt_boxes' + (str(r) if r else '')
+        boxes = data_dict.get(key)
+        if boxes is None:
+            continue
+        inside = box_utils.mask_boxes_outside_range_numpy(boxes, self.point_cloud_range,
+                                                          min_num_corners=config.get('min_num_corners', 1))
+        data_dict[key] = boxes[inside]
+        if r == 0 and 'gt_tracklets' in data_dict:
+            data_dict['gt_tracklets'] = data_dict['gt_tracklets'][inside]
+            data_dict['num_bbs_in_tracklets'] = data_dict['num_bbs_in_tracklets'][inside]
+    return data_dict
+
+
 def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=False, use_fused_rpn_targets=False,
             use_fused_roi_targets=False, use_fused_losses=False, use_fused_part_pool=False, use_fused_optimizer=False, use_fused_roi_grid=False,
-            use_fused_box_decode=False, use_fused_kitti_eval=False):
+            use_fused_box_decode=False, use_fused_kitti_eval=False, use_device_input_discard=False):
     """Register everything listed in the module docstring.  `reference_root`: put that checkout first on sys.path."""
     if reference_root is not None and reference_root not in sys.path:
         sys.path.insert(0, reference_root)
@@ -396,6 +437,12 @@ def install(use_fused_backbones=False, reference_root=None, use_fused_roi_pool=F
         ev.get_official_eval_result = kitti_eval.get_official_eval_result
         ev.get_coco_eval_result = kitti_eval.get_coco_eval_result
         ev.rotate_iou_gpu_eval = kitti_eval.rotate_iou_eval
+    if use_device_input_discard:
+        ds = importlib.import_module('pcdet.datasets.dataset').DatasetTemplate
+        ds.input_point_discard = _keep_points
+        dp = importlib.import_module('pcdet.datasets.processor.data_processor').DataProcessor
+        dp.shuffle_points = _shuffle_later
+        dp.mask_points_and_boxes_outside_range = _mask_boxes_only
     if use_fused_optimizer:
         import os
         tools = os.path.join(reference_root, 'tools') if reference_root is not None else None
