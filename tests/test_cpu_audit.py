@@ -8,8 +8,12 @@ import torch
 from oracle import audit
 
 
-@pytest.mark.parametrize('training', [True, False])
-def test_bn_relu_matches_torch_batchnorm(training):
+@pytest.mark.parametrize('training,adversarial', [(True, False), (False, False), (False, True), (True, True)],
+                         ids=['True', 'False', 'eval-adversarial', 'train-adversarial'])
+def test_bn_relu_matches_torch_batchnorm(training, adversarial):
+    """adversarial: the BatchNorm state of the step audit's running-statistics cases — gamma negative on every third
+    channel, running statistics of the scale of x with the mean shifted by half a standard deviation, and one channel with
+    running_var = 0 (eps alone under the square root)"""
     torch.manual_seed(0)
     n, c, eps, mom = 300, 16, 1e-3, 0.01
     x = (torch.randn(n, c, dtype=torch.float64) * torch.linspace(0.2, 3.0, c, dtype=torch.float64)
@@ -20,6 +24,12 @@ def test_bn_relu_matches_torch_batchnorm(training):
         bn.bias.copy_(torch.linspace(-0.3, 0.3, c))
         bn.running_mean.copy_(torch.linspace(-0.1, 0.1, c))
         bn.running_var.copy_(torch.linspace(0.5, 1.5, c))
+        if adversarial:
+            bn.weight[::3] *= -1
+            sd = x.std(0)
+            bn.running_mean.copy_(x.mean(0) + 0.5 * sd * torch.where(torch.arange(c) % 2 == 0, 1.0, -1.0).double())
+            bn.running_var.copy_(sd ** 2 * torch.linspace(0.5, 2.0, c, dtype=torch.float64))
+            bn.running_var[5] = 0.0
     rm0, rv0 = bn.running_mean.clone(), bn.running_var.clone()
     bn.train(training)
     xt = x.clone().requires_grad_(True)

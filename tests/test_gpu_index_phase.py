@@ -35,11 +35,14 @@ LAUNCHES_L_PAPER = 4 * 5 + 4 * 5 + 3 * (7 + 2) + 20 + 2
 
 
 def _runs(monkeypatch):
-    from virconv_b200 import executor
-    runs, real = [], executor.run_plan
+    """every executor run of a forward, with its input coordinates and the library launches its call enqueued"""
+    from virconv_b200 import _lib, executor
+    runs, real, lib = [], executor.run_plan, _lib.load()
 
     def run_plan(plan, feats, coords, *a, **kw):
+        l0 = lib.vc_launch_count()
         run, res = real(plan, feats, coords, *a, **kw)
+        run.launches = lib.vc_launch_count() - l0
         run.coords0 = coords.clone()        # (the input index set is the caller's tensor, not in the arena)
         runs.append(run)
         return run, res
@@ -127,13 +130,13 @@ def _equal(got, want, what):
     assert got.shape == want.shape and np.array_equal(got, want), what
 
 
-def _check_run(run, bd):
+def _check_run(run, bd, trans=None):
     """Every index op of `run` against the oracle -> the overflow value static mode must report.  Per index set the oracle
     keeps `full`, the whole set, and `held`, the rows the executor holds: the first min(capacity, count) of it.  Composed
     semantics (csrc/rulebook.cu header): a strided conv's output set is built from its input's whole set, its tables and
-    every other op from the held rows."""
+    every other op from the held rows.  trans: the [B, 3] transform of the run's projections (default bd['aug_param'])."""
     from virconv_b200 import executor
-    calibs, aug, batch = bd['calib'], bd['aug_param'].numpy(), bd['batch_size']
+    calibs, batch = bd['calib'], bd['batch_size']
 
     def count(iset):   # (capacity, count) of an executor index set
         cap = run.query(2, iset)[1]
@@ -176,7 +179,7 @@ def _check_run(run, bd):
             _equal(pn, (want >= 0).sum(1).astype(np.int32), 'pair counts of rulebook %d' % rb)
         elif kind == executor.OP_INDEX2UV:
             assert (row[22], row[23]) == (1400, 600)   # the oracle's pixel clamp
-            uv = ouv.index2uv(held[a], batch, calibs, row[21], aug)
+            uv = ouv.index2uv(held[a], batch, calibs, row[21], bd['aug_param'].numpy() if trans is None else trans)
             _equal(run.indices(b)[0][:len(uv)], uv, 'projection %d' % b)
             full[b] = held[b] = uv
             shape[b] = [row[6], row[7]]
@@ -216,6 +219,51 @@ def test_virconv_t_plans(monkeypatch):
     for run in runs:
         _check_run(run, bd)
     assert launches == LAUNCHES_T
+
+
+def _launches_no_discard(plan):
+    """Library launches of one forward of a plan without layer discards, from its ops: the first stage's submanifold rulebook
+    (hash insert + probe: 2), the chain of its strided convs composed (4) with their tables in one launch (1), the later
+    stages' submanifold rulebooks one launch per kind (2), one fused conv + BatchNorm launch per layer, the weight images
+    and the input's bf16 cast (2).  A plan with projections (index2uv, 2-D rulebooks) is counted by LAUNCHES_L / _T."""
+    from virconv_b200 import executor
+    kinds = [r[0] for r in plan.rows_i]
+    assert executor.OP_INDEX2UV not in kinds and executor.OP_DISCARD not in kinds
+    n_conv, n_subm = kinds.count(executor.OP_CONV_RB), kinds.count(executor.OP_SUBM_RB)
+    assert n_conv >= 1 and n_subm >= 2
+    return 2 + (4 + 1) + 2 + len(plan.layers) + 2
+
+
+def test_virconv_t_eval_rot3_packed_grid(monkeypatch):
+    """VirConv-T's test-time forward at bench.py's eval_rot3 size: the LiDAR plan over the ROT_NUM = 3 copies of 40 000 voxels
+    packed along x into [81, 1600, 4 * 1408].  Its input rows are in concat order — copy, then scene — so not batch-contiguous
+    as the training input is; every table must still equal the oracle's.  Then each copy's virtual-point plan, its
+    projections under that copy's transform."""
+    from virconv_b200 import parallel, scenes
+    from virconv_b200.backbone import VirConv8x
+    m = VirConv8x(CFG8, 8, [1408, 1600, 80], precision='bf16')
+    fill_module(m, 667)
+    m.to(DEV).eval()
+    R = 3
+    b = scenes.make_batch_mm(parallel.shard_scene_ids(100, 0, 1, 2), 16384, 80000, 40000, training=False, rot_num=R)
+    bd = {k: torch.from_numpy(v.copy()).to(DEV) for k, v in b.arrays.items()}
+    bd.update(batch_size=b.batch_size, calib=b.calib, transform_param=torch.from_numpy(b.transform_param.copy()))
+    runs, _ = _forward(m, bd, monkeypatch, n_runs=1 + R)
+    lidar = runs[0]
+    assert lidar.plan is m._plan_lidar()
+    W = m.sparse_shape[2]
+    assert lidar.query(2, 0)[3:6] == [m.sparse_shape[0], m.sparse_shape[1], 4 * W]
+    c = lidar.coords0.cpu().numpy()
+    assert len(c) == sum(bd['voxel_coords' + s].shape[0] for s in ['', '1', '2'])
+    copy_of = c[:, 3] // W
+    assert np.all(np.diff(copy_of) >= 0) and set(copy_of.tolist()) == set(range(R))
+    assert np.any(np.diff(c[:, 0]) < 0)               # scene 1 of copy 0 comes before scene 0 of copy 1
+    assert _check_run(lidar, bd) == 0
+    assert lidar.launches == _launches_no_discard(lidar.plan)
+    tp = bd['transform_param'].numpy()
+    for i, run in enumerate(runs[1:]):
+        assert run.plan is m._plan_mm()
+        _check_run(run, bd, tp[:, i])
 
 
 def test_paper_stvd_device_discards(monkeypatch):
