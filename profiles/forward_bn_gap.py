@@ -3,7 +3,7 @@ kernel's duration, the gap from its end to the BN apply's start, the BN apply's 
 torch.profiler over ~20 replays of the captured VirConv-L training step (GraphedStep with the in-graph voxeliser, bench's
 batch and loss).  With the BN apply fused into the conv (VIRCONV_CONV_BN_FUSED=1) the apply columns read 0 and the conv
 column includes it.  Per replay it also prints the index phase: the span from the first index kernel (hash insert, probes,
-strided-conv count / emit / tables, projections) to the last, the time from the voxeliser's last kernel to the first conv,
+bitmap lookups, strided-conv count / emit / tables, projections) to the last, the time from the voxeliser's last kernel to the first conv,
 and the span of the forward's conv chain.  Run on the GPU:
 
     python profiles/forward_bn_gap.py [--replays 20]
@@ -25,7 +25,7 @@ from virconv_b200.backbone import VirConvL8x  # noqa: E402
 from virconv_b200.graph import GraphedStep, masked_mean  # noqa: E402
 
 CONV, APPLY, REDUCE = 'tc_conv_persist', 'bn_apply_relu', 'bn_sums_reduce'
-INDEX = re.compile(r'\b(hash_insert|subm_probe|conv_mark|scan_local|scan_blocks|conv_emit_indices|conv_tables|index2uv|g2_[a-z_]+|'
+INDEX = re.compile(r'\b(hash_insert|subm_probe|subm_lookup|conv_mark|scan_local|scan_blocks|conv_emit_indices|conv_tables|conv_fwd_lookup|index2uv|g2_[a-z_]+|'
                    r'stvd_gather_idx)_kernel')
 VOX = re.compile(r'\b(vox_[a-z]+|vscan_local)_kernel')
 

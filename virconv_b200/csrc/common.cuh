@@ -164,9 +164,33 @@ struct TablesStage {  // one strided conv's tables (conv_rulebook_tables_dev)
     const int32_t *shape, *ksize, *stride, *pad, *dil;
     int n_out;
     ConvRank rank;
-    int32_t *nbr_fwd, *nbr_bwd, *pair_num;
+    int32_t *nbr_fwd, *nbr_bwd, *pair_num;   // nbr_fwd NULL: written by conv_fwd_lookup_batch_dev instead
 };
 int conv_tables_batch_dev(const TablesStage* st, int n_st, int batch_size, cudaStream_t stream);
+// Over chain levels (conv_chain_rank): a level's rows are its bitmap's set bits in rank order, so a cell's row is its rank,
+// and a rank at or past the level's held rows (n, or *n_dev) is absent.
+struct SubmLookupStage {   // one submanifold rulebook over a chain level's output set, `rank` that level's bitmap
+    const int32_t* idx;
+    int n;
+    const int* n_dev;
+    int ndim;
+    const int32_t *shape, *ksize, *dil;
+    ConvRank rank;
+    int32_t *nbr, *pair_num;
+};
+int subm_lookup_batch_dev(const SubmLookupStage* st, int n_st, int batch_size, cudaStream_t stream);
+struct FwdLookupStage {    // nbr_fwd of a chained strided conv whose input set is the chain level `in_rank`
+    const int32_t* out_idx;          // the conv's output rows
+    int n_out;
+    const int* n_out_dev;
+    int n_in;                        // the input level's held rows
+    const int* n_in_dev;
+    ConvRank in_rank;
+    int ndim;
+    const int32_t *shape, *ksize, *stride, *pad, *dil;   // shape: the input level's
+    int32_t* nbr_fwd;
+};
+int conv_fwd_lookup_batch_dev(const FwdLookupStage* st, int n_st, int batch_size, cudaStream_t stream);
 struct UVStage {     // one projection (index2uv_dev)
     const int32_t* idx;
     int n;
@@ -274,7 +298,8 @@ bool tc2_ch_ok(int c);
 int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_t* nbr, long long pitch, float* out, int n_rows,
              const int* n_dev, int K, double* bn_sums, int* err, cudaStream_t stream, const float* addend,
              int* tile_counter = nullptr, int flags = 0,   // flags: bit 0 sparse offsets (strided dgrad), bit 1 no index kernel
-                                                           // beside it (the conv + BN grid takes 2 CTAs/SM)
+                                                           // beside it (the conv + BN grid takes 2 CTAs/SM), bit 2 zeros
+                                                           // in out's rows [*n_dev, n_rows)
              int in_ld = 0,                                // row pitch of in_bf16 (0: kc)
              double* bn_part = nullptr,                    // deterministic BN sums: [tiles, 2, nr] per 128-row tile (bn_sums NULL)
              const BnTail* bn = nullptr,                   // forward only: BN + ReLU in the same launch when g_conv_bn_fused

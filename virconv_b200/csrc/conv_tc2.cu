@@ -90,6 +90,7 @@ struct PArgs {
     int w_resident;            // all K weight slices stay in shared memory for the whole launch (else: streamed with the ring)
     int scan_k;                // the loader lists the kernel offsets that touch each tile (strided-conv dgrad: most do not)
     int ntb_alloc;             // neighbour-table buffers in shared memory (2 when two CTAs share an SM, else P_NTB)
+    int zero_tail;             // store zeros into out's rows [count, n_host) (a static-mode input gradient)
     int* err;
     BnTail bn;                 // bn.bar != NULL: BatchNorm + ReLU after a grid-wide barrier (forward, cooperative launch)
 };
@@ -592,6 +593,12 @@ done:
         // a CTA that was handed no tile must still see its weight copy land before it exits (the copy targets its smem)
         mbar_wait_t(&wres_bar, 0u, a.err, 0x150);
     }
+    if (a.zero_tail) {   // (the tiles store rows below the count only)
+        float4* o4 = reinterpret_cast<float4*>(a.out);
+        const size_t c4 = a.out_c / 4;
+        for (size_t i = (size_t)n * c4 + (size_t)blockIdx.x * blockDim.x + tid; i < (size_t)a.n_host * c4; i += (size_t)gridDim.x * blockDim.x)
+            o4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
     __syncthreads();
     if (a.bn.bar == nullptr) return;
 
@@ -826,7 +833,7 @@ int tc2_conv(int kc, int nr, const void* in_bf16, const void* wimg, const int32_
     }
     a.in = (const __nv_bfloat16*)in_bf16; a.in_c = kc; a.in_ld = in_ld; a.wimg = (const unsigned char*)wimg; a.nbr = nbr; a.pitch = pitch;
     a.out = out; a.out_c = nr; a.addend = addend; a.bn_sums = bn_part ? nullptr : bn_sums; a.bn_part = bn_part; a.n_dev = n_dev; a.n_host = n_rows; a.tile_counter = tile_counter;
-    a.K = K; a.S = 0; a.w_resident = 0; a.ntb_alloc = P_NTB; a.scan_k = flags & 1;
+    a.K = K; a.S = 0; a.w_resident = 0; a.ntb_alloc = P_NTB; a.scan_k = flags & 1; a.zero_tail = n_dev != nullptr && (flags & 4);
     a.err = err;
     a.bn = BnTail{};
     bool done_dummy = false;

@@ -531,8 +531,11 @@ int fwd_discard(FwdCtx& C, int i, const int* o) {
     return VC_OK;
 }
 
-// The tables of all the chain's strided convs in one launch (conv_tables_batch_dev) on the chain's stream.
-// Their nbr_fwd tables lie back to back and their pair counts too: one -1 fill and one zeroing.
+// The tables of all the chain's strided convs on the chain's stream: nbr_bwd, pair counts and level 0's nbr_fwd in one
+// launch (conv_tables_batch_dev), and the nbr_fwd of the levels whose input set is the previous level's output by lookup
+// in that level's bitmap (conv_fwd_lookup_batch_dev), which writes every entry.  Level 0's input set (the voxels) has no
+// bitmap: its nbr_fwd is scattered from the input rows into a -1 filled table.  The nbr_fwd tables lie back to back and
+// the pair counts too: one fill and one zeroing.
 int fwd_chain_tables(FwdCtx& C, const int* ops, int L, int s) {
     size_t fwd_ints = 0, pn_ints = 0;
     for (int l = 0; l < L; ++l) {
@@ -543,6 +546,7 @@ int fwd_chain_tables(FwdCtx& C, const int* ops, int L, int s) {
     VC_ALLOC(fwd_all, int32_t*, fwd_ints * 4);
     VC_ALLOC(pn_all, int32_t*, pn_ints * 4);
     TablesStage ts[CONV_CHAIN_MAX];
+    FwdLookupStage fs[CONV_CHAIN_MAX];
     for (int l = 0, fo = 0, po = 0; l < L; ++l) {
         const int* o = C.op(ops[l]);
         const ISet& I = C.S->iset[o[F_A]];
@@ -552,13 +556,18 @@ int fwd_chain_tables(FwdCtx& C, const int* ops, int L, int s) {
         fo += R.K * (R.n_out > 0 ? R.n_out : 1);
         po += R.K;
         ts[l] = TablesStage{I.idx, I.n, I.n_dev, I.ndim, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL, R.n_out, C.chain[ops[l]].rank,
-                            R.nbr, R.nbr_bwd, R.pair_num};
+                            l == 0 ? R.nbr : nullptr, R.nbr_bwd, R.pair_num};
+        if (l > 0)
+            fs[l - 1] = FwdLookupStage{C.S->iset[o[F_B]].idx, R.n_out, R.n_out_dev, I.n, I.n_dev, C.chain[ops[l - 1]].rank, I.ndim,
+                                       I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL, R.nbr};
         C.batched[ops[l]] = true;
     }
     if (C.do_idx) {
+        const RBk& R0 = C.S->rb[C.op(ops[0])[F_C]];
         VC_CUDA(cudaMemsetAsync(pn_all, 0, pn_ints * 4, C.st[s]));
-        VC_CUDA(cudaMemsetAsync(fwd_all, 0xFF, fwd_ints * 4, C.st[s]));
+        VC_CUDA(cudaMemsetAsync(fwd_all, 0xFF, (size_t)R0.K * R0.n_out * 4, C.st[s]));
         VC_TRY(conv_tables_batch_dev(ts, L, C.S->batch_size, C.st[s]));
+        VC_TRY(conv_fwd_lookup_batch_dev(fs, L - 1, C.S->batch_size, C.st[s]));
     }
     RBk& R0 = C.S->rb[C.op(ops[0])[F_C]];
     C.produced(R0, s);   // one event for the batch
@@ -570,9 +579,10 @@ int fwd_chain_tables(FwdCtx& C, const int* ops, int L, int s) {
 }
 
 // The submanifold rulebooks and projections over the chain's output sets (the stage 2-4 work of the plan's
-// image-branch stream), one launch per kind: hash insert + probe of the 3-D sets, index2uv, hash insert + probe of the
-// projected sets.  Applies when all of them run on one stream and probe alike; else each op keeps its own launches.  The
-// deterministic mode's 2-D rulebooks (the gather-form dgrad's `rep` rows) stay per op.
+// image-branch stream), one launch per kind: bitmap lookup of the 3-D sets (each is a chain level), index2uv, hash insert +
+// probe of the projected sets (their pixels collide: many-to-one tables).  Applies when all of them run on one stream and
+// the 2-D ones probe alike; else each op keeps its own launches.  The deterministic mode's 2-D rulebooks (the gather-form
+// dgrad's `rep` rows) stay per op.
 int fwd_chain_stages(FwdCtx& C, int i0, const int* ops, int L) {
     int sub3[IDX_BATCH_MAX], uvop[IDX_BATCH_MAX], sub2[IDX_BATCH_MAX], n3 = 0, nuv = 0, n2 = 0, s = -1;
     bool ok = true;
@@ -594,7 +604,6 @@ int fwd_chain_stages(FwdCtx& C, int i0, const int* ops, int L) {
         for (int u = 0; u < nuv; ++u) from_uv |= o[F_A] == C.op(uvop[u])[F_B];
         if (o[F_KIND] == OP_SUBM_RB && from_uv && !(C.S->deterministic && !o[F_X0])) take(j, sub2, n2);
     }
-    for (int a = 1; a < n3; ++a) ok &= C.op(sub3[a])[F_X0] == C.op(sub3[0])[F_X0];
     for (int a = 1; a < n2; ++a) ok &= C.op(sub2[a])[F_X0] == C.op(sub2[0])[F_X0];
     if (!ok || s < 0) return VC_OK;
     for (int a = 0; a < n3; ++a) {
@@ -615,9 +624,8 @@ int fwd_chain_stages(FwdCtx& C, int i0, const int* ops, int L) {
     VC_ALLOC(pn_all, int32_t*, pn_ints * 4);
     if (C.do_idx && pn_ints) VC_CUDA(cudaMemsetAsync(pn_all, 0, pn_ints * 4, C.st[s]));
     int32_t* pn = pn_all;
-    // 3-D: per stage its table, then its hash table right behind it, so the mirrored rows (k > centre, -1) and the hash table
-    // (EMPTY) are one 0xFF fill
-    SubmStage st3[IDX_BATCH_MAX];
+    // 3-D: by lookup in the bitmap of the chain level each index set is (every table entry written, nothing to clear)
+    SubmLookupStage st3[IDX_BATCH_MAX];
     for (int a = 0; a < n3; ++a) {
         const int* o = C.op(sub3[a]);
         ISet& I = C.S->iset[o[F_A]];
@@ -625,19 +633,15 @@ int fwd_chain_stages(FwdCtx& C, int i0, const int* ops, int L) {
         R.n_in = R.n_out = I.n;
         R.n_in_dev = R.n_out_dev = I.n_dev;
         VC_ALLOC(nbr, int32_t*, (size_t)R.K * I.n * 4);
-        const size_t wsb = vc_subm_rulebook_ws_bytes(I.n);
-        VC_ALLOC(ws, void*, wsb);
         R.nbr = nbr; R.pair_num = pn;
         pn += R.K;
-        st3[a] = SubmStage{I.idx, I.n, I.n_dev, I.ndim, I.shape, o + F_KS, o + F_DL, R.nbr, R.pair_num, ws, wsb};
-        if (C.do_idx && I.n > 0) {
-            char* from = subm_sym(I.ndim, o + F_KS, R.unique != 0) ? (char*)(nbr + (size_t)(R.K / 2 + 1) * I.n) : (char*)ws;
-            VC_CUDA(cudaMemsetAsync(from, 0xFF, (char*)ws + wsb - from, C.st[s]));
-        }
+        int l = 0;
+        while (C.op(ops[l])[F_B] != o[F_A]) ++l;
+        st3[a] = SubmLookupStage{I.idx, I.n, I.n_dev, I.ndim, I.shape, o + F_KS, o + F_DL, C.chain[ops[l]].rank, R.nbr, R.pair_num};
         C.batched[sub3[a]] = true;
     }
     if (n3) {
-        if (C.do_idx) VC_TRY(subm_rulebook_batch_dev(st3, n3, C.S->batch_size, C.op(sub3[0])[F_X0] != 0, C.st[s]));
+        if (C.do_idx) VC_TRY(subm_lookup_batch_dev(st3, n3, C.S->batch_size, C.st[s]));
         RBk& R0 = C.S->rb[C.op(sub3[0])[F_C]];
         C.produced(R0, s);
         for (int a = 1; a < n3; ++a) {
@@ -1422,8 +1426,9 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
             case K_DGRAD_TC:
                 VC_TRY(contribute_fused(C, X, [&](float* dst, const float* addend) -> int {
                     Timed t(L.dgrad, li, st);
+                    // (static mode: the slot's gradient has zero rows past its count, as every BN output has)
                     return tc2_conv(L.cout, L.cin, dxb, L.wimg_dgrad, table, R.n_in, dst, R.n_in, R.n_in_dev, R.K, nullptr, C.err, st,
-                                    addend, L.tile_ctr + 1, R.subm ? 0 : 1);
+                                    addend, L.tile_ctr + 1, (R.subm ? 0 : 1) | 4);
                 }));
                 break;
             case K_DGRAD_F32:

@@ -8,7 +8,8 @@
 //   hash      2^h x uint64, entry = (linear_key << 24) | row, EMPTY = ~0   (ws of vc_subm_rulebook)
 //   nbr       [K, N_out] int32 — row o of offset-plane k is written by thread o: fully coalesced
 //   bitmap    1 bit per OUTPUT cell (batch-major linear index), + per-word exclusive popcount rank
-//             (ws of vc_conv_rulebook_*) — gives the sorted, duplicate-free output set with no sort.
+//             (ws of vc_conv_rulebook_*) — gives the sorted, duplicate-free output set with no sort, and a cell's row in
+//             it by one bit test and one rank (the neighbour tables over a chain level's output set: no hash table).
 // Roofline: all kernels here are HBM/L2-latency bound integer work (no FLOPs); algorithmic bytes per
 // input voxel are stated in DESIGN.md §kernels.
 //
@@ -307,11 +308,34 @@ __global__ void __launch_bounds__(1024) scan_blocks_kernel(uint32_t* block_sum, 
     scan_segment(block_sum, n_blocks, n_out, cap, overflow);
 }
 
-__device__ __forceinline__ int cell_rank(const uint32_t* __restrict__ bitmap, const uint32_t* __restrict__ word_rank,
-                                         const uint32_t* __restrict__ block_sum, long long lin) {
-    long long w = lin >> 5;
-    uint32_t word = __ldg(bitmap + w);
-    return (int)(__ldg(block_sum + (w / SCAN_WORDS)) + __ldg(word_rank + w) + __popc(word & ((1u << (lin & 31)) - 1u)));
+// Rows of the cells along one x run of a ranked set of which the first n rows are held: a cell's row is its rank, or -1
+// when the cell is not in the set or ranks past the held rows (static mode: an overflowing level holds its first `cap`
+// cells only).  Successive cells of a run mostly share a bitmap word: the word and its rank are loaded together, once per
+// word.
+struct RunRows {
+    const ConvRank& r;
+    int n;
+    long long wc = -1;
+    uint32_t word = 0, base = 0;
+    __device__ __forceinline__ RunRows(const ConvRank& r_, int n_) : r(r_), n(n_) {}
+    __device__ __forceinline__ int row(long long lin) {
+        const long long w = lin >> 5;
+        if (w != wc) {
+            wc = w;
+            word = __ldg(r.bitmap + w);
+            base = __ldg(r.block_sum + (w / SCAN_WORDS)) + __ldg(r.word_rank + w);
+        }
+        const uint32_t bit = 1u << (lin & 31);
+        if (!(word & bit)) return -1;
+        const int row = (int)(base + __popc(word & (bit - 1u)));
+        return row < n ? row : -1;
+    }
+};
+
+// pair counts: per offset k, warp ballot -> shared counter cnt[k] -> (caller) one atomic per block
+__device__ __forceinline__ void count_pairs(int* cnt, int k, bool hit) {
+    const unsigned m = __ballot_sync(0xffffffffu, hit);
+    if ((threadIdx.x & 31) == 0 && m) atomicAdd(&cnt[k], __popc(m));
 }
 
 __global__ void conv_emit_indices_kernel(const uint32_t* __restrict__ bitmap, const uint32_t* __restrict__ word_rank,
@@ -445,36 +469,176 @@ struct TablesBatch {
     TablesEntry e[IDX_BATCH_MAX];
 };
 
-__global__ void __launch_bounds__(256) conv_tables_kernel(const __grid_constant__ TablesBatch tb) {   // grid (row blocks, max K)
+// One thread per input row, as the lookup kernels below: the output cells of the offsets along x lie on one x run of the
+// output bitmap (RunRows).
+__global__ void __launch_bounds__(256) conv_tables_kernel(const __grid_constant__ TablesBatch tb) {   // one thread per row
     const int i = batch_entry(tb.blk0, tb.E, blockIdx.x);
     const TablesEntry& e = tb.e[i];
     const Geom& g = e.g;
-    const int k = blockIdx.y;
-    if (k >= g.K) return;
-    __shared__ int cnt;
+    const int xd = g.ndim - 1, kx = g.ksize[xd];
+    __shared__ int cnt[MAXK];
+    if (threadIdx.x < g.K) cnt[threadIdx.x] = 0;
+    __syncthreads();
     const int pitch_in = e.n;             // nbr_bwd rows are [K][input capacity], nbr_fwd rows [K][n_out = output capacity]
     const int n = e.n_dev != nullptr ? min(e.n, __ldg(e.n_dev)) : e.n;
-    if (threadIdx.x == 0) cnt = 0;
-    __syncthreads();
     const int row = (blockIdx.x - tb.blk0[i]) * blockDim.x + threadIdx.x;
-    int orow = -1;
+    int b = 0, c[VC_MAX_NDIM] = {}, off[VC_MAX_NDIM];
+    bool in = false;
     if (row < n) {
-        int b, c[VC_MAX_NDIM];
         load_index(e.idx, row, g.ndim, b, c);
-        long long lin = out_cell(g, b, c, k);
-        if (lin >= 0) {
-            orow = cell_rank(e.r.bitmap, e.r.word_rank, e.r.block_sum, lin);
-            if (orow < e.n_out) e.nbr_fwd[(size_t)k * e.n_out + orow] = row;  // unique writer: (o,k) determines the input cell
-            else orow = -1;                                                    // beyond the output capacity (overflow flagged)
-        }
-        e.nbr_bwd[(size_t)k * pitch_in + row] = orow;
-    } else if (row < pitch_in) {
-        e.nbr_bwd[(size_t)k * pitch_in + row] = -1;   // static mode: rows between the count and the capacity
+        in = index_ok(g, b, c);
     }
-    unsigned m = __ballot_sync(0xffffffffu, orow >= 0);
-    if ((threadIdx.x & 31) == 0 && m) atomicAdd(&cnt, __popc(m));
+    for (int k0 = 0; k0 < g.K; k0 += kx) {   // the offset groups
+        bool ok = in;
+        long long lin = b;
+        decode_k(g, k0, off);
+        for (int d = 0; d < xd; ++d) {
+            const int num = c[d] + g.pad[d] - off[d] * g.dil[d], o = num / g.stride[d];
+            ok &= (num >= 0) & (o * g.stride[d] == num) & (o < g.oshape[d]);
+            lin = lin * g.oshape[d] + o;
+        }
+        lin *= g.oshape[xd];
+        RunRows rr(e.r, e.n_out);   // (a rank at or past the output capacity: overflow, flagged by the count)
+        for (int j = 0; j < kx; ++j) {
+            const int num = c[xd] + g.pad[xd] - j * g.dil[xd], o = num / g.stride[xd];
+            int orow = -1;
+            if (row < n) {
+                if (ok && num >= 0 && o * g.stride[xd] == num && o < g.oshape[xd]) {
+                    orow = rr.row(lin + o);
+                    if (orow >= 0 && e.nbr_fwd != nullptr)   // (else conv_fwd_lookup_kernel writes it)
+                        e.nbr_fwd[(size_t)(k0 + j) * e.n_out + orow] = row;   // unique writer: (o,k) determines the input cell
+                }
+                e.nbr_bwd[(size_t)(k0 + j) * pitch_in + row] = orow;
+            } else if (row < pitch_in) {
+                e.nbr_bwd[(size_t)(k0 + j) * pitch_in + row] = -1;   // static mode: rows between the count and the capacity
+            }
+            count_pairs(cnt, k0 + j, orow >= 0);
+        }
+    }
     __syncthreads();
-    if (e.pair_num != nullptr && threadIdx.x == 0 && cnt) atomicAdd(&e.pair_num[k], cnt);
+    if (e.pair_num != nullptr && threadIdx.x < g.K && cnt[threadIdx.x]) atomicAdd(&e.pair_num[threadIdx.x], cnt[threadIdx.x]);
+}
+
+// Lookups in a chain level's ranked output bitmap.  A chain level's rows are the set bits of its bitmap in rank order
+// (conv_emit_indices_kernel), so the row of a cell of that set is one bit test and one rank: no hash table, and each
+// table entry is written by the thread of its row, coalesced.  One thread per row, which loads the row's index once and
+// walks its offset groups: a group is the offsets that differ along x only (the last dimension, fastest in both the
+// offset and the cell order), whose cells lie along one x run of the bitmap (RunRows).  A neighbour cell is rejected per
+// dimension against the grid, never by linear-index arithmetic (x = W is the next row's x = 0, and the last cell of one
+// scene is the first of the next).
+
+// nbr_fwd of the chained strided convs whose input set is the previous level's output set (conv_fwd_lookup_batch_dev):
+// output row o and offset k look up the input cell o * stride - pad + k * dil in the input level's bitmap.  The pair
+// counts come from conv_tables_kernel's nbr_bwd.
+struct FwdLookupEntry {
+    const int32_t* out_idx;
+    const int *n_out_dev, *n_in_dev;
+    ConvRank in_rank;
+    int32_t* nbr_fwd;
+    Geom g;
+    int n_out, n_in;
+};
+struct FwdLookupBatch {
+    int E;
+    int blk0[IDX_BATCH_MAX + 1];
+    FwdLookupEntry e[IDX_BATCH_MAX];
+};
+
+__global__ void __launch_bounds__(256) conv_fwd_lookup_kernel(const __grid_constant__ FwdLookupBatch fb) {   // one thread per row
+    const int i = batch_entry(fb.blk0, fb.E, blockIdx.x);
+    const FwdLookupEntry& e = fb.e[i];
+    const Geom& g = e.g;
+    const int xd = g.ndim - 1, kx = g.ksize[xd];
+    const int n = e.n_out_dev != nullptr ? min(e.n_out, __ldg(e.n_out_dev)) : e.n_out;
+    const int n_in = e.n_in_dev != nullptr ? min(e.n_in, __ldg(e.n_in_dev)) : e.n_in;
+    const int row = (blockIdx.x - fb.blk0[i]) * blockDim.x + threadIdx.x;
+    if (row >= e.n_out) return;
+    int b = 0, c[VC_MAX_NDIM] = {}, off[VC_MAX_NDIM];
+    bool in = row < n;   // (static mode: rows between the count and the capacity have no neighbours)
+    if (in) {
+        load_index(e.out_idx, row, g.ndim, b, c);
+        in = b >= 0 && b < g.batch;
+    }
+    const int x0 = c[xd] * g.stride[xd] - g.pad[xd];
+    for (int k0 = 0; k0 < g.K; k0 += kx) {   // the offset groups
+        bool ok = in;
+        long long lin = b;
+        decode_k(g, k0, off);
+        for (int d = 0; d < xd; ++d) {
+            const int v = c[d] * g.stride[d] - g.pad[d] + off[d] * g.dil[d];
+            ok &= (v >= 0) & (v < g.shape[d]);
+            lin = lin * g.shape[d] + v;
+        }
+        lin *= g.shape[xd];
+        RunRows rr(e.in_rank, n_in);
+        for (int j = 0; j < kx; ++j) {
+            const int x = x0 + j * g.dil[xd];
+            e.nbr_fwd[(size_t)(k0 + j) * e.n_out + row] = ok && x >= 0 && x < g.shape[xd] ? rr.row(lin + x) : -1;
+        }
+    }
+}
+
+// Submanifold rulebooks over chain levels' output sets (subm_lookup_batch_dev), laid out as SubmBatch, every offset
+// looked up; the centre identity and the static-mode -1 tail as in subm_probe_kernel.
+struct LookupEntry {
+    const int32_t* idx;
+    const int* n_dev;
+    ConvRank rank;
+    int32_t *nbr, *pair_num;
+    Geom g;
+    int n;
+};
+struct LookupBatch {
+    int E;
+    int blk0[IDX_BATCH_MAX + 1];
+    LookupEntry e[IDX_BATCH_MAX];
+};
+
+__global__ void __launch_bounds__(256) subm_lookup_kernel(const __grid_constant__ LookupBatch lb) {   // one thread per row
+    const int i = batch_entry(lb.blk0, lb.E, blockIdx.x);
+    const LookupEntry& e = lb.e[i];
+    const Geom& g = e.g;
+    const int xd = g.ndim - 1, kx = g.ksize[xd];
+    __shared__ int cnt[MAXK];
+    if (threadIdx.x < g.K) cnt[threadIdx.x] = 0;
+    __syncthreads();
+    const int pitch = e.n;                // table rows are [K][capacity]
+    const int n = e.n_dev != nullptr ? min(e.n, __ldg(e.n_dev)) : e.n;
+    const int row = (blockIdx.x - lb.blk0[i]) * blockDim.x + threadIdx.x;
+    int b = 0, c[VC_MAX_NDIM] = {}, off[VC_MAX_NDIM], centre = 0;
+    for (int d = 0; d < g.ndim; ++d) centre = centre * g.ksize[d] + g.ksize[d] / 2;
+    bool in = false;
+    if (row < n) {
+        load_index(e.idx, row, g.ndim, b, c);
+        in = index_ok(g, b, c);
+    }
+    const int x0 = c[xd] - kx / 2 * g.dil[xd];
+    for (int k0 = 0; k0 < g.K; k0 += kx) {   // the offset groups
+        bool ok = in;
+        long long lin = b;
+        decode_k(g, k0, off);
+        for (int d = 0; d < xd; ++d) {
+            const int v = c[d] + (off[d] - g.ksize[d] / 2) * g.dil[d];
+            ok &= (v >= 0) & (v < g.shape[d]);
+            lin = lin * g.shape[d] + v;
+        }
+        lin *= g.shape[xd];
+        RunRows rr(e.rank, n);
+        for (int j = 0; j < kx; ++j) {
+            const int x = x0 + j * g.dil[xd];
+            int res = -1;
+            if (row < n) {
+                if (k0 + j == centre) res = row;   // identity (spconv Native: out = features @ W[centre])
+                else if (ok && x >= 0 && x < g.shape[xd]) res = rr.row(lin + x);
+                e.nbr[(size_t)(k0 + j) * pitch + row] = res;
+            } else if (row < pitch) {
+                e.nbr[(size_t)(k0 + j) * pitch + row] = -1;    // static mode: rows between the count and the capacity have no neighbours
+            }
+            count_pairs(cnt, k0 + j, res >= 0);
+        }
+    }
+    __syncthreads();
+    if (e.pair_num != nullptr && threadIdx.x < g.K && cnt[threadIdx.x]) atomicAdd(&e.pair_num[threadIdx.x], cnt[threadIdx.x]);
 }
 
 // one block per offset: order-preserving compaction of nbr[k, :] into spconv-style pairs
@@ -775,27 +939,71 @@ int vc::subm_rulebook_batch_dev(const SubmStage* st, int n_st, int batch_size, b
 }
 
 // The tables of up to IDX_BATCH_MAX strided convs in one launch.  The caller has filled every nbr_fwd with -1 and zeroed the
-// pair counts.
+// pair counts; a stage without nbr_fwd (NULL) gets it from conv_fwd_lookup_batch_dev.
 int vc::conv_tables_batch_dev(const TablesStage* st, int n_st, int batch_size, cudaStream_t stream) {
     VC_CHECK_ARG(n_st >= 1 && n_st <= IDX_BATCH_MAX, "%d stages in one batch", n_st);
     TablesBatch tb;
     memset(&tb, 0, sizeof(tb));
-    int K = 1;
     for (int i = 0; i < n_st; ++i) {
         const TablesStage& s = st[i];
         TablesEntry& e = tb.e[tb.E];
         int rc = make_geom(e.g, s.ndim, batch_size, s.shape, s.ksize, s.stride, s.pad, s.dil);
         if (rc) return rc;
         if (s.n == 0) continue;
-        VC_CHECK_ARG(s.idx && s.nbr_bwd && (s.n_out == 0 || s.nbr_fwd), "null pointer");
+        VC_CHECK_ARG(s.idx && s.nbr_bwd, "null pointer");
         e.idx = s.idx; e.n = s.n; e.n_dev = s.n_dev; e.n_out = s.n_out; e.r = s.rank;
         e.nbr_fwd = s.nbr_fwd; e.nbr_bwd = s.nbr_bwd; e.pair_num = s.pair_num;
-        K = e.g.K > K ? e.g.K : K;
         tb.blk0[tb.E + 1] = tb.blk0[tb.E] + cdiv(s.n, 256);
         ++tb.E;
     }
     if (tb.E == 0) return VC_OK;
-    conv_tables_kernel<<<dim3(tb.blk0[tb.E], K), 256, 0, stream>>>(tb);
+    conv_tables_kernel<<<tb.blk0[tb.E], 256, 0, stream>>>(tb);
+    VC_LAUNCH_CHECK();
+    return VC_OK;
+}
+
+// nbr_fwd of up to IDX_BATCH_MAX chained strided convs in one launch; every entry of each table is written (no fill).
+int vc::conv_fwd_lookup_batch_dev(const FwdLookupStage* st, int n_st, int batch_size, cudaStream_t stream) {
+    VC_CHECK_ARG(n_st >= 1 && n_st <= IDX_BATCH_MAX, "%d stages in one batch", n_st);
+    FwdLookupBatch fb;
+    memset(&fb, 0, sizeof(fb));
+    for (int i = 0; i < n_st; ++i) {
+        const FwdLookupStage& s = st[i];
+        FwdLookupEntry& e = fb.e[fb.E];
+        int rc = make_geom(e.g, s.ndim, batch_size, s.shape, s.ksize, s.stride, s.pad, s.dil);
+        if (rc) return rc;
+        if (s.n_out == 0) continue;
+        VC_CHECK_ARG(s.out_idx && s.nbr_fwd && s.in_rank.bitmap && s.n_in >= 0, "bad arguments");
+        e.out_idx = s.out_idx; e.n_out = s.n_out; e.n_out_dev = s.n_out_dev; e.n_in = s.n_in; e.n_in_dev = s.n_in_dev;
+        e.in_rank = s.in_rank; e.nbr_fwd = s.nbr_fwd;
+        fb.blk0[fb.E + 1] = fb.blk0[fb.E] + cdiv(s.n_out, 256);
+        ++fb.E;
+    }
+    if (fb.E == 0) return VC_OK;
+    conv_fwd_lookup_kernel<<<fb.blk0[fb.E], 256, 0, stream>>>(fb);
+    VC_LAUNCH_CHECK();
+    return VC_OK;
+}
+
+// Submanifold rulebooks of up to IDX_BATCH_MAX chain levels in one launch.  The caller has zeroed the pair counts.
+int vc::subm_lookup_batch_dev(const SubmLookupStage* st, int n_st, int batch_size, cudaStream_t stream) {
+    VC_CHECK_ARG(n_st >= 1 && n_st <= IDX_BATCH_MAX, "%d stages in one batch", n_st);
+    LookupBatch lb;
+    memset(&lb, 0, sizeof(lb));
+    for (int i = 0; i < n_st; ++i) {
+        const SubmLookupStage& s = st[i];
+        LookupEntry& e = lb.e[lb.E];
+        int rc = make_geom(e.g, s.ndim, batch_size, s.shape, s.ksize, nullptr, nullptr, s.dil);
+        if (rc) return rc;
+        VC_CHECK_ARG(s.n >= 0, "row count %d out of range", s.n);
+        if (s.n == 0) continue;
+        VC_CHECK_ARG(s.idx && s.nbr && s.rank.bitmap, "null pointer");
+        e.idx = s.idx; e.n = s.n; e.n_dev = s.n_dev; e.rank = s.rank; e.nbr = s.nbr; e.pair_num = s.pair_num;
+        lb.blk0[lb.E + 1] = lb.blk0[lb.E] + cdiv(s.n, 256);
+        ++lb.E;
+    }
+    if (lb.E == 0) return VC_OK;
+    subm_lookup_kernel<<<lb.blk0[lb.E], 256, 0, stream>>>(lb);
     VC_LAUNCH_CHECK();
     return VC_OK;
 }
