@@ -222,15 +222,16 @@ __device__ __forceinline__ void red_add_v2(float* p, float a, float b) {
 // both used MN-major (the reduction runs over the rows).  A group = 128 / CI kernel offsets stacked along M; warpgroup wg
 // owns M rows [64 wg, 64 wg + 64), i.e. starts 64 / CI gathered tiles into the stage.  acc[g] is group g of the pass; a group
 // index only known at run time selects its accumulator through an unrolled compare (registers cannot be indexed).
+// acc_in = 0: the stage's first MMA overwrites the group's accumulators instead of adding to them (a fresh sum).
 template <int CI, int CO, int NKS, int MAXG, int A_BYTES>
-__device__ __forceinline__ void wgrad_stage_mma(float (&acc)[MAXG][CO / 2], int g, uint32_t a_s, uint32_t b_s) {
+__device__ __forceinline__ void wgrad_stage_mma(float (&acc)[MAXG][CO / 2], int g, uint32_t a_s, uint32_t b_s, uint32_t acc_in) {
 #pragma unroll
     for (int gg = 0; gg < MAXG; ++gg) {
         if (gg == g) {
 #pragma unroll
             for (int m = 0; m < NKS; ++m)      // 16 rows per MMA
                 wgmma_bf16<CO, 1, 1>(acc[gg], gmma_desc_mn<2 * CI>(a_s + (uint32_t)(m * 32 * CI), (uint32_t)A_BYTES),
-                                     gmma_desc_mn<2 * CO>(b_s + (uint32_t)(m * 32 * CO), 16u), 1u);
+                                     gmma_desc_mn<2 * CO>(b_s + (uint32_t)(m * 32 * CO), 16u), m == 0 ? acc_in : 1u);
         }
     }
 }

@@ -2,16 +2,16 @@
 //
 //   dW[k] (C_in x C_out) = sum over output rows o of  in[nbr[k,o], :]^T (x) dout[o, :]
 //
-// Ring stages of 64 rows (16 KB), <= 111 KB shared memory and 416 threads per CTA, so that a wgrad CTA and a dgrad CTA of the
+// Ring stages of 64 rows (16 KB), <= 111 KB shared memory and 448 threads per CTA, so that a wgrad CTA and a dgrad CTA of the
 // main stream can share an SM: the plan executor runs this kernel on its own stream beside the dgrad chain.
 // Same machinery as the persistent forward kernel (conv_tc2.cu): persistent CTAs walk 128-row output tiles (dynamic tile
-// counter), a loader warp stages the tile's neighbour-table slice (cp.async into a 2-deep shared ring), 4 producer warps
-// gather the rows with 16-byte cp.async into 32/64/128-byte-swizzled tiles, two consumer warpgroups (64 accumulator rows
-// each) issue the MMAs.  What differs:
+// counter), a loader warp stages each tile's neighbour-table slice (bulk copies completing on an mbarrier) into a ring of
+// 2-4 tile slots, a dout warp fills the slot's dout tile, 4 producer warps gather the rows with 16-byte cp.async into
+// 32/64/128-byte-swizzled tiles, two consumer warpgroups (64 accumulator rows each) issue the MMAs.  What differs:
 //   * the gathered tile is used MN-MAJOR (the reduction runs over the 128 rows): the row-major swizzled tile the forward
 //     kernel builds is exactly the canonical Major-MN layout, and G = 128 / C_in kernel offsets are stacked along the MMA
 //     M dimension through the descriptor's leading-byte offset (one ring stage = G half tiles);
-//   * the second operand is the tile of dout itself (contiguous rows, loaded once per tile, double buffered);
+//   * the second operand is the tile of dout itself (contiguous rows, loaded once per tile into the tile's slot);
 //   * the accumulators of the pass's offset groups (<= 64 / C_out, 32 registers per thread: two CTAs fit an SM) stay
 //     resident in registers across all tiles of the CTA (more groups: more passes, blockIdx.y); at the end each CTA adds
 //     its [K, C_in, C_out] partial into ONE fp32 scratch image with 8-byte vector reductions.  Per-CTA partials re-read by a
@@ -33,12 +33,12 @@ namespace {
 // stream).  A ring stage is HALF a tile (64 rows) of the GW offsets of one accumulator group: 16 KB; the two producer groups
 // (2 warps each) own the two halves.
 constexpr int W_CONS_WARPS = 8;                                    // two consumer warpgroups
-constexpr int W_WARP_LOADER = W_CONS_WARPS, W_WARP_PROD0 = W_WARP_LOADER + 1, W_GROUPS = 2, W_GROUP_WARPS = 2;
+constexpr int W_WARP_LOADER = W_CONS_WARPS, W_WARP_DOUT = W_WARP_LOADER + 1, W_WARP_PROD0 = W_WARP_DOUT + 1;
+constexpr int W_GROUPS = 2, W_GROUP_WARPS = 2;
 constexpr int W_PROD_WARPS = W_GROUPS * W_GROUP_WARPS;             // 4
-constexpr int W_THREADS = 32 * (W_WARP_PROD0 + W_PROD_WARPS);      // 416
-constexpr int W_PROD_THREADS = 32 * W_PROD_WARPS;
+constexpr int W_THREADS = 32 * (W_WARP_PROD0 + W_PROD_WARPS);      // 448: still 72 registers per thread at two CTAs per SM
 constexpr int W_MAX_STAGES = 8;
-constexpr int W_NTB = 2;
+constexpr int W_MAX_NT = 4;                                       // tile slots (table slice + dout tile) a CTA loads ahead
 constexpr int W_HROWS = TCM / 2;                                   // rows of a ring stage
 constexpr int W_ROWS_PER_PROD = W_HROWS / W_GROUP_WARPS;           // 32
 constexpr int W_ACC = 64;                                          // accumulator columns (x 64 rows) per consumer warpgroup
@@ -67,6 +67,7 @@ struct WArgs {
     int n_host;
     int* tile_counter;          // [passes] or NULL
     int K, S, groups_per_pass;
+    int NT;                     // tile slots in shared memory (see launch_wgrad3)
     int det_chunks;             // > 0: deterministic mode, scratch = [det_chunks][K][in_c][out_c] (see tc3_wgrad)
     int* err;
 };
@@ -85,17 +86,20 @@ __global__ void __launch_bounds__(W_THREADS, 2) tc_wgrad_half_kernel(const WArgs
     using C = WCfg2<CI, CO>;
     constexpr int W_MAXG = W_ACC / CO, W_STAGES_PER_GROUP = 2, W_MMAS_PER_STAGE = W_HROWS / 16;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    const int S = a.S, K = a.K;
+    const int S = a.S, K = a.K, NT = a.NT;
     unsigned char* ring = smem_raw;                                              // [S][GW x A half tile]
-    unsigned char* dout_s = smem_raw + (size_t)S * C::STAGE;                     // [2][B tile]
-    int* nbr_s = reinterpret_cast<int*>(dout_s + 2 * C::B_BYTES);                // [W_NTB][kcount][128]
+    unsigned char* dout_s = smem_raw + (size_t)S * C::STAGE;                     // [NT][B tile]
+    int* nbr_s = reinterpret_cast<int*>(dout_s + (size_t)NT * C::B_BYTES);     // [NT][kcount][128]
     __shared__ __align__(8) uint64_t full_bar[W_MAX_STAGES];
     __shared__ __align__(8) uint64_t empty_bar[W_MAX_STAGES];
-    __shared__ __align__(8) uint64_t tbl_full[W_NTB], tbl_empty[W_NTB];
-    __shared__ __align__(8) uint64_t dout_full[2], dout_empty[2];
-    __shared__ int tile_s[W_NTB];
+    __shared__ __align__(8) uint64_t tbl_full[W_MAX_NT], tbl_empty[W_MAX_NT];
+    __shared__ __align__(8) uint64_t dout_full[W_MAX_NT], dout_empty[W_MAX_NT];
+    __shared__ __align__(8) uint64_t claim_bar[W_MAX_NT];
+    __shared__ int tile_s[W_MAX_NT];
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    // the role index read through a shuffle: the compiler can then tell that the consumer branch is warp-uniform, and does not
+    // serialize its wgmma instructions
+    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
     // this pass's slice of the kernel offsets (passes only when the accumulators of all groups exceed W_ACC columns)
     const int n_groups_total = (K + C::GW - 1) / C::GW;
     const int g_begin = blockIdx.y * a.groups_per_pass;
@@ -110,13 +114,12 @@ __global__ void __launch_bounds__(W_THREADS, 2) tc_wgrad_half_kernel(const WArgs
             mbar_init(&full_bar[s], 32 * W_GROUP_WARPS + W_GROUP_WARPS);
             mbar_init(&empty_bar[s], 2);                       // one arrive per consumer warpgroup
         }
-        for (int b = 0; b < W_NTB; ++b) {
-            mbar_init(&tbl_full[b], 1);                        // loader
-            mbar_init(&tbl_empty[b], W_PROD_WARPS + W_CONS_WARPS);   // producers + consumers
-        }
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(&dout_full[b], W_PROD_THREADS);          // every producer thread (cp.async arrive)
+        for (int b = 0; b < NT; ++b) {
+            mbar_init(&tbl_full[b], 1);                        // loader (arrive.expect_tx of the bulk copies, or a plain arrive)
+            mbar_init(&tbl_empty[b], W_PROD_WARPS + W_CONS_WARPS + 1);   // producers + consumers + dout loader
+            mbar_init(&dout_full[b], 32);                      // every dout-loader lane (cp.async arrive)
             mbar_init(&dout_empty[b], 2);                      // one arrive per consumer warpgroup
+            mbar_init(&claim_bar[b], 1);                       // loader: tile_s holds the slot's tile
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -131,24 +134,20 @@ __global__ void __launch_bounds__(W_THREADS, 2) tc_wgrad_half_kernel(const WArgs
     const int tpc = a.det_chunks > 0 ? max(1, (n_tiles + a.det_chunks - 1) / a.det_chunks) : 0;
     const int n_chunks = tpc > 0 ? (n_tiles + tpc - 1) / tpc : 0;
     const size_t part_floats = (size_t)K * a.in_c * a.out_c;
-    int ntb = W_NTB;            // table buffers in use == tiles a CTA holds claimed at once (see conv_tc2.cu)
-    if (counter != nullptr) {
-        int d = n_tiles / (3 * (int)gridDim.x);
-        d = d < 1 ? 1 : (d > W_NTB - 1 ? W_NTB - 1 : d);
-        ntb = d + 1;
-    }
     __syncthreads();
 
     if (warp == W_WARP_LOADER) {
         // ------------------------------------------------------------ tile scheduler + neighbour-table loader
-        const bool vec_ok = (reinterpret_cast<uintptr_t>(a.nbr) & 15u) == 0 && (a.pitch & 3) == 0;
-        const int lag = ntb - 1;
-        int tq0 = -1, tq1 = -1, tq2 = -1, tq3 = -1;
+        // Tile slot it % NT holds the tile's table slice and its dout tile.  The slice (one 512-byte span per kernel offset) comes
+        // in by bulk copies that complete on tbl_full, up to NT tiles ahead of the producers.  claim_bar publishes the slot's tile
+        // before its table lands, so the dout warp starts on the dout tile at once; neither this warp nor the producers wait for
+        // a dout buffer.
+        const bool bulk_ok = (reinterpret_cast<uintptr_t>(a.nbr) & 15u) == 0 && (a.pitch & 3) == 0;
         bool stop = false;
         int claimed = 0;
         int c_next = 0, c_end = 0;          // deterministic mode: the rest of the claimed chunk
         for (int it = 0;; ++it) {
-            const int tb = it % ntb;
+            const int tb = it % NT;
             int tile = -1;
             if (!stop && tpc > 0) {
                 if (c_next >= c_end) {
@@ -181,64 +180,57 @@ __global__ void __launch_bounds__(W_THREADS, 2) tc_wgrad_half_kernel(const WArgs
                     stop = true;
                 }
             }
-            switch (it & 3) {
-                case 0: tq0 = tile; break;
-                case 1: tq1 = tile; break;
-                case 2: tq2 = tile; break;
-                default: tq3 = tile; break;
+            if (it >= NT) W_WAIT(&tbl_empty[tb], (uint32_t)(((it / NT) - 1) & 1), 0x201);
+            if (lane == 0) tile_s[tb] = tile;
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&claim_bar[tb]);
+            if (tile < 0) {
+                if (lane == 0) mbar_arrive(&tbl_full[tb]);
+                break;
             }
-            if (it >= ntb) W_WAIT(&tbl_empty[tb], (uint32_t)(((it / ntb) - 1) & 1), 0x201);
-            if (tile >= 0) {
-                int* dst = nbr_s + (size_t)tb * k_count * TCM;
-                const int base = tile * TCM;
-                if (vec_ok && (long long)base + TCM <= a.pitch) {
-                    uint32_t d = smem_u32(dst) + lane * 16;
-                    const int32_t* sp = a.nbr + (size_t)k_begin * a.pitch + base + lane * 4;
-                    for (int k = 0; k < k_count; ++k, d += TCM * 4, sp += a.pitch) cp_async16_s(d, sp, true);
-                } else {
-                    for (int k = 0; k < k_count; ++k) {
+            int* dst = nbr_s + (size_t)tb * k_count * TCM;
+            const int base = tile * TCM;
+            if (bulk_ok && (long long)base + TCM <= a.pitch) {
+                // the producers treat the rows at or past n as missing, whatever the table holds there
+                if (lane == 0) mbar_expect_tx(&tbl_full[tb], (uint32_t)(k_count * TCM * 4));
+                __syncwarp();
+                for (int k = lane; k < k_count; k += 32)
+                    bulk_g2s(smem_u32(dst + k * TCM), a.nbr + (size_t)(k_begin + k) * a.pitch + base, TCM * 4, &tbl_full[tb]);
+            } else {
+                for (int k = 0; k < k_count; ++k)
 #pragma unroll
-                        for (int q = 0; q < 4; ++q) {
-                            const int row = base + q * 32 + lane;
-                            if (row < n) {
-                                asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"(smem_u32(dst + k * TCM + q * 32 + lane)),
-                                             "l"(a.nbr + (size_t)(k_begin + k) * a.pitch + row));
-                            } else {
-                                dst[k * TCM + q * 32 + lane] = -1;
-                            }
-                        }
+                    for (int q = 0; q < 4; ++q) {
+                        const int row = base + q * 32 + lane;
+                        dst[k * TCM + q * 32 + lane] = row < n ? __ldg(a.nbr + (size_t)(k_begin + k) * a.pitch + row) : -1;
                     }
-                }
-            }
-            cp_async_commit();
-            if (it >= lag) {
-                const int pi = it - lag;
-                if (lag == 3) cp_async_wait<3>(); else if (lag == 2) cp_async_wait<2>(); else cp_async_wait<1>();
                 __syncwarp();
-                const int ptb = pi % ntb;
-                const int ptile = (pi & 3) == 0 ? tq0 : (pi & 3) == 1 ? tq1 : (pi & 3) == 2 ? tq2 : tq3;
-                if (ptile >= 0 && ptile * TCM + TCM > n) {
-                    int* dst = nbr_s + (size_t)ptb * k_count * TCM;
-                    const int r0 = ptile * TCM + lane * 4;
-                    for (int k = 0; k < k_count; ++k) {
-                        int4 v = reinterpret_cast<const int4*>(dst + k * TCM)[lane];
-                        if (r0 + 0 >= n) v.x = -1;
-                        if (r0 + 1 >= n) v.y = -1;
-                        if (r0 + 2 >= n) v.z = -1;
-                        if (r0 + 3 >= n) v.w = -1;
-                        reinterpret_cast<int4*>(dst + k * TCM)[lane] = v;
-                    }
-                }
-                if (lane == 0) tile_s[ptb] = ptile;
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tbl_full[ptb]);
-                if (ptile < 0) break;
+                if (lane == 0) mbar_arrive(&tbl_full[tb]);
             }
+        }
+    } else if (warp == W_WARP_DOUT) {
+        // ------------------------------------------------------------ dout loader
+        // the tile of dout (second operand of every group of the tile): contiguous rows, copied by the 32 lanes' cp.async into
+        // its swizzled image (a bulk copy cannot swizzle) once the consumers have retired the slot's previous tile
+        for (int it = 0;; ++it) {
+            const int tb = it % NT;
+            W_WAIT(&claim_bar[tb], (uint32_t)((it / NT) & 1), 0x202);
+            const int tile = tile_s[tb];
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&tbl_empty[tb]);
+            if (tile < 0) break;
+            const int base = tile * TCM;
+            if (it >= NT) W_WAIT(&dout_empty[tb], (uint32_t)(((it / NT) - 1) & 1), 0x203);
+            const uint32_t b_s = smem_u32(dout_s) + (uint32_t)tb * C::B_BYTES;
+            for (int q = lane; q < TCM * C::CPB; q += 32) {
+                const int r = q / C::CPB, c = q % C::CPB;
+                const bool v = base + r < n && c * 8 < a.out_c;
+                cp_async16_s(b_s + swz_off<C::RB>(r, c), v ? a.dout + (size_t)(base + r) * a.out_c + c * 8 : a.dout, v);
+            }
+            cp_async_arrive_noinc(&dout_full[tb]);
         }
     } else if (warp >= W_WARP_PROD0) {
         // ------------------------------------------------------------ gather producers
         const int grp = (warp - W_WARP_PROD0) / W_GROUP_WARPS, pw = (warp - W_WARP_PROD0) % W_GROUP_WARPS;   // grp = half of the tile
-        const int ptid = tid - W_WARP_PROD0 * 32;
         constexpr int CW = C::CPA < 4 ? C::CPA : 4;
         constexpr int RPI = 32 / CW;
         constexpr int NIT = W_ROWS_PER_PROD / RPI;
@@ -249,33 +241,21 @@ __global__ void __launch_bounds__(W_THREADS, 2) tc_wgrad_half_kernel(const WArgs
         bool ch_ok[NCG];
 #pragma unroll
         for (int i = 0; i < NIT; ++i) {
-            rows[i] = pw * W_ROWS_PER_PROD + i * RPI + r_sub;
+            rows[i] = grp * W_HROWS + pw * W_ROWS_PER_PROD + i * RPI + r_sub;
 #pragma unroll
-            for (int cg = 0; cg < NCG; ++cg) dst_off[i][cg] = swz_off<C::RA>(rows[i], cg * CW + c_sub);
+            for (int cg = 0; cg < NCG; ++cg) dst_off[i][cg] = swz_off<C::RA>(rows[i] - grp * W_HROWS, cg * CW + c_sub);
         }
 #pragma unroll
         for (int cg = 0; cg < NCG; ++cg) ch_ok[cg] = (cg * CW + c_sub) * 8 < a.in_c;
         const uint32_t ring_s = smem_u32(ring);
         int s = 0, wr = 0, turn = 0;
         for (int it = 0;; ++it) {
-            const int tb = it % ntb, db = it & 1;
-            W_WAIT(&tbl_full[tb], (uint32_t)((it / ntb) & 1), 0x211);
+            const int tb = it % NT;
+            W_WAIT(&tbl_full[tb], (uint32_t)((it / NT) & 1), 0x211);
             const int tile = tile_s[tb];
             if (tile < 0) break;
             const int* tbl = nbr_s + (size_t)tb * k_count * TCM;
-            const int base = tile * TCM;
-            // the tile of dout (second operand of every group of this tile): contiguous rows, swizzled image, loaded by all
-            // producer threads together
-            if (it >= 2) W_WAIT(&dout_empty[db], (uint32_t)(((it >> 1) - 1) & 1), 0x212);
-            {
-                const uint32_t b_s = smem_u32(dout_s) + (uint32_t)db * C::B_BYTES;
-                for (int q = ptid; q < TCM * C::CPB; q += W_PROD_THREADS) {
-                    const int r = q / C::CPB, c = q % C::CPB;
-                    const bool v = base + r < n && c * 8 < a.out_c;
-                    cp_async16_s(b_s + swz_off<C::RB>(r, c), v ? a.dout + (size_t)(base + r) * a.out_c + c * 8 : a.dout, v);
-                }
-                cp_async_arrive_noinc(&dout_full[db]);
-            }
+            const int rows_left = n - tile * TCM;       // rows at or past it are missing (the last tile's tail)
             for (int gs = 0; gs < 2 * g_count; ++gs) {         // stage (group g, half h) = 2 g + h; half h belongs to producer group h
                 const int g = gs >> 1;
                 if (turn == grp) {
@@ -284,7 +264,7 @@ __global__ void __launch_bounds__(W_THREADS, 2) tc_wgrad_half_kernel(const WArgs
                     for (int j = 0; j < C::GW; ++j) {
                         const int kk = g * C::GW + j;
 #pragma unroll
-                        for (int i = 0; i < NIT; ++i) src[j][i] = kk < k_count ? tbl[kk * TCM + grp * W_HROWS + rows[i]] : -1;
+                        for (int i = 0; i < NIT; ++i) src[j][i] = kk < k_count && rows[i] < rows_left ? tbl[kk * TCM + rows[i]] : -1;
                     }
                     if (wr > 0) W_WAIT(&empty_bar[s], (uint32_t)((wr - 1) & 1), 0x213);
                     const uint32_t st_s = ring_s + (uint32_t)s * C::STAGE;
@@ -317,7 +297,7 @@ __global__ void __launch_bounds__(W_THREADS, 2) tc_wgrad_half_kernel(const WArgs
             if (lane == 0) mbar_arrive(&tbl_empty[tb]);
         }
     } else {
-        // ------------------------------------------------------------ consumers: MMAs into register accumulators, one flush at the end
+        // ------------------------------------------------------------ consumers: MMAs into register accumulators, one flush per run
         const int wg = warp >> 2, t = tid & 127;
         float acc[W_MAXG][CO / 2];
 #pragma unroll
@@ -328,61 +308,60 @@ __global__ void __launch_bounds__(W_THREADS, 2) tc_wgrad_half_kernel(const WArgs
         const uint32_t ring_a = smem_u32(ring) + (uint32_t)(wg * (64 / CI) * C::A_BYTES), dout_a = smem_u32(dout_s);
         int s = 0;
         uint32_t ph = 0;
-        int n_done = 0;
-        int chunk = -1;                          // deterministic mode: chunk the accumulators belong to
-        for (int it = 0;; ++it) {
-            const int tb = it % ntb, db = it & 1;
-            W_WAIT(&tbl_full[tb], (uint32_t)((it / ntb) & 1), 0x221);
-            const int tile = tile_s[tb];
-            if (tile < 0) break;
-            if (tpc > 0 && tile / tpc != chunk) {
-                if (n_done > 0) {                // the previous chunk is complete: its partial image, then start from zero
-#pragma unroll
-                    for (int gg = 0; gg < W_MAXG; ++gg) wg_fence_acc(acc[gg]);
-                    wgrad_flush<CI, CO, W_MAXG>(acc, wg, t, g_count, k_begin, k_count, a.in_c, a.out_c,
-                                                a.scratch + (size_t)chunk * part_floats);
-#pragma unroll
-                    for (int gg = 0; gg < W_MAXG; ++gg)
-#pragma unroll
-                        for (int j = 0; j < CO / 2; ++j) acc[gg][j] = 0.f;
+        int it = 0;
+        for (bool more = true; more;) {
+            // one run of tiles summed into the accumulators, then one flush: the whole CTA, or in deterministic mode one chunk
+            int chunk = -1, n_done = 0;
+            for (;; ++it) {
+                const int tb = it % NT;
+                W_WAIT(&tbl_full[tb], (uint32_t)((it / NT) & 1), 0x221);
+                const int tile = tile_s[tb];
+                if (tile < 0) {
+                    more = false;
+                    break;
                 }
-                chunk = tile / tpc;
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tbl_empty[tb]);
-            if (!mbar_spin(doutf0 + 8u * db, (uint32_t)((it >> 1) & 1), 4096u) &&
-                !mbar_wait_t_addr(doutf0 + 8u * db, (uint32_t)((it >> 1) & 1), a.err, 0x222))
-                goto done;
-            const uint32_t b_s = dout_a + (uint32_t)db * C::B_BYTES;
-            int prev = -1;                       // ring slot whose MMAs may still be in flight
-            for (int gs = 0; gs < W_STAGES_PER_GROUP * g_count; ++gs) {
-                if (!mbar_spin(full0 + 8u * s, ph, 4096u) && !mbar_wait_t_addr(full0 + 8u * s, ph, a.err, 0x223)) goto done;
-                fence_async_smem();     // generic-proxy (cp.async, st.shared) writes -> visible to the tensor core's async proxy
-                wg_fence();
-                wgrad_stage_mma<CI, CO, W_MMAS_PER_STAGE, W_MAXG, C::A_BYTES>(
-                    acc, gs / W_STAGES_PER_GROUP, ring_a + (uint32_t)s * C::STAGE,
-                    b_s + (uint32_t)((gs % W_STAGES_PER_GROUP) * W_MMAS_PER_STAGE * 16 * C::RB));
-                wg_commit();
-                wg_wait<1>();                    // the previous stage's MMAs have completed: release its ring slot
-                if (prev >= 0 && t == 0) mbar_arrive(&empty_bar[prev]);
-                prev = s;
-                if (++s == S) {
-                    s = 0;
-                    ph ^= 1u;
+                if (tpc > 0) {
+                    if (n_done == 0) chunk = tile / tpc;
+                    else if (tile / tpc != chunk) break;      // the chunk is complete; this tile starts the next run
                 }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&tbl_empty[tb]);
+                if (!mbar_spin(doutf0 + 8u * tb, (uint32_t)((it / NT) & 1), 4096u) &&
+                    !mbar_wait_t_addr(doutf0 + 8u * tb, (uint32_t)((it / NT) & 1), a.err, 0x222))
+                    goto done;
+                const uint32_t b_s = dout_a + (uint32_t)tb * C::B_BYTES;
+                int prev = -1;                       // ring slot whose MMAs may still be in flight
+                for (int gs = 0; gs < W_STAGES_PER_GROUP * g_count; ++gs) {
+                    if (!mbar_spin(full0 + 8u * s, ph, 4096u) && !mbar_wait_t_addr(full0 + 8u * s, ph, a.err, 0x223)) goto done;
+                    fence_async_smem();     // generic-proxy (cp.async, st.shared) writes -> visible to the tensor core's async proxy
+                    wg_fence();
+                    wgrad_stage_mma<CI, CO, W_MMAS_PER_STAGE, W_MAXG, C::A_BYTES>(
+                        acc, gs / W_STAGES_PER_GROUP, ring_a + (uint32_t)s * C::STAGE,
+                        b_s + (uint32_t)((gs % W_STAGES_PER_GROUP) * W_MMAS_PER_STAGE * 16 * C::RB),
+                        n_done > 0 || gs % W_STAGES_PER_GROUP != 0 ? 1u : 0u);
+                    wg_commit();
+                    wg_wait<1>();                    // the previous stage's MMAs have completed: release its ring slot
+                    if (prev >= 0 && t == 0) mbar_arrive(&empty_bar[prev]);
+                    prev = s;
+                    if (++s == S) {
+                        s = 0;
+                        ph ^= 1u;
+                    }
+                }
+                wg_wait<0>();
+                if (t == 0) {
+                    mbar_arrive(&empty_bar[prev]);
+                    mbar_arrive(&dout_empty[tb]);
+                }
+                ++n_done;
             }
-            wg_wait<0>();
-            if (t == 0) {
-                if (prev >= 0) mbar_arrive(&empty_bar[prev]);
-                mbar_arrive(&dout_empty[db]);
-            }
-            ++n_done;
+#pragma unroll
+            for (int gg = 0; gg < W_MAXG; ++gg) wg_fence_acc(acc[gg]);
+            // (the next run's first MMA of each group starts its sum afresh: no zeroing of the accumulators here)
+            if (n_done > 0)
+                wgrad_flush<CI, CO, W_MAXG>(acc, wg, t, g_count, k_begin, k_count, a.in_c, a.out_c,
+                                            a.scratch + (tpc > 0 ? (size_t)chunk * part_floats : 0));
         }
-#pragma unroll
-        for (int gg = 0; gg < W_MAXG; ++gg) wg_fence_acc(acc[gg]);
-        if (n_done > 0)
-            wgrad_flush<CI, CO, W_MAXG>(acc, wg, t, g_count, k_begin, k_count, a.in_c, a.out_c,
-                                        a.scratch + (tpc > 0 ? (size_t)chunk * part_floats : 0));
     }
 done:
     cp_async_wait<0>();
@@ -408,15 +387,22 @@ int launch_wgrad3(const WArgs& a0, int n_cap, int max_ctas, cudaStream_t stream)
     int gpp = (n_groups + passes - 1) / passes;
     const int kcount = gpp * C::GW < a.K ? gpp * C::GW : a.K;
     a.groups_per_pass = gpp;
-    const size_t fixed = 2 * (size_t)C::B_BYTES + (size_t)W_NTB * kcount * TCM * 4;
-    int S = (int)((W_SMEM_BUDGET - fixed) / C::STAGE);
-    if (S > W_MAX_STAGES) S = W_MAX_STAGES;
+    const size_t slot = (size_t)C::B_BYTES + (size_t)kcount * TCM * 4;     // one tile slot: dout tile + table slice
+    auto stages = [&](int nt) {
+        const long long s = ((long long)W_SMEM_BUDGET - (long long)nt * (long long)slot) / C::STAGE;
+        return (int)(s > W_MAX_STAGES ? W_MAX_STAGES : s);
+    };
+    // as many tile slots as fit without taking a stage from the gather ring (the stages hold most of the bytes in flight)
+    int NT = 2;
+    while (NT < W_MAX_NT && stages(NT + 1) >= stages(2)) ++NT;
+    const int S = stages(NT);
     if (S < 2) {
         set_error("tensor-core wgrad: no room for the operand ring (K=%d, %d->%d)", a.K, CI, CO);
         return VC_ERR_UNSUPPORTED;
     }
     a.S = S;
-    const size_t smem = (size_t)S * C::STAGE + fixed;
+    a.NT = NT;
+    const size_t smem = (size_t)S * C::STAGE + (size_t)NT * slot;
     auto kern = tc_wgrad_half_kernel<CI, CO>;
     static bool attr_done = false;
     if (!attr_done) {
@@ -448,7 +434,7 @@ int tc3_wgrad(int cin, int cout, const void* in_bf16, const void* dout_bf16, con
     }
     a.in = (const __nv_bfloat16*)in_bf16; a.in_c = cin; a.in_ld = in_ld; a.dout = (const __nv_bfloat16*)dout_bf16; a.out_c = cout; a.nbr = nbr;
     a.pitch = pitch; a.scratch = scratch; a.n_dev = n_dev; a.n_host = n_rows; a.tile_counter = tile_counter; a.K = K; a.S = 0;
-    a.groups_per_pass = 0; a.err = err; a.det_chunks = det_chunks;
+    a.groups_per_pass = 0; a.NT = 0; a.err = err; a.det_chunks = det_chunks;
     const int ci = tc_pad16(cin), co = tc_pad16(cout);
 #define VC_W_CASE(A, B) \
     if (ci == A && co == B) return launch_wgrad3<A, B>(a, n_rows, max_ctas, stream);
