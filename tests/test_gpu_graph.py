@@ -179,6 +179,33 @@ def test_graph_recaptures_when_a_batch_does_not_fit(lib_built):
     assert abs(float(loss) - l_big) < 1e-5 * max(1.0, abs(l_big))
 
 
+def test_capture_outlives_unreachable_graphs_of_earlier_steps(lib_built):
+    """An earlier GraphedStep dropped inside a reference cycle keeps its CUDA graphs until the cyclic collector runs, and a
+    graph destroyed during another capture invalidates that capture.  The collector runs here in the middle of the capture
+    (from the loss function), so it must find no such graph left."""
+    import gc
+    from virconv_b200.graph import GraphedStep
+    model = _model('bf16')
+    batch = _batch([35, 36], n_lidar=2048, n_virtual=3000, max_voxels=2500)
+    old = GraphedStep(model, _loss, margin=1.3, grain=256)
+    old(batch)
+    torch.cuda.synchronize()
+    old.cycle = old
+    del old
+
+    def loss_collecting(out):
+        if torch.cuda.is_current_stream_capturing():
+            gc.collect()
+        return _loss(out)
+
+    l0, _, _ = _exact(model, batch)
+    step = GraphedStep(model, loss_collecting, margin=1.3, grain=256)
+    loss = step(batch)
+    torch.cuda.synchronize()
+    assert step.recaptures == 1
+    assert abs(float(loss) - l0) < 1e-5 * max(1.0, abs(l0))
+
+
 def test_graph_resets_the_input_tail_of_a_shrinking_batch(lib_built):
     """A larger batch, then a smaller one through the same captured step (voxelised batches): the published x_conv1, whose
     indices are the graph's input coordinates, keeps its -1 tail past `num_rows` — no row of the larger batch is left

@@ -28,10 +28,12 @@ LAUNCHES_T = (2 + 4 + 1 + 2 + 12 + 2) + (5 + 4 + 1 + 5 + 19 + 2)
 # deterministic mode: stages 2-4's 2-D rulebooks one batch per op, for their `rep` rows (6 launches instead of 2), and the
 # row groups of the gather-form dgrad for each of the four 2-D rulebooks (gather2d_prep_dev: 6 launches each)
 LAUNCHES_L_DET = LAUNCHES_L + 4 + 4 * 6
-# paper-mode StVD: a layer discard between strided convs, so no chain: per strided conv its count (mark, two scans), emit
-# and tables (5), every stage's index work one call per op (5), per discard site the row selection (7) and the gathers
-# of its indices and features (2)
-LAUNCHES_L_PAPER = 4 * 5 + 4 * 5 + 3 * (7 + 2) + 20 + 2
+# paper-mode StVD: a layer discard after vir_conv1..3 ends a chain, so vir_conv2's and vir_conv3's down convs are chains of
+# one and vir_conv4's down conv and conv_out a chain of two.  Stage 1's index work as in LAUNCHES_L (5); per chain its
+# count and emit (mark, two scans, emit: 4) and its tables (1), plus the chain of two's lookup of level 1's nbr_fwd (1);
+# stages 2-4's 3-D rulebook, projection and 2-D rulebook one launch per kind (1 + 1 + 2); per discard site the row
+# selection (7) and the gathers of its indices and features (2); 20 layers, the weight images and the input's bf16 cast
+LAUNCHES_L_PAPER = 5 + 3 * (4 + 1) + 1 + 3 * (1 + 1 + 2) + 3 * (7 + 2) + 20 + 2
 
 
 def _runs(monkeypatch):
@@ -266,8 +268,8 @@ def test_virconv_t_eval_rot3_packed_grid(monkeypatch):
         _check_run(run, bd, tp[:, i])
 
 
-def test_paper_stvd_device_discards(monkeypatch):
-    """VirConv-L's paper-mode StVD discards rows after vir_conv1..3: the strided convs are built level by level"""
+def test_paper_stvd_chains_of_one_and_two(monkeypatch):
+    """VirConv-L's paper-mode StVD discards rows after vir_conv1..3: the strided convs are built as chains of one, one, two"""
     bd = dict(_batch([5, 6]), stvd_seed=torch.tensor([1234], dtype=torch.int64, device=DEV))
     runs, launches = _forward(_model(40, discard_mode='paper', discard_rng='device'), bd, monkeypatch)
     from virconv_b200 import executor

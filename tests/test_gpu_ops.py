@@ -57,7 +57,9 @@ def test_subm2d_rulebook_with_duplicates(lib_built, n, shape):
 
 GEOS = [dict(ksize=3, stride=2, padding=1), dict(ksize=3, stride=2, padding=(0, 1, 1)),
         dict(ksize=(3, 1, 1), stride=(2, 1, 1), padding=0), dict(ksize=3, stride=1, padding=1),
-        dict(ksize=(3, 3, 3), stride=(2, 2, 2), padding=0), dict(ksize=2, stride=2, padding=0)]
+        dict(ksize=(3, 3, 3), stride=(2, 2, 2), padding=0), dict(ksize=2, stride=2, padding=0),
+        dict(ksize=3, stride=2, padding=2, dilation=(2, 3, 2)),     # dilated: marked per kernel offset
+        dict(ksize=3, stride=2, padding=1, ndim=2)]                 # 2-D: the last two dimensions of `shape`
 
 
 @pytest.mark.parametrize('geo', GEOS)
@@ -65,10 +67,12 @@ GEOS = [dict(ksize=3, stride=2, padding=1), dict(ksize=3, stride=2, padding=(0, 
 def test_conv_rulebook_bit_exact(lib_built, geo, n, batch, shape):
     from virconv_b200 import ops
     rng = np.random.default_rng(n)
+    shape = shape[3 - geo.get('ndim', 3):]
     c = _coords(rng, n, batch, shape)
+    dl = geo.get('dilation', 1)
     rb = ops.build_conv_rulebook(torch.from_numpy(c).to(_dev()), batch, shape, geo['ksize'], geo['stride'],
-                                 geo['padding'])
-    oi, osh, nf, nb = orb.conv_rulebook(c, shape, geo['ksize'], geo['stride'], geo['padding'])
+                                 geo['padding'], dl)
+    oi, osh, nf, nb = orb.conv_rulebook(c, shape, geo['ksize'], geo['stride'], geo['padding'], dl)
     assert rb.out_shape == osh
     assert np.array_equal(rb.out_indices.cpu().numpy(), oi)           # ascending linear index, batch major
     assert np.array_equal(rb.nbr.cpu().numpy(), nf)

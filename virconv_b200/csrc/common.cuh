@@ -103,33 +103,19 @@ int subm_rulebook_dev(const int32_t* indices, int n, const int* n_dev, int ndim,
                       const int32_t* ksize, const int32_t* dilation, int32_t* nbr, int32_t* pair_num, void* ws, size_t ws_bytes,
                       cudaStream_t stream, int32_t* rep = nullptr,   // rep (optional): [n] lowest row at each row's coordinate
                       bool unique = false);   // every coordinate held by one row: half the probes (the table is its own transpose)
-int conv_rulebook_count_dev(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size,
-                            const int32_t* spatial_shape, const int32_t* ksize, const int32_t* stride, const int32_t* padding,
-                            const int32_t* dilation, int32_t* n_out_dev, int cap_out, int* overflow, void* ws, size_t ws_bytes,
-                            cudaStream_t stream);
-int conv_rulebook_fill_phases(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size,
-                              const int32_t* spatial_shape, const int32_t* ksize, const int32_t* stride, const int32_t* padding,
-                              const int32_t* dilation, int n_out, int32_t* out_indices, int32_t* nbr_fwd, int32_t* nbr_bwd,
-                              int32_t* pair_num, void* ws, size_t ws_bytes, cudaStream_t stream, int phases);
-// where a strided conv's output bitmap and its ranks lie: in the workspace of vc_conv_rulebook_count (conv_rank_of) or in
-// that of a chain of strided convs (conv_chain_rank)
+// where a strided conv's output bitmap and its ranks lie in the workspace of its chain (conv_chain_rank)
 struct ConvRank {
     const uint32_t *bitmap, *word_rank, *block_sum;
 };
-ConvRank conv_rank_of(int ndim, int batch_size, const int32_t* out_shape, const void* ws);
-// nbr_fwd (-1 filled here) / nbr_bwd / pair counts of one strided conv from its ranked output bitmap
-int conv_rulebook_tables_dev(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size, const int32_t* spatial_shape,
-                             const int32_t* ksize, const int32_t* stride, const int32_t* padding, const int32_t* dilation, int n_out,
-                             ConvRank rank, int32_t* nbr_fwd, int32_t* nbr_bwd, int32_t* pair_num, cudaStream_t stream);
-// L chained strided convs (rulebook.cu header: each level's input set is the previous level's output set): every level's
-// output set from the first input set, in one mark + scan pass and one emit
+// L chained strided convs (rulebook.cu header: each level's input set is the previous level's output set; a single strided
+// conv is a chain of one): every level's output set from the first input set, in one mark + scan pass and one emit
 constexpr int CONV_CHAIN_MAX = 4;
 struct ConvChain {
     int L, ndim, batch;
     const int32_t* shape0;   // input spatial shape of level 0; level l + 1's is level l's output shape
     const int32_t *ksize[CONV_CHAIN_MAX], *stride[CONV_CHAIN_MAX], *pad[CONV_CHAIN_MAX], *dil[CONV_CHAIN_MAX];
 };
-bool conv_chain_composable(const ConvChain& ch);   // dilation 1 everywhere (the rule needs it), 2 <= L <= CONV_CHAIN_MAX
+bool conv_chain_composable(const ConvChain& ch);   // 1 <= L <= CONV_CHAIN_MAX, dilation 1 everywhere when L >= 2
 size_t conv_chain_ws_bytes(const ConvChain& ch);
 ConvRank conv_chain_rank(const ConvChain& ch, const void* ws, int level);
 // n_out_dev [L]: each level's row count; caps (NULL: no clamp) [L]: capacities, a larger count is clamped and reported
@@ -139,7 +125,7 @@ int conv_chain_count_dev(const ConvChain& ch, const int32_t* indices, int n, con
 int conv_chain_emit_dev(const ConvChain& ch, int32_t* const* out_idx, const int* caps, void* ws, size_t ws_bytes, cudaStream_t stream);
 
 // The per-stage index work of up to IDX_BATCH_MAX stages, one launch per kind (rulebook.cu, misc.cu): the same results as
-// one call per stage (subm_rulebook_dev and conv_rulebook_tables_dev are batches of one).  The caller owns the buffers and
+// one call per stage (subm_rulebook_dev and vc_conv_rulebook_fill are batches of one).  The caller owns the buffers and
 // clears them first (so that the regions of all stages can be cleared together): hash tables to 0xFF, a mirrored table's
 // rows k > centre to -1, pair counts to 0, nbr_fwd to -1.
 constexpr int IDX_BATCH_MAX = 4;
@@ -156,7 +142,7 @@ struct SubmStage {   // one submanifold rulebook (subm_rulebook_dev); table: vc_
     int32_t* rep;    // optional [n]: lowest row at each row's coordinate (the stage then probes every offset)
 };
 int subm_rulebook_batch_dev(const SubmStage* st, int n_st, int batch_size, bool unique, cudaStream_t stream);
-struct TablesStage {  // one strided conv's tables (conv_rulebook_tables_dev)
+struct TablesStage {  // one strided conv's tables (nbr_bwd, pair counts, nbr_fwd scattered from the input rows)
     const int32_t* idx;
     int n;
     const int* n_dev;

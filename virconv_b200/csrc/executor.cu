@@ -316,8 +316,7 @@ struct FwdCtx : Ctx {
     bool do_idx, do_feat, two;   // do_idx / do_feat: enqueue the index / feature operators (both unless phased)
     bool idx_first;              // the whole index phase is enqueued before this walk: no index kernel runs beside a conv
     bool batched[MAX_OPS];       // op enqueued by a batched call of its chain (fwd_chain_tables, fwd_chain_stages)
-    // per strided conv op: where its ranked output bitmap lies (for the tables); done: count and indices are enqueued
-    struct { ConvRank rank; bool done; } chain[MAX_OPS];
+    ConvRank rank[MAX_I];        // per index set a strided conv wrote: where its ranked output bitmap lies (for the tables)
     template <class T>
     void produced(T& r, int s) {   // r was written on stream s: consumers on the other streams wait for r.ev
         r.prod = s;
@@ -406,59 +405,6 @@ int fwd_subm_rb(FwdCtx& C, int i, const int* o, int s) {
     return VC_OK;
 }
 
-// count + row-count read-back + output indices of strided conv op j (its input index set must exist)
-int fwd_conv_count(FwdCtx& C, int j) {
-    const int* o = C.op(j);
-    const int s = C.two ? o[F_STREAM] : 0;
-    cudaStream_t st = C.st[s];
-    ISet& I = C.S->iset[o[F_A]];
-    ISet& O = C.S->iset[o[F_B]];
-    RBk& R = C.S->rb[o[F_C]];
-    VC_CHECK_ARG(I.ndim == o[F_NDIM], "op %d: index set %d has the wrong ndim", j, o[F_A]);
-    VC_TRY(wait_for(C, I.ev, I.prod, s));
-    int32_t oshape[3] = {0, 0, 0};
-    VC_TRY(vc_conv_out_shape(I.ndim, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL, oshape));
-    const size_t wsb = vc_conv_rulebook_ws_bytes(I.ndim, C.S->batch_size, oshape);
-    VC_ALLOC(ws, void*, wsb);
-    VC_ALLOC(n_dev, int32_t*, 4);
-    int n_out;
-    if (C.S->is_static) {
-        n_out = C.caps[o[F_B]];
-        VC_CHECK_ARG(n_out > 0, "op %d: static mode needs a capacity for index set %d", j, o[F_B]);
-        if (C.do_idx)
-            VC_TRY(conv_rulebook_count_dev(I.idx, I.n, I.n_dev, I.ndim, C.S->batch_size, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL,
-                                           n_dev, n_out, C.overflow, ws, wsb, st));
-    } else {
-        VC_TRY(conv_rulebook_count_dev(I.idx, I.n, nullptr, I.ndim, C.S->batch_size, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL,
-                                       n_dev, 0, nullptr, ws, wsb, st));
-        VC_CUDA(cudaMemcpyAsync(C.pinned + (C.n_syncs & 7), n_dev, 4, cudaMemcpyDeviceToHost, st));
-        // the tensor-core kernels' pipeline-timeout flag rides along with the first read-back of a step (it reports on the
-        // kernels of EARLIER steps: a wedged mbarrier wait must not go unnoticed in production — ADVICE r1)
-        if (C.n_syncs == 0 && C.err != nullptr) VC_CUDA(cudaMemcpyAsync(C.pinned + 15, C.err, 4, cudaMemcpyDeviceToHost, st));
-        VC_CUDA(cudaStreamSynchronize(st));        // the one data-dependent size per strided conv
-        n_out = C.pinned[C.n_syncs & 7];
-        if (C.n_syncs == 0 && C.err != nullptr && C.pinned[15] != 0) {
-            set_error("a tensor-core kernel's pipeline wait timed out in an earlier step (error flag %d): its results are invalid",
-                      C.pinned[15]);
-            return VC_ERR_PIPELINE;
-        }
-        ++C.n_syncs;
-    }
-    R.n_in = I.n; R.n_out = n_out;
-    R.n_in_dev = I.n_dev; R.n_out_dev = C.S->is_static ? n_dev : nullptr;
-    O.n = n_out; O.ndim = I.ndim; O.n_dev = R.n_out_dev;
-    for (int d = 0; d < 3; ++d) O.shape[d] = oshape[d];
-    VC_ALLOC(oidx, int32_t*, (size_t)(n_out > 0 ? n_out : 1) * (1 + I.ndim) * 4);
-    O.idx = oidx;
-    if (C.S->is_static && C.do_idx) VC_CUDA(cudaMemsetAsync(oidx, 0xFF, (size_t)n_out * (1 + I.ndim) * 4, st));   // defined tail (-1) for the published indices
-    if (C.do_idx)
-        VC_TRY(conv_rulebook_fill_phases(I.idx, I.n, I.n_dev, I.ndim, C.S->batch_size, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL,
-                                         n_out, O.idx, nullptr, nullptr, nullptr, ws, wsb, st, 1));
-    C.produced(O, s);
-    C.chain[j] = {conv_rank_of(I.ndim, C.S->batch_size, oshape, ws), true};
-    return VC_OK;
-}
-
 double op_rate(const int* o) {   // the float64 rate of a DISCARD op, stored as two int32 halves
     const uint64_t bits = (uint64_t)(uint32_t)o[F_KS] | ((uint64_t)(uint32_t)o[F_KS + 1] << 32);
     double r;
@@ -498,14 +444,14 @@ int fwd_discard_keep(FwdCtx& C, int j) {
     O.idx = oidx; O.n = k; O.ndim = I.ndim; O.n_dev = C.S->is_static ? kept_dev : nullptr;
     for (int d = 0; d < 3; ++d) O.shape[d] = I.shape[d];
     C.produced(O, s);
-    C.chain[j].done = true;
     return VC_OK;
 }
 
-// DISCARD op i: its index part (unless the strided convs' chain ran it), then the feature gather on the main stream — the
-// kept fp32 rows (the published x_conv*) and their bf16 rounding (the next down conv's operand), zero tail in static mode
+// DISCARD op i: its index part (unless the first strided conv's read-backs ran it), then the feature gather on the main
+// stream — the kept fp32 rows (the published x_conv*) and their bf16 rounding (the next down conv's operand), zero tail in
+// static mode
 int fwd_discard(FwdCtx& C, int i, const int* o) {
-    if (!C.chain[i].done) VC_TRY(fwd_discard_keep(C, i));
+    if (!C.S->iset[o[F_B]].idx) VC_TRY(fwd_discard_keep(C, i));
     const Disc& D = C.S->disc[i];
     ISet& O = C.S->iset[o[F_B]];
     FSlot& X = C.S->f[o[F_CIN]];
@@ -555,10 +501,10 @@ int fwd_chain_tables(FwdCtx& C, const int* ops, int L, int s) {
         R.nbr = fwd_all + fo; R.nbr_bwd = nbr_bwd; R.pair_num = pn_all + po;
         fo += R.K * (R.n_out > 0 ? R.n_out : 1);
         po += R.K;
-        ts[l] = TablesStage{I.idx, I.n, I.n_dev, I.ndim, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL, R.n_out, C.chain[ops[l]].rank,
+        ts[l] = TablesStage{I.idx, I.n, I.n_dev, I.ndim, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL, R.n_out, C.rank[o[F_B]],
                             l == 0 ? R.nbr : nullptr, R.nbr_bwd, R.pair_num};
         if (l > 0)
-            fs[l - 1] = FwdLookupStage{C.S->iset[o[F_B]].idx, R.n_out, R.n_out_dev, I.n, I.n_dev, C.chain[ops[l - 1]].rank, I.ndim,
+            fs[l - 1] = FwdLookupStage{C.S->iset[o[F_B]].idx, R.n_out, R.n_out_dev, I.n, I.n_dev, C.rank[o[F_A]], I.ndim,
                                        I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL, R.nbr};
         C.batched[ops[l]] = true;
     }
@@ -567,7 +513,7 @@ int fwd_chain_tables(FwdCtx& C, const int* ops, int L, int s) {
         VC_CUDA(cudaMemsetAsync(pn_all, 0, pn_ints * 4, C.st[s]));
         VC_CUDA(cudaMemsetAsync(fwd_all, 0xFF, (size_t)R0.K * R0.n_out * 4, C.st[s]));
         VC_TRY(conv_tables_batch_dev(ts, L, C.S->batch_size, C.st[s]));
-        VC_TRY(conv_fwd_lookup_batch_dev(fs, L - 1, C.S->batch_size, C.st[s]));
+        if (L > 1) VC_TRY(conv_fwd_lookup_batch_dev(fs, L - 1, C.S->batch_size, C.st[s]));
     }
     RBk& R0 = C.S->rb[C.op(ops[0])[F_C]];
     C.produced(R0, s);   // one event for the batch
@@ -635,9 +581,7 @@ int fwd_chain_stages(FwdCtx& C, int i0, const int* ops, int L) {
         VC_ALLOC(nbr, int32_t*, (size_t)R.K * I.n * 4);
         R.nbr = nbr; R.pair_num = pn;
         pn += R.K;
-        int l = 0;
-        while (C.op(ops[l])[F_B] != o[F_A]) ++l;
-        st3[a] = SubmLookupStage{I.idx, I.n, I.n_dev, I.ndim, I.shape, o + F_KS, o + F_DL, C.chain[ops[l]].rank, R.nbr, R.pair_num};
+        st3[a] = SubmLookupStage{I.idx, I.n, I.n_dev, I.ndim, I.shape, o + F_KS, o + F_DL, C.rank[o[F_A]], R.nbr, R.pair_num};
         C.batched[sub3[a]] = true;
     }
     if (n3) {
@@ -707,27 +651,39 @@ int fwd_chain_stages(FwdCtx& C, int i0, const int* ops, int L) {
     return VC_OK;
 }
 
-// The strided convs chained from op i (each one's input set is the previous one's output set, no layer discard in the plan
-// between them): every level's count and output indices in one composed pass (rulebook.cu), one host read in exact mode.
-// Leaves C.chain[i].done unset where the rule does not apply (a single conv, a dilation); the caller then takes the
-// per-level path.
-int fwd_conv_chain(FwdCtx& C, int i) {
+// The chain of strided convs from op i (rulebook.cu header): op i and the strided convs after it that each read the
+// previous one's output set, up to CONV_CHAIN_MAX and no further than a layer discard; a dilated conv is a chain of its own.
+// A function of the plan alone.  -> L, the chain's ops and geometry
+int chain_from(const FwdCtx& C, int i, int* ops, ConvChain& ch) {
     const int* o0 = C.op(i);
-    ISet& I = C.S->iset[o0[F_A]];
-    int ops[CONV_CHAIN_MAX];
-    ConvChain ch{};
+    ch = ConvChain{};
+    ch.ndim = o0[F_NDIM]; ch.batch = C.S->batch_size; ch.shape0 = C.S->iset[o0[F_A]].shape;
     for (int j = i, cur = o0[F_A]; j < C.n_ops && ch.L < CONV_CHAIN_MAX; ++j) {
         const int* o = C.op(j);
         if (o[F_KIND] == OP_DISCARD) break;
         if (o[F_KIND] != OP_CONV_RB) continue;
-        if (o[F_A] != cur || o[F_NDIM] != o0[F_NDIM] || C.chain[j].done) break;
-        ops[ch.L] = j;
-        ch.ksize[ch.L] = o + F_KS; ch.stride[ch.L] = o + F_ST; ch.pad[ch.L] = o + F_PD; ch.dil[ch.L] = o + F_DL;
-        ++ch.L;
+        if (o[F_A] != cur || o[F_NDIM] != o0[F_NDIM]) break;
+        const int l = ch.L++;
+        ch.ksize[l] = o + F_KS; ch.stride[l] = o + F_ST; ch.pad[l] = o + F_PD; ch.dil[l] = o + F_DL;
+        if (!conv_chain_composable(ch)) {   // a dilated level, or one after a dilated level 0
+            --ch.L;
+            break;
+        }
+        ops[l] = j;
         cur = o[F_B];
     }
-    ch.ndim = I.ndim; ch.batch = C.S->batch_size; ch.shape0 = I.shape;
-    if (!I.idx || I.ndim != o0[F_NDIM] || !conv_chain_composable(ch)) return VC_OK;
+    return ch.L;
+}
+
+// count + row-count read-back + output indices of the chain from op i: every level's count and output indices in one
+// composed pass (rulebook.cu), one host read of all of them in exact mode
+int fwd_chain_count(FwdCtx& C, int i) {
+    const int* o0 = C.op(i);
+    ISet& I = C.S->iset[o0[F_A]];
+    VC_CHECK_ARG(I.idx && I.ndim == o0[F_NDIM], "op %d: index set %d not built / wrong ndim", i, o0[F_A]);
+    int ops[CONV_CHAIN_MAX];
+    ConvChain ch;
+    chain_from(C, i, ops, ch);
     const int s = C.two ? o0[F_STREAM] : 0;
     cudaStream_t st = C.st[s];
     VC_TRY(wait_for(C, I.ev, I.prod, s));
@@ -746,7 +702,8 @@ int fwd_conv_chain(FwdCtx& C, int i) {
     } else {
         VC_TRY(conv_chain_count_dev(ch, I.idx, I.n, nullptr, n_dev, nullptr, nullptr, ws, wsb, st));
         VC_CUDA(cudaMemcpyAsync(C.pinned + 8, n_dev, 4 * ch.L, cudaMemcpyDeviceToHost, st));
-        // (the pipeline-timeout flag rides along with the first read-back of a step, as in fwd_conv_count)
+        // the tensor-core kernels' pipeline-timeout flag rides along with the first read-back of a step (it reports on the
+        // kernels of EARLIER steps: a wedged mbarrier wait must not go unnoticed in production — ADVICE r1)
         if (C.n_syncs == 0 && C.err != nullptr) VC_CUDA(cudaMemcpyAsync(C.pinned + 15, C.err, 4, cudaMemcpyDeviceToHost, st));
         VC_CUDA(cudaStreamSynchronize(st));        // the data-dependent sizes of all the chain's convs at once
         for (int l = 0; l < ch.L; ++l) n_out[l] = C.pinned[8 + l];
@@ -771,52 +728,38 @@ int fwd_conv_chain(FwdCtx& C, int i) {
         VC_ALLOC(oi, int32_t*, (size_t)(n_out[l] > 0 ? n_out[l] : 1) * (1 + In.ndim) * 4);
         O.idx = oidx[l] = oi;
         if (C.S->is_static && C.do_idx) VC_CUDA(cudaMemsetAsync(oi, 0xFF, (size_t)n_out[l] * (1 + In.ndim) * 4, st));
-        C.chain[ops[l]] = {conv_chain_rank(ch, ws, l), true};
+        C.rank[o[F_B]] = conv_chain_rank(ch, ws, l);
     }
     if (C.do_idx) VC_TRY(conv_chain_emit_dev(ch, oidx, n_out, ws, wsb, st));
     for (int l = 0; l < ch.L; ++l) C.produced(C.S->iset[C.op(ops[l])[F_B]], s);
-    VC_TRY(fwd_chain_tables(C, ops, ch.L, s));
-    return fwd_chain_stages(C, i, ops, ch.L);
+    return VC_OK;
 }
 
 int fwd_conv_rb(FwdCtx& C, int i, const int* o, int s) {
-    // First strided conv reached: the strided convs chained from it get their counts and output indices from one composed
-    // pass (fwd_conv_chain).  Where the chain rule does not apply (a layer discard between two strided convs, a dilation, a
-    // single conv), the loop below builds them level by level: the count -> (host reads the row count) -> emit-indices
-    // chain of EVERY strided conv of the plan, back to back.  Each link only needs the previous link's output indices, and
-    // it is the only part of the forward the host has to wait for; the neighbour tables, submanifold rulebooks and
-    // projections queue up behind it without further synchronisation.
-    if (!C.chain[i].done) VC_TRY(fwd_conv_chain(C, i));
-    if (!C.chain[i].done) {
+    // First strided conv reached.  In exact mode the host reads here the row counts of EVERY chain of strided convs in the
+    // plan, back to back: each chain's count -> (host read) -> emit, and the row selection of each layer discard between
+    // chains (the next count reads its rows), in plan order.  That is the only part of the forward the host has to wait
+    // for, and each read waits for counting work only; the neighbour tables, submanifold rulebooks and projections queue up
+    // behind it without further synchronisation.  Static mode reads nothing on the host, so it keeps the natural order
+    // (count -> indices -> tables per chain): the tables of an early chain do not queue behind the counting of later ones.
+    if (!C.S->iset[o[F_B]].idx) {
         if (C.S->is_static) {
-            // no host read to wait for: keep the natural order (count -> indices -> tables per stage), so the tables of an
-            // early stage are not queued behind the counting kernels of all later ones
-            VC_TRY(fwd_conv_count(C, i));
+            VC_TRY(fwd_chain_count(C, i));
         } else {
-            // (a layer discard between two strided convs selects its rows in the same chain: the next count reads them)
             for (int j = i; j < C.n_ops; ++j) {
                 const int* oj = C.op(j);
-                if (oj[F_KIND] == OP_CONV_RB && C.S->iset[oj[F_A]].idx) VC_TRY(fwd_conv_count(C, j));
-                else if (oj[F_KIND] == OP_DISCARD && !C.chain[j].done && C.S->iset[oj[F_A]].idx) VC_TRY(fwd_discard_keep(C, j));
+                if ((oj[F_KIND] != OP_CONV_RB && oj[F_KIND] != OP_DISCARD) || C.S->iset[oj[F_B]].idx || !C.S->iset[oj[F_A]].idx)
+                    continue;
+                VC_TRY(oj[F_KIND] == OP_CONV_RB ? fwd_chain_count(C, j) : fwd_discard_keep(C, j));
             }
         }
     }
-    VC_CHECK_ARG(C.chain[i].done, "op %d: index set %d not built", i, o[F_A]);
-    if (C.batched[i]) return VC_OK;
-    ISet& I = C.S->iset[o[F_A]];
-    ISet& O = C.S->iset[o[F_B]];
-    RBk& R = C.S->rb[o[F_C]];
-    VC_TRY(wait_for(C, I.ev, I.prod, s));
-    VC_TRY(wait_for(C, O.ev, O.prod, s));
-    VC_ALLOC(nbr, int32_t*, (size_t)R.K * (R.n_out > 0 ? R.n_out : 1) * 4);
-    VC_ALLOC(nbr_bwd, int32_t*, (size_t)R.K * I.n * 4);
-    VC_ALLOC(pn, int32_t*, (size_t)R.K * 4);
-    R.nbr = nbr; R.nbr_bwd = nbr_bwd; R.pair_num = pn;
-    if (C.do_idx)
-        VC_TRY(conv_rulebook_tables_dev(I.idx, I.n, I.n_dev, I.ndim, C.S->batch_size, I.shape, o + F_KS, o + F_ST, o + F_PD, o + F_DL,
-                                        R.n_out, C.chain[i].rank, R.nbr, R.nbr_bwd, R.pair_num, C.st[s]));
-    C.produced(R, s);
-    return VC_OK;
+    VC_CHECK_ARG(C.S->iset[o[F_B]].idx, "op %d: index set %d not built", i, o[F_A]);
+    int ops[CONV_CHAIN_MAX];
+    ConvChain ch;
+    const int L = chain_from(C, i, ops, ch);
+    VC_TRY(fwd_chain_tables(C, ops, L, s));
+    return fwd_chain_stages(C, i, ops, L);
 }
 
 int fwd_index2uv(FwdCtx& C, int i, const int* o, int s) {

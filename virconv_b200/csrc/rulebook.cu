@@ -8,25 +8,29 @@
 //   hash      2^h x uint64, entry = (linear_key << 24) | row, EMPTY = ~0   (ws of vc_subm_rulebook)
 //   nbr       [K, N_out] int32 — row o of offset-plane k is written by thread o: fully coalesced
 //   bitmap    1 bit per OUTPUT cell (batch-major linear index), + per-word exclusive popcount rank
-//             (ws of vc_conv_rulebook_*) — gives the sorted, duplicate-free output set with no sort, and a cell's row in
-//             it by one bit test and one rank (the neighbour tables over a chain level's output set: no hash table).
+//             (ws of a chain of strided convs, vc_conv_rulebook_*) — gives the sorted, duplicate-free output set with
+//             no sort, and a cell's row in it by one bit test and one rank (the neighbour tables over a chain level's
+//             output set: no hash table).
 // Roofline: all kernels here are HBM/L2-latency bound integer work (no FLOPs); algorithmic bytes per
 // input voxel are stated in DESIGN.md §kernels.
 //
-// Chained strided convs (conv_chain_*): L <= 4 regular convs where each one's input set is the previous one's output set
-// (no layer discard between them).  Their output sets are built from the FIRST input set in one pass instead of L
-// dependent count -> scan -> emit rounds.  Composition rule: with dilation 1, input coordinate c reaches output coordinate o
+// Every strided conv is built as a chain (conv_chain_*): 1 <= L <= 4 regular convs where each one's input set is the
+// previous one's output set (no layer discard between them); a single strided conv is a chain of one.  Their output sets
+// are built from the FIRST input set in one pass instead of L dependent count -> scan -> emit rounds.  Composition rule:
+// with dilation 1, input coordinate c reaches output coordinate o
 // of a level exactly when o * stride lies in [c + pad - (ksize - 1), c + pad] and 0 <= o < oshape, and the grid test and
 // the window factor per dimension (the batch index passes through).  So the level-1 cells reached from one input voxel are
 // a product of per-dimension integer intervals; the cells reached from an interval [lo, hi] are again one interval
 // (c + pad - off covers [lo + pad - ksize + 1, hi + pad] without a hole, so every multiple of the stride in it is hit), and
 // the union over a product of intervals is the product of the per-dimension unions.  Level l's output set is therefore the
 // union over input voxels of one product of intervals, computed level by level from the voxel's own coordinates: exactly
-// the set the per-level chain builds from the previous level's emitted indices, marked into the same bitmap and ranked in
-// the same order (so every index set, count and table is bit-identical).  One exception, only when a capacity is too small:
-// the per-level chain derives level l + 1 from the first `cap` rows of an overflowing level l, the composed pass from all of
-// its cells, so the counts of the levels AFTER the first overflowing one may be larger (the overflow is reported either way
-// and such a step is recomputed with larger capacities).
+// the set the level-by-level definition (oracle/rulebook.py) builds from the previous level's output indices, in the same
+// ascending cell order (so every index set, count and table is bit-identical); with L = 1 the rule IS that definition.  A
+// dilation leaves holes in a level's window, so the rule needs dilation 1 at every level of a chain of two or more; a
+// dilated strided conv is a chain of one, its level 0 marked cell by cell per kernel offset (out_cell).  One exception,
+// only when a capacity is too small: the level-by-level definition derives level l + 1 from the first `cap` rows of an
+// overflowing level l, the composed pass from all of its cells, so the counts of the levels AFTER the first overflowing one
+// may be larger (the overflow is reported either way and such a step is recomputed with larger capacities).
 #include "common.cuh"
 
 namespace vc {
@@ -218,16 +222,8 @@ __device__ __forceinline__ long long out_cell(const Geom& g, int b, const int* c
     return lin;
 }
 
-__global__ void conv_mark_kernel(const int32_t* __restrict__ idx, int n, const int* __restrict__ n_dev, Geom g,
-                                 uint32_t* bitmap) {   // grid (rows, K)
-    if (n_dev != nullptr) n = min(n, __ldg(n_dev));
-    int row = blockIdx.x * blockDim.x + threadIdx.x;
-    if (row >= n) return;
-    int b, c[VC_MAX_NDIM];
-    load_index(idx, row, g.ndim, b, c);
-    long long lin = out_cell(g, b, c, blockIdx.y);
-    if (lin < 0) return;
-    uint32_t bit = 1u << (lin & 31);
+__device__ __forceinline__ void mark_cell(uint32_t* bitmap, long long lin) {
+    const uint32_t bit = 1u << (lin & 31);
     uint32_t* w = bitmap + (lin >> 5);
     if (!(*w & bit)) atomicOr(w, bit);
 }
@@ -303,11 +299,6 @@ __device__ __forceinline__ void scan_segment(uint32_t* block_sum, int n_blocks, 
     }
 }
 
-__global__ void __launch_bounds__(1024) scan_blocks_kernel(uint32_t* block_sum, int n_blocks, int32_t* n_out, int cap,
-                                                           int* overflow) {
-    scan_segment(block_sum, n_blocks, n_out, cap, overflow);
-}
-
 // Rows of the cells along one x run of a ranked set of which the first n rows are held: a cell's row is its rank, or -1
 // when the cell is not in the set or ranks past the held rows (static mode: an overflowing level holds its first `cap`
 // cells only).  Successive cells of a run mostly share a bitmap word: the word and its rank are loaded together, once per
@@ -338,36 +329,12 @@ __device__ __forceinline__ void count_pairs(int* cnt, int k, bool hit) {
     if ((threadIdx.x & 31) == 0 && m) atomicAdd(&cnt[k], __popc(m));
 }
 
-__global__ void conv_emit_indices_kernel(const uint32_t* __restrict__ bitmap, const uint32_t* __restrict__ word_rank,
-                                         const uint32_t* __restrict__ block_sum, long long n_words, Geom g,
-                                         int32_t* __restrict__ out_idx, int cap) {
-    long long w = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (w >= n_words) return;
-    uint32_t word = bitmap[w];
-    if (!word) return;
-    int row = (int)(block_sum[w / SCAN_WORDS] + word_rank[w]);
-    while (word) {
-        int bit = __ffs(word) - 1;
-        word &= word - 1;
-        if (row >= cap) return;           // capacity overflow (flagged by scan_blocks_kernel)
-        long long lin = (w << 5) + bit;
-        int c[VC_MAX_NDIM];
-        for (int d = g.ndim - 1; d >= 0; --d) {
-            c[d] = (int)(lin % g.oshape[d]);
-            lin /= g.oshape[d];
-        }
-        int32_t* o = out_idx + (size_t)row * (1 + g.ndim);
-        o[0] = (int32_t)lin;
-        for (int d = 0; d < g.ndim; ++d) o[1 + d] = c[d];
-        ++row;
-    }
-}
-
 // chained strided convs (file header): per level the geometry, where its bitmap / ranks start in the concatenated
 // workspace (w0 words, b0 scan blocks: every level starts on a SCAN_WORDS boundary, so a scan block never spans two
 // levels), and for the emit its output buffer and capacity.  Passed by value.
 struct ChainDesc {
     int L;
+    int dilated;   // level 0 has a dilation (then L = 1)
     Geom g[CONV_CHAIN_MAX];
     long long w0[CONV_CHAIN_MAX + 1];
     int b0[CONV_CHAIN_MAX + 1];
@@ -375,9 +342,8 @@ struct ChainDesc {
     int cap[CONV_CHAIN_MAX];
 };
 
-// The chain's kernels overload the per-level ones they stand for (conv_mark / scan_blocks / conv_emit_indices), so that a
-// profile names them alike.
-// grid (rows, L): the cells of level blockIdx.y reached from one input row, the product of its per-dimension intervals
+// grid (rows, L): the cells of level blockIdx.y reached from one input row, the product of its per-dimension intervals.
+// A dilated level 0: grid (rows, K), the cell of kernel offset blockIdx.y.
 __global__ void conv_mark_kernel(const int32_t* __restrict__ idx, int n, const int* __restrict__ n_dev, ChainDesc cd,
                                   uint32_t* bitmap) {
     if (n_dev != nullptr) n = min(n, __ldg(n_dev));
@@ -386,6 +352,11 @@ __global__ void conv_mark_kernel(const int32_t* __restrict__ idx, int n, const i
     const int level = blockIdx.y;
     int b, lo[VC_MAX_NDIM], hi[VC_MAX_NDIM];
     load_index(idx, row, cd.g[0].ndim, b, lo);
+    if (cd.dilated) {
+        const long long lin = out_cell(cd.g[0], b, lo, blockIdx.y);
+        if (lin >= 0) mark_cell(bitmap, lin);
+        return;
+    }
     if (!index_ok(cd.g[0], b, lo)) return;
     for (int d = 0; d < cd.g[0].ndim; ++d) hi[d] = lo[d];
     for (int l = 0; l <= level; ++l) {
@@ -406,9 +377,7 @@ __global__ void conv_mark_kernel(const int32_t* __restrict__ idx, int n, const i
     while (true) {
         long long lin = b;
         for (int d = 0; d < g.ndim; ++d) lin = lin * g.oshape[d] + c[d];
-        const uint32_t bit = 1u << (lin & 31);
-        uint32_t* w = bm + (lin >> 5);
-        if (!(*w & bit)) atomicOr(w, bit);
+        mark_cell(bm, lin);
         int d = g.ndim - 1;   // next cell of the product, last dimension fastest
         while (d >= 0 && c[d] == hi[d]) { c[d] = lo[d]; --d; }
         if (d < 0) break;
@@ -423,7 +392,7 @@ __global__ void __launch_bounds__(1024) scan_blocks_kernel(uint32_t* block_sum, 
         scan_segment(block_sum + cd.b0[l], cd.b0[l + 1] - cd.b0[l], n_out + l, cd.cap[l], overflow);
 }
 
-// one thread per word of all levels (conv_emit_indices_kernel over the level the word belongs to)
+// one thread per word of all levels: the output indices of the word's set bits, in rank order
 __global__ void conv_emit_indices_kernel(const uint32_t* __restrict__ bitmap, const uint32_t* __restrict__ word_rank,
                                   const uint32_t* __restrict__ block_sum, ChainDesc cd) {
     const long long w = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -439,7 +408,7 @@ __global__ void conv_emit_indices_kernel(const uint32_t* __restrict__ bitmap, co
     while (word) {
         int bit = __ffs(word) - 1;
         word &= word - 1;
-        if (row >= cap) return;
+        if (row >= cap) return;           // capacity overflow (flagged by scan_blocks_kernel)
         long long lin = (wl << 5) + bit;
         int c[VC_MAX_NDIM];
         for (int d = g.ndim - 1; d >= 0; --d) {
@@ -777,128 +746,6 @@ extern "C" int vc_conv_out_shape(int ndim, const int32_t* spatial_shape, const i
     return VC_OK;
 }
 
-namespace {
-struct ConvWs {
-    long long n_words;
-    int n_blocks;
-    uint32_t *bitmap, *word_rank, *block_sum;
-    size_t bytes;
-};
-ConvWs conv_ws_layout(int ndim, int batch_size, const int32_t* oshape, void* ws) {
-    ConvWs w;
-    long long cells = batch_size;
-    for (int d = 0; d < ndim; ++d) cells *= oshape[d];
-    w.n_words = (cells + 31) / 32;
-    w.n_blocks = (int)((w.n_words + SCAN_WORDS - 1) / SCAN_WORDS);
-    size_t a = ((size_t)w.n_words * 4 + 255) / 256 * 256;
-    size_t b = ((size_t)w.n_blocks * 4 + 255) / 256 * 256;
-    char* p = (char*)ws;
-    w.bitmap = (uint32_t*)p;
-    w.word_rank = (uint32_t*)(p + a);
-    w.block_sum = (uint32_t*)(p + 2 * a);
-    w.bytes = 2 * a + b;
-    return w;
-}
-}  // namespace
-
-extern "C" size_t vc_conv_rulebook_ws_bytes(int ndim, int batch_size, const int32_t* out_shape) {
-    return conv_ws_layout(ndim, batch_size, out_shape, nullptr).bytes;
-}
-
-// cap_out > 0: the caller's output buffers hold cap_out rows (static mode): the count is clamped, *overflow gets the real total
-int vc::conv_rulebook_count_dev(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size,
-                                const int32_t* spatial_shape, const int32_t* ksize, const int32_t* stride,
-                                const int32_t* padding, const int32_t* dilation, int32_t* n_out_dev, int cap_out, int* overflow,
-                                void* ws, size_t ws_bytes, cudaStream_t stream) {
-    Geom g;
-    int rc = make_geom(g, ndim, batch_size, spatial_shape, ksize, stride, padding, dilation);
-    if (rc) return rc;
-    VC_CHECK_ARG(n >= 0 && n_out_dev && ws && batch_size > 0, "bad arguments");
-    ConvWs w = conv_ws_layout(ndim, batch_size, g.oshape, ws);
-    VC_CHECK_ARG(w.n_words < (1LL << 31), "output grid too large");
-    if (ws_bytes < w.bytes) {
-        set_error("conv rulebook workspace %zu < %zu", ws_bytes, w.bytes);
-        return VC_ERR_WORKSPACE;
-    }
-    VC_CUDA(cudaMemsetAsync(w.bitmap, 0, (size_t)w.n_words * 4, stream));
-    if (n > 0) {
-        conv_mark_kernel<<<dim3(cdiv(n, 256), g.K), 256, 0, stream>>>(indices, n, n_dev, g, w.bitmap);
-        VC_LAUNCH_CHECK();
-    }
-    scan_local_kernel<<<w.n_blocks, 256, 0, stream>>>(w.bitmap, w.n_words, w.word_rank, w.block_sum);
-    VC_LAUNCH_CHECK();
-    scan_blocks_kernel<<<1, 1024, 0, stream>>>(w.block_sum, w.n_blocks, n_out_dev, cap_out, overflow);
-    VC_LAUNCH_CHECK();
-    return VC_OK;
-}
-
-extern "C" int vc_conv_rulebook_count(const int32_t* indices, int n, int ndim, int batch_size,
-                                      const int32_t* spatial_shape, const int32_t* ksize, const int32_t* stride,
-                                      const int32_t* padding, const int32_t* dilation, int32_t* n_out_dev, void* ws,
-                                      size_t ws_bytes, vc_stream_t stream_) {
-    return vc::conv_rulebook_count_dev(indices, n, nullptr, ndim, batch_size, spatial_shape, ksize, stride, padding, dilation,
-                                       n_out_dev, 0, nullptr, ws, ws_bytes, (cudaStream_t)stream_);
-}
-
-extern "C" int vc_conv_rulebook_fill(const int32_t* indices, int n, int ndim, int batch_size,
-                                     const int32_t* spatial_shape, const int32_t* ksize, const int32_t* stride,
-                                     const int32_t* padding, const int32_t* dilation, int n_out, int32_t* out_indices,
-                                     int32_t* nbr_fwd, int32_t* nbr_bwd, int32_t* pair_num, void* ws, size_t ws_bytes,
-                                     vc_stream_t stream_) {
-    return vc::conv_rulebook_fill_phases(indices, n, nullptr, ndim, batch_size, spatial_shape, ksize, stride, padding, dilation, n_out,
-                                         out_indices, nbr_fwd, nbr_bwd, pair_num, ws, ws_bytes, (cudaStream_t)stream_, 3);
-}
-
-// phases: bit 0 = emit the output indices, bit 1 = build the neighbour tables.  The plan executor runs the emit phase of
-// every strided conv first (the next conv's row count depends on it and the host waits for that), the tables later.
-// (n_dev != NULL: n / n_out are the capacities of the input / output index sets, the real input count is *n_dev)
-int vc::conv_rulebook_fill_phases(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size, const int32_t* spatial_shape,
-                                  const int32_t* ksize, const int32_t* stride, const int32_t* padding,
-                                  const int32_t* dilation, int n_out, int32_t* out_indices, int32_t* nbr_fwd,
-                                  int32_t* nbr_bwd, int32_t* pair_num, void* ws, size_t ws_bytes, cudaStream_t stream,
-                                  int phases) {
-    Geom g;
-    int rc = make_geom(g, ndim, batch_size, spatial_shape, ksize, stride, padding, dilation);
-    if (rc) return rc;
-    ConvWs w = conv_ws_layout(ndim, batch_size, g.oshape, ws);
-    if (ws_bytes < w.bytes) {
-        set_error("conv rulebook workspace %zu < %zu", ws_bytes, w.bytes);
-        return VC_ERR_WORKSPACE;
-    }
-    if ((phases & 1) && n_out > 0) {
-        VC_CHECK_ARG(out_indices, "null output pointer");
-        conv_emit_indices_kernel<<<cdiv(w.n_words, 256), 256, 0, stream>>>(w.bitmap, w.word_rank, w.block_sum,
-                                                                            w.n_words, g, out_indices, n_out);
-        VC_LAUNCH_CHECK();
-    }
-    if (!(phases & 2)) return VC_OK;
-    return conv_rulebook_tables_dev(indices, n, n_dev, ndim, batch_size, spatial_shape, ksize, stride, padding, dilation, n_out,
-                                    ConvRank{w.bitmap, w.word_rank, w.block_sum}, nbr_fwd, nbr_bwd, pair_num, stream);
-}
-
-ConvRank vc::conv_rank_of(int ndim, int batch_size, const int32_t* out_shape, const void* ws) {
-    ConvWs w = conv_ws_layout(ndim, batch_size, out_shape, const_cast<void*>(ws));
-    return ConvRank{w.bitmap, w.word_rank, w.block_sum};
-}
-
-// one strided conv: its own clears, then a batch of one
-int vc::conv_rulebook_tables_dev(const int32_t* indices, int n, const int* n_dev, int ndim, int batch_size,
-                                 const int32_t* spatial_shape, const int32_t* ksize, const int32_t* stride, const int32_t* padding,
-                                 const int32_t* dilation, int n_out, ConvRank rank, int32_t* nbr_fwd, int32_t* nbr_bwd,
-                                 int32_t* pair_num, cudaStream_t stream) {
-    Geom g;
-    int rc = make_geom(g, ndim, batch_size, spatial_shape, ksize, stride, padding, dilation);
-    if (rc) return rc;
-    if (pair_num) VC_CUDA(cudaMemsetAsync(pair_num, 0, sizeof(int32_t) * g.K, stream));
-    if (n_out > 0) {
-        VC_CHECK_ARG(nbr_fwd, "null output pointer");
-        VC_CUDA(cudaMemsetAsync(nbr_fwd, 0xFF, (size_t)g.K * n_out * 4, stream));
-    }
-    const TablesStage s{indices, n, n_dev, ndim, spatial_shape, ksize, stride, padding, dilation, n_out, rank, nbr_fwd, nbr_bwd,
-                        pair_num};
-    return conv_tables_batch_dev(&s, 1, batch_size, stream);
-}
-
 bool vc::subm_sym(int ndim, const int32_t* ksize, bool unique) {
     bool sym = unique;
     for (int d = 0; d < ndim; ++d) sym &= (ksize[d] & 1) == 1;
@@ -1009,41 +856,43 @@ int vc::subm_lookup_batch_dev(const SubmLookupStage* st, int n_st, int batch_siz
 }
 
 namespace {
-// the chain's geometry and workspace layout: bitmap [W words], word ranks [W], block sums [B], W = cd.w0[L], B = cd.b0[L]
+// scan blocks of one level's bitmap: every level starts on a SCAN_WORDS boundary, so a scan block never spans two levels
+int level_blocks(int ndim, int batch, const int32_t* oshape) {
+    long long cells = batch;
+    for (int d = 0; d < ndim; ++d) cells *= oshape[d];
+    return (int)(((cells + 31) / 32 + SCAN_WORDS - 1) / SCAN_WORDS);
+}
+// the chain's workspace: bitmap [W words], word ranks [W], block sums [B], W = B * SCAN_WORDS, B = cd.b0[L]
+size_t chain_bytes(int blocks) { return (size_t)blocks * SCAN_WORDS * 8 + ((size_t)blocks * 4 + 255) / 256 * 256; }
 struct ChainWs {
     uint32_t *bitmap, *word_rank, *block_sum;
     size_t bytes;
 };
 int chain_layout(const ConvChain& ch, ChainDesc& cd, ChainWs& w, const void* ws) {
-    VC_CHECK_ARG(ch.L >= 1 && ch.L <= CONV_CHAIN_MAX, "chain of %d strided convs", ch.L);
+    VC_CHECK_ARG(conv_chain_composable(ch), "chain of %d strided convs (2 or more need dilation 1)", ch.L);
     memset(&cd, 0, sizeof(cd));
     cd.L = ch.L;
     const int32_t* shape = ch.shape0;
     for (int l = 0; l < ch.L; ++l) {
         int rc = make_geom(cd.g[l], ch.ndim, ch.batch, shape, ch.ksize[l], ch.stride[l], ch.pad[l], ch.dil[l]);
         if (rc) return rc;
-        for (int d = 0; d < ch.ndim; ++d) VC_CHECK_ARG(cd.g[l].dil[d] == 1, "chained strided convs need dilation 1");
         shape = cd.g[l].oshape;
-        long long cells = ch.batch;
-        for (int d = 0; d < ch.ndim; ++d) cells *= cd.g[l].oshape[d];
-        const long long words = (cells + 31) / 32;
-        const int blocks = (int)((words + SCAN_WORDS - 1) / SCAN_WORDS);
-        cd.b0[l + 1] = cd.b0[l] + blocks;
-        cd.w0[l + 1] = cd.w0[l] + (long long)blocks * SCAN_WORDS;
+        cd.b0[l + 1] = cd.b0[l] + level_blocks(ch.ndim, ch.batch, cd.g[l].oshape);
+        cd.w0[l + 1] = (long long)cd.b0[l + 1] * SCAN_WORDS;
     }
+    for (int d = 0; d < ch.ndim; ++d) cd.dilated |= cd.g[0].dil[d] != 1;
     VC_CHECK_ARG(cd.w0[ch.L] < (1LL << 31), "output grids too large");
-    const size_t a = ((size_t)cd.w0[ch.L] * 4 + 255) / 256 * 256, b = ((size_t)cd.b0[ch.L] * 4 + 255) / 256 * 256;
-    char* p = (char*)const_cast<void*>(ws);
-    w.bitmap = (uint32_t*)p;
-    w.word_rank = (uint32_t*)(p + a);
-    w.block_sum = (uint32_t*)(p + 2 * a);
-    w.bytes = 2 * a + b;
+    w.bitmap = (uint32_t*)const_cast<void*>(ws);
+    w.word_rank = w.bitmap + cd.w0[ch.L];
+    w.block_sum = w.word_rank + cd.w0[ch.L];
+    w.bytes = chain_bytes(cd.b0[ch.L]);
     return VC_OK;
 }
 }  // namespace
 
 bool vc::conv_chain_composable(const ConvChain& ch) {
-    if (ch.L < 2 || ch.L > CONV_CHAIN_MAX) return false;
+    if (ch.L < 1 || ch.L > CONV_CHAIN_MAX) return false;
+    if (ch.L == 1) return true;   // level 0 alone: a dilation is marked per kernel offset
     for (int l = 0; l < ch.L; ++l)
         for (int d = 0; d < ch.ndim; ++d)
             if (ch.dil[l][d] != 1) return false;
@@ -1077,7 +926,7 @@ int vc::conv_chain_count_dev(const ConvChain& ch, const int32_t* indices, int n,
     for (int l = 0; l < ch.L; ++l) cd.cap[l] = caps ? caps[l] : 0;
     VC_CUDA(cudaMemsetAsync(w.bitmap, 0, (size_t)cd.w0[ch.L] * 4, stream));
     if (n > 0) {
-        conv_mark_kernel<<<dim3(cdiv(n, 256), ch.L), 256, 0, stream>>>(indices, n, n_dev, cd, w.bitmap);
+        conv_mark_kernel<<<dim3(cdiv(n, 256), cd.dilated ? cd.g[0].K : ch.L), 256, 0, stream>>>(indices, n, n_dev, cd, w.bitmap);
         VC_LAUNCH_CHECK();
     }
     scan_local_kernel<<<cd.b0[ch.L], 256, 0, stream>>>(w.bitmap, cd.w0[ch.L], w.word_rank, w.block_sum);
@@ -1102,6 +951,47 @@ int vc::conv_chain_emit_dev(const ConvChain& ch, int32_t* const* out_idx, const 
     conv_emit_indices_kernel<<<cdiv(cd.w0[ch.L], 256), 256, 0, stream>>>(w.bitmap, w.word_rank, w.block_sum, cd);
     VC_LAUNCH_CHECK();
     return VC_OK;
+}
+
+// The per-operator strided conv: a chain of one.  The count leaves its ranked output bitmap in `ws`; the fill emits the
+// output indices and builds the tables from it.
+extern "C" size_t vc_conv_rulebook_ws_bytes(int ndim, int batch_size, const int32_t* out_shape) {
+    return chain_bytes(level_blocks(ndim, batch_size, out_shape));
+}
+
+extern "C" int vc_conv_rulebook_count(const int32_t* indices, int n, int ndim, int batch_size,
+                                      const int32_t* spatial_shape, const int32_t* ksize, const int32_t* stride,
+                                      const int32_t* padding, const int32_t* dilation, int32_t* n_out_dev, void* ws,
+                                      size_t ws_bytes, vc_stream_t stream_) {
+    const ConvChain ch{1, ndim, batch_size, spatial_shape, {ksize}, {stride}, {padding}, {dilation}};
+    return conv_chain_count_dev(ch, indices, n, nullptr, n_out_dev, nullptr, nullptr, ws, ws_bytes, (cudaStream_t)stream_);
+}
+
+extern "C" int vc_conv_rulebook_fill(const int32_t* indices, int n, int ndim, int batch_size,
+                                     const int32_t* spatial_shape, const int32_t* ksize, const int32_t* stride,
+                                     const int32_t* padding, const int32_t* dilation, int n_out, int32_t* out_indices,
+                                     int32_t* nbr_fwd, int32_t* nbr_bwd, int32_t* pair_num, void* ws, size_t ws_bytes,
+                                     vc_stream_t stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    const ConvChain ch{1, ndim, batch_size, spatial_shape, {ksize}, {stride}, {padding}, {dilation}};
+    Geom g;
+    int rc = make_geom(g, ndim, batch_size, spatial_shape, ksize, stride, padding, dilation);
+    if (rc) return rc;
+    const size_t need = conv_chain_ws_bytes(ch);
+    if (!ws || ws_bytes < need) {
+        set_error("conv rulebook workspace %zu < %zu", ws_bytes, need);
+        return VC_ERR_WORKSPACE;
+    }
+    if (n_out > 0) {
+        VC_CHECK_ARG(nbr_fwd, "null output pointer");
+        rc = conv_chain_emit_dev(ch, &out_indices, &n_out, ws, ws_bytes, stream);
+        if (rc) return rc;
+    }
+    if (pair_num) VC_CUDA(cudaMemsetAsync(pair_num, 0, sizeof(int32_t) * g.K, stream));
+    if (n_out > 0) VC_CUDA(cudaMemsetAsync(nbr_fwd, 0xFF, (size_t)g.K * n_out * 4, stream));
+    const TablesStage s{indices, n, nullptr, ndim, spatial_shape, ksize, stride, padding, dilation, n_out,
+                        conv_chain_rank(ch, ws, 0), nbr_fwd, nbr_bwd, pair_num};
+    return conv_tables_batch_dev(&s, 1, batch_size, stream);
 }
 
 extern "C" int vc_pairs_from_nbr(const int32_t* nbr, int K, int n, int32_t* pairs, int32_t* pair_num,

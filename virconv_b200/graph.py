@@ -34,6 +34,8 @@ static body and its own reaction to an overflow.
 """
 from __future__ import annotations
 
+import gc
+
 import torch
 
 from . import _lib, executor, ops, preprocess
@@ -400,10 +402,20 @@ class _Captured:
         lib = _lib.load()
         l0 = lib.vc_launch_count()
         graphs, outs = [], []
-        for body in bodies:
-            graphs.append(torch.cuda.CUDAGraph())
-            with torch.cuda.graph(graphs[-1]):
-                outs.append(body(batch))
+        # A CUDA graph destroyed during a capture invalidates it: torch frees a graph with CUDA calls that the capture mode
+        # refuses.  A graph of an earlier step left in an unreachable reference cycle is freed whenever the cyclic collector
+        # next runs, so collect such garbage here and keep the collector off until the captures end.
+        gc.collect()
+        gc_was_on = gc.isenabled()
+        gc.disable()
+        try:
+            for body in bodies:
+                graphs.append(torch.cuda.CUDAGraph())
+                with torch.cuda.graph(graphs[-1]):
+                    outs.append(body(batch))
+        finally:
+            if gc_was_on:
+                gc.enable()
         self.launches_per_replay = int(lib.vc_launch_count() - l0)     # this library's kernels inside one replay
         self.graphs = graphs
         self.recaptures += 1
