@@ -461,6 +461,17 @@ int vc_voxel_pool_bn_fold(int C, long long n, int training, const double* moment
                           double* stat, vc_stream_t stream);
 int vc_voxel_pool_bn_grad(int C, long long n, int training, const double* sums, const double* moments, const float* w_pos,
                           const float* gamma, const double* stat, float* dw, float* dgamma, float* dbeta, vc_stream_t stream);
+/* SyncBatchNorm2d as the position branch's BatchNorm over several ranks (train mode): the caller all-reduces
+ * [moments (9), n] (float64, n = the rank's M * nsample) and passes the sum as moments10 — statistics and the running update
+ * then come from the union of the ranks' slots.  vc_voxel_pool_bn_grad_sync: sums and moments are the rank's own, gsums
+ * [C, 4] the all-reduced sums and n_glob the all-reduced slot count (moments10[9]); the coupling term of dw takes the global
+ * mean of dy and of dy*xhat, dgamma / dbeta stay local (torch's SyncBatchNorm backward). */
+int vc_voxel_pool_bn_fold_sync(int C, int training, const double* moments10, const float* w_pos, const float* gamma,
+                               const float* beta, float* running_mean, float* running_var, long long* num_batches_tracked,
+                               double eps, double momentum, float* scale, float* shift, double* stat, vc_stream_t stream);
+int vc_voxel_pool_bn_grad_sync(int C, const double* n_glob, const double* sums, const double* gsums, const double* moments,
+                               const float* w_pos, const float* gamma, const double* stat, float* dw, float* dgamma,
+                               float* dbeta, vc_stream_t stream);
 int vc_voxel_pool_fwd(int M, int C, int nsample, const float* features_in, const float* xyz, const float* new_xyz,
                       const int32_t* idx, const unsigned char* empty_mask, const float* w_pos, const float* scale,
                       const float* shift, float* pooled, unsigned char* argmax, vc_stream_t stream);
@@ -806,6 +817,33 @@ int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, int n_ops, 
 int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_ops, const uint64_t* layer_ptrs, const float* layer_f,
                      int n_layers, const int32_t* pub_slots, const uint64_t* ext_grads, int n_pub, void* arena,
                      size_t arena_bytes, int32_t* err_flag, void* state, vc_stream_t stream, vc_stream_t wgrad_stream);
+/* SyncBatchNorm across ranks (torch.nn.SyncBatchNorm semantics; training mode only — eval uses the running statistics).
+ * vc_exec_forward_sync / vc_exec_backward_sync are vc_exec_forward_seeded / vc_exec_backward plus a caller-owned float64
+ * exchange buffer `xchg`, host slot offsets xchg_off [n_layers, 2] (in doubles: forward slot, backward slot of each layer)
+ * and a host callback.  With exchange_fn NULL (world size 1) they are the plain calls.  Otherwise every conv + BN layer runs
+ * conv with epilogue sums -> exchange -> BN apply (never the fused conv + BN launch), and its BN backward runs reduce ->
+ * exchange -> element-wise apply:
+ *   forward slot  [sum x (cout), sum x^2 (cout), row count] — the count written by a kernel (static mode: from the device
+ *                 count); after the exchange the statistics divide by the all-reduced count, the running statistics use it
+ *                 for the unbiased variance;
+ *   backward slot [sum g (cout), sum g*xhat (cout)] — the local d_gamma / d_beta are written before the exchange and stay
+ *                 local; dx takes the all-reduced sums and the forward slot's global count.
+ * exchange_fn(user, layer, direction 0 forward / 1 backward, slot, n doubles) is called on the host at each exchange point
+ * and must enqueue the in-place sum of the slot over all ranks on main_stream / `stream` (under CUDA-graph capture it runs
+ * once, at capture time); non-zero return fails the call.  Every rank makes the same calls in the same order.  In the
+ * deterministic mode the local sums keep their fixed order.  The backward reads the forward slots: same buffer. */
+typedef int (*vc_bn_exchange_fn)(void* user, int layer, int direction, double* slot, int n);
+int vc_exec_forward_sync(const int32_t* ops_i, const float* ops_f, int n_ops, const uint64_t* layer_ptrs, const float* layer_f,
+                         int n_layers, const float* feats0, int c0, const int32_t* idx0, int n0, const int32_t* shape0,
+                         int batch_size, const float* proj_params, int training, int precision, int flags, void* arena,
+                         size_t arena_bytes, int32_t* pinned_host, int32_t* err_flag, void* state, size_t state_bytes,
+                         vc_stream_t main_stream, vc_stream_t side_stream, int side_waits_main, const int32_t* caps,
+                         const int32_t* n0_dev, int32_t* overflow_flag, vc_stream_t side2_stream, const int64_t* rng_seed_dev,
+                         double* xchg, const int64_t* xchg_off /*host*/, vc_bn_exchange_fn exchange_fn, void* exchange_user);
+int vc_exec_backward_sync(const int32_t* ops_i, const float* ops_f, int n_ops, const uint64_t* layer_ptrs, const float* layer_f,
+                          int n_layers, const int32_t* pub_slots, const uint64_t* ext_grads, int n_pub, void* arena,
+                          size_t arena_bytes, int32_t* err_flag, void* state, vc_stream_t stream, vc_stream_t wgrad_stream,
+                          double* xchg, const int64_t* xchg_off, vc_bn_exchange_fn exchange_fn, void* exchange_user);
 /* Read a state blob.  what 0: out[0] = arena bytes in use, out[1] = of them, the deterministic mode's partials, tables and
  * operands, out[2] = deterministic mode;  1 (feature slot id): f32 ptr, bf16 ptr, rows, c, row pitch of f32 / bf16,
  * gradient ptr, row pitch of the gradient (after vc_exec_backward: the slot's final input gradient; a published slot no

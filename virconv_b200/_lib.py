@@ -21,6 +21,8 @@ _HOSTF = ctypes.POINTER(c_float)
 _HOSTD = ctypes.POINTER(c_double)
 _HOSTP = ctypes.POINTER(c_void_p)        # host array of device pointers
 _D = c_double
+# vc_bn_exchange_fn: (user, layer, direction, slot, n doubles) -> 0 on success
+EXCHANGE_FN = ctypes.CFUNCTYPE(c_int, c_void_p, c_int, c_int, c_void_p, c_int)
 
 # name -> (restype, argtypes).  Every symbol include/virconv_b200.h declares.
 SIGNATURES = {
@@ -104,6 +106,8 @@ SIGNATURES = {
     'vc_voxel_pool_bn_fold': (_I, [_I, ctypes.c_longlong, _I, _P, _P, _P, _P, _P, _P, _P, ctypes.c_double, ctypes.c_double,
                                    _P, _P, _P, _P]),
     'vc_voxel_pool_bn_grad': (_I, [_I, ctypes.c_longlong, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    'vc_voxel_pool_bn_fold_sync': (_I, [_I, _I, _P, _P, _P, _P, _P, _P, _P, ctypes.c_double, ctypes.c_double, _P, _P, _P, _P]),
+    'vc_voxel_pool_bn_grad_sync': (_I, [_I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'vc_voxel_pool_fwd': (_I, [_I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'vc_voxel_pool_bwd': (_I, [_I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'vc_voxel_pool_det_config': (_I, [_I]),
@@ -144,7 +148,10 @@ SIGNATURES = {
                              _P, _P, _P, _P]),
     'vc_exec_forward_seeded': (_I, [_P, _P, _I, _P, _P, _I, _P, _I, _P, _I, _HOST, _I, _P, _I, _I, _I, _P, _Z, _P, _P, _P, _Z, _P, _P,
                                     _I, _P, _P, _P, _P, _P]),
+    'vc_exec_forward_sync': (_I, [_P, _P, _I, _P, _P, _I, _P, _I, _P, _I, _HOST, _I, _P, _I, _I, _I, _P, _Z, _P, _P, _P, _Z, _P, _P,
+                                  _I, _P, _P, _P, _P, _P, _P, _P, EXCHANGE_FN, _P]),
     'vc_exec_backward': (_I, [_P, _P, _I, _P, _P, _I, _P, _P, _I, _P, _Z, _P, _P, _P, _P]),
+    'vc_exec_backward_sync': (_I, [_P, _P, _I, _P, _P, _I, _P, _P, _I, _P, _Z, _P, _P, _P, _P, _P, _P, EXCHANGE_FN, _P]),
     'vc_exec_query': (_I, [_P, _I, _I, _P]),
     'vc_exec_timing': (_I, [_I]),
     'vc_exec_timing_read': (_I, [_P, _P, _I]),

@@ -28,7 +28,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import executor, ops
+from . import executor, ops, sync_bn
 from . import spconv_compat as spconv
 
 
@@ -263,6 +263,18 @@ class _VirConvBackbone(nn.Module):
         keep = given[site] if given is not None else stvd_keep_rows(t.features.shape[0], self.layer_discard_rate)
         return discard_rows(t, keep)
 
+    # -- SyncBatchNorm (sync_bn): `bn_reducer` replaces the all-reduce of the exchanged BN sums ---------------------
+    bn_reducer = None
+
+    def _no_module_path_under_sync(self, plan, reason):
+        """SyncBatchNorm layers exchanging their sums: every rank must issue the same collectives in the same order.  A reason
+        that is the same on every rank (VIRCONV_EXECUTOR=0, host-drawn StVD, the module types) sends every rank to the module
+        path, where torch's SyncBatchNorm exchanges in step; a reason that depends on the rank's own batch or call raises
+        instead (the other ranks would wait for its plan's exchanges)."""
+        if reason in _RANK_DEPENDENT and sync_bn.active(self, [bn for _, bn in plan.layers]):
+            raise RuntimeError('VirConv backbone: SyncBatchNorm across ranks runs through the plan executor on every rank, and '
+                               'this forward cannot (%s)' % reason)
+
     # -- native plans (csrc/executor.cu): the whole forward / backward of a stream in one C-ABI call each ------
     def _cached_plan(self, attr, build):
         """The plan cached under `attr`, rebuilt by build() when there is none or it is stale (a sub-module was replaced after
@@ -301,7 +313,8 @@ class _VirConvBackbone(nn.Module):
         StaticSpec (capacity-sized feats / coords)."""
         ci = spconv._as_i32(coords)
         run, res = executor.run_plan(plan, feats, ci, shape, batch_size, proj, plan.layers[0][1].training,
-                                     plan.layers[0][0].precision, inputs_ready=inputs_ready, static=static, seed=seed)
+                                     plan.layers[0][0].precision, inputs_ready=inputs_ready, static=static, seed=seed,
+                                     reducer=sync_bn.reducer_for(self, [bn for _, bn in plan.layers]), tag=stream)
         # (graph.GraphedStep sizes each stream's capacities from an exact run.)  The default stream '' is left to
         # note_last_run's default, so that wrappers of it taking (model, run) keep working for one-stream models
         if stream:
@@ -335,6 +348,7 @@ class _VirConvBackbone(nn.Module):
             return xs
         if refusal is not None:
             raise ValueError(refusal % reason)
+        self._no_module_path_under_sync(plan, reason)
         _module_path_under_determinism(reason)
         proj = ops.projection_params(batch_dict.get('calib'), trans, batch_size, feats.device)
         x = spconv.SparseConvTensor(feats, coords.int(), self.sparse_shape, batch_size)
@@ -437,6 +451,12 @@ def _module_path_under_determinism(reason):
         raise RuntimeError(msg)
 
 
+# module-path reasons that depend on one rank's batch or call rather than on the model or the configuration
+NO_VOXELS, GRAD_INTO_FEATURES = 'no input voxels', 'gradient into the voxel features'
+MIXED_MODES = 'BatchNorm layers in mixed train / eval modes'
+_RANK_DEPENDENT = (NO_VOXELS, GRAD_INTO_FEATURES, MIXED_MODES)
+
+
 def _module_path_reason(feats, plan=None, discard=False):
     """None when a forward over `feats` may run through the executor `plan`, else why it takes the per-operator module path.
     discard: it applies host-drawn or caller-given StVD kept rows.  Without a plan (a caller that only knows the plan did
@@ -446,15 +466,15 @@ def _module_path_reason(feats, plan=None, discard=False):
     if not feats.is_cuda:
         return 'features not on a CUDA device'
     if feats.shape[0] == 0:
-        return 'no input voxels'
+        return NO_VOXELS
     if feats.requires_grad:          # (the plan does not propagate a gradient into the voxel features; the module path does)
-        return 'gradient into the voxel features'
+        return GRAD_INTO_FEATURES
     if discard:
         return 'host-drawn or caller-given StVD layer discard'
     if plan is not None and not plan.eligible():    # (dtype / layout / module type may change under .half(), .to())
-        return 'SyncBatchNorm, momentum=None, bias or a non-fp32 module'
+        return 'SyncBatchNorm on mixed process groups, momentum=None, bias or a non-fp32 module'
     if plan is None or any(bn.training != plan.layers[0][1].training for _, bn in plan.layers):
-        return 'BatchNorm layers in mixed train / eval modes'
+        return MIXED_MODES
     return None
 
 
@@ -651,6 +671,7 @@ class VirConv8x(_VirConvBackbone):
             return self._run(plan, feats, coords, shape, batch_size, None, '', static=static)[1]
         if static is not None:
             raise ValueError('VirConv8x static mode: the LiDAR stream cannot run through the plan executor (%s)' % reason)
+        self._no_module_path_under_sync(plan, reason)
         _module_path_under_determinism(reason)
         x = spconv.SparseConvTensor(feats, coords.int(), shape, batch_size)
         x1 = self.conv1(self.conv_input(x))

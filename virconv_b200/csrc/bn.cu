@@ -21,7 +21,10 @@ __global__ void __launch_bounds__(256) bn_apply_relu_kernel(
     const float4* __restrict__ x, const double* __restrict__ sums, int n_rows, const int* __restrict__ n_dev, int c,
     const float* __restrict__ gamma, const float* __restrict__ beta, float* running_mean, float* running_var,
     long long* num_batches_tracked, float momentum, float eps, int training, float4* __restrict__ y, int y_ld4,
-    uint2* __restrict__ y_bf16, int yb_ld4, float* __restrict__ stats_out, int relu, int tail_zero) {
+    uint2* __restrict__ y_bf16, int yb_ld4, float* __restrict__ stats_out, int relu, int tail_zero,
+    const double* __restrict__ n_glob) {
+    // n_glob (SyncBatchNorm, else NULL): the row count over all ranks the statistics divide by, sums then being the
+    // all-reduced ones.
     // n_dev (static mode): the row count lives in device memory, n_rows is the capacity of the buffers; with tail_zero the
     // rows [count, capacity) of the outputs are written as zeros (published tensors keep a defined tail).
     // y_ld4 / yb_ld4: row pitch of the outputs in float4 / uint2 units (>= c/4: the output may be a column slice of a
@@ -35,7 +38,8 @@ __global__ void __launch_bounds__(256) bn_apply_relu_kernel(
     const int cg = (int)(i0 % c4);
     __shared__ float sc_s[128], sh_s[128];
     if (threadIdx.x < c)   // one thread per channel derives scale / shift (float64 once per block, not per thread)
-        bn_channel(training ? sums[threadIdx.x] : 0.0, training ? sums[c + threadIdx.x] : 0.0, threadIdx.x, c, n_rows, gamma, beta,
+        bn_channel(training ? sums[threadIdx.x] : 0.0, training ? sums[c + threadIdx.x] : 0.0, threadIdx.x, c,
+                   n_glob != nullptr ? (int)__ldg(n_glob) : n_rows, gamma, beta,
                    running_mean, running_var, momentum, eps, training, sc_s, sh_s, blockIdx.x == 0, stats_out);
     if (training && blockIdx.x == 0 && threadIdx.x == 0 && num_batches_tracked != nullptr) *num_batches_tracked += 1;
     __syncthreads();
@@ -194,7 +198,9 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const float4* __restr
                                                            const int* __restrict__ n_dev, int c, int training,
                                                            float4* __restrict__ dx, uint2* __restrict__ dx_bf16,
                                                            float* __restrict__ dgamma, float* __restrict__ dbeta, int tail_zero,
-                                                           const double* __restrict__ part) {
+                                                           const double* __restrict__ part, const double* __restrict__ n_glob) {
+    // n_glob (SyncBatchNorm, else NULL): bsums are the all-reduced sums, *n_glob the row count over all ranks; dgamma /
+    // dbeta are then NULL (the local ones were written before the exchange)
     const int cap_rows = n_rows;
     if (n_dev != nullptr) n_rows = min(n_rows, __ldg(n_dev));
     const int c4 = c / 4;
@@ -215,7 +221,7 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const float4* __restr
         const float mean = stats[2 * c + ch], invstd = stats[3 * c + ch];
         const float gi = gamma[ch] * invstd;
         if (training) {
-            const double nn = (double)(n_rows > 0 ? n_rows : 1);
+            const double nn = n_glob != nullptr ? __ldg(n_glob) : (double)(n_rows > 0 ? n_rows : 1);
             const float k1 = (float)(Q / nn) * invstd;
             a_s[ch] = gi;
             b_s[ch] = -gi * k1;
@@ -225,7 +231,7 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const float4* __restr
             b_s[ch] = 0.f;
             d_s[ch] = 0.f;
         }
-        if (blockIdx.x == 0) {
+        if (blockIdx.x == 0 && dgamma != nullptr) {
             dbeta[ch] = (float)S;
             dgamma[ch] = (float)Q;
         }
@@ -260,6 +266,20 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const float4* __restr
             if (dx_bf16 != nullptr) dx_bf16[i] = make_uint2(0u, 0u);
         }
     }
+}
+
+// SyncBatchNorm: a rank's local sums [2, c] into its exchange slot before the all-reduce.  Forward (dgamma == NULL):
+// slot = [sum x (c), sum x^2 (c), row count] (the count from n_dev in static mode).  Backward: slot = [sum g (c),
+// sum g*xhat (c)], and the local dbeta / dgamma (which stay local: DDP averages them) are written from the same sums.
+__global__ void __launch_bounds__(256) bn_sync_pack_kernel(const double* __restrict__ sums, int c, int n_rows,
+                                                           const int* __restrict__ n_dev, double* __restrict__ slot,
+                                                           float* __restrict__ dgamma, float* __restrict__ dbeta) {
+    for (int j = threadIdx.x; j < 2 * c; j += blockDim.x) {
+        const double v = sums[j];
+        slot[j] = v;
+        if (dgamma != nullptr) (j < c ? dbeta[j] : dgamma[j - c]) = (float)v;
+    }
+    if (dgamma == nullptr && threadIdx.x == 0) slot[2 * c] = (double)(n_dev != nullptr ? min(n_rows, __ldg(n_dev)) : n_rows);
 }
 
 // backward, both passes in ONE cooperative launch (grid-wide barrier between the reduction and the apply): 20 launches fewer per
@@ -389,16 +409,16 @@ using namespace vc;
 int vc::bn_apply_relu_dev(const float* x, const double* sums, int n_rows, const int* n_dev, int c, const float* gamma,
                           const float* beta, float* running_mean, float* running_var, long long* num_batches_tracked,
                           float momentum, float eps, int training, float* y, int y_ld, void* y_bf16, int yb_ld,
-                          float* stats_out, int relu, int tail_zero, cudaStream_t stream) {
+                          float* stats_out, int relu, int tail_zero, cudaStream_t stream, const double* n_glob) {
     VC_CHECK_ARG(c_ok(c) && n_rows >= 0, "bad bn args c=%d rows=%d", c, n_rows);
     VC_CHECK_ARG(gamma && beta && running_mean && running_var && stats_out, "null pointer");
     VC_CHECK_ARG(!training || sums, "training-mode BN needs the conv's channel sums");
-    VC_CHECK_ARG(!training || n_rows > 0, "training-mode BN over zero rows");
+    VC_CHECK_ARG(!training || n_rows > 0 || n_glob, "training-mode BN over zero rows");
     VC_CHECK_ARG(n_rows == 0 || (x && (y || y_bf16)), "null pointer");
     VC_CHECK_ARG(y_ld % 4 == 0 && yb_ld % 4 == 0 && y_ld >= c && yb_ld >= c, "bad output pitch");
     bn_apply_relu_kernel<<<dim3(ew_blocks((size_t)n_rows * c / 4)), dim3(256), 0, stream>>>((const float4*)x, sums, n_rows, n_dev,
         c, gamma, beta, running_mean, running_var, num_batches_tracked, momentum, eps, training, (float4*)y, y_ld / 4,
-        (uint2*)y_bf16, yb_ld / 4, stats_out, relu, tail_zero);
+        (uint2*)y_bf16, yb_ld / 4, stats_out, relu, tail_zero, n_glob);
     VC_LAUNCH_CHECK();
     return VC_OK;
 }
@@ -454,7 +474,50 @@ int vc::bn_relu_bwd_dev(const float* dy, int dy_ld, const float* x, const float*
     }
     bn_bwd_apply_kernel<<<dim3(ew_blocks((size_t)n * c / 4)), dim3(256), 0, stream>>>((const float4*)dy, dy_ld / 4,
         (const float4*)x, gamma, stats, bsums, n, n_dev, c, training, (float4*)dx, (uint2*)dx_bf16, dgamma, dbeta, tail_zero,
-        (const double*)part);
+        (const double*)part, nullptr);
+    VC_LAUNCH_CHECK();
+    return VC_OK;
+}
+
+int vc::bn_sync_pack_dev(const double* sums, int c, int n_rows, const int* n_dev, double* slot, float* dgamma, float* dbeta,
+                         cudaStream_t stream) {
+    VC_CHECK_ARG(c_ok(c) && n_rows >= 0 && sums && slot && (dgamma == nullptr) == (dbeta == nullptr), "bad bn exchange args");
+    bn_sync_pack_kernel<<<1, 256, 0, stream>>>(sums, c, n_rows, n_dev, slot, dgamma, dbeta);
+    VC_LAUNCH_CHECK();
+    return VC_OK;
+}
+
+// SyncBatchNorm backward, first half: the local (sum g, sum g*xhat) into bsums [2, c] (zeroed by the caller; deterministic
+// mode: chunk partials `part`, added in chunk order), then the local dbeta / dgamma and the exchange slot [2c]
+int vc::bn_relu_bwd_local_dev(const float* dy, int dy_ld, const float* x, const float* stats, int n, const int* n_dev, int c,
+                              double* bsums, double* part, float* dgamma, float* dbeta, double* slot, cudaStream_t stream) {
+    VC_CHECK_ARG(c_ok(c) && n >= 0 && bsums && stats && dgamma && dbeta && slot, "bad args n=%d c=%d", n, c);
+    VC_CHECK_ARG(dy_ld % 4 == 0 && dy_ld >= c, "bad gradient pitch");
+    if (n > 0) {
+        VC_CHECK_ARG(dy && x, "null pointer");
+        const int c4 = c / 4, rowlanes = 256 / c4;
+        int blocks = (n + rowlanes - 1) / rowlanes;
+        if (blocks > 296) blocks = 296;
+        bn_bwd_reduce_kernel<<<dim3(blocks), dim3(256), (size_t)rowlanes * 2 * c * sizeof(float), stream>>>(
+            (const float4*)dy, dy_ld / 4, (const float4*)x, stats, n, n_dev, c, bsums, part);
+        VC_LAUNCH_CHECK();
+        if (part != nullptr) {
+            const int rc = bn_sums_reduce_dev(part, n, n_dev, BN_DET_ROWS, c, bsums, stream);
+            if (rc) return rc;
+        }
+    }
+    return bn_sync_pack_dev(bsums, c, n, n_dev, slot, dgamma, dbeta, stream);
+}
+
+// second half, after the exchange: dx from the all-reduced sums and the global row count n_glob (device float64)
+int vc::bn_relu_bwd_apply_dev(const float* dy, int dy_ld, const float* x, const float* gamma, const float* stats,
+                              const double* bsums, const double* n_glob, float* dx, void* dx_bf16, int n, const int* n_dev, int c,
+                              int tail_zero, cudaStream_t stream) {
+    VC_CHECK_ARG(c_ok(c) && n >= 0 && bsums && n_glob && stats && gamma, "bad args n=%d c=%d", n, c);
+    VC_CHECK_ARG(n == 0 || (dy && x && (dx || dx_bf16)), "null pointer");
+    bn_bwd_apply_kernel<<<dim3(ew_blocks((size_t)n * c / 4)), dim3(256), 0, stream>>>((const float4*)dy, dy_ld / 4,
+        (const float4*)x, gamma, stats, bsums, n, n_dev, c, 1, (float4*)dx, (uint2*)dx_bf16, nullptr, nullptr, tail_zero,
+        nullptr, n_glob);
     VC_LAUNCH_CHECK();
     return VC_OK;
 }

@@ -191,7 +191,7 @@ int index2uv_batch_dev(const UVStage* st, int n_st, int batch_size, const float*
 int bn_apply_relu_dev(const float* x, const double* sums, int n_rows, const int* n_dev, int c, const float* gamma,
                       const float* beta, float* running_mean, float* running_var, long long* num_batches_tracked, float momentum,
                       float eps, int training, float* y, int y_ld, void* y_bf16, int yb_ld, float* stats_out, int relu,
-                      int tail_zero, cudaStream_t stream);
+                      int tail_zero, cudaStream_t stream, const double* n_glob = nullptr);
 // part (deterministic mode, else NULL): [cdiv(n, BN_DET_ROWS), 2, c] float64 chunk partials, summed in chunk order
 int bn_relu_bwd_dev(const float* dy, int dy_ld, const float* x, const float* gamma, const float* stats, float* dx, void* dx_bf16,
                     float* dgamma, float* dbeta, int n, const int* n_dev, int c, int training, double* bsums, int tail_zero,
@@ -200,6 +200,15 @@ int bn_relu_bwd_dev(const float* dy, int dy_ld, const float* x, const float* gam
 int bn_sums_reduce_dev(const double* part, int cap_rows, const int* n_dev, int rows_per_part, int c, double* sums,
                        cudaStream_t stream);
 static constexpr int BN_DET_ROWS = 512;   // rows per chunk of the deterministic BN backward reduction
+// SyncBatchNorm exchange (executor.cu): local sums into a rank's float64 slot before the all-reduce, and the backward split
+// around it (bn.cu states the layouts); n_glob: device float64, the row count over all ranks
+int bn_sync_pack_dev(const double* sums, int c, int n_rows, const int* n_dev, double* slot, float* dgamma, float* dbeta,
+                     cudaStream_t stream);
+int bn_relu_bwd_local_dev(const float* dy, int dy_ld, const float* x, const float* stats, int n, const int* n_dev, int c,
+                          double* bsums, double* part, float* dgamma, float* dbeta, double* slot, cudaStream_t stream);
+int bn_relu_bwd_apply_dev(const float* dy, int dy_ld, const float* x, const float* gamma, const float* stats,
+                          const double* bsums, const double* n_glob, float* dx, void* dx_bf16, int n, const int* n_dev, int c,
+                          int tail_zero, cudaStream_t stream);
 int cat2_dev(const float* a, const float* b, float* out, void* out_bf16, int n, const int* n_dev, int ca, int cb, cudaStream_t stream);
 int index2uv_dev(const int32_t* indices, int n, const int* n_dev, int batch_size, const float* params, const float* grid,
                  int stride, int u_max, int v_max, int32_t* uv_out, cudaStream_t stream);

@@ -220,7 +220,14 @@ struct Ctx {
     Arena A;
     cudaStream_t st[3];   // forward: main, index stream, second index stream (image branch); backward: main, wgrad
     int32_t* err;
+    // SyncBatchNorm (vc_exec_forward_sync / vc_exec_backward_sync; xfn NULL: plain BatchNorm): the caller's float64 exchange
+    // buffer, its slot offsets [n_layers, 2] (forward, backward) and the callback that all-reduces a slot
+    double* xchg;
+    const int64_t* xoff;
+    vc_bn_exchange_fn xfn;
+    void* xuser;
     const int* op(int i) const { return oi + (size_t)i * OPI; }
+    double* xslot(int layer, int dir) const { return xchg + xoff[2 * layer + dir]; }
     template <class T>
     T* P(int layer, int col) const { return reinterpret_cast<T*>(lp[(size_t)layer * P_COLS + col]); }
 };
@@ -237,6 +244,16 @@ struct Ctx {
         set_error("plan executor: arena too small (%zu bytes given, > %zu needed)", C.A.cap, C.A.used); \
         return VC_ERR_WORKSPACE;                                                                       \
     }
+
+// SyncBatchNorm: the caller all-reduces slot `dir` (0 forward, 1 backward) of layer `li` over the ranks, enqueued on the main
+// stream (under capture: captured there, once)
+int exchange(Ctx& C, int li, int dir, int n) {
+    if (C.xfn(C.xuser, li, dir, C.xslot(li, dir), n) != 0) {
+        set_error("SyncBatchNorm exchange of layer %d (%s) failed", li, dir ? "backward" : "forward");
+        return VC_ERR_INVALID;
+    }
+    return VC_OK;
+}
 
 // make `consumer` stream wait for a resource produced on the other stream
 int wait_for(Ctx& C, int& ev, int prod, int consumer) {
@@ -829,6 +846,9 @@ int fwd_cbr(FwdCtx& C, int i, const int* o, int s) {
         S->det_bytes += pb;
     }
     bool bn_done = false;
+    // SyncBatchNorm over more than one rank: conv with epilogue sums -> exchange -> apply (the fused conv + BN cannot wait
+    // for the other ranks' sums)
+    const bool sync = C.xfn != nullptr && S->training;
     if (L.fwd == K_FWD_TC && R.n_out > 0) {
         if (!X.bf16) {   // no producer wrote a shadow (network input): cast once
             VC_CHECK_ARG(X.ld == X.c, "op %d: no bf16 copy of a strided input", i);
@@ -843,7 +863,7 @@ int fwd_cbr(FwdCtx& C, int i, const int* o, int s) {
                         C.S->is_static, L.tile_ctr + CTR_BN_BAR};
         if (C.do_feat)
             VC_TRY(tc2_conv(L.cin, L.cout, X.bf16, L.wimg_fwd, R.nbr, R.n_out, x, R.n_out, R.n_out_dev, R.K, sums, C.err, st, nullptr,
-                            L.tile_ctr, C.idx_first ? 2 : 0, X.ld, part, &bt, &bn_done));
+                            L.tile_ctr, C.idx_first ? 2 : 0, X.ld, part, sync ? nullptr : &bt, &bn_done));
     } else {   // (also a tensor-core layer without output rows)
         const size_t wsb = vc_conv_ws_bytes(L.cin, L.cout, R.K);
         VC_ALLOC(ws, void*, wsb);
@@ -856,10 +876,18 @@ int fwd_cbr(FwdCtx& C, int i, const int* o, int s) {
     }
     if (C.do_feat && !bn_done && part && R.n_out > 0)
         VC_TRY(bn_sums_reduce_dev(part, R.n_out, R.n_out_dev, VC_TILE_ROWS, L.cout, L.sums, st));
+    const double* sums_in = L.sums;
+    const double* n_glob = nullptr;
+    if (C.do_feat && sync) {   // slot = [sum x, sum x^2, rows], all-reduced in place
+        VC_TRY(bn_sync_pack_dev(L.sums, L.cout, R.n_out, R.n_out_dev, C.xslot(li, 0), nullptr, nullptr, st));
+        VC_TRY(exchange(C, li, 0, 2 * L.cout + 1));
+        sums_in = C.xslot(li, 0);
+        n_glob = sums_in + 2 * L.cout;
+    }
     if (C.do_feat && !bn_done)
-        VC_TRY(bn_apply_relu_dev(x, L.sums, R.n_out, R.n_out_dev, L.cout, C.P<const float>(li, P_GAMMA), C.P<const float>(li, P_BETA),
+        VC_TRY(bn_apply_relu_dev(x, sums_in, R.n_out, R.n_out_dev, L.cout, C.P<const float>(li, P_GAMMA), C.P<const float>(li, P_BETA),
                                  C.P<float>(li, P_RM), C.P<float>(li, P_RV), C.P<long long>(li, P_NBT), C.lf[2 * li + 1], C.lf[2 * li],
-                                 S->training, y, y_ld, yb, y_ld, stats, 1, C.S->is_static, st));
+                                 S->training, y, y_ld, yb, y_ld, stats, 1, C.S->is_static, st, n_glob));
     Y.f32 = y; Y.bf16 = yb; Y.rows = R.n_out; Y.c = L.cout; Y.ld = y_ld; Y.n_dev = R.n_out_dev;
     C.produced(Y, s);
     return VC_OK;
@@ -995,7 +1023,8 @@ int exec_forward(const int32_t* ops_i, const float* ops_f, int n_ops, const uint
                  const float* proj_params, int training, int precision, int flags, void* arena, size_t arena_bytes,
                  int32_t* pinned_host, int32_t* err_flag, void* state, size_t state_bytes, vc_stream_t main_stream,
                  vc_stream_t side_stream, int side_waits_main, const int32_t* caps, const int32_t* n0_dev, int32_t* overflow_flag,
-                 vc_stream_t side2_stream, const int64_t* rng_seed_dev, bool idx_first) {
+                 vc_stream_t side2_stream, const int64_t* rng_seed_dev, bool idx_first, double* xchg, const int64_t* xchg_off,
+                 vc_bn_exchange_fn exchange_fn, void* exchange_user) {
     // static mode and phased execution: include/virconv_b200.h.  Both phases walk the whole plan with the same
     // deterministic bump allocation, so they agree on every address and leave the same state blob.
     const bool is_static = n0_dev != nullptr;
@@ -1032,6 +1061,7 @@ int exec_forward(const int32_t* ops_i, const float* ops_f, int n_ops, const uint
     C.proj = proj_params; C.seed = rng_seed_dev; C.caps = caps; C.overflow = overflow_flag; C.pinned = pinned_host;
     C.do_idx = phase != 2; C.do_feat = phase != 1; C.two = C.st[0] != C.st[1];
     C.idx_first = idx_first;
+    C.xchg = xchg; C.xoff = xchg_off; C.xfn = exchange_fn; C.xuser = exchange_user;
     plan_step(C, c0, precision, training);
 
     VC_TRY(ev_init());
@@ -1119,6 +1149,21 @@ extern "C" int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, 
                                       void* state, size_t state_bytes, vc_stream_t main_stream, vc_stream_t side_stream,
                                       int side_waits_main, const int32_t* caps, const int32_t* n0_dev, int32_t* overflow_flag,
                                       vc_stream_t side2_stream, const int64_t* rng_seed_dev) {
+    return vc_exec_forward_sync(ops_i, ops_f, n_ops, layer_ptrs, layer_f, n_layers, feats0, c0, idx0, n0, shape0, batch_size,
+                                proj_params, training, precision, flags, arena, arena_bytes, pinned_host, err_flag, state,
+                                state_bytes, main_stream, side_stream, side_waits_main, caps, n0_dev, overflow_flag, side2_stream,
+                                rng_seed_dev, nullptr, nullptr, nullptr, nullptr);
+}
+
+extern "C" int vc_exec_forward_sync(const int32_t* ops_i, const float* ops_f, int n_ops, const uint64_t* layer_ptrs,
+                                    const float* layer_f, int n_layers, const float* feats0, int c0, const int32_t* idx0, int n0,
+                                    const int32_t* shape0, int batch_size, const float* proj_params, int training, int precision,
+                                    int flags, void* arena, size_t arena_bytes, int32_t* pinned_host, int32_t* err_flag,
+                                    void* state, size_t state_bytes, vc_stream_t main_stream, vc_stream_t side_stream,
+                                    int side_waits_main, const int32_t* caps, const int32_t* n0_dev, int32_t* overflow_flag,
+                                    vc_stream_t side2_stream, const int64_t* rng_seed_dev, double* xchg, const int64_t* xchg_off,
+                                    vc_bn_exchange_fn exchange_fn, void* exchange_user) {
+    VC_CHECK_ARG(!exchange_fn || (xchg && xchg_off), "a SyncBatchNorm exchange needs its buffer and slot offsets");
     // Static mode (no host read splits the index phase): the index walk first, then the feature walk, so that no index
     // kernel is resident while the convs run and the fused conv + BN grids take two CTAs per SM (conv_tc2.cu launch_persist).
     const bool idx_first = n0_dev != nullptr && ((flags >> 8) & 3) == 0 && side_stream != nullptr && side_stream != main_stream;
@@ -1126,11 +1171,12 @@ extern "C" int vc_exec_forward_seeded(const int32_t* ops_i, const float* ops_f, 
     if (idx_first)
         VC_TRY(exec_forward(ops_i, ops_f, n_ops, layer_ptrs, layer_f, n_layers, feats0, c0, idx0, n0, shape0, batch_size, proj_params,
                             training, precision, f | (1 << 8), arena, arena_bytes, pinned_host, err_flag, state, state_bytes,
-                            main_stream, side_stream, side_waits_main, caps, n0_dev, overflow_flag, side2_stream, rng_seed_dev, false));
+                            main_stream, side_stream, side_waits_main, caps, n0_dev, overflow_flag, side2_stream, rng_seed_dev, false,
+                            xchg, xchg_off, exchange_fn, exchange_user));
     return exec_forward(ops_i, ops_f, n_ops, layer_ptrs, layer_f, n_layers, feats0, c0, idx0, n0, shape0, batch_size, proj_params,
                         training, precision, idx_first ? f | (2 << 8) : flags, arena, arena_bytes, pinned_host, err_flag, state,
                         state_bytes, main_stream, side_stream, side_waits_main, caps, n0_dev, overflow_flag, side2_stream, rng_seed_dev,
-                        idx_first);
+                        idx_first, xchg, xchg_off, exchange_fn, exchange_user);
 }
 
 namespace vc {
@@ -1202,7 +1248,17 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
                                 const float* layer_f, int n_layers, const int32_t* pub_slots, const uint64_t* ext_grads,
                                 int n_pub, void* arena, size_t arena_bytes, int32_t* err_flag, void* state,
                                 vc_stream_t stream_, vc_stream_t wgrad_stream_) {
+    return vc_exec_backward_sync(ops_i, ops_f, n_ops, layer_ptrs, layer_f, n_layers, pub_slots, ext_grads, n_pub, arena, arena_bytes,
+                                 err_flag, state, stream_, wgrad_stream_, nullptr, nullptr, nullptr, nullptr);
+}
+
+extern "C" int vc_exec_backward_sync(const int32_t* ops_i, const float* ops_f, int n_ops, const uint64_t* layer_ptrs,
+                                     const float* layer_f, int n_layers, const int32_t* pub_slots, const uint64_t* ext_grads,
+                                     int n_pub, void* arena, size_t arena_bytes, int32_t* err_flag, void* state,
+                                     vc_stream_t stream_, vc_stream_t wgrad_stream_, double* xchg, const int64_t* xchg_off,
+                                     vc_bn_exchange_fn exchange_fn, void* exchange_user) {
     VC_TRY(check_plan(ops_i, n_ops, n_layers));
+    VC_CHECK_ARG(!exchange_fn || (xchg && xchg_off), "a SyncBatchNorm exchange needs its buffer and slot offsets");
     State* S = (State*)state;
     VC_CHECK_ARG(S && S->magic == STATE_MAGIC && S->n_ops == n_ops && S->n_layers == n_layers, "state does not belong to this plan");
     VC_CHECK_ARG(arena && layer_ptrs && (n_pub == 0 || (pub_slots && ext_grads)), "null argument");
@@ -1213,6 +1269,7 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
     C.st[1] = wgrad_stream_ ? (cudaStream_t)wgrad_stream_ : (cudaStream_t)stream_;
     C.st[2] = C.st[1];
     C.err = err_flag;
+    C.xchg = xchg; C.xoff = xchg_off; C.xfn = exchange_fn; C.xuser = exchange_user;
     g_ev_next = 0;
     cudaStream_t st = C.st[0];
     cudaStream_t wst = C.st[1];      // weight gradients: off the dgrad chain's critical path
@@ -1296,6 +1353,10 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
             VC_CUDA(cudaMemsetAsync(dw, 0, wn * 4, st));
             VC_CUDA(cudaMemsetAsync(dgamma, 0, (size_t)L.cout * 4, st));
             VC_CUDA(cudaMemsetAsync(dbeta, 0, (size_t)L.cout * 4, st));
+            if (C.xfn != nullptr && training && Y.grad_state != G_EMPTY) {   // (no rows here, but the other ranks' exchange waits)
+                VC_CUDA(cudaMemsetAsync(C.xslot(li, 1), 0, (size_t)2 * L.cout * 8, st));
+                VC_TRY(exchange(C, li, 1, 2 * L.cout));
+            }
             continue;
         }
         const size_t elems = (size_t)R.n_out * L.cout;
@@ -1320,8 +1381,18 @@ extern "C" int vc_exec_backward(const int32_t* ops_i, const float* ops_f, int n_
             bpart = t;
             S->det_bytes += pb + (g2 ? elems * (L.dgrad == K_DGRAD_GATHER2D_TC ? 2 : 4) : 0);
         }
-        VC_TRY(bn_relu_bwd_dev(Y.grad, Y.gld, L.x, C.P<const float>(li, P_GAMMA), L.stats, dx, dxb, dgamma, dbeta, R.n_out, R.n_out_dev,
-                               L.cout, training, L.sums + 2 * L.cout, S->is_static, st, bpart));
+        if (C.xfn != nullptr && training) {
+            // SyncBatchNorm: local sums (and the local dgamma / dbeta) -> exchange -> dx from the all-reduced sums and the
+            // forward slot's global row count
+            VC_TRY(bn_relu_bwd_local_dev(Y.grad, Y.gld, L.x, L.stats, R.n_out, R.n_out_dev, L.cout, L.sums + 2 * L.cout, bpart, dgamma,
+                                         dbeta, C.xslot(li, 1), st));
+            VC_TRY(exchange(C, li, 1, 2 * L.cout));
+            VC_TRY(bn_relu_bwd_apply_dev(Y.grad, Y.gld, L.x, C.P<const float>(li, P_GAMMA), L.stats, C.xslot(li, 1),
+                                         C.xslot(li, 0) + 2 * L.cout, dx, dxb, R.n_out, R.n_out_dev, L.cout, S->is_static, st));
+        } else {
+            VC_TRY(bn_relu_bwd_dev(Y.grad, Y.gld, L.x, C.P<const float>(li, P_GAMMA), L.stats, dx, dxb, dgamma, dbeta, R.n_out,
+                                   R.n_out_dev, L.cout, training, L.sums + 2 * L.cout, S->is_static, st, bpart));
+        }
         // the wgrad needs dx / its bf16 shadow: on its own stream it waits for this event, and it is enqueued after the
         // dgrad, which is on the critical path (the dgrad's CTAs reach the SMs first)
         const int bn_ev = two ? record_on(C, 0) : -1;

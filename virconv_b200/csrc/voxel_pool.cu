@@ -216,13 +216,14 @@ __device__ __forceinline__ void moments_to_cov(const double* __restrict__ m, dou
 
 // one thread per channel: the BatchNorm2d of the position branch (rule 4), folded; running statistics as torch's
 // _BatchNorm (momentum < 0: cumulative average); stat [C, 2] = mean, invstd for the backward
-__global__ void pool_bn_fold_kernel(int C, double n, int training, const double* __restrict__ moments,
+__global__ void pool_bn_fold_kernel(int C, double n, const double* __restrict__ n_dev, int training, const double* __restrict__ moments,
                                     const float* __restrict__ w_pos, const float* __restrict__ gamma,
                                     const float* __restrict__ beta, float* __restrict__ running_mean,
                                     float* __restrict__ running_var, long long* __restrict__ num_batches_tracked, double eps,
                                     double momentum, float* __restrict__ scale, float* __restrict__ shift,
                                     double* __restrict__ stat) {
     const int c = threadIdx.x;
+    if (n_dev != nullptr) n = *n_dev;   // (SyncBatchNorm: the slot count over all ranks)
     const long long nbt = training ? num_batches_tracked[0] + 1 : 0;
     __syncthreads();
     if (training && c == 0) num_batches_tracked[0] = nbt;
@@ -253,8 +254,9 @@ __global__ void pool_bn_fold_kernel(int C, double n, int training, const double*
 }
 
 // one thread per channel: dW_pos, dgamma, dbeta from the per-channel sums of the pooling backward (rule 6)
-__global__ void pool_bn_grad_kernel(int C, double n, int training, const double* __restrict__ sums,
-                                    const double* __restrict__ moments, const float* __restrict__ w_pos,
+// gsums / n_dev (SyncBatchNorm, else NULL): the all-reduced sums and slot count; sums and moments stay the rank's own
+__global__ void pool_bn_grad_kernel(int C, double n, const double* __restrict__ n_dev, int training, const double* __restrict__ sums,
+                                    const double* __restrict__ gsums, const double* __restrict__ moments, const float* __restrict__ w_pos,
                                     const float* __restrict__ gamma, const double* __restrict__ stat, float* __restrict__ dw,
                                     float* __restrict__ dgamma, float* __restrict__ dbeta) {
     const int c = threadIdx.x;
@@ -264,6 +266,10 @@ __global__ void pool_bn_grad_kernel(int C, double n, int training, const double*
     const double sdy = sums[c * 4 + 0], sdyr[3] = {sums[c * 4 + 1], sums[c * 4 + 2], sums[c * 4 + 3]};
     // x = w r before BN, xhat = (x - mean) invstd:  dbeta = sum dy, dgamma = sum dy xhat
     const double dg = (sdyr[0] * w[0] + sdyr[1] * w[1] + sdyr[2] * w[2] - mean * sdy) * invstd;
+    const double* gs = gsums != nullptr ? gsums : sums;
+    const double gsdy = gs[c * 4 + 0];
+    const double gdg = gsums != nullptr ? (gs[c * 4 + 1] * w[0] + gs[c * 4 + 2] * w[1] + gs[c * 4 + 3] * w[2] - mean * gsdy) * invstd : dg;
+    if (n_dev != nullptr) n = *n_dev;
     const double k = gamma[c] * invstd;
     for (int j = 0; j < 3; j++) {
         double d = sdyr[j];
@@ -273,7 +279,7 @@ __global__ void pool_bn_grad_kernel(int C, double n, int training, const double*
             const double s[3][3] = {{moments[3], moments[4], moments[5]}, {moments[4], moments[6], moments[7]},
                                     {moments[5], moments[7], moments[8]}};
             const double sxr = (s[j][0] * w[0] + s[j][1] * w[1] + s[j][2] * w[2] - mean * moments[j]) * invstd;
-            d = d - sdy / n * moments[j] - dg / n * sxr;
+            d = d - gsdy / n * moments[j] - gdg / n * sxr;
         }
         dw[c * 3 + j] = (float)(k * d);
     }
@@ -496,7 +502,7 @@ extern "C" int vc_voxel_pool_bn_fold(int C, long long n, int training, const dou
     VC_CHECK_ARG(C > 0 && C <= 1024 && n > 0, "bad voxel_pool_bn_fold arguments");
     VC_CHECK_ARG(w_pos && gamma && beta && running_mean && running_var && scale && shift && stat, "null pointer");
     VC_CHECK_ARG(!training || (moments && num_batches_tracked), "train mode needs moments and num_batches_tracked");
-    pool_bn_fold_kernel<<<1, (C + 31) / 32 * 32, 0, stream>>>(C, (double)n, training, moments, w_pos, gamma, beta, running_mean,
+    pool_bn_fold_kernel<<<1, (C + 31) / 32 * 32, 0, stream>>>(C, (double)n, nullptr, training, moments, w_pos, gamma, beta, running_mean,
                                                               running_var, num_batches_tracked, eps, momentum, scale, shift,
                                                               stat);
     VC_LAUNCH_CHECK();
@@ -509,7 +515,34 @@ extern "C" int vc_voxel_pool_bn_grad(int C, long long n, int training, const dou
     cudaStream_t stream = (cudaStream_t)stream_;
     VC_CHECK_ARG(C > 0 && C <= 1024 && n > 0, "bad voxel_pool_bn_grad arguments");
     VC_CHECK_ARG(sums && w_pos && gamma && stat && dw && dgamma && dbeta && (!training || moments), "null pointer");
-    pool_bn_grad_kernel<<<1, (C + 31) / 32 * 32, 0, stream>>>(C, (double)n, training, sums, moments, w_pos, gamma, stat, dw,
+    pool_bn_grad_kernel<<<1, (C + 31) / 32 * 32, 0, stream>>>(C, (double)n, nullptr, training, sums, nullptr, moments, w_pos, gamma,
+                                                              stat, dw, dgamma, dbeta);
+    VC_LAUNCH_CHECK();
+    return VC_OK;
+}
+
+extern "C" int vc_voxel_pool_bn_fold_sync(int C, int training, const double* moments10, const float* w_pos, const float* gamma,
+                                          const float* beta, float* running_mean, float* running_var,
+                                          long long* num_batches_tracked, double eps, double momentum, float* scale, float* shift,
+                                          double* stat, vc_stream_t stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    VC_CHECK_ARG(C > 0 && C <= 1024 && training, "bad voxel_pool_bn_fold_sync arguments (train mode only)");
+    VC_CHECK_ARG(moments10 && num_batches_tracked && w_pos && gamma && beta && running_mean && running_var && scale && shift && stat,
+                 "null pointer");
+    pool_bn_fold_kernel<<<1, (C + 31) / 32 * 32, 0, stream>>>(C, 1.0, moments10 + 9, training, moments10, w_pos, gamma, beta,
+                                                              running_mean, running_var, num_batches_tracked, eps, momentum, scale,
+                                                              shift, stat);
+    VC_LAUNCH_CHECK();
+    return VC_OK;
+}
+
+extern "C" int vc_voxel_pool_bn_grad_sync(int C, const double* n_glob, const double* sums, const double* gsums,
+                                          const double* moments, const float* w_pos, const float* gamma, const double* stat,
+                                          float* dw, float* dgamma, float* dbeta, vc_stream_t stream_) {
+    cudaStream_t stream = (cudaStream_t)stream_;
+    VC_CHECK_ARG(C > 0 && C <= 1024, "bad voxel_pool_bn_grad_sync arguments");
+    VC_CHECK_ARG(n_glob && sums && gsums && moments && w_pos && gamma && stat && dw && dgamma && dbeta, "null pointer");
+    pool_bn_grad_kernel<<<1, (C + 31) / 32 * 32, 0, stream>>>(C, 1.0, n_glob, 1, sums, gsums, moments, w_pos, gamma, stat, dw,
                                                               dgamma, dbeta);
     VC_LAUNCH_CHECK();
     return VC_OK;

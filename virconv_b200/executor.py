@@ -16,7 +16,7 @@ import weakref
 import numpy as np
 import torch
 
-from . import _lib, ops
+from . import _lib, ops, sync_bn
 from ._lib import check
 
 ENABLED = os.environ.get('VIRCONV_EXECUTOR', '1') != '0'
@@ -72,6 +72,7 @@ class Plan:
         self.iset_group = {0: 0}
         self.no_grad = {0}            # feature slots no parameter gradient flows into (the input and discards of it)
         self._final = None
+        self._slots = None
         # per-device run-time state (dies with the plan, i.e. with the model that owns it)
         self.arena_bytes = {}         # (device index, training) -> arena size handed out (monotone)
         self.arena_used = {}          # (device index, training) -> largest number of arena bytes a step really used
@@ -90,6 +91,7 @@ class Plan:
         self.rows_i.append([kind, stream, a, b, c, ndim, *ks, *st, *pd, *dl, cin, cout, layer, x0, x1, x2])
         self.rows_f.append(list(f) + [0.0] * (OPF - len(f)))
         self._final = None
+        self._slots = None
 
     def subm_rb(self, iset, ndim, ksize, dilation=1, unique=True, keys=(), stream=1):
         """stream: 1 = index stream, 2 = second index stream (the image branch: its projection + 2-D rulebooks depend on a
@@ -199,14 +201,33 @@ class Plan:
             out += [conv.weight, bn.weight, bn.bias]
         return out
 
+    def sync_slots(self):
+        """SyncBatchNorm exchange layout (vc_exec_forward_sync): -> (int64 [n_layers, 2] offsets in float64 elements of each
+        layer's forward slot [sum x (C), sum x^2 (C), rows] and backward slot [sum g (C), sum g*xhat (C)], total elements).
+        The slots of a layer are adjacent, layers follow in plan order."""
+        if self._slots is None:
+            off, rows = 0, []
+            for conv, _ in self.layers:
+                c = conv.out_channels
+                rows.append([off, off + 2 * c + 1])
+                off += 4 * c + 1
+            self._slots = (np.ascontiguousarray(np.array(rows, dtype=np.int64).reshape(-1, 2)), off)
+        return self._slots
+
     def eligible(self):
-        """Every layer is conv(bias=False) + a plain affine BatchNorm1d with running statistics and a fixed momentum (what the
-        VirConv blocks build), all parameters / buffers fp32 and contiguous.  SyncBatchNorm (statistics across ranks), a
-        cumulative-average BatchNorm (momentum=None) or a half-precision model go through the module path instead."""
+        """Every layer is conv(bias=False) + a plain affine BatchNorm1d or SyncBatchNorm with running statistics and a fixed
+        momentum (what the VirConv blocks build, or convert_sync_batchnorm makes of them), all parameters / buffers fp32 and
+        contiguous, and SyncBatchNorm layers all of them on one process group.  A cumulative-average BatchNorm
+        (momentum=None) or a half-precision model goes through the module path instead."""
         def f32(*ts):
             return all(t is not None and t.dtype == torch.float32 and t.is_contiguous() for t in ts)
-        return all(conv.bias is None and type(bn) is torch.nn.BatchNorm1d and bn.affine and bn.track_running_stats
-                   and bn.momentum is not None and f32(conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var)
+        try:
+            sync_bn.group_of([bn for _, bn in self.layers])
+        except ValueError:
+            return False
+        return all(conv.bias is None and type(bn) in (torch.nn.BatchNorm1d, torch.nn.SyncBatchNorm) and bn.affine
+                   and bn.track_running_stats and bn.momentum is not None
+                   and f32(conv.weight, bn.weight, bn.bias, bn.running_mean, bn.running_var)
                    for conv, bn in self.layers)
 
     def is_current(self):
@@ -230,16 +251,17 @@ def _pinned(device):
 ARENA_GRAIN = 64 << 20
 
 
-def _arena_bytes(plan, n0, device, with_bwd=True):
+def _arena_bytes(plan, n0, device, with_bwd=True, headroom=1.3):
     """Arena size for a step.  First use of a plan: a generous guess from the input row count (VirConv-L uses ~16 KB per
     input voxel, forward + backward; a forward alone about half).  Afterwards: the largest bytes-per-input-row an earlier
     step of the same plan really used (recorded by the backward / the eval forward) times this step's rows plus 30 %
     head-room — monotone per plan, so the caching allocator keeps handing back the same block, and an eval-only or
-    small-batch user does not reserve the training worst case (ADVICE r1: rows*24 KB + 256 MB over-reserved ~2x)."""
+    small-batch user does not reserve the training worst case (ADVICE r1: rows*24 KB + 256 MB over-reserved ~2x).  `headroom`:
+    the factor over the largest use seen (larger under a SyncBatchNorm exchange, which cannot re-run a walk that ran out)."""
     key = (device.index, bool(with_bwd))
     per_row = plan.arena_used.get(key, 0.0)
     if per_row:
-        want = int(1.3 * per_row * int(n0)) + (32 << 20)
+        want = int(headroom * per_row * int(n0)) + (32 << 20)
     else:
         # (fixed part: bitmaps / hash tables / weight images / per-layer scratch do not shrink with the batch — a 14 k-voxel
         #  training step uses 540 MB, an 80 k-voxel one 1.1 GB)
@@ -583,15 +605,48 @@ def _index_streams(dev, inputs_ready=False):
     return side, (ops.side2(dev) if (side is not None and THREE_STREAMS and not inputs_ready) else None)
 
 
+_NO_EXCHANGE = (None, None, _lib.EXCHANGE_FN(), None)     # (a NULL vc_bn_exchange_fn: plain BatchNorm)
+
+
+class _Exchange:
+    """One step's SyncBatchNorm exchange (sync_bn): the float64 slot buffer (Plan.sync_slots; alive from the forward to its
+    backward, which reads the forward slots' global counts) and the vc_bn_exchange_fn callback that hands a slot to
+    `reducer(slot, (tag, layer, 'forward' | 'backward'))`.  An exception in the reducer fails the C call and is re-raised."""
+
+    def __init__(self, plan, reducer, tag, dev):
+        self.off, n = plan.sync_slots()
+        self.buf = empty_scratch(max(n, 1), torch.float64, dev)    # (every slot is written before it is reduced)
+        self.reducer, self.tag, self.error = reducer, tag, None
+        self.fn = _lib.EXCHANGE_FN(self._call)
+
+    def _call(self, user, layer, direction, ptr, n):
+        try:
+            i = (ptr - self.buf.data_ptr()) // 8
+            self.reducer(self.buf[i:i + n], (self.tag, int(layer), 'backward' if direction else 'forward'))
+            return 0
+        except BaseException as e:      # (an exception must not cross the C frames)
+            self.error = e
+            return 1
+
+    def args(self):
+        return self.buf.data_ptr(), self.off.ctypes.data, self.fn, None
+
+    def raise_error(self):
+        if self.error is not None:
+            e, self.error = self.error, None
+            raise e
+
+
 def _exec_forward(plan, feats, coords, spatial_shape, batch_size, proj, training, precision, static, arena, side, side2,
-                  side_waits_main, seed=None):
-    """One vc_exec_forward_seeded call (only one phase where static.phase says so) -> (return code, state blob).  seed:
-    device int64[1] of the plan's layer discards.  torch.are_deterministic_algorithms_enabled() selects the deterministic
-    mode (flags bit 2), which the state records for the backward; a captured graph keeps the mode of its capture."""
+                  side_waits_main, seed=None, xchg=None):
+    """One vc_exec_forward_sync call (only one phase where static.phase says so) -> (return code, state blob).  seed:
+    device int64[1] of the plan's layer discards; xchg: the _Exchange of a SyncBatchNorm step, else None.
+    torch.are_deterministic_algorithms_enabled() selects the deterministic mode (flags bit 2), which the state records for
+    the backward; a captured graph keeps the mode of its capture."""
     oi, of, lf, _, _ = plan.finalize()
     tab, lib, dev = _layer_ptrs(plan), _lib.load(), feats.device
     state = np.zeros(lib.vc_exec_state_bytes(), dtype=np.uint8)
-    return lib.vc_exec_forward_seeded(
+    rc = lib.vc_exec_forward_sync(
         oi.ctypes.data, of.ctypes.data, oi.shape[0], tab.ctypes.data, lf.ctypes.data, len(plan.layers), feats.data_ptr(),
         feats.shape[1], coords.data_ptr(), feats.shape[0], _lib.host_i32(spatial_shape), int(batch_size),
         proj.data_ptr() if proj is not None else None, int(training), int(precision == 'bf16'),
@@ -601,7 +656,10 @@ def _exec_forward(plan, feats, coords, spatial_shape, batch_size, proj, training
         side.cuda_stream if side is not None else None, int(side_waits_main),
         static.caps_array().ctypes.data if static is not None else None, static.n_dev.data_ptr() if static is not None else None,
         static.overflow.data_ptr() if static is not None else None, side2.cuda_stream if side2 is not None else None,
-        seed.data_ptr() if seed is not None else None), state
+        seed.data_ptr() if seed is not None else None, *(xchg.args() if xchg is not None else _NO_EXCHANGE))
+    if xchg is not None:
+        xchg.raise_error()
+    return rc, state
 
 
 class PlanFn(torch.autograd.Function):
@@ -609,7 +667,7 @@ class PlanFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, plan, holder, feats, coords, spatial_shape, batch_size, proj, training, precision, inputs_ready, static,
-                with_bwd, seed, *params):
+                with_bwd, seed, xchg, *params):
         ctx.set_materialize_grads(False)     # published tensors the loss does not touch arrive as None, not as zeros
         dev = feats.device
         feats = feats.contiguous()
@@ -620,8 +678,11 @@ class PlanFn(torch.autograd.Function):
             inputs_ready = False             # under capture the side stream must fork from the capturing stream
         else:
             inflight = _throttle(plan, dev)
-        for attempt in range(3):
-            nbytes = _arena_bytes(plan, n0, dev, with_bwd)
+        for attempt in range(3 if xchg is None else 1):
+            # (SyncBatchNorm: no re-run — the exchanges of the failed walk were already enqueued, the other ranks would pair
+            #  them with the wrong ones.  So twice the largest arena use per input row seen so far instead of 1.3x; a batch
+            #  denser than that still fails, on its rank, and the other ranks wait in their exchanges: DESIGN.md section 6)
+            nbytes = _arena_bytes(plan, n0, dev, with_bwd, 1.3 if xchg is None else 2.0)
             if static is not None and static.arena is not None:
                 arena = static.arena              # phased execution: the index phase already built its part in there
             elif static is not None:
@@ -638,7 +699,8 @@ class PlanFn(torch.autograd.Function):
             else:
                 arena = _alloc_arena(plan, nbytes, dev, None)
             rc, state = _exec_forward(plan, feats, coords, spatial_shape, batch_size, proj, training, precision, static, arena,
-                                      side_obj, side2_obj, side_waits_main=not (inputs_ready and side_obj is not None), seed=seed)
+                                      side_obj, side2_obj, side_waits_main=not (inputs_ready and side_obj is not None), seed=seed,
+                                      xchg=xchg)
             if rc != VC_ERR_WORKSPACE:
                 break
             # too small (first use of a plan on an unusually dense batch): the call is restartable — nothing it enqueued is
@@ -651,6 +713,7 @@ class PlanFn(torch.autograd.Function):
             inflight.append(tail)
         run = _Run(plan, arena, state, precision)
         run.static, run.n0, run.training, run.with_bwd, run.feats = static, n0, bool(training), bool(with_bwd), feats
+        run.xchg = xchg
         holder.append(run)
         if not with_bwd:
             _note_arena_use(plan, dev, False, run.query(0, 0)[0], n0)
@@ -678,10 +741,14 @@ class PlanFn(torch.autograd.Function):
         if ws is not None and run.static is None:
             flat.record_stream(ws)
             run.arena.record_stream(ws)
-        rc = lib.vc_exec_backward(oi.ctypes.data, of.ctypes.data, oi.shape[0], tab.ctypes.data, lf.ctypes.data, len(plan.layers),
-                                  slots.ctypes.data, ext.ctypes.data, len(gs), run.arena.data_ptr(), run.arena.numel(),
-                                  ops.tc_error_flag(dev).data_ptr(), run.state.ctypes.data, ops._stream(),
-                                  ws.cuda_stream if ws is not None else None)
+        xchg = run.xchg
+        rc = lib.vc_exec_backward_sync(oi.ctypes.data, of.ctypes.data, oi.shape[0], tab.ctypes.data, lf.ctypes.data,
+                                       len(plan.layers), slots.ctypes.data, ext.ctypes.data, len(gs), run.arena.data_ptr(),
+                                       run.arena.numel(), ops.tc_error_flag(dev).data_ptr(), run.state.ctypes.data, ops._stream(),
+                                       ws.cuda_stream if ws is not None else None,
+                                       *(xchg.args() if xchg is not None else _NO_EXCHANGE))
+        if xchg is not None:
+            xchg.raise_error()
         if rc == VC_ERR_WORKSPACE:
             # (a forward taken without autograd's knowledge of a later backward: the next step's arena is sized for it)
             plan.arena_bytes[(dev.index, run.with_bwd)] = 2 * run.arena.numel()
@@ -690,7 +757,7 @@ class PlanFn(torch.autograd.Function):
         run.flat_grad = flat
         views = flat.split(sizes)
         out = [v.view_as(p) for v, p in zip(views, plan.params())]
-        return (None,) * 13 + tuple(out)
+        return (None,) * 14 + tuple(out)
 
 
 def run_index(plan, feats, coords_i32, spatial_shape, batch_size, proj, training, precision, static, seed=None):
@@ -704,13 +771,15 @@ def run_index(plan, feats, coords_i32, spatial_shape, batch_size, proj, training
 
 
 def run_plan(plan, feats, coords_i32, spatial_shape, batch_size, proj, training, precision, inputs_ready=False, static=None,
-             seed=None):
+             seed=None, reducer=None, tag=''):
     """-> (run record, {name: (features, indices, spatial_shape, bf16 shadow, device row count or None)}).  `coords_i32`
     [N,4] int32 contiguous (b,z,y,x).  inputs_ready: the caller vouches that `coords_i32` and `proj` are complete in the
     SIDE stream's order (resident from an earlier step, or produced on / synchronised with ops.side(device).stream): the
     index pipeline then does not wait for the main stream and overlaps the previous step's backward.  static: a StaticSpec
     (capacity-sized tensors, device row counts, no host synchronisation: CUDA-graph capturable).  seed: device int64[1], the
-    draw of the plan's layer discards (Plan.discard), read on the index stream after everything queued on main so far."""
+    draw of the plan's layer discards (Plan.discard), read on the index stream after everything queued on main so far.
+    reducer (training only): the SyncBatchNorm exchange — `reducer(slot, (tag, layer, 'forward' | 'backward'))` sums a float64
+    slot over the ranks on the current stream (sync_bn); None: plain BatchNorm."""
     ops._require_cuda(feats, coords_i32)
     assert coords_i32.dtype == torch.int32 and coords_i32.is_contiguous()
     inputs_ready = inputs_ready and seed is None       # (the seed is drawn on main: the index stream must wait for it)
@@ -726,8 +795,9 @@ def run_plan(plan, feats, coords_i32, spatial_shape, batch_size, proj, training,
         aliases = [p.detach().requires_grad_(True) for p in params]
         static.param_aliases = {id(p): a for p, a in zip(params, aliases)}
         params = aliases
+    xchg = _Exchange(plan, reducer, tag, feats.device) if (reducer is not None and training) else None
     outs = PlanFn.apply(plan, holder, feats, coords_i32, list(spatial_shape), batch_size, proj, training, precision,
-                        bool(inputs_ready), static, with_bwd, seed, *params)
+                        bool(inputs_ready), static, with_bwd, seed, xchg, *params)
     run = holder[0]
     res = {}
     for (name, slot, iset), f in zip(plan.published, outs):

@@ -38,7 +38,7 @@ import gc
 
 import torch
 
-from . import _lib, executor, ops, preprocess
+from . import _lib, executor, ops, preprocess, sync_bn
 
 
 class _MaskedMean(torch.autograd.Function):
@@ -196,19 +196,23 @@ class _Inputs:
         self.n_host = torch.zeros((self.SLOTS, ns), dtype=torch.int32).pin_memory()
         self._stage_ev, self._stage = [None] * self.SLOTS, 0
 
+    def fits(self, batch):
+        """Every stream of `batch` fits the input buffers."""
+        if self.fe is not None:
+            return all(batch['points' + c].shape[0] <= self.raw[c].shape[0] for c in self.copy_sfx())
+        key = 'points' if self.vox is not None else 'voxel_features'
+        return all(batch[key + st.sfx].shape[0] <= (st.cap_pts if self.vox is not None else st.cap0) for st in self.streams)
+
     def load(self, batch, transforms):
         """Copy one batch into the buffers (asynchronous, current stream), with `transforms` (one per copy) for the projection
         blocks; False (nothing copied) when a stream does not fit.  Rows a larger earlier batch left behind are reset to the
         tail values, so that the voxeliser drops them and the published input index set (x_conv1's indices, which are the
         coordinate buffer) keeps its -1 tail."""
-        if self.fe is not None:
-            if any(batch['points' + c].shape[0] > self.raw[c].shape[0] for c in self.copy_sfx()):
-                return False
-        else:
+        if not self.fits(batch):
+            return False
+        if self.fe is None:
             key = 'points' if self.vox is not None else 'voxel_features'
             ns = [batch[key + st.sfx].shape[0] for st in self.streams]
-            if any(n > (st.cap_pts if self.vox is not None else st.cap0) for st, n in zip(self.streams, ns)):
-                return False
         slot = self._stage
         self._stage = (slot + 1) % self.SLOTS
         if self._stage_ev[slot] is not None:
@@ -445,7 +449,10 @@ class GraphedStep(_Captured):
         The exact and warm-up runs of a capture update nothing, and a re-capture keeps the optimizer's state.  Parameters are
         updated in place at fixed addresses: the executor re-casts its bf16 operands from them in every replay, so the next
         replay computes with the new weights with no further action.  A world size above one is refused: the gradient
-        all-reduce has to sit between backward and update (use parallel.allreduce_gradients and the eager step())."""
+        all-reduce has to sit between backward and update (use parallel.allreduce_gradients and the eager step()).
+
+        SyncBatchNorm over more than one rank: the graph replays the exchanges' all-reduces, and every call first agrees with
+        the other ranks on whether to grow and re-capture (_call_in_step), so that all ranks re-capture together."""
         self.model, self.loss_fn = model, loss_fn
         self.params = list(model.parameters()) if params is None else list(params)
         super().__init__(self.params[0].device, voxelizer, margin, grain, warmup)
@@ -457,6 +464,7 @@ class GraphedStep(_Captured):
         self.optimizer, self.max_grad_norm = optimizer, max_grad_norm
         self._binding = None          # the optimizer's segment table of the current capture (set by _bind_optimizer)
         self.check_overflow = check_overflow
+        self._group = None            # (SyncBatchNorm across ranks, its process group): _rank_group, on the first call
         self.inputs = _Inputs(getattr(model, 'static_streams', ('',)), self.vox, self._vox_arg)
 
     @property
@@ -519,10 +527,37 @@ class GraphedStep(_Captured):
         self._binding = None
         self.loss, = self._capture(batch, self._exact, self._warm, [self._static_step], self._bind_optimizer)
 
+    def _rank_group(self):
+        """(True, process group) when the model's SyncBatchNorm layers exchange over more than one rank, else (False, None)."""
+        if self._group is None:
+            sync = [m for m in self.model.modules() if isinstance(m, torch.nn.SyncBatchNorm)]
+            self._group = (True, sync[0].process_group) if sync and sync_bn.world_size(sync) > 1 else (False, None)
+        return self._group
+
+    def _call_in_step(self, batch, group):
+        """__call__ under SyncBatchNorm across ranks.  A re-capture runs eager steps whose exchanges are real collectives, so
+        the ranks must grow and re-capture together: the decision is one all-reduce (MAX) of [largest overflow so far, this
+        batch does not fit], taken after the previous replay has finished (its flags are then in on every rank).  This waits
+        for the previous replay on every call: the host does not run ahead of the GPU in this mode."""
+        torch.cuda.current_stream(self.dev).synchronize()
+        worst = self.flags.worst() if self.check_overflow else 0
+        vote = torch.tensor([worst, 0 if self.inputs.fits(batch) else 1], dtype=torch.int32, device=self.dev)
+        torch.distributed.all_reduce(vote, op=torch.distributed.ReduceOp.MAX, group=group)
+        if max(vote.tolist()):
+            self._grow(batch)
+        assert self._load(batch)
+        self.graphs[0].replay()
+        if self.check_overflow:
+            self.flags.push()
+        return self.loss
+
     def __call__(self, batch):
         """-> the step's loss (a device tensor owned by the graph: read or copy it before the next call)."""
         if not self.graphs:
             self._recapture(batch)
+        sync, group = self._rank_group()
+        if sync:
+            return self._call_in_step(batch, group)
         if self.optimizer is not None:
             self.optimizer.stage_hyper()
             if self.check_overflow:
@@ -600,6 +635,9 @@ class PipelinedStep:
                              'in-graph update: pass optimizer= to GraphedStep, or call the optimizer\'s step() after each call')
         if (kwargs.get('voxelizer') or {}).get('input_discard') is not None:
             raise ValueError('PipelinedStep does not run the StVD input front end (voxelizer input_discard): use GraphedStep')
+        if sync_bn.world_size(list(model.modules())) > 1:
+            raise ValueError('PipelinedStep runs the feature phase of step t beside the index phase of step t+1 and has no '
+                             'SyncBatchNorm exchange across ranks: use GraphedStep')
         if streams != ('',):
             raise ValueError('PipelinedStep phases a one-stream backbone (VirConvL8x); %s has the input streams %s, which have '
                              'no phased form: use GraphedStep' % (type(model).__name__, streams))

@@ -16,7 +16,7 @@ from typing import List
 import torch
 import torch.nn as nn
 
-from . import _lib, ops
+from . import _lib, ops, sync_bn
 from ._lib import check
 from .roi_pool import VoxelQueryAndGrouping, _i32
 
@@ -66,7 +66,7 @@ class _VoxelPool(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, features_in, w_pos, gamma, beta, xyz, new_xyz, new_coords, point_indices, bn, max_range, radius,
-                nsample):
+                nsample, reducer, tag):
         lib = _lib.load()
         dev = features_in.device
         N, C = features_in.shape
@@ -81,11 +81,25 @@ class _VoxelPool(torch.autograd.Function):
         scale = torch.empty((C,), dtype=torch.float32, device=dev)
         shift = torch.empty((C,), dtype=torch.float32, device=dev)
         stat = torch.empty((C, 2), dtype=torch.float64, device=dev)
-        check(lib.vc_voxel_pool_bn_fold(C, n, int(training), ops._p(moments), w32.data_ptr(), gamma.data_ptr(),
-                                        beta.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
-                                        bn.num_batches_tracked.data_ptr(), float(bn.eps),
-                                        -1.0 if bn.momentum is None else float(bn.momentum), scale.data_ptr(),
-                                        shift.data_ptr(), stat.data_ptr(), ops._stream()), 'vc_voxel_pool_bn_fold')
+        momentum = -1.0 if bn.momentum is None else float(bn.momentum)
+        sync = reducer is not None and training
+        if sync:
+            # SyncBatchNorm: [moments, slot count] summed over the ranks, the statistics over the union of their slots
+            m10 = torch.empty((10,), dtype=torch.float64, device=dev)
+            m10[:9].copy_(moments)
+            m10[9:].fill_(float(n))
+            reducer(m10, (tag, 0, 'forward'))
+            check(lib.vc_voxel_pool_bn_fold_sync(C, 1, m10.data_ptr(), w32.data_ptr(), gamma.data_ptr(), beta.data_ptr(),
+                                                 bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
+                                                 bn.num_batches_tracked.data_ptr(), float(bn.eps), momentum, scale.data_ptr(),
+                                                 shift.data_ptr(), stat.data_ptr(), ops._stream()), 'vc_voxel_pool_bn_fold_sync')
+            ctx.sync = (reducer, tag, m10)
+        else:
+            check(lib.vc_voxel_pool_bn_fold(C, n, int(training), ops._p(moments), w32.data_ptr(), gamma.data_ptr(),
+                                            beta.data_ptr(), bn.running_mean.data_ptr(), bn.running_var.data_ptr(),
+                                            bn.num_batches_tracked.data_ptr(), float(bn.eps), momentum, scale.data_ptr(),
+                                            shift.data_ptr(), stat.data_ptr(), ops._stream()), 'vc_voxel_pool_bn_fold')
+            ctx.sync = None
         pooled = torch.empty((M, C), dtype=torch.float32, device=dev)
         argmax = torch.empty((M, C), dtype=torch.uint8, device=dev)
         check(lib.vc_voxel_pool_fwd(M, C, int(nsample), features_in.data_ptr(), xyz.data_ptr(), new_xyz.data_ptr(),
@@ -126,13 +140,24 @@ class _VoxelPool(torch.autograd.Function):
         dw = torch.empty((C, 3, 1, 1), dtype=torch.float32, device=dev)
         dgamma = torch.empty((C,), dtype=torch.float32, device=dev)
         dbeta = torch.empty((C,), dtype=torch.float32, device=dev)
-        check(lib.vc_voxel_pool_bn_grad(C, n, int(training), sums.data_ptr(), moments.data_ptr() if training else None,
-                                        w32.data_ptr(), gamma.data_ptr(), stat.data_ptr(), dw.data_ptr(), dgamma.data_ptr(),
-                                        dbeta.data_ptr(), ops._stream()), 'vc_voxel_pool_bn_grad')
-        return grad_features_in, dw, dgamma, dbeta, None, None, None, None, None, None, None, None
+        if ctx.sync is not None:
+            # the [C, 4] sums over all ranks for the coupling term of dw; dgamma / dbeta and the local sum dy * r stay local
+            reducer, tag, m10 = ctx.sync
+            gsums = sums.clone()
+            reducer(gsums, (tag, 0, 'backward'))
+            check(lib.vc_voxel_pool_bn_grad_sync(C, m10[9:].data_ptr(), sums.data_ptr(), gsums.data_ptr(), moments.data_ptr(),
+                                                 w32.data_ptr(), gamma.data_ptr(), stat.data_ptr(), dw.data_ptr(),
+                                                 dgamma.data_ptr(), dbeta.data_ptr(), ops._stream()),
+                  'vc_voxel_pool_bn_grad_sync')
+        else:
+            check(lib.vc_voxel_pool_bn_grad(C, n, int(training), sums.data_ptr(), moments.data_ptr() if training else None,
+                                            w32.data_ptr(), gamma.data_ptr(), stat.data_ptr(), dw.data_ptr(), dgamma.data_ptr(),
+                                            dbeta.data_ptr(), ops._stream()), 'vc_voxel_pool_bn_grad')
+        return grad_features_in, dw, dgamma, dbeta, None, None, None, None, None, None, None, None, None, None
 
 
-def voxel_pool(features_in, xyz, new_xyz, new_coords, voxel2point_indices, mlp_pos, max_range, radius, nsample):
+def voxel_pool(features_in, xyz, new_xyz, new_coords, voxel2point_indices, mlp_pos, max_range, radius, nsample, owner=None,
+               tag=0):
     """One grouper of NeighborVoxelSAModuleMSG between mlps_in[k] and mlps_out[k], fused.
 
     features_in [N, C] fp32 (the output of mlps_in[k], rows as in voxel2point_indices), xyz [N, 3], new_xyz [M, 3],
@@ -141,19 +166,26 @@ def voxel_pool(features_in, xyz, new_xyz, new_coords, voxel2point_indices, mlp_p
     M * nsample slots and its running statistics advance.
     -> pooled [M, C] fp32 (differentiable in features_in and mlp_pos's parameters), argmax [M, C] uint8 (first maximising
     slot), idx [M, nsample] int32 (global rows), empty [M] bool, moments [9] float64 of the relative positions (train mode;
-    None in eval mode)."""
+    None in eval mode).
+    A SyncBatchNorm mlp_pos[1] in train mode takes its statistics over the ranks of its process group (sync_bn; moments and
+    gradient sums exchanged through `owner.bn_reducer` when set, else all_reduce; `tag` names the grouper in the reducer's
+    key).  At world size 1 without a reducer it is the BatchNorm2d above."""
     ops._require_cuda(features_in, xyz, new_xyz, new_coords, voxel2point_indices)
     assert features_in.dtype == torch.float32 and xyz.dtype == torch.float32 and new_xyz.dtype == torch.float32
     conv, bn = mlp_pos[0], mlp_pos[1]
     pooled, argmax, idx, empty, moments = _VoxelPool.apply(
         features_in.contiguous(), conv.weight, bn.weight, bn.bias, xyz.contiguous(), new_xyz.contiguous(), _i32(new_coords),
-        _i32(voxel2point_indices), bn, tuple(max_range), radius, int(nsample))
+        _i32(voxel2point_indices), bn, tuple(max_range), radius, int(nsample), sync_bn.reducer_for(owner, [bn]),
+        ('voxel_pool', tag))
     return pooled, argmax, idx, empty.bool(), moments
 
 
 class NeighborVoxelSAModuleMSG(nn.Module):
     """`NeighborVoxelSAModuleMSG` (voxel_pool_modules.py:8-130): same constructor, submodules (state_dict keys and
-    shapes), initialisation, forward signature and output, with each grouper's query .. max-pool fused (voxel_pool)."""
+    shapes), initialisation, forward signature and output, with each grouper's query .. max-pool fused (voxel_pool).
+    `bn_reducer` (sync_bn) replaces the all-reduce of a SyncBatchNorm position branch's exchanged sums."""
+
+    bn_reducer = None
 
     def __init__(self, *, query_ranges: List[List[int]], radii: List[float], nsamples: List[int], mlps: List[List[int]],
                  use_xyz: bool = True, pool_method='max_pool'):
@@ -213,7 +245,7 @@ class NeighborVoxelSAModuleMSG(nn.Module):
             features_in = features_in.view(-1, features_in.shape[-1])
             g = self.groupers[k]
             pooled = voxel_pool(features_in, xyz, new_xyz, new_coords, v2p, self.mlps_pos[k], g.max_range, g.radius,
-                                g.nsample)[0]
+                                g.nsample, owner=self, tag=k)[0]
             new_features = self.mlps_out[k](pooled.t().unsqueeze(0))       # (1, C, M)
             new_features_list.append(new_features.squeeze(dim=0).permute(1, 0))
         return torch.cat(new_features_list, dim=1)
