@@ -60,6 +60,12 @@ int vc_set_tc_variant(int variant);
  * unless 2 is forced or no index kernel runs beside it (the plan executor's static mode with side streams, which enqueues
  * the whole index phase before the first feature kernel). */
 int vc_conv_tc2_config(int ctas_per_sm);
+/* Host-only: the shared-memory plan the persistent tensor-core conv takes for a cin -> cout layer with K offsets under the
+ * current vc_conv_tc2_config, for a launch that takes BatchNorm channel sums (bn_sums != 0: the forward of a conv + BN layer,
+ * whose epilogue needs a staging buffer) or not (a dgrad, a plain forward).  out[0] = ring stages, out[1] = 1 when all K
+ * weight slices stay resident in shared memory (else they stream with the ring), out[2] = CTAs per SM, out[3] = dynamic
+ * shared memory per CTA in bytes. */
+int vc_conv_tc2_plan(int cin, int cout, int K, int bn_sums, int32_t* out);
 /* The plan executor's weight-gradient launches (csrc/wgrad_tc3.cu): variant must be 1 (the only kernel); max_ctas > 0 caps
  * the CTAs of each launch, over all its passes; 0, the default: half the SMs for each pass, so that each CTA shares its
  * SM with a dgrad CTA of the main stream. */

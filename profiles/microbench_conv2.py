@@ -2,7 +2,10 @@
     python profiles/microbench_conv2.py            # VIRCONV_LIB=<.so> times another build of the library
 For every conv layer of VirConv-L on the bench batch: forward and gather-dgrad through the C ABI (weight-image prep
 launch included in both), median of 7 CUDA-event timings with the L2 flushed in between, and the maximum relative
-difference to the fp32 kernel fed bf16-rounded operands."""
+difference to the fp32 kernel fed bf16-rounded operands.  Each layer line ends with the kernel's shared-memory plan
+(vc_conv_tc2_plan: ring stages S, resident weights w or streamed s, CTAs per SM) for the forward timed here, the forward
+with BatchNorm sums of the training step (fwd+bn) and the dgrad."""
+import ctypes
 import os
 import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -61,6 +64,12 @@ def bf16r(t):
     return t.to(torch.bfloat16).to(torch.float32)
 
 
+def plan(kc, nr, K, bn_sums=0):
+    out = (ctypes.c_int32 * 4)()
+    _lib.check(lib.vc_conv_tc2_plan(kc, nr, K, bn_sums, out), 'vc_conv_tc2_plan')
+    return f'S={out[0]}{"w" if out[1] else "s"}x{out[2]}'
+
+
 tot = {}
 for li, (feats, weight, rb) in enumerate(calls):
     cout, cin = weight.shape[0], weight.shape[-1]
@@ -91,6 +100,7 @@ for li, (feats, weight, rb) in enumerate(calls):
     print(f'L{li:02d} {"subm" if rb.subm else "conv"}{rb.ndim}d {cin:2d}->{cout:2d} K={rb.K:2d} N_in={feats.shape[0]:6d} N_out={rb.n_out:6d} '
           f'P={P:8d} ' + ' '.join(f'{k}={v:6.1f}us' for k, v in sorted(res.items())) +
           f'  fwd: {by / res["fwd"] / 1e3:7.1f} GB/s {2 * P * cin * cout / res["fwd"] / 1e6:6.1f} TF/s'
-          f'  maxrel fwd {d_f:.1e}' + (f' dgrad {d_d:.1e}' if d_d is not None else ''), flush=True)
+          f'  maxrel fwd {d_f:.1e}' + (f' dgrad {d_d:.1e}' if d_d is not None else '') +
+          f'  plan fwd {plan(cin, cout, rb.K)} fwd+bn {plan(cin, cout, rb.K, 1)}' + (f' dgrad {plan(cout, cin, rb.K)}' if gather_dgrad else ''), flush=True)
 print('TOTAL us', {k: round(v, 1) for k, v in sorted(tot.items())})
 print('error flag', int(err.item()))

@@ -33,6 +33,7 @@ SIGNATURES = {
     'vc_set_conv_bn_fused': (_I, [_I]),
     'vc_set_tc_variant': (_I, [_I]),
     'vc_conv_tc2_config': (_I, [_I]),
+    'vc_conv_tc2_plan': (_I, [_I, _I, _I, _I, _HOST]),
     'vc_conv_wgrad_tc3_config': (_I, [_I, _I]),
     'vc_wgrad_launch_geometry': (_I, [_I, _I, _I, _I, _I, _HOST]),
     'vc_subm_rulebook_ws_bytes': (_Z, [_I]),

@@ -8,10 +8,11 @@
 // 448 threads per CTA:
 //   warps 0-7   two consumer warpgroups, one per 64-row half of the tile: wait for a ring stage, issue its wgmma.mma_async
 //               (m64 x C_out x 16, accumulator in registers), release the stage once the MMAs reading it have completed
-//               (wgmma.wait_group 1: the next stage's MMAs are already queued); after the tile's last stage the accumulator
-//               goes through a half-tile shared staging buffer to coalesced fp32 stores (+ addend); BatchNorm channel sums per
-//               tile in fp32 over fixed row groups, accumulated per CTA in float64 (scheduling independent), one set of
-//               atomics per CTA;
+//               (wgmma.wait_group 1: the next stage's MMAs are already queued); after the tile's last stage each warpgroup
+//               stores its 64 rows straight from the accumulator registers (fp32, + addend).  A launch that takes BatchNorm
+//               channel sums instead sends the accumulator through a half-tile shared staging buffer to coalesced fp32
+//               stores, with the sums per tile in fp32 over fixed row groups, accumulated per CTA in float64 (scheduling
+//               independent), one set of atomics per CTA;
 //   warp  8     tile scheduler + table loader: claims a tile, cp.async's its K x 128 slice of the neighbour table into one of
 //               2-4 shared buffers one tile ahead, fixes rows beyond the (device) row count to -1 and — for the dgrad of a
 //               strided conv — lists the kernel offsets that reach the tile at all (lane-parallel scan);
@@ -68,7 +69,7 @@ struct PCfg {
     static constexpr int A_BYTES = TCM * ROWB;               // one offset's gathered tile
     static constexpr int B_BYTES = NR * ROWB;                // one offset's weight slice
     static constexpr int STG_LD = NR + 1;                    // staging row pitch (floats)
-    static constexpr int STG_BYTES = (TCM / 2) * STG_LD * 4;   // half a tile at a time
+    static constexpr int STG_BYTES = (TCM / 2) * STG_LD * 4;   // half a tile at a time (launches with BatchNorm sums only)
 };
 
 struct PArgs {
@@ -175,7 +176,7 @@ __global__ void __launch_bounds__(P_THREADS, P_GROUPS == 1 ? 2 : 1) tc_conv_pers
     unsigned char* ring = smem_raw;                                              // [S][G x A (| G x B)]
     unsigned char* wimg_s = smem_raw + (size_t)S * stage_bytes;                  // [K][B] when resident
     int* nbr_s = reinterpret_cast<int*>(wimg_s + wres_bytes);                    // [P_NTB][K][128]
-    float* stg = reinterpret_cast<float*>(nbr_s + (size_t)a.ntb_alloc * K * TCM); // [64][STG_LD]
+    float* stg = reinterpret_cast<float*>(nbr_s + (size_t)a.ntb_alloc * K * TCM); // [64][STG_LD] (with BN sums)
     __shared__ __align__(8) uint64_t full_bar[P_MAX_STAGES];
     __shared__ __align__(8) uint64_t empty_bar[P_MAX_STAGES];
     __shared__ __align__(8) uint64_t tbl_full[P_NTB], tbl_empty[P_NTB];
@@ -184,7 +185,9 @@ __global__ void __launch_bounds__(P_THREADS, P_GROUPS == 1 ? 2 : 1) tc_conv_pers
     __shared__ int klist_s[P_NTB][MAXK_TC];
     __shared__ double red_s[2][P_CONS_THREADS];
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    // the role index read through a shuffle: the compiler can then tell that the consumer branch is warp-uniform, and does not
+    // serialize its wgmma instructions
+    const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
 #ifdef VC_TC_TRACE
     long long* const trc = blockIdx.x == 0 ? g_trace2 : nullptr;      // (read once: a stamp must not cost a global load)
 #endif
@@ -515,6 +518,37 @@ __global__ void __launch_bounds__(P_THREADS, P_GROUPS == 1 ? 2 : 1) tc_conv_pers
             wg_fence_acc(acc);
             if (prev >= 0 && t == 0) mbar_arrive(&empty_bar[prev]);
             const bool empty_tile = nk == 0;
+            if (a.bn_sums == nullptr && a.bn_part == nullptr) {
+                // no BatchNorm sums: each warpgroup stores its own 64 rows straight from the accumulators, two adjacent columns
+                // per float2 (wg_col); the four lanes of a row cover 32 contiguous bytes, one sector.  The addend is loaded
+                // first (independent loads, all in flight together); the same element is read and written by this thread
+                // only, so `addend` may alias `out`.  No shared memory, and the two warpgroups do not wait for each other
+                const int r0 = base + wg * 64 + wg_row(0, t);       // this thread's rows: r0 and r0 + 8
+                const bool ok0 = r0 < n, ok1 = r0 + 8 < n;
+                if (empty_tile) {        // (the registers still hold the last tile)
+#pragma unroll
+                    for (int j = 0; j < NR / 2; ++j) acc[j] = 0.f;
+                }
+                if (a.addend != nullptr) {
+#pragma unroll
+                    for (int j = 0; j < NR / 2; j += 2) {
+                        const int c = wg_col(j, t);
+                        if (((j & 2) ? ok1 : ok0) && c < oc) {
+                            const float2 w = *reinterpret_cast<const float2*>(a.addend + (size_t)(r0 + (j & 2) * 4) * oc + c);
+                            acc[j] += w.x;
+                            acc[j + 1] += w.y;
+                        }
+                    }
+                }
+#pragma unroll
+                for (int j = 0; j < NR / 2; j += 2) {
+                    const int c = wg_col(j, t);
+                    if (((j & 2) ? ok1 : ok0) && c < oc)
+                        *reinterpret_cast<float2*>(a.out + (size_t)(r0 + (j & 2) * 4) * oc + c) = make_float2(acc[j], acc[j + 1]);
+                }
+                if (tid == 0) P_TRACE(5, tr2);
+                continue;
+            }
             // two halves of 64 rows through a [64][NR + 1] staging buffer (half the shared memory of a full-tile buffer: what
             // lets two CTAs share an SM): the warpgroup owning the half unloads its accumulator, then all 8 warps store it
             const int oc4 = oc >> 2;
@@ -619,8 +653,11 @@ done:
         ok = grid_barrier(b.bar, 2 * gridDim.x, a.err, &ok_s);
     }
     if (!ok) return;
-    float* sc_s = stg;            // (the staging buffer is dead: >= 64 x 17 floats)
-    float* sh_s = stg + oc;
+    // scale / shift in the dead operand ring (>= 2 x 16 KB; a launch without BN sums, e.g. an eval-mode BN, has no staging
+    // buffer), whose last accesses were the async proxy's (bulk copies, wgmma reads)
+    float* sc_s = reinterpret_cast<float*>(ring);
+    float* sh_s = sc_s + oc;
+    fence_async_smem();
     if (tid < oc)
         bn_channel(b.training ? __ldcg(b.sums + tid) : 0.0, b.training ? __ldcg(b.sums + oc + tid) : 0.0, tid, oc, n, b.gamma, b.beta,
                    b.running_mean, b.running_var, b.momentum, b.eps, b.training, sc_s, sh_s, blockIdx.x == 0, b.stats);
@@ -677,10 +714,11 @@ struct PPlan {
 };
 
 // shared-memory plan of one CTA under a budget: weights resident if they fit beside a ring of >= min_stages, else streamed
+// (staged: the launch takes BatchNorm sums, whose epilogue needs the staging buffer)
 template <int KC, int NR>
-bool plan_smem(int K, size_t budget, int ntb, size_t resident_max, int min_stages, PPlan& p) {
+bool plan_smem(int K, size_t budget, int ntb, size_t resident_max, int min_stages, bool staged, PPlan& p) {
     using C = PCfg<KC, NR>;
-    const size_t fixed = (size_t)ntb * K * TCM * 4 + C::STG_BYTES;
+    const size_t fixed = (size_t)ntb * K * TCM * 4 + (staged ? C::STG_BYTES : 0);
     const size_t wbytes = ((size_t)K * C::B_BYTES + 1023) & ~(size_t)1023;
     if (fixed + (size_t)min_stages * C::G * C::A_BYTES > budget) return false;
     int s_res = 0;
@@ -698,21 +736,28 @@ bool plan_smem(int K, size_t budget, int ntb, size_t resident_max, int min_stage
     return true;
 }
 
+// Two CTAs per SM (half the shared memory each, 2 table buffers) when the ring still has VC_P_MIN_STAGES2 stages: two
+// independent pipelines per SM (each a serial chain of barrier wait -> MMA issue -> release per stage) and room for CTAs
+// of another stream's kernel.  Otherwise one CTA with the whole SM.
+template <int KC, int NR>
+int choose_plan(int K, bool staged, PPlan& p, int& ctas) {
+    ctas = 1;
+    const size_t budget2 = (size_t)(227 * 1024) / 2 - 7 * 1024;      // static shared memory + 1 KB/CTA reserved by the driver
+    if (P_GROUPS == 1 && g_p_ctas != 1 && plan_smem<KC, NR>(K, budget2, 2, 28 * 1024, VC_P_MIN_STAGES2, staged, p)) {
+        ctas = 2;
+    } else if (!plan_smem<KC, NR>(K, SMEM_BUDGET, P_NTB, P_W_RESIDENT_MAX, 2, staged, p)) {
+        set_error("tensor-core conv: no room for the operand ring (K=%d, %d->%d)", K, KC, NR);
+        return VC_ERR_UNSUPPORTED;
+    }
+    return VC_OK;
+}
+
 template <int KC, int NR>
 int launch_persist(const PArgs& a0, int n_cap, cudaStream_t stream, bool* bn_done, bool coop2) {
     PArgs a = a0;
-    // Two CTAs per SM (half the shared memory each, 2 table buffers) when the ring still has VC_P_MIN_STAGES2 stages: two
-    // independent pipelines per SM (each a serial chain of barrier wait -> MMA issue -> release per stage) and room for CTAs
-    // of another stream's kernel.  Otherwise one CTA with the whole SM.
     PPlan p;
     int ctas = 1;
-    const size_t budget2 = (size_t)(227 * 1024) / 2 - 7 * 1024;      // static shared memory + 1 KB/CTA reserved by the driver
-    if (P_GROUPS == 1 && g_p_ctas != 1 && plan_smem<KC, NR>(a.K, budget2, 2, 28 * 1024, VC_P_MIN_STAGES2, p)) {
-        ctas = 2;
-    } else if (!plan_smem<KC, NR>(a.K, SMEM_BUDGET, P_NTB, P_W_RESIDENT_MAX, 2, p)) {
-        set_error("tensor-core conv: no room for the operand ring (K=%d, %d->%d)", a.K, KC, NR);
-        return VC_ERR_UNSUPPORTED;
-    }
+    if (const int rc = choose_plan<KC, NR>(a.K, a.bn_sums != nullptr || a.bn_part != nullptr, p, ctas)) return rc;
     a.S = p.S;
     a.w_resident = p.resident;
     a.ntb_alloc = p.ntb;
@@ -867,6 +912,29 @@ extern "C" int vc_debug_set_trace2(long long* buf) {
 extern "C" int vc_conv_tc2_config(int ctas_per_sm) {
     VC_CHECK_ARG(ctas_per_sm >= 0 && ctas_per_sm <= 2, "CTAs per SM must be 0 (automatic), 1 or 2");
     vc::g_p_ctas = ctas_per_sm;
+    return VC_OK;
+}
+
+extern "C" int vc_conv_tc2_plan(int cin, int cout, int K, int bn_sums, int32_t* out) {
+    VC_CHECK_ARG(out != nullptr, "null pointer");
+    if (!vc::tc2_ch_ok(cin) || !vc::tc2_ch_ok(cout) || K < 1 || K > vc::MAXK_TC) {
+        vc::set_error("tensor-core conv: unsupported shape (%d -> %d channels, K=%d)", cin, cout, K);
+        return VC_ERR_UNSUPPORTED;
+    }
+    vc::PPlan p{};
+    int ctas = 1, rc = VC_ERR_UNSUPPORTED;
+    const int kcp = vc::tc_pad16(cin), nrp = vc::tc_pad16(cout);
+#define VC_P_CASE(A, B) \
+    if (kcp == A && nrp == B) rc = vc::choose_plan<A, B>(K, bn_sums != 0, p, ctas);
+    VC_P_CASE(16, 16) VC_P_CASE(16, 32) VC_P_CASE(16, 64)
+    VC_P_CASE(32, 16) VC_P_CASE(32, 32) VC_P_CASE(32, 64)
+    VC_P_CASE(64, 16) VC_P_CASE(64, 32) VC_P_CASE(64, 64)
+#undef VC_P_CASE
+    if (rc) return rc;
+    out[0] = p.S;
+    out[1] = p.resident;
+    out[2] = ctas;
+    out[3] = (int32_t)p.smem;
     return VC_OK;
 }
 
